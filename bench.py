@@ -1,7 +1,7 @@
-"""LW-DETR inference throughput benchmark (BASELINE.json: images/sec at 640x640, per-GPU batch, N B200s).
+"""LW-DETR inference throughput benchmark (BASELINE.json: images/sec at 640x640, per-GPU batch, N H100s).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--config small] [--batch 32] [--dtype fp16]
-    python bench.py --impl reference ...      # the unmodified reference's CPU forward (baseline/_ref) on the host cores
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--config small] [--batch 32] [--dtype fp16] [--dump-outputs DIR]
+    python bench.py --impl reference ...      # the unmodified reference's CPU forward (oracle/_ref) on the host cores
     torchrun --nproc-per-node N bench.py --gpus N ...   # one process per GPU, image-sharded replicas
 
 One "step" = one forward pass of `batch` synthetic 640x640 images per GPU through the C-ABI engine
@@ -30,15 +30,8 @@ FLOPS_PER_IMAGE = {"tiny": 21.40e9, "small": 31.76e9, "medium": 83.93e9, "large"
 
 
 def peaks():
-    p = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            m = json.load(f)
-        p.update({k: m[k] for k in ("hbm_gbs", "bf16_tflops", "bf16_tflops_sustained") if k in m})
-        p["source"] = "measured"
-    except Exception:
-        pass
-    return p
+    # H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 / FP16 - ceilings, not rates this project reached
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler(threading.Thread):
@@ -103,8 +96,7 @@ class ClockSampler(threading.Thread):
 def cpu_reference_run(cfg_name, steps, warmup, sample_batch, dtype_name, full_batch=0, budget_s=0.0):
     """The reference's CPU forward on the host cores, fp32, all the threads that help.
     kind "reference": the UNMODIFIED reference model built by its own models.build_model(args) (tools/ref_import.py;
-    /root/reference in the build container, the byte-identical copy under baseline/_ref on the GPU box, staged by
-    tools/vendor_reference.py at build() time), cross-attention through its ms_deform_attn_core_pytorch path - the path
+    the byte-identical copy under oracle/_ref, staged by oracle/vendor_reference.py at build() time), cross-attention through its ms_deform_attn_core_pytorch path - the path
     the reference itself takes on the CPU.  kind "port": the oracle port (oracle/lwdetr_oracle.py), only when no
     reference tree is available."""
     sys.path.insert(0, os.path.join(ROOT, "tools"))
@@ -157,7 +149,7 @@ def cpu_reference_run(cfg_name, steps, warmup, sample_batch, dtype_name, full_ba
         fwd()
     dt = time.perf_counter() - t0
     per_step = sample_batch * chunks
-    what = "unmodified reference models.build_model forward (baseline/_ref)" if kind == "reference" else "fp32 torch CPU oracle port"
+    what = "unmodified reference models.build_model forward (oracle/_ref)" if kind == "reference" else "fp32 torch CPU oracle port"
     return {"value": steps * per_step / dt, "unit": "images/s", "cores": torch.get_num_threads(), "kind": kind,
             "sample": "%d step(s) of %d synthetic 640x640 image(s) each (%d forward(s) of %d), LW-DETR-%s, fp32, %s, best of thread counts up to %d"
                       % (steps, per_step, chunks, sample_batch, cfg_name, what, ncpu),
@@ -178,6 +170,8 @@ def main():
     ap.add_argument("--profile-out", default=None, help="write the per-op timing table (JSON) here")
     ap.add_argument("--no-per-config", action="store_true", help="skip the per_config block (the other four BASELINE configs, N = 1 only)")
     ap.add_argument("--e2e-input", default="uint8", choices=["uint8", "fp32"], help="what the end-to-end arm holds on the host")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step returned (pred_logits, pred_boxes) as DIR/<name>.npy, float32")
     a = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -217,7 +211,7 @@ def main():
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
     r = measure_config(cfg_name, batch, dtype_name, a.steps, warmup, dev, rank, world, local, graph=not a.no_graph, pdl=not a.no_pdl,
-                       profile_out=a.profile_out, clocks=True, e2e_input=a.e2e_input)
+                       profile_out=a.profile_out, clocks=True, e2e_input=a.e2e_input, dump_outputs=a.dump_outputs if rank == 0 else None)
 
     cpu = None
     if rank == 0 and world == 1:
@@ -228,7 +222,7 @@ def main():
             cpu = {"error": repr(ex)}
 
     # ---- the other BASELINE configurations, measured in the same run (N = 1 only; a few seconds each): the bench line of
-    # the headline config stays the contract, this block is the driver-visible evidence for the rest of the model family
+    # the headline config stays the contract, this block is the evidence for the rest of the model family
     per_config = None
     if rank == 0 and world == 1 and not a.no_per_config:
         per_config = {}
@@ -264,7 +258,7 @@ def main():
 
 
 def measure_config(cfg_name, batch, dtype_name, steps, warmup, dev, rank, world, local, graph=True, pdl=True, profile_out=None, clocks=True,
-                   e2e_input="uint8"):
+                   e2e_input="uint8", dump_outputs=None):
     """One LW-DETR configuration on this rank's GPU: device-resident throughput, end-to-end throughput through the public
     module call with host inputs, batch-1 latencies and the per-kernel table.  Returns a dict (see main)."""
     import torch.distributed as dist
@@ -292,7 +286,8 @@ def measure_config(cfg_name, batch, dtype_name, steps, warmup, dev, rank, world,
         replicas_agree = bool(all(torch.equal(s_, allsig[0]) for s_ in allsig))     # bit-identical replicas after the broadcast
     eng.set_option("cuda_graph", 1 if graph else 0)
     eng.set_option("pdl", 1 if pdl else 0)
-    # inputs: two distinct device batches (fp32, 4.9 MB/image => larger than the 126 MB L2 at batch >= 26)
+    # inputs: two distinct device batches (fp32, 4.9 MB/image => larger than the 50 MB L2 at batch >= 11), seeded: the same
+    # arguments give the same inputs in every run
     xs = [synth_images(batch, seed=100 * rank + i).to(dev) for i in range(2)]
     in_bytes = xs[0].numel() * 4
 
@@ -316,7 +311,10 @@ def measure_config(cfg_name, batch, dtype_name, steps, warmup, dev, rank, world,
         barrier()
         return ms.item()
 
-    dev_step = lambda i: eng.forward(xs[i & 1], want_aux=False)
+    last = {}
+
+    def dev_step(i):
+        last["out"] = eng.forward(xs[i & 1], want_aux=False)
     for i in range(warmup):
         dev_step(i)
     sampler = ClockSampler(local)
@@ -326,6 +324,12 @@ def measure_config(cfg_name, batch, dtype_name, steps, warmup, dev, rank, world,
     load_t0 = time.time()
     ms_total = timed(dev_step, steps)
     load_t1 = time.time()
+    if dump_outputs:
+        # what the last timed step handed to its caller (batch x queries x 91 logits and x 4 boxes: a few MB, stored whole)
+        import numpy as np
+        os.makedirs(dump_outputs, exist_ok=True)
+        for k in ("pred_logits", "pred_boxes"):
+            np.save(os.path.join(dump_outputs, k + ".npy"), last["out"][k].float().cpu().numpy())
     if rank == 0 and clocks:
         # a short timed region can fall between two 100 ms nvidia-smi samples: keep the same step running
         # (untimed) until at least three samples were taken under this load
@@ -402,7 +406,7 @@ def measure_config(cfg_name, batch, dtype_name, steps, warmup, dev, rank, world,
         return world * batch * steps / (ms.item() * 1e-3), host[0].numel() * host[0].element_size()
 
     d2h = hl[0].numel() * 4 + hb[0].numel() * 4
-    d2h_stream = torch.cuda.Stream(device=dev)         # read-back on its own stream: +3 % end to end in a same-process A/B on the B200
+    d2h_stream = torch.cuda.Stream(device=dev)         # read-back on its own stream: so the next forward does not queue behind the copy
     e2e_value, h2d = e2e_measure(e2e_input, d2h_stream)
     other = "fp32" if e2e_input == "uint8" else "uint8"
     e2e_other, h2d_other = e2e_measure(other, d2h_stream)
@@ -478,31 +482,24 @@ def measure_config(cfg_name, batch, dtype_name, steps, warmup, dev, rank, world,
         if tens_t >= hbm_t:
             ach = gfl / (gms * 1e-3) / 1e12
             roof = {"kernel": name, "launches_per_step": n, "bound": "tensor", "achieved": ach, "peak": pk["bf16_tflops"], "unit": "TFLOP/s",
-                    "frac": ach / pk["bf16_tflops"], "traffic": None, "share_of_step": gms / tot, "peak_source": pk["source"] + " (burst)"}
+                    "frac": ach / pk["bf16_tflops"], "traffic": None, "share_of_step": gms / tot, "peak_source": pk["source"]}
         else:
             ach = gby / (gms * 1e-3) / 1e9
             roof = {"kernel": name, "launches_per_step": n, "bound": "hbm", "achieved": ach, "peak": pk["hbm_gbs"], "unit": "GB/s",
                     "frac": ach / pk["hbm_gbs"], "traffic": None, "share_of_step": gms / tot, "peak_source": pk["source"]}
-        # DRAM traffic per launch of this kernel from a committed ncu --set full capture (profiles/kernel_traffic.json);
-        # null when no capture exists for this config / batch / dtype.  Compare with the algorithmic bytes per launch.
         roof["algorithmic_bytes_per_launch"] = gby / n
-        try:
-            with open(os.path.join(ROOT, "profiles", "kernel_traffic.json")) as f:
-                roof["traffic"] = json.load(f).get("%s:%d:%s:%s" % (cfg_name, batch, dtype_name, name))
-        except Exception:
-            pass
         if name.endswith("attn"):
             # attention at head dim 16/32 is bound by exp (MUFU, 16 ex2/clk/SM), not by the tensor pipe: report that too
             dh = (cfg.vit_dim // cfg.vit_heads) if name in ("glb_attn", "win_attn") else (cfg.hidden_dim // cfg.sa_nheads)
             gexp = gfl / (4.0 * dh) / (gms * 1e-3) / 1e9
-            mufu_peak = 16 * 148 * 1.965                      # Gexp/s at the maximum SM clock
+            mufu_peak = 16 * 132 * 1.98                       # Gexp/s at the H100 SXM's maximum SM clock
             roof["exp_bound"] = {"achieved_gexp_s": gexp, "peak_gexp_s": mufu_peak, "frac": gexp / mufu_peak,
-                                 "note": "softmax exp count / MUFU.EX2 throughput (16/clk/SM x 148 SMs x 1.965 GHz)"}
+                                 "note": "softmax exp count / MUFU.EX2 throughput (16/clk/SM x 132 SMs x 1.98 GHz)"}
         # per-op bandwidths come from back-to-back repeats of the same op (Engine::profile_ops): working sets below the
-        # 126 MB L2 are L2-warm there, so "gbps" of a small op is NOT an HBM figure - it is labelled as such
+        # 50 MB L2 are L2-warm there, so "gbps" of a small op is NOT an HBM figure - it is labelled as such
         table = [{"op": k, "launches": v[3], "ms": v[0], "share": v[0] / tot, "gflop": v[1] / 1e9, "mbytes": v[2] / 1e6,
                   "tflops": (v[1] / (v[0] * 1e-3) / 1e12) if v[0] > 0 else 0, "gbps": (v[2] / (v[0] * 1e-3) / 1e9) if v[0] > 0 else 0,
-                  "gbps_is_l2_warm": bool(v[2] / max(1, v[3]) < 126e6)}
+                  "gbps_is_l2_warm": bool(v[2] / max(1, v[3]) < 50e6)}
                  for k, v in sorted(groups.items(), key=lambda kv: -kv[1][0])]
         if profile_out:
             with open(profile_out, "w") as f:
@@ -512,7 +509,7 @@ def measure_config(cfg_name, batch, dtype_name, steps, warmup, dev, rank, world,
     step_bytes = sum(p[2] for p in prof) if prof else 0.0
     tensor_frac = value * FLOPS_PER_IMAGE[cfg_name] / (peaks()["bf16_tflops_sustained"] * 1e12)
     config_extra = {"l2": "no flush needed: inputs alternate between two fp32 batches of %.0f MB and one step streams %.1f GB of "
-                          "activations and weights through the kernels (>> 126 MB L2), so nothing survives from step to step"
+                          "activations and weights through the kernels (>> 50 MB L2), so nothing survives from step to step"
                           % (in_bytes / 1e6, step_bytes / 1e9),
                     "cuda_graph": graph, "pdl": pdl, "weight_broadcast_bytes": bcast_bytes, "replicas_bit_identical": replicas_agree,
                     "model_gflop_per_image": FLOPS_PER_IMAGE[cfg_name] / 1e9, "whole_model_tensor_frac_of_sustained": tensor_frac}

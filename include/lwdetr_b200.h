@@ -1,5 +1,5 @@
 /*
- * lwdetr_b200 - C ABI of the B200-native LW-DETR inference path.
+ * lwdetr_b200 - C ABI of the CUDA-native (sm_90a) LW-DETR inference path.
  *
  * Every entry point takes plain pointers and sizes (no torch types).  Device pointers are CUDA
  * device addresses on the current device; `stream` is a cudaStream_t passed as void* (NULL = the
@@ -25,9 +25,6 @@ enum { LWDETR_F16 = 0, LWDETR_BF16 = 1 };
 enum { LWDETR_ACT_NONE = 0, LWDETR_ACT_RELU = 1, LWDETR_ACT_GELU = 2, LWDETR_ACT_SILU = 3 };
 
 LWDETR_API const char* lwdetr_last_error(void);
-/* Debug aid: with LWDETR_B200_DEBUG_WAIT=1 in the environment the attention kernel's barrier waits time out after ~50 ms and
- * record where; this prints the records to stderr (they live in mapped host memory and survive the device fault). */
-LWDETR_API int lwdetr_debug_dump(void);
 LWDETR_API int lwdetr_abi_version(void);
 
 /* ------------------------------------------------------------------------------------------------
@@ -36,7 +33,7 @@ LWDETR_API int lwdetr_abi_version(void);
  * ---------------------------------------------------------------------------------------------- */
 
 /* out[rowmap(m), n] = resid[m', n] + gamma[n] * act(sum_k A[m,k] W[n,k] + bias[n])
- * tcgen05/TMA GEMM standing in for F.linear / 1x1 conv / ConvTranspose2d(k2,s2)
+ * wgmma/TMA GEMM standing in for F.linear / 1x1 conv / ConvTranspose2d(k2,s2)
  * (models/backbone/vit.py:120-140,206-220; projector.py:85-98,165-190; transformer.py:27-39).
  *   A [M, lda] 16-bit, W [N, K] 16-bit, K % 64 == 0, bias/gamma fp32 [N] or NULL,
  *   resid 16-bit [*, ld_resid] or NULL (row m % resid_mod when resid_mod > 0),

@@ -1,6 +1,6 @@
 """Drop-in for the reference's compiled pybind11 module `MultiScaleDeformableAttention`
 (models/ops/setup.py:53, src/vision.cpp:13-16): same module name, same two functions, same argument order, so
-models/ops/functions/ms_deform_attn_func.py:23 (`import MultiScaleDeformableAttention as MSDA`) binds to the B200
+models/ops/functions/ms_deform_attn_func.py:23 (`import MultiScaleDeformableAttention as MSDA`) binds to the CUDA-native
 kernels without any edit when lw-detr_b200/ precedes the reference tree on PYTHONPATH.
 
     ms_deform_attn_forward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, im2col_step) -> output
@@ -10,7 +10,7 @@ kernels without any edit when lw-detr_b200/ precedes the reference tree on PYTHO
 Both go through the C ABI (include/lwdetr_b200.h: lwdetr_ms_deform_attn_forward / _backward).  Like the reference
 op (ms_deform_attn.h:19-35) they raise RuntimeError for CPU tensors ("Not implemented on the CPU") and for
 non-contiguous tensors; unlike it the forward also accepts float16 / bfloat16, and float64 inputs are computed in
-float32 (B200 has no useful fp64 rate) and returned as float64."""
+float32 (the H100's fp64 rate is no use to a gather) and returned as float64."""
 import torch
 
 from b200 import capi

@@ -1,1 +1,1 @@
-"""Host-side glue of the B200-native LW-DETR path (ctypes binding, configs, synthetic weights)."""
+"""Host-side glue of the CUDA-native (H100, sm_90a) LW-DETR path (ctypes binding, configs, synthetic weights)."""

@@ -19,7 +19,6 @@ _vp, _i, _f, _i64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_int6
 _SIGNATURES = {
     "lwdetr_last_error": (ctypes.c_char_p, []),
     "lwdetr_abi_version": (_i, []),
-    "lwdetr_debug_dump": (_i, []),
     "lwdetr_gemm": (_i, [_i, _vp, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "lwdetr_conv3x3": (_i, [_i, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp]),
     "lwdetr_layernorm": (_i, [_i, _vp, _i, _vp, _i, _vp, _vp, _f, _i64, _i, _vp]),
@@ -275,7 +274,7 @@ class Engine:
     def __init__(self, cfg, dtype, device=None):
         import torch
         if not torch.cuda.is_available():
-            raise RuntimeError("lwdetr_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+            raise RuntimeError("lwdetr_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.cfg, self.dtype = cfg, dtype
         self._h = _vp()
         cs = config_struct(cfg)

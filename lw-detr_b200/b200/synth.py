@@ -5,7 +5,7 @@ bbox_embed layer lwdetr.py:90-91, MSDeformAttn sampling_offsets.weight / attenti
 ms_deform_attn.py:80-94, attention biases); zeros would hide bugs, so every tensor here is random
 with a scale that keeps activations O(1) through the whole network (checked in
 tests/test_oracle.py).  Values depend only on (config, seed) and the installed torch CPU RNG, so the
-same call reproduces the same weights in the build container and on the GPU box.
+same call reproduces the same weights on every machine.
 """
 import math
 

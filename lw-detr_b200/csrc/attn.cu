@@ -9,10 +9,10 @@
 //
 // Kernels in this file (register-resident flash attention: mma.sync m16n8k16 with fp32 accumulation, K/V chunks
 // in a 3-stage cp.async ring, exp2 against the running maximum of the raw scores):
-//   attn_kernel       - sequences longer than 112 tokens: global attention at head dim 16, decoder self-attention
-//   attn_short_kernel - the 100-token windows, persistent CTAs walking (window, head) items
-// Long packed-qkv sequences at head dim >= 32 are dispatched to the tcgen05 kernel in attn_tc.cu instead
-// (attention_launch below; measured crossover in DESIGN.md 3.1).
+//   attn_kernel       - sequences longer than 112 tokens (decoder self-attention)
+//   attn_short_kernel - sequences of up to 112 tokens, persistent CTAs walking (sequence, head) items
+// The packed qkv matrix of the ViT blocks is dispatched to the wgmma / TMA kernel in attn_wg.cu instead
+// (attention_launch below); these kernels serve q / k / v given as separate matrices.
 #include "attn.h"
 #include "launch.h"
 #include "ptx.cuh"
@@ -361,7 +361,7 @@ static int launch_short(const AttnArgs& a, cudaStream_t st) {
   constexpr int LDS = DH + 8;
   const size_t smem = static_cast<size_t>(3) * (112 + 256) * LDS * sizeof(T);
   if (int e = ensure_max_dyn_smem(reinterpret_cast<const void*>(attn_short_kernel<T, DH, PM>), 200 * 1024)) return e;
-  static int ctas_per_sm = 0;   // a property of the kernel image and the sm_100a SM, identical on every device of a B200 box
+  static int ctas_per_sm = 0;   // a property of the kernel image and the sm_90a SM, identical on every device of a node
   if (!ctas_per_sm) {
     int n = 0;
     cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_short_kernel<T, DH, PM>, 7 * 32, smem);
@@ -418,43 +418,17 @@ static int dispatch(const AttnArgs& a, int dh, cudaStream_t st) {
   return -2;
 }
 
-int attention_tc_launch(int dtype, const AttnArgs& a, int dh, int C, cudaStream_t st);      // attn_tc.cu
-int attention_slots_launch(int dtype, const AttnArgs& a, int dh, int C, cudaStream_t st);   // attn_slots.cu
+int attention_wg_launch(int dtype, const AttnArgs& a, int dh, int C, cudaStream_t st);      // attn_wg.cu
 
-// Slot kernel (attn_slots.cu: tcgen05, one thread per row, partly polynomial exp2) for packed qkv:
-//   0 = never, 1 = head dim 16 always + head dim 32 for sequences of <= 128 tokens (the ViT windows),
-//   2 (default) = head dim 32 for every sequence length as well (global attention, B200, isolated: medium B=64 612 us against
-//   825 us of the attn_tc.cu kernel, large B=32 334 against 424).  Environment override for A/B measurements only.
-static int slots_policy() {
-  static int v = [] {
-    const char* e = getenv("LWDETR_B200_ATTN_SLOTS");
-    return e ? atoi(e) : 2;
-  }();
-  return v;
-}
-
-// 0 = mma.sync flash kernel everywhere, 1 = tcgen05 kernel for long packed-qkv sequences with dh >= 32 (default; measured
-// 18-22 % faster there, 10 % slower at dh = 16 where the mma.sync kernel's 6 warps per scheduler hide latency better),
-// 2 = tcgen05 kernel for every long packed-qkv sequence.  Environment override for A/B measurements only.
-static int tc_policy() {
-  static int v = [] {
-    const char* e = getenv("LWDETR_B200_ATTN_TC");
-    return e ? atoi(e) : 1;
-  }();
-  return v;
-}
-
+// Packed qkv (the ViT blocks) runs on the wgmma / TMA kernel of attn_wg.cu at every sequence length; separate q / k / v
+// matrices (decoder self-attention) take the mma.sync kernels above.
 int attention_launch(int dtype, const AttnArgs& a, int dh, cudaStream_t st) {
   const long long dk = (static_cast<const char*>(a.k) - static_cast<const char*>(a.q)) / 2;
   const long long dv = (static_cast<const char*>(a.v) - static_cast<const char*>(a.q)) / 2;
   const bool packed = dk > 0 && dv == 2 * dk && a.ldq == a.ldk && a.ldq == a.ldv && dk == static_cast<long long>(a.heads) * dh &&
-                      a.ldq >= 3 * dk && (reinterpret_cast<uintptr_t>(a.q) & 15) == 0;
-  const int sp = slots_policy();
-  if (packed && sp > 0 && (dh == 16 || (dh == 32 && (a.seqlen <= 128 || sp >= 2))))
-    return attention_slots_launch(dtype, a, dh, static_cast<int>(dk), st);
-  const int pol = tc_policy();
-  if (packed && a.seqlen >= 512 && (pol == 2 || (pol == 1 && dh >= 32)))
-    return attention_tc_launch(dtype, a, dh, static_cast<int>(dk), st);
+                      a.ldq >= 3 * dk && (a.ldq % 8) == 0 && (reinterpret_cast<uintptr_t>(a.q) & 15) == 0 &&
+                      (a.ldo % 8) == 0 && (reinterpret_cast<uintptr_t>(a.o) & 15) == 0;   // TMA rows and the 16-byte output stores
+  if (packed && (dh == 16 || dh == 32 || dh == 64)) return attention_wg_launch(dtype, a, dh, static_cast<int>(dk), st);
   return dtype == DT_BF16 ? dispatch<__nv_bfloat16>(a, dh, st) : dispatch<__half>(a, dh, st);
 }
 

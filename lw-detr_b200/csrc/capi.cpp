@@ -17,7 +17,6 @@
 #include "msda.h"
 #include "rowops.h"
 
-namespace lwb { int attention_slots_debug_dump(); }   // attn_slots.cu
 
 namespace {
 thread_local std::string g_err;
@@ -127,7 +126,6 @@ int lwdetr_ms_deform_attn_backward(const float* value, const int64_t* spatial_sh
   return 0;
 }
 
-int lwdetr_debug_dump(void) { return lwb::attention_slots_debug_dump(); }
 
 int lwdetr_msda_forward(int dtype, const void* value_hm, int64_t v_image_stride, const void* offs_logits, int ld_ol, const float* ref,
                         const float* valid_ratio, void* out, int ld_out, int B, int S, int Lq, int M, int L, int P,

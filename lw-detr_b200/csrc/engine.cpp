@@ -1,5 +1,5 @@
 // LW-DETR forward engine (host side).  Packs a reference-format checkpoint into kernel-native
-// layouts once, then runs a fixed schedule of hand-written sm_100a kernels per batch:
+// layouts once, then runs a fixed schedule of hand-written sm_90a kernels per batch:
 //   patch gather -> [LN, qkv GEMM, fused attention, proj GEMM(+layer-scale+residual), LN, fc1 GEMM(GELU),
 //   fc2 GEMM(+layer-scale+residual)] x depth -> projector (1x1 / implicit 3x3 / pixel-shuffle GEMMs,
 //   channel LN writing the decoder memory directly) -> two-stage selection (GEMMs, row max, top-k,

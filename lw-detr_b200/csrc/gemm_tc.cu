@@ -1,13 +1,14 @@
-// tcgen05 / TMA GEMM family (see gemm_tc.h).  Persistent CTA PAIRS (clusters of 2, one pair per two SMs)
-// compute 256 x BN output tiles with tcgen05.mma.cta_group::2 - a single-CTA tcgen05.mma was measured at about
-// half of the pair rate on this part (profiles/r01c_gemm_timeline.txt), so every GEMM of the path runs paired:
-//   warp 0   : TMA producer (one elected lane, in BOTH CTAs): its CTA's 128 x 64 A tile and its HALF of the
-//              BN x 64 W tile per k-block, credited to the leader CTA's "full" barrier
-//   warp 1   : TMEM allocator; in the leader CTA also the tcgen05.mma issuer (one lane) - accumulators are
-//              double buffered in TMEM (each CTA holds its 128 rows), commits are multicast to both CTAs
-//   warps 2-17: epilogue, four warps per TMEM lane quarter: tcgen05.ld -> LayerNorm-fold / bias / activation /
-//              layer-scale / residual -> 16-bit (or fp32) rows to global, optional row re-ordering / pixel shuffle,
-//              optional per-row (sum, sum^2) statistics for the next LayerNorm-fused GEMM.
+// wgmma / TMA GEMM family (see gemm_tc.h).  Persistent CTAs (one per SM) walk 128 x BN output tiles:
+//   warp 0 (of the producer warpgroup): TMA producer (one elected lane): the 128 x 64 A tile and the BN x 64 W tile per
+//              k-block into a ring of shared-memory stages (full / empty mbarriers); the warpgroup gives its registers
+//              to the consumers (setmaxnreg)
+//   warps 4-11: two consumer warpgroups, 64 rows each: wgmma.mma_async m64nBNk16 straight out of the swizzled stages,
+//              fp32 accumulators in registers, one k-block of MMAs in flight while the next stage is awaited; then the
+//              epilogue of their own rows: the accumulators pass through a per-warp shared-memory staging area, 64 columns
+//              at a time, so that every row is finished by two threads on 16-column chunks - LayerNorm-fold / bias /
+//              activation / layer-scale / residual -> 16-bit (or fp32) rows to global, optional row re-ordering / pixel
+//              shuffle, optional per-row (sum, M2) statistics for the next LayerNorm-fused GEMM.  The producer keeps
+//              filling the ring with the next tile's stages while the epilogue runs.
 // Replaces, on the LW-DETR path, every F.linear / nn.Conv2d / nn.ConvTranspose2d call listed in
 // SURVEY.md appendix B (reference: models/backbone/vit.py:120-140,206-220, projector.py:85-132,
 // transformer.py:27-39,466-517, ops/modules/ms_deform_attn.py:112-143, lwdetr.py:149-159).
@@ -15,6 +16,7 @@
 #include "launch.h"
 #include "ptx.cuh"
 #include "tma_util.h"
+#include "wgmma.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -26,9 +28,12 @@ namespace lwb {
 static constexpr int BM = 128;
 static constexpr int BK = 64;
 static constexpr int A_STAGE_BYTES = BM * BK * 2;
-static constexpr int EPI_WARPS = 16;                      // two groups of 8 (alternate tiles); in a group two warps per TMEM lane quarter, half of the columns each
-static constexpr int GEMM_THREADS = 64 + 32 * EPI_WARPS;
+static constexpr int MMA_WARPS = 8;                       // two consumer warpgroups of 64 rows; warp w owns rows 16w .. 16w+15
+static constexpr int GEMM_THREADS = 128 + 32 * MMA_WARPS; // producer warpgroup + consumers
 static constexpr int MAX_STAGES = 8;
+static constexpr int STG_LD = 68;                         // floats per staged accumulator row: 64 columns + 4 (bank spread)
+static constexpr int STG_BYTES = MMA_WARPS * 16 * STG_LD * 4;
+
 
 // Exact (erf) GELU, nn.GELU() default used by timm's Mlp (vit.py:184).  gelu(x) = x*Phi(x) with
 // Phi(-|x|) = 0.5*erfc(|x|/sqrt2) from Abramowitz-Stegun 7.1.26 (|erf error| <= 1.5e-7):
@@ -46,11 +51,10 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return fmaf(-ax * t, p * e, fmaxf(x, 0.f));
 }
 
-// The same exact-erf GELU for a PAIR on the packed fp32x2 pipe, without the MUFU: gelu(x) = x * (0.5 + xc * q(xc^2)), xc = x
+// The same exact-erf GELU for a PAIR of values (ptx.cuh f2_*), without the MUFU: gelu(x) = x * (0.5 + xc * q(xc^2)), xc = x
 // clamped to [-4.5, 4.5], q a degree-9 polynomial fitted to erf(x/sqrt2) / (2x) (weighted least squares at Chebyshev nodes;
 // fp32 Horner: max |error| 7.4e-5 at |x| ~ 4.46 where gelu ~ 4.46, < 1e-5 for |x| < 3 (tests/test_numerics_cpu.py); beyond the clamp Phi(-4.5) = 3.4e-6
-// multiplies x).  16 instructions per pair (8 per element) against 14 per element for gelu_erf - the fc1 epilogue is bound by
-// its instruction count, not by the tensor core (DESIGN.md section 3).
+// multiplies x).  FMA pipe only, where gelu_erf spends two MUFU operations per element.
 __device__ __forceinline__ uint64_t gelu_erf2(uint64_t x2) {
   float x0, x1;
   f2_unpack(x2, x0, x1);
@@ -74,16 +78,16 @@ __device__ __forceinline__ uint64_t gelu_erf2(uint64_t x2) {
 struct TileCoord {
   int m_tile, n_tile, n0, cb, cy0, cx0;
 };
-// pair-tile index -> this CTA's (m_tile, n_tile); n fastest, so neighbouring pairs share the A rows in L2
-__device__ __forceinline__ TileCoord decode_tile(const GemmArgs& p, int ptile, int rank, int BN) {
+// tile index -> (m_tile, n_tile); n fastest, so CTAs running at the same time share the A rows in L2
+__device__ __forceinline__ TileCoord decode_tile(const GemmArgs& p, int tile, int BN) {
   TileCoord t;
-  t.n_tile = ptile % p.n_tiles;
-  t.m_tile = 2 * (ptile / p.n_tiles) + rank;     // may be == m_tiles for the odd tail: loads are OOB zero-fill, stores masked
+  t.n_tile = tile % p.n_tiles;
+  t.m_tile = tile / p.n_tiles;
   t.n0 = t.n_tile * BN;
   t.cb = t.cy0 = t.cx0 = 0;
   if (p.a_mode != AMODE_PLAIN) {
     const int per_img = p.tiles_x * p.tiles_y;
-    t.cb = t.m_tile / per_img;                    // == batch for the odd tail: out of bounds in the TMA batch dimension
+    t.cb = t.m_tile / per_img;
     const int r = t.m_tile % per_img;
     t.cy0 = (r / p.tiles_x) * p.TH;
     t.cx0 = (r % p.tiles_x) * p.TW;
@@ -91,10 +95,12 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmArgs& p, int ptile, i
   return t;
 }
 
-// Persistent CTA pairs: pair q (= blockIdx.x / 2) walks pair-tiles q, q + npairs, ...  A pair-tile is two
-// vertically adjacent 128-row m-tiles (CTA rank 0 / 1) times one BN-wide n-tile.  The smem ring (TMA -> MMA)
-// runs continuously across tiles and the accumulator is double buffered in TMEM, so the epilogue of tile i
-// overlaps the loads and MMAs of tile i+1.
+// keeps the compiler from moving uses of the accumulators across the asynchronous MMAs' wait
+template <int N> __device__ __forceinline__ void fence_regs(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
 // EP (epilogue specialisation): EP_GENERIC keeps every feature behind runtime flags; the others compile the
 // features of the hot GEMMs in or out so the per-element instruction count stays minimal:
 //   EP_BIAS      out = acc + bias                     (16-bit out, plain rows, no LN / residual / activation)
@@ -111,126 +117,76 @@ __device__ __forceinline__ float4 lds128(const float* p) {
 }
 
 template <typename T, int BN, int EP>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmArgs p) {
-  constexpr int B_HALF_BYTES = (BN / 2) * BK * 2;                             // this CTA's half of the W tile
-  constexpr uint32_t ACC_STRIDE = BN <= 64 ? 64 : (BN <= 128 ? 128 : 256);   // TMEM columns per accumulator buffer
-  constexpr uint32_t TMEM_COLS = 2 * ACC_STRIDE;
+  constexpr int B_STAGE_BYTES = BN * BK * 2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int stages = p.stages;
   uint8_t* sA = smem;
   uint8_t* sB = smem + stages * A_STAGE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sB + stages * B_HALF_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sB + stages * B_STAGE_BYTES);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
-  uint64_t* acc_full = empty_bar + MAX_STAGES;      // [2]
-  uint64_t* acc_empty = acc_full + 2;               // [2]  (used in the leader CTA)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* s_vec = reinterpret_cast<float*>(full_bar + 32);   // 256 B of barriers, then {bias | gamma | colsum}[n_tiles * BN]
+  float* s_stage = reinterpret_cast<float*>(full_bar + 32);   // 256 B of barriers, then the accumulator staging [warp][16][STG_LD]
+  float* s_vec = s_stage + MMA_WARPS * 16 * STG_LD;           // then {bias | gamma | colsum}[n_tiles * BN]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();          // 0 = leader
-  const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-  const int m_pairs = (p.m_tiles + 1) >> 1;
-  const int num_ptiles = m_pairs * p.n_tiles;
+  const int num_tiles = p.m_tiles * p.n_tiles;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < stages; ++s) {
-      mbar_init(&full_bar[s], 2);                   // leader: own arrive.expect_tx + the peer's remote arrive
-      mbar_init(&empty_bar[s], 1);                  // one multicast tcgen05.commit
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_empty[b], p.epi_groups == 2 ? EPI_WARPS : 2 * EPI_WARPS);   // the epilogue warps (of one group / of both) in each of the two CTAs
+      mbar_init(&full_bar[s], 1);                   // the producer's arrive.expect_tx
+      mbar_init(&empty_bar[s], MMA_WARPS);          // one elected arrival per consumer warp
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc2(tmem_slot, TMEM_COLS);
-    tmem_relinquish2();
-  }
-  tc_fence_before();
-  cluster_sync_all();                               // barriers of BOTH CTAs are initialised before any remote use
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
   pdl_sync();   // the prologue above touched no global data; everything below reads the predecessor's output
 
-  if (warp == 0) {
-    if (lane == 0) {
-      // ------------------------------------------------------------------ TMA producer (both CTAs)
+  if (warp < 4) {
+    reg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      // ------------------------------------------------------------------ TMA producer
       uint32_t ring = 0;
-      for (int pt = pair; pt < num_ptiles; pt += npairs) {
-        const TileCoord tc = decode_tile(p, pt, static_cast<int>(rank), BN);
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const TileCoord tc = decode_tile(p, tile, BN);
         for (int kb = 0; kb < p.kblocks; ++kb, ++ring) {
           const int s = ring % stages;
           const uint32_t ph = (ring / stages) & 1;
           mbar_wait(&empty_bar[s], ph ^ 1);
+          mbar_arrive_expect_tx(&full_bar[s], p.a_stage_tx + B_STAGE_BYTES);
           uint8_t* a_dst = sA + s * A_STAGE_BYTES;
           if (p.a_mode == AMODE_PLAIN) {
-            tma2_load_2d(a_dst, &tmA, &full_bar[s], kb * BK, tc.m_tile * BM);
+            tma_load_2d(a_dst, &tmA, &full_bar[s], kb * BK, tc.m_tile * BM);
           } else {
             const int tap = kb / p.cin_blocks;
             const int c0 = (kb % p.cin_blocks) * BK;
             const int dy = tap / 3, dx = tap % 3;
             if (p.a_mode == AMODE_CONV3_S1) {
-              tma2_load_4d(a_dst, &tmA, &full_bar[s], c0, tc.cx0 + dx - 1, tc.cy0 + dy - 1, tc.cb);
+              tma_load_4d(a_dst, &tmA, &full_bar[s], c0, tc.cx0 + dx - 1, tc.cy0 + dy - 1, tc.cb);
             } else {
               // input row iy = 2*oy + dy - 1 = 2*(oy + yoff) + py ; same for columns
               const int py = (dy == 1) ? 0 : 1, yoff = (dy == 0) ? -1 : 0;
               const int px = (dx == 1) ? 0 : 1, xoff = (dx == 0) ? -1 : 0;
-              tma2_load_5d(a_dst, &tmA, &full_bar[s], px * p.lda + c0, tc.cx0 + xoff, py, tc.cy0 + yoff, tc.cb);
+              tma_load_5d(a_dst, &tmA, &full_bar[s], px * p.lda + c0, tc.cx0 + xoff, py, tc.cy0 + yoff, tc.cb);
             }
           }
-          tma2_load_2d(sB + s * B_HALF_BYTES, &tmB, &full_bar[s], kb * BK, tc.n0 + static_cast<int>(rank) * (BN / 2));
-          if (rank == 0) mbar_arrive_expect_tx(&full_bar[s], 2u * (p.a_stage_tx + B_HALF_BYTES));
-          else mbar_arrive_cluster(&full_bar[s], 0);
+          tma_load_2d(sB + s * B_STAGE_BYTES, &tmB, &full_bar[s], kb * BK, tc.n0);
         }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {
-      // ------------------------------------------------------------------ MMA issuer (leader CTA only)
-      constexpr uint32_t idesc = umma_idesc_f16(Cvt<T>::is_bf16, 2 * BM, BN);
-      uint32_t ring = 0;
-      int it = 0;
-      for (int pt = pair; pt < num_ptiles; pt += npairs, ++it) {
-        const int buf = it & 1;
-        mbar_wait(&acc_empty[buf], ((it >> 1) & 1) ^ 1);     // both epilogues have drained this accumulator buffer
-        tc_fence_after();
-        const uint32_t tacc = tmem_base + buf * ACC_STRIDE;
-        for (int kb = 0; kb < p.kblocks; ++kb, ++ring) {
-          const int s = ring % stages;
-          const uint32_t ph = (ring / stages) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint64_t adesc = umma_desc_k128(smem_u32(sA + s * A_STAGE_BYTES));
-          const uint64_t bdesc = umma_desc_k128(smem_u32(sB + s * B_HALF_BYTES));
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            // advance 16 elements (32 B) along K inside the 128 B swizzle row: +2 in 16-byte units
-            umma2_f16_ss(tacc, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma2_commit_both(&empty_bar[s]);                   // frees the stage in both CTAs
-        }
-        umma2_commit_both(&acc_full[buf]);
       }
     }
   } else {
-    // -------------------------------------------------------------------- epilogue (16 warps, both CTAs)
-    const int quarter = warp & 3;               // TMEM lanes [32*quarter, 32*quarter+32) (hardware: warp_id % 4)
-    // The 16 epilogue warps form TWO GROUPS.  With many tiles per CTA (epi_groups = 2: qkv, fc1, ...) the groups take alternate
-    // tiles (group g owns accumulator buffer g): while one group is in the latency-bound head of its tile (statistics, TMEM
-    // pull, residual) or in its stores, the other one is in its arithmetic - as one group the four warps of a scheduler moved in
-    // lock step and left the FMA pipe idle half of the time (fc1: FMA pipe 52 % busy at an FMA-bound epilogue,
-    // profiles/r02_ncu_gemm_small.txt).  Measured in the small / B = 32 step: qkv 257 -> 233 us, fc1 364 -> 353 us per 10
-    // launches.  With two or three tiles per CTA (proj, fc2, the projector) halving the warps per tile only stretches the tail
-    // (fc2 274 -> 309 us), so there both groups split every tile (epi_groups = 1: group g takes half of the pull rounds).
-    const int grp = (warp - 2) >> 3;
-    const int chalf = ((warp - 2) >> 2) & 1;    // which half of the tile's 16-column chunks this warp owns
-    const int r = quarter * 32 + lane;          // row inside this CTA's 128-row tile
+    reg_inc<232>();
+    // -------------------------------------------------------------------- MMA + epilogue (two warpgroups)
+    const int cw = warp - 4;                    // consumer warp: rows [16*cw, 16*cw + 16) of the tile
+    const int wg = cw >> 2;                     // its warpgroup: rows [64*wg, 64*wg + 64)
+    const int g = lane >> 2, t4 = lane & 3;     // accumulator fragment: rows 16*cw + g (+8), columns 8j + 2*t4 (+1)
+    const int chalf = lane & 1;                 // epilogue: two threads per row, this one takes chunks 4i + 2*chalf, +1
+    const int r = cw * 16 + (lane >> 1);        // row inside the 128-row tile (epilogue)
+    float* stg = s_stage + cw * 16 * STG_LD;
     constexpr bool GEN = EP == EP_GENERIC;
     const bool has_gamma = (GEN || EP == EP_RESID) && p.gamma != nullptr;
     const bool ln_in = GEN ? (p.stats_in != nullptr) : (EP == EP_LN || EP == EP_LN_GELU);
@@ -238,44 +194,22 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const bool has_resid = (GEN || EP == EP_RESID) && p.resid != nullptr;
     const bool do_stats = (GEN || EP == EP_RESID) && p.stats_out != nullptr;
     const bool plain_out = !GEN;                 // 16-bit, rows in place, no pixel shuffle
-    // Stage the bias / layer-scale / LayerNorm column-sum vectors of ALL n-tiles once per CTA (epilogue warps only,
-    // while the producer / MMA warps already stream the first tile): the per-tile epilogue then has no dependent
-    // global loads except the (prefetched) residual and the per-row LayerNorm statistics.
+    // Stage the bias / layer-scale / LayerNorm column-sum vectors of ALL n-tiles once per CTA (consumer warps only,
+    // while the producer already streams the first tile): the per-tile epilogue then has no dependent global loads
+    // except the residual and the per-row LayerNorm statistics.
     {
       const int npad_all = p.n_tiles * BN;
-      for (int i = threadIdx.x - 64; i < npad_all; i += 32 * EPI_WARPS) {
+      for (int i = threadIdx.x - 128; i < npad_all; i += 32 * MMA_WARPS) {
         const bool in = i < p.N;
         s_vec[i] = (p.bias != nullptr && in) ? __ldg(p.bias + i) : 0.f;
         s_vec[npad_all + i] = (p.gamma != nullptr && in) ? __ldg(p.gamma + i) : 1.f;
         s_vec[2 * npad_all + i] = (p.colsum != nullptr && in) ? __ldg(p.colsum + i) : 0.f;
       }
-      asm volatile("bar.sync 1, %0;" ::"n"(32 * EPI_WARPS) : "memory");
+      asm volatile("bar.sync 1, %0;" ::"n"(32 * MMA_WARPS) : "memory");
     }
-    int it = 0;
-    const int n_my_tiles = pair < num_ptiles ? (num_ptiles - pair + npairs - 1) / npairs : 0;
-    // Tile walk without a division per tile (plain GEMMs; ncu counted ~180 of the 324 instructions a warp spends per qkv tile
-    // in tile decoding, row bookkeeping and the statistics reduction - more than on its 48 output columns): pair-tile index
-    // pt = m_pair * n_tiles + n_tile advances by npairs = d_mp * n_tiles + d_nt with a carry.
-    const bool plain = p.a_mode == AMODE_PLAIN;
-    const bool alt = p.epi_groups == 2;
-    const int tstep = alt ? 2 * npairs : npairs;        // this group's next tile
-    const int d_mp = tstep / p.n_tiles, d_nt = tstep - d_mp * p.n_tiles;
-    const int pt0 = alt ? pair + grp * npairs : pair;
-    int w_nt = pt0 % p.n_tiles, w_mp = pt0 / p.n_tiles;
-    auto plain_tile = [&](int nt, int mp) {
-      TileCoord t;
-      t.n_tile = nt;
-      t.m_tile = 2 * mp + static_cast<int>(rank);
-      t.n0 = nt * BN;
-      t.cb = t.cy0 = t.cx0 = 0;
-      return t;
-    };
-    // LayerNorm statistics of a row: the producer's partial (sum, sum of squares) pairs.  The partials of the NEXT tile's rows
-    // are requested at the start of a tile and reduced at its end (first four in registers), so the L2 round trip that used to
-    // stall the first use (13 % of all samples of the qkv GEMM on one FADD) overlaps the tile's own work.
-    float nx_mean = 0.f, nx_rstd = 1.f;
     // combine equal-width partials (sum_p, M2_p): mean = sum(sum_p) / C, var = [sum(M2_p) + n_p * sum((sum_p / n_p - mean)^2)] / C
     const float part_n = p.stats_parts_in > 0 ? 1.f / (p.ln_inv_c * p.stats_parts_in) : 1.f, part_inv_n = 1.f / part_n;
+
     auto stats_of = [&](long long mrow, float& mean, float& rstd) {
       float s1 = 0.f, m2 = 0.f;
       for (int i = 0; i < p.stats_parts_in; ++i) s1 += __ldg(p.stats_in + mrow * p.stats_parts_in + i).x;
@@ -287,23 +221,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
       rstd = rsqrtf(m2 * p.ln_inv_c + p.ln_eps);
     };
-    if (ln_in && plain && pt0 < num_ptiles) {
-      const long long m0 = static_cast<long long>(2 * w_mp + static_cast<int>(rank)) * BM + r;
-      if (m0 < p.M) stats_of(m0, nx_mean, nx_rstd);
-    }
-    it = alt ? grp : 0;
-    const int it_step = alt ? 2 : 1;
-    for (int pt = pt0; pt < num_ptiles; pt += tstep, it += it_step) {
-      const TileCoord tc = plain ? plain_tile(w_nt, w_mp) : decode_tile(p, pt, static_cast<int>(rank), BN);
-      // next tile of this group
-      w_nt += d_nt;
-      w_mp += d_mp;
-      if (w_nt >= p.n_tiles) {
-        w_nt -= p.n_tiles;
-        ++w_mp;
-      }
+    uint32_t ring = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const TileCoord tc = decode_tile(p, tile, BN);
       const int n0 = tc.n0;
-      const int buf = it & 1;
       int m, b = 0, y = 0, x = 0;
       bool valid;
       if (p.a_mode == AMODE_PLAIN) {
@@ -340,25 +261,30 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const float* s_bias = s_vec + n0;
       const float* s_gamma = s_vec + npad + n0;
       const float* s_csum = s_vec + 2 * npad + n0;
-      // fused LayerNorm (consumer): combine the producer's partial sums of this row
+      // fused LayerNorm (consumer): combine the producer's partial sums of this row; the loads overlap the MMAs below
       float ln_mean = 0.f, ln_rstd = 1.f;
-      float2 nq[4];
-      long long nx_row = -1;
-      if (ln_in && plain) {
-        ln_mean = nx_mean;                            // reduced at the end of the previous tile (or before the loop)
-        ln_rstd = nx_rstd;
-        if (pt + tstep < num_ptiles) {
-          const long long mn = static_cast<long long>(2 * w_mp + static_cast<int>(rank)) * BM + r;
-          if (mn < p.M) {
-            nx_row = mn;
+      if (ln_in && valid) stats_of(m, ln_mean, ln_rstd);
+
+      // ------------------------------------------------------------------ main loop: this warpgroup's 64 x BN accumulator
+      float acc[BN / 2];
+      for (int kb = 0; kb < p.kblocks; ++kb, ++ring) {
+        const int s = ring % stages;
+        mbar_wait(&full_bar[s], (ring / stages) & 1);
+        const uint64_t adesc = wgmma_desc(smem_u32(sA + s * A_STAGE_BYTES + wg * (64 * BK * 2)), 128);
+        const uint64_t bdesc = wgmma_desc(smem_u32(sB + s * B_STAGE_BYTES), 128);
+        wgmma_fence();
 #pragma unroll
-            for (int i = 0; i < 4; ++i)
-              if (i < p.stats_parts_in) nq[i] = __ldg(p.stats_in + mn * p.stats_parts_in + i);
-          }
+        for (int k = 0; k < BK / 16; ++k)     // 16 elements (32 B) along K inside the 128 B swizzle row: +2 in 16-byte units
+          Wgmma<Cvt<T>::is_bf16, BN>::ss(acc, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        if (kb > 0) {                          // the previous k-block's MMAs are done: hand its stage back
+          wgmma_wait<1>();
+          if (lane == 0) mbar_arrive(&empty_bar[(ring - 1) % stages]);
         }
-      } else if (ln_in && valid) {
-        stats_of(m, ln_mean, ln_rstd);
       }
+      wgmma_wait<0>();
+      fence_regs(acc);
+      if (lane == 0) mbar_arrive(&empty_bar[(ring - 1) % stages]);
       // Row statistics for the fused LayerNorm of the consumer, SHIFTED by the first value of the slice: sums of (x - K) and
       // (x - K)^2 do not cancel when the row mean is large against its spread (real checkpoints; E[x^2] - mean^2 would).
       float st_sum = 0.f, st_sq = 0.f, st_K = 0.f;
@@ -372,7 +298,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int nrem = p.N - n;                     // may be <= 0 for the padded tail of the last n-tile
         if (!valid || nrem <= 0) return;
         const bool full = nrem >= 16;
-        // packed fp32x2 from here on (FFMA2 / FADD2 / FMUL2): half the issue slots of the scalar form
+        // fp32 pairs from here on (ptx.cuh f2_*: adjacent columns travel together)
         uint64_t w[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) w[j] = f2_pack(v[2 * j], v[2 * j + 1]);
@@ -518,44 +444,30 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         return false;
       };
 
-      constexpr int CH_PER_WARP = BN / 16 / 2;
-      // The slice is pulled G chunks (16 columns each) at a time - the kernel runs at 96 registers per thread - and the TMEM
-      // buffer goes back to the MMA warp right after this warp's LAST pull, before that round's math / stores.
-      constexpr int G = CH_PER_WARP % 3 == 0 ? 3 : (CH_PER_WARP >= 4 ? 2 : 1);
-      constexpr int NR = CH_PER_WARP / G;               // pull rounds per column half: 4 / 2 / 2 / 2 for BN = 256 / 192 / 128 / 64
-      static_assert(CH_PER_WARP % G == 0 && NR % 2 == 0, "chunk rounds");
-      const int rd0 = alt ? 0 : grp * (NR / 2), rd1 = alt ? NR : rd0 + NR / 2;   // this warp's rounds
-      const int c_first = chalf * CH_PER_WARP;
-      U8 rr_cur, rr_nxt;
-      bool rv_cur = resid_prefetch(c_first + rd0 * G, rr_cur), rv_nxt = false;
-
-      mbar_wait(&acc_full[buf], (it >> 1) & 1);
-      tc_fence_after();
-      const uint32_t taddr_row = tmem_base + buf * ACC_STRIDE + (static_cast<uint32_t>(quarter * 32) << 16);
-      float v[G][16];
-#pragma unroll 1                                    // one copy of the (large) chunk code: the rounds differ only in their column offset
-      for (int rd = rd0; rd < rd1; ++rd) {
-        __syncwarp();                                 // tcgen05.ld is .sync.aligned: reconverge first
+      // ------------------------------------------------------------------ epilogue, 64 columns per pass
 #pragma unroll
-        for (int i = 0; i < G; ++i) tmem_ld_x16(taddr_row + (c_first + rd * G + i) * 16, v[i]);
-        tmem_ld_wait();
-        if (rd == rd1 - 1) {
-          tc_fence_before();
-          __syncwarp();
-          // (the release of the last two tiles is never consumed: skipping it also guarantees that no remote arrive is
-          //  still in flight when the pair leaves through the relaxed cluster rendezvous below)
-          if (lane == 0 && it + 2 < n_my_tiles) {
-            if (rank == 0) mbar_arrive(&acc_empty[buf]);
-            else mbar_arrive_cluster(&acc_empty[buf], 0);
-          }
+      for (int pc = 0; pc < BN / 64; ++pc) {
+        __syncwarp();                                  // the previous pass has been read
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int a0 = 4 * (8 * pc + j), col = 8 * j + 2 * t4;
+          *reinterpret_cast<float2*>(stg + g * STG_LD + col) = make_float2(acc[a0], acc[a0 + 1]);
+          *reinterpret_cast<float2*>(stg + (g + 8) * STG_LD + col) = make_float2(acc[a0 + 2], acc[a0 + 3]);
         }
+        __syncwarp();
+#pragma unroll 1                                       // one copy of the (large) chunk code per pass
+        for (int i = 0; i < 2; ++i) {
+          const int cl = 2 * chalf + i, c = 4 * pc + cl;
+          U8 rr;
+          const bool rv = resid_prefetch(c, rr);
+          float v[16];
+          const float* src = stg + (lane >> 1) * STG_LD + cl * 16;
 #pragma unroll
-        for (int i = 0; i < G; ++i) {
-          const int c = rd * G + i;
-          if (c + 1 < rd1 * G) rv_nxt = resid_prefetch(c_first + c + 1, rr_nxt);
-          finish_chunk(c_first + c, v[i], rr_cur, rv_cur);
-          rr_cur = rr_nxt;
-          rv_cur = rv_nxt;
+          for (int q = 0; q < 4; ++q) {
+            const float4 f = lds128(src + 4 * q);
+            v[4 * q] = f.x; v[4 * q + 1] = f.y; v[4 * q + 2] = f.z; v[4 * q + 3] = f.w;
+          }
+          finish_chunk(c, v, rr, rv);
         }
       }
       if (do_stats && valid) {
@@ -563,38 +475,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         // (gemm_build checks N % BN == 0 for producers), which is all the consumer needs to combine them (Chan et al.)
         const float nn = static_cast<float>(st_n > 0 ? st_n : 1);
         const float part_sum = fmaf(nn, st_K, st_sum), part_m2 = fmaxf(st_sq - st_sum * st_sum / nn, 0.f);
-        p.stats_out[static_cast<long long>(m) * p.stats_parts_out + (alt ? tc.n_tile * 2 + chalf : tc.n_tile * 4 + chalf * 2 + grp)] = make_float2(part_sum, part_m2);
-      }
-      if (nx_row >= 0) {                              // statistics of the next tile's row: the requests above have landed by now
-        float s1 = 0.f, m2 = 0.f;
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-          if (i < p.stats_parts_in) s1 += nq[i].x;
-        for (int i = 4; i < p.stats_parts_in; ++i) s1 += __ldg(p.stats_in + nx_row * p.stats_parts_in + i).x;
-        nx_mean = s1 * p.ln_inv_c;
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-          if (i < p.stats_parts_in) {
-            const float dm = nq[i].x * part_inv_n - nx_mean;
-            m2 += nq[i].y + part_n * dm * dm;
-          }
-        for (int i = 4; i < p.stats_parts_in; ++i) {
-          const float2 q = __ldg(p.stats_in + nx_row * p.stats_parts_in + i);
-          const float dm = q.x * part_inv_n - nx_mean;
-          m2 += q.y + part_n * dm * dm;
-        }
-        nx_rstd = rsqrtf(m2 * p.ln_inv_c + p.ln_eps);
+        p.stats_out[static_cast<long long>(m) * p.stats_parts_out + tc.n_tile * 2 + chalf] = make_float2(part_sum, part_m2);
       }
     }
   }
-
-  tc_fence_before();
-  cluster_sync_relaxed();                           // nobody frees TMEM / exits while its peer may still use it
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, TMEM_COLS);
-  }
 }
+
 
 // ------------------------------------------------------------------------------------------- host
 static int encode(CUtensorMap* tm, int dtype, int rank, const void* base, const cuuint64_t* dims,
@@ -617,9 +503,9 @@ static int pick_bn(int N, int m_tiles) {
     }
     bn = best;
   }
-  // Small problems: prefer more CTAs over wider tiles so that all 148 SMs get work.
-  auto tiles = [&](int b) { return static_cast<long long>((m_tiles + 1) / 2) * ((N + b - 1) / b); };
-  while (bn > 64 && tiles(bn) < 74) {
+  // Small problems: prefer more CTAs over wider tiles so that every SM gets work.
+  auto tiles = [&](int b) { return static_cast<long long>(m_tiles) * ((N + b - 1) / b); };
+  while (bn > 64 && tiles(bn) < num_sms()) {
     const int nb = bn == 256 ? 128 : (bn == 192 ? 64 : 64);
     if (((N + nb - 1) / nb) * nb - N > ((N + bn - 1) / bn) * bn - N + 32) break;
     bn = nb;
@@ -711,31 +597,27 @@ int gemm_build(const GemmDesc& d, GemmOp* op, std::string* err) {
   {
     const cuuint64_t dims[2] = {static_cast<cuuint64_t>(d.K), static_cast<cuuint64_t>(d.N)};
     const cuuint64_t strides[1] = {static_cast<cuuint64_t>(d.K) * 2};
-    const cuuint32_t box[2] = {BK, static_cast<cuuint32_t>(bn / 2)};      // each CTA of a pair loads half of the n-tile
+    const cuuint32_t box[2] = {BK, static_cast<cuuint32_t>(bn)};
     if (encode(&op->tb, d.dtype, 2, d.W, dims, strides, box, err)) return -1;
   }
-  const int stage_bytes = A_STAGE_BYTES + (bn / 2) * BK * 2;
+  const int stage_bytes = A_STAGE_BYTES + bn * BK * 2;
   const size_t vec_bytes = 3 * 4 * static_cast<size_t>(a.n_tiles) * bn;     // bias | gamma | colsum for all n-tiles
-  int stages = static_cast<int>((206 * 1024 - vec_bytes) / stage_bytes);
+  int stages = static_cast<int>((225 * 1024 - STG_BYTES - vec_bytes) / stage_bytes);
   stages = std::min(stages, MAX_STAGES);
   stages = std::max(2, std::min(stages, std::max(2, 2 * a.kblocks)));
   a.stages = stages;
   a.m_tiles = m_tiles;
-  op->smem = 1024 + static_cast<size_t>(stages) * stage_bytes + 256 + vec_bytes;
-  const long long ptiles = static_cast<long long>((m_tiles + 1) / 2) * a.n_tiles;
-  op->grid = 2u * static_cast<unsigned>(std::min<long long>(ptiles, num_sms() / 2));
-  // epilogue groups on alternate tiles once a CTA pair has at least six tiles to walk (see the kernel); the LayerNorm
-  // partials a producer writes per row follow: one per (n-tile, column half) or one per (n-tile, column half, group)
-  a.epi_groups = ptiles >= 6LL * (op->grid / 2) ? 2 : 1;
-  if (const char* e = getenv("LWDETR_B200_GEMM_GROUPS")) a.epi_groups = atoi(e) == 2 ? 2 : 1;   // A/B measurements
-  a.stats_parts_out = a.n_tiles * (a.epi_groups == 2 ? 2 : 4);
+  op->smem = 1024 + static_cast<size_t>(stages) * stage_bytes + 256 + STG_BYTES + vec_bytes;
+  const long long tiles = static_cast<long long>(m_tiles) * a.n_tiles;
+  op->grid = static_cast<unsigned>(std::min<long long>(tiles, num_sms()));
+  a.stats_parts_out = a.n_tiles * 2;     // the LayerNorm partials a producer writes per row: one per (n-tile, column half)
   op->flops = 2.0 * d.M * static_cast<double>(d.N) * d.K;
   return 0;
 }
 
 template <typename T, int BN, int EP>
 static int launch_inst(const GemmOp& op, cudaStream_t st) {
-  if (int e = ensure_max_dyn_smem(reinterpret_cast<const void*>(gemm_tc_kernel<T, BN, EP>), 226 * 1024)) return e;
+  if (int e = ensure_max_dyn_smem(reinterpret_cast<const void*>(gemm_tc_kernel<T, BN, EP>), 227 * 1024)) return e;
   launch_k(gemm_tc_kernel<T, BN, EP>, dim3(op.grid), dim3(GEMM_THREADS), op.smem, st, op.ta, op.tb, op.args);
   return static_cast<int>(cudaGetLastError());
 }

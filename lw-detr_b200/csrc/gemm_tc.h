@@ -1,4 +1,4 @@
-// tcgen05 + TMA GEMM family used for every linear / convolution of the LW-DETR forward.
+// wgmma + TMA GEMM family used for every linear / convolution of the LW-DETR forward.
 //   out[row_map(m), n] = epilogue( sum_k A[m, k] * W[n, k] )
 // A is gathered by TMA either from a plain row-major matrix, or implicitly (im2col-free) from an
 // NHWC feature map for 3x3 convolutions (stride 1 and 2).  W is always [N, K] row-major, i.e. the
@@ -49,7 +49,6 @@ struct GemmArgs {
   int stats_parts_in;
   const float* colsum;      // [N] fp32 (consumer)
   float ln_inv_c, ln_eps;   // 1/C of the normalised dimension, epsilon
-  int epi_groups;           // 2: the two 8-warp epilogue groups take alternate tiles (many tiles per CTA); 1: both work on every tile
 };
 
 // Host description of one GEMM.

@@ -9,7 +9,7 @@
 //    ([image][head][token][16], gemm_tc "head-major" epilogue), so everything one (image, head) can ever sample is
 //    ONE contiguous slab (51 KB at 40x40).  Persistent CTAs (one per SM, 20 warps) walk the (image, head) items: the
 //    slab is streamed - in bands of <= 1680 tokens - into a four-stage shared-memory ring with 1-D bulk copies
-//    (cp.async.bulk + mbarrier complete_tx; measured 7.0 TB/s at this chunk size with tools/ubench/stream_rate.cu),
+//    (cp.async.bulk + mbarrier complete_tx; tools/ubench/stream_rate.cu measures what that path streams per chunk size),
 //    the threads (two per (query, head): half of the samples each, all 16 channels) take the bilinear corners out of
 //    shared memory.  DRAM sees the value tensor exactly once, as a linear stream; the softmax over
 //    the L*P logits, the sampling-location arithmetic (incl. valid ratios of padded batches) and the weighted sum
@@ -62,17 +62,15 @@ __device__ __forceinline__ uint64_t shfl_xor1_b64(uint64_t v) {
   return (static_cast<uint64_t>(hi) << 32) | lo;
 }
 
-// ncu of the earlier versions of this kernel (history in DESIGN.md 3.2; current capture: profiles/r02_ncu_msda_medium.txt) showed it bound by
-// its own instruction stream and by a tail, not by memory: 735 instructions per (query, head) - a fifth of them integer
-// divisions of the item / pass bookkeeping, another third register shuffling around the 16-bit -> fp32 unpack - at 36 % issue
-// utilisation, with half-CTAs that each walked whole (image, head) items (3.46 items per half at medium / B = 64: 14 % tail).
-// Hence:
+// The kernel is bound by its own instruction stream and by its tail rather than by memory (integer divisions in the item /
+// pass bookkeeping, register shuffling around the 16-bit -> fp32 unpack, and a tail when half-CTAs each walk whole
+// (image, head) items).  Hence:
 //   * the whole CTA (20 warps) works on ONE (image, head) slab at a time; slabs stream through a 4-stage ring filled by one
 //     elected thread (cp.async.bulk + mbarrier complete_tx), so up to three slabs are in flight behind the one being sampled;
 //   * TWO threads per (query, head): each takes half of the L*P samples (all 16 channels), the pair exchanges halves of its
 //     partial sums with 8 shuffles and each stores 8 channels - 600 of 640 threads busy at nq = 300;
 //   * item / image / head counters are incremental (no division in any loop), the unpack is two ALU operations per pair,
-//     the accumulation runs on packed fp32x2 FMAs.
+//     the accumulation runs on fp32 pairs (ptx.cuh f2_*: two scalar FMAs each on sm_90).
 template <typename T, int NL, int NP>   // levels, points per head and level
 __global__ void __launch_bounds__(MS_THREADS, 1) msda_fwd_kernel(const __grid_constant__ MsdaArgs p) {
   constexpr int LP = NL * NP;

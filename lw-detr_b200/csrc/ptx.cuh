@@ -1,6 +1,6 @@
-// Thin inline-PTX wrappers for the sm_100a features the LW-DETR kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld) and
-// 256-bit global accesses.  Everything here is device-only and header-only.
+// Thin inline-PTX wrappers for the sm_90a features the LW-DETR kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma shared-memory descriptors (the MMAs themselves are in wgmma.cuh)
+// and wide global accesses.  Everything here is device-only and header-only.
 #pragma once
 #include <cuda.h>          // CUtensorMap (types only, libcuda is never linked)
 #include <cuda_runtime.h>
@@ -56,8 +56,8 @@ __device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
 }
 // Bounded wait: a pipeline bug must surface as a trap (CUDA error), never as a hung GPU.  The spin loop is kept
 // to try_wait + counter + branch (try_wait itself suspends the thread for a while): waiting warps share issue
-// slots with the working ones, and a clock read / 64-bit compare per iteration showed up in ncu as ~30% of all
-// executed instructions of the attention kernel.  The clock is only consulted every 4096 failed tries.
+// slots with the working ones, so a clock read / 64-bit compare per iteration would be a large share of what a waiting
+// kernel executes.  The clock is only consulted every 4096 failed tries.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   uint32_t spins = 0;
@@ -107,144 +107,26 @@ __device__ __forceinline__ void bulk_load(void* dst, const void* src, uint32_t b
                : "memory");
 }
 
-// ----------------------------------------------------------------------------- clusters / CTA pairs
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-// execution-only rendezvous of the cluster (no memory ordering: nothing written here is read by the peer afterwards)
-__device__ __forceinline__ void cluster_sync_relaxed() {
-  __syncwarp();
-  asm volatile("barrier.cluster.arrive.relaxed;" ::: "memory");
-  asm volatile("barrier.cluster.wait;" ::: "memory");
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  __syncwarp();
-  asm volatile("barrier.cluster.arrive.release;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire;" ::: "memory");
-}
-// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of this cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(smem_u32(bar)), "r"(cta)
-      : "memory");
-}
-// TMA loads issued by either CTA of a pair; the transaction bytes are credited to the LEADER CTA's barrier
-// (peer bit of the barrier address cleared), as the cta_group::2 MMA consumes both halves together.
-static constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-__device__ __forceinline__ void tma2_load_2d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma2_load_4d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
-      "[%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma2_load_5d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, "
-      "%7}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t* slot_in_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_in_smem)), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// One MMA for the CTA pair: D[256 x N] (128 rows in each CTA's TMEM) (+)= A[256 x 16] * B[N x 16]^T, A rows and
-// B rows split half/half between the two CTAs' shared memories at identical offsets.  Issued by the leader only.
-__device__ __forceinline__ void umma2_f16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit: arrive (once all earlier MMAs of this thread completed) on the barrier at this offset in BOTH CTAs
-__device__ __forceinline__ void umma2_commit_both(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(static_cast<uint16_t>(3))
-               : "memory");
-}
 
-// ----------------------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot_in_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_in_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], fp16/bf16 inputs, fp32 accumulate, one CTA.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once every previously issued tcgen05.mma of this thread has completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns: thread t of the warp receives row (lane_base + t).
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// Shared-memory matrix descriptor for a K-major bf16/fp16 tile stored as 128-byte rows with the
-// 128B TMA swizzle (8-row x 128 B atoms, 1024 B apart): SBO = 1024 B, LBO unused (=1), version 1.
-__device__ __forceinline__ uint64_t umma_desc_k128(uint32_t smem_addr) {
+// ----------------------------------------------------------------------------- wgmma operands
+// Shared-memory matrix descriptor of a 16-bit tile whose rows are `pitch` bytes (32 / 64 / 128) written by TMA with the
+// swizzle of the same span: 8-row groups `8 * pitch` bytes apart (stride byte offset), leading byte offset unused (one
+// swizzle span covers the whole row).  The same descriptor serves a K-major operand (rows = M or N) and an MN-major
+// one (rows = K, transposed by the tensor core).  Advancing 16 elements along a K-major row adds 32 bytes (+2).
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr, uint32_t pitch) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
-  d |= static_cast<uint64_t>(1) << 16;            // leading byte offset (ignored for swizzled K-major)
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;    // stride byte offset between 8-row groups
-  d |= static_cast<uint64_t>(1) << 46;            // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;            // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>((8 * pitch) >> 4) << 32;
+  d |= static_cast<uint64_t>(pitch == 128 ? 1 : (pitch == 64 ? 2 : 3)) << 62;   // SWIZZLE_128B / 64B / 32B
   return d;
 }
-// kind::f16 instruction descriptor: fp32 accumulate, A/B both K-major.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(bool bf16, int m, int n) {
-  return (1u << 4) | ((bf16 ? 1u : 0u) << 7) | ((bf16 ? 1u : 0u) << 10) | (static_cast<uint32_t>(n >> 3) << 17) |
-         (static_cast<uint32_t>(m >> 4) << 24);
-}
+template <int N> __device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
-// ----------------------------------------------------------------------------- packed fp32x2 arithmetic (sm_100: FFMA2 / FADD2 / FMUL2)
-// Two fp32 lanes per instruction in a 64-bit register pair: halves the issue slots of FMA-bound epilogues and softmax loops.
+// ----------------------------------------------------------------------------- fp32 pairs
+// Two fp32 values carried in a 64-bit register pair (epilogues and softmax loops work on adjacent columns); sm_90 has no
+// packed fp32x2 arithmetic, so every operation is two scalar instructions.
 __device__ __forceinline__ uint64_t f2_pack(float a, float b) {
   uint64_t r;
   asm("mov.b64 %0, {%1,%2};" : "=l"(r) : "f"(a), "f"(b));
@@ -252,23 +134,28 @@ __device__ __forceinline__ uint64_t f2_pack(float a, float b) {
 }
 __device__ __forceinline__ void f2_unpack(uint64_t v, float& a, float& b) { asm("mov.b64 {%0,%1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
 __device__ __forceinline__ uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  f2_unpack(a, a0, a1);
+  f2_unpack(b, b0, b1);
+  f2_unpack(c, c0, c1);
+  return f2_pack(fmaf(a0, b0, c0), fmaf(a1, b1, c1));
 }
 __device__ __forceinline__ uint64_t f2_add(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  f2_unpack(a, a0, a1);
+  f2_unpack(b, b0, b1);
+  return f2_pack(a0 + b0, a1 + b1);
 }
 __device__ __forceinline__ uint64_t f2_mul(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  f2_unpack(a, a0, a1);
+  f2_unpack(b, b0, b1);
+  return f2_pack(a0 * b0, a1 * b1);
 }
 
-// 2^(s*c - m) for a PAIR of scores without the MUFU (the exp-bound attention kernels move a fraction of their exponentials
-// to the FMA pipe): t = round(s*c - m) + 1.5*2^23 by one FFMA2, the fraction f = s*c - m - round(..) in [-0.5, 0.5] by
+
+// 2^(s*c - m) for a PAIR of scores without the MUFU (the exp-bound attention kernels can move a fraction of their exponentials
+// to the FMA pipe): t = round(s*c - m) + 1.5*2^23 by one FMA per score, the fraction f = s*c - m - round(..) in [-0.5, 0.5] by
 // two more, a degree-3 polynomial for 2^f (max relative error 7.5e-5, an order of magnitude below the 16-bit rounding
 // of P) and the integer part added into the exponent field.  The raw scores are clamped at smin = (m - 125)/c first:
 // below that 2^x is 0 for every purpose here, and an unclamped argument would wrap the exponent field.
@@ -293,19 +180,18 @@ __device__ __forceinline__ void exp2_poly2(float s0, float s1, float smin, uint6
 struct __align__(16) U4 { uint32_t x, y, z, w; };
 struct __align__(32) U8 { uint32_t v[8]; };
 
+// 32 bytes as two 16-byte accesses (sm_90 has no 256-bit global load / store)
 __device__ __forceinline__ U8 ldg256(const void* p) {
   U8 r;
-  asm volatile("ld.global.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]), "=r"(r.v[4]), "=r"(r.v[5]), "=r"(r.v[6]),
-                 "=r"(r.v[7])
-               : "l"(p));
+  asm volatile("ld.global.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]) : "l"(p));
+  asm volatile("ld.global.v4.b32 {%0,%1,%2,%3}, [%4+16];" : "=r"(r.v[4]), "=r"(r.v[5]), "=r"(r.v[6]), "=r"(r.v[7]) : "l"(p));
   return r;
 }
 __device__ __forceinline__ void stg256(void* p, const U8& r) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(r.v[0]), "r"(r.v[1]), "r"(r.v[2]),
-               "r"(r.v[3]), "r"(r.v[4]), "r"(r.v[5]), "r"(r.v[6]), "r"(r.v[7])
-               : "memory");
+  asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(r.v[0]), "r"(r.v[1]), "r"(r.v[2]), "r"(r.v[3]) : "memory");
+  asm volatile("st.global.v4.b32 [%0+16], {%1,%2,%3,%4};" ::"l"(p), "r"(r.v[4]), "r"(r.v[5]), "r"(r.v[6]), "r"(r.v[7]) : "memory");
 }
+
 
 // ----------------------------------------------------------------------------- 16-bit conversions
 template <typename T> struct Cvt;

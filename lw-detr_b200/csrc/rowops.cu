@@ -194,7 +194,7 @@ int layernorm_launch(int dtype, const LayerNormArgs& a, cudaStream_t st) {
 // ----------------------------------------------------------------------------------- patch gather
 // Image [B,3,S,S] (fp32 or 16-bit, NCHW) -> A [B*G*G, 3*256] 16-bit with rows in WINDOW-MAJOR token
 // order and k = c*256 + py*16 + px, so that the 16x16/s16 patch-embedding conv (vit.py:79-83)
-// becomes one tcgen05 GEMM whose output is already in the layout of vit.py:353-358.
+// becomes one wgmma GEMM whose output is already in the layout of vit.py:353-358.
 template <typename T, typename TIn>
 __global__ void __launch_bounds__(256) patch_gather_kernel(const TIn* __restrict__ img, T* __restrict__ A, int B, int S) {
   pdl_sync();   // programmatic dependent launch: release the successor, wait for the predecessor (launch.h)

@@ -37,12 +37,12 @@ int current_device_sms() {
   static std::mutex mu;
   static std::map<int, int> sms;
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   std::lock_guard<std::mutex> lk(mu);
   auto it = sms.find(dev);
   if (it != sms.end()) return it->second;
   int v = 0;
-  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
   sms[dev] = v;
   return v;
 }

@@ -1,5 +1,5 @@
 """Drop-in for the reference's `models` package (models/__init__.py:16-17): `build_model(args)` returns
-(model, criterion, postprocessors) where `model` is the B200-native LWDETR module."""
+(model, criterion, postprocessors) where `model` is the CUDA-native LWDETR module."""
 from .lwdetr import build
 
 

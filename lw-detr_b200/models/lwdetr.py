@@ -1,8 +1,8 @@
-"""B200-native LW-DETR module with the reference's `models.lwdetr` surface (lwdetr.py:36-216, 509-619):
+"""CUDA-native (H100, sm_90a) LW-DETR module with the reference's `models.lwdetr` surface (lwdetr.py:36-216, 509-619):
 LWDETR (an nn.Module whose parameters carry the reference's state_dict names), PostProcess, build().
 
 The forward pass is NOT PyTorch: LWDETR.forward hands the image batch to the C-ABI engine
-(include/lwdetr_b200.h, lwdetr_forward), which runs the hand-written sm_100a kernel schedule.  There is
+(include/lwdetr_b200.h, lwdetr_forward), which runs the hand-written sm_90a kernel schedule.  There is
 no CPU / eager fallback: without the built library or without a CUDA device, forward raises."""
 import os
 
@@ -173,7 +173,7 @@ class PostProcess(nn.Module):
 
 class InferenceOnlyCriterion(nn.Module):
     """build() returns a criterion for API compatibility (lwdetr.py:596-619).  Losses / Hungarian matching
-    are training-side and out of scope of the B200 inference path (SURVEY.md section 2)."""
+    are training-side and out of scope of the inference path (SURVEY.md section 2)."""
 
     def __init__(self, weight_dict):
         super().__init__()

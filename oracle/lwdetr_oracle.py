@@ -6,8 +6,7 @@ Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl refere
 this file; the product path (lw-detr_b200/) never does and has no CPU fallback.
 
 Pinning: tests/test_oracle.py checks this oracle against golden vectors produced by the UNMODIFIED
-reference imported in the build container (tools/make_goldens.py -> tests/golden/*.npz) for all five
-released configurations; when /root/reference is present the same test also compares live.  The
+reference (tools/make_goldens.py -> tests/golden/*.npz) for all five released configurations.  The
 reference itself ships no golden vectors for this path (SURVEY.md 8c), so the goldens are outputs of
 the reference code run on torch 2.11 CPU.
 

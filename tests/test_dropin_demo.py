@@ -1,7 +1,7 @@
 """The reference's own caller, demo/demo.py, driven UNMODIFIED against the drop-in (SURVEY.md 8b, INTEGRATION.md 1):
 PYTHONPATH=<repo>/lw-detr_b200:<reference tree>.  `from models import build_model` resolves to this repo, everything else
-(`util.get_param_dicts`, `util.misc`, torchvision transforms) to the reference.  The reference tree is /root/reference in
-the build container and its byte-identical staged copy baseline/_ref (tools/vendor_reference.py) on the GPU box."""
+(`util.get_param_dicts`, `util.misc`, torchvision transforms) to the reference.  The reference tree is the
+byte-identical staged copy oracle/_ref (oracle/vendor_reference.py, made by build() from a reference checkout)."""
 import os
 import subprocess
 import sys
@@ -49,7 +49,7 @@ print("RESULT " + json.dumps(info))
 def _reference_tree():
     import ref_import
     if not ref_import.available() or not os.path.isfile(os.path.join(ref_import.REF, "demo", "demo.py")):
-        pytest.skip("no reference tree with demo/demo.py (neither /root/reference nor baseline/_ref)")
+        pytest.skip("no reference tree with demo/demo.py (oracle/_ref is staged by build() from a reference checkout)")
     return ref_import.REF
 
 

@@ -1,4 +1,4 @@
-"""tcgen05/TMA GEMM family vs. fp32 torch math on the same 16-bit-rounded operands (kernel-level)."""
+"""wgmma/TMA GEMM family vs. fp32 torch math on the same 16-bit-rounded operands (kernel-level)."""
 import pytest
 import torch
 import torch.nn.functional as F

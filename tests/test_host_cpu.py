@@ -184,16 +184,3 @@ def test_bench_clock_sampler_windows_and_reasons():
     assert r["sm_mhz"] == 1965.0 and r["sm_max_mhz"] == 1965.0 and r["reasons"] == ["sw_power_cap"] and r["samples"] == 4
     assert s.summary(40.0, 50.0) == {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["unavailable"]}
     assert "hw_slowdown" in s.summary()["reasons"]
-
-
-def test_kernel_traffic_table_keys():
-    """profiles/kernel_traffic.json is what bench.py reads for roofline.traffic: keys are config:batch:dtype:op."""
-    import json
-    from b200.config import CONFIGS
-    with open(os.path.join(ROOT, "profiles", "kernel_traffic.json")) as f:
-        t = json.load(f)
-    for k, v in t.items():
-        if k.startswith("_"):
-            continue
-        cfg, batch, dtype, op = k.split(":")
-        assert cfg in CONFIGS and int(batch) > 0 and dtype in ("fp16", "bf16") and op and isinstance(v, int) and v > 0

@@ -27,10 +27,10 @@ REL_L2 = {torch.float16: 1e-3, torch.bfloat16: 8e-3}
 @pytest.mark.parametrize("nseq,seqlen,heads,dh", [(32, 100, 12, 16), (2, 1600, 12, 16), (16, 100, 12, 32), (1, 1600, 12, 32),
                                                   (16, 100, 12, 64), (1, 1600, 12, 64), (3, 300, 8, 32), (2, 100, 8, 32),
                                                   (2, 300, 12, 32), (5, 37, 4, 16),
-                                                  # tcgen05 path (packed qkv, seqlen >= 512, dh >= 32): ragged tails, single-tile last CTA
+                                                  # wgmma path (packed qkv): ragged tails, single-tile last CTA
                                                   (2, 700, 6, 32), (3, 640, 4, 64), (2, 520, 4, 32), (1, 1153, 4, 64),
-                                                  # slot kernel (attn_slots.cu: packed qkv, dh 16 any length, dh 32 windows): lock-step groups of
-                                                  # 1-4 query tiles, ragged key tails, more (window, head) items than slots, single-item launches
+                                                  # head dim 16 at any length, head dim 32 windows: one to ten query tiles, ragged key
+                                                  # tails, a second warpgroup with no rows, many (window, head) items, single-item launches
                                                   (3, 300, 4, 16), (2, 129, 4, 16), (1, 1153, 4, 16), (2, 513, 12, 16), (1, 64, 4, 16), (7, 128, 4, 16),
                                                   (640, 100, 12, 16), (70, 100, 12, 32), (3, 1, 4, 16), (2, 65, 4, 32)])
 def test_attention_matches_softmax_reference(dt, nseq, seqlen, heads, dh):
@@ -47,8 +47,8 @@ def test_attention_matches_softmax_reference(dt, nseq, seqlen, heads, dh):
     err = (out.float() - ref).abs().max().item()
     assert err <= _tol(dt) * ref.abs().max().item(), err
     assert _rel_l2(out.float(), ref) <= REL_L2[dt]
-    # per-row bound: no query row may be off by more than a few 16-bit ulps of its own magnitude (measured worst row 4.8e-3 fp16
-    # at 1153 keys: the rounding of P, averaged over the keys, against a row norm that is itself an average)
+    # per-row bound: no query row may be off by more than a few 16-bit ulps of its own magnitude (the rounding
+    # of P, averaged over the keys, against a row norm that is itself an average)
     row_err = (out.float() - ref).norm(dim=1) / (ref.norm(dim=1) + 1e-6)
     assert row_err.max().item() <= 8 * REL_L2[dt], row_err.max().item()
 
@@ -57,7 +57,7 @@ def test_attention_matches_softmax_reference(dt, nseq, seqlen, heads, dh):
 @pytest.mark.parametrize("dh", [16, 32, 64])
 def test_attention_late_dominant_keys(dt, dh):
     """Keys whose scores dwarf everything seen before arrive late in the sequence: the lazily tracked row maximum of
-    the tcgen05 kernel has to move (O rescaled in TMEM) several times, and rows must still normalise exactly."""
+    the kernel has to move (O rescaled) several times, and rows must still normalise exactly."""
     from b200 import capi
     nseq, seqlen, heads = 2, 1600, 4
     g = torch.Generator(device="cuda").manual_seed(dh)
@@ -330,15 +330,15 @@ def test_ms_deform_attn_backward_operator(N, M, D, Lq, L, P, shapes):
 
 
 def _reference_ops_package():
-    """The reference's models/ops Python package (functions/, modules/) from /root/reference or its staged copy
-    baseline/_ref, with OUR MultiScaleDeformableAttention module standing in for the compiled one."""
+    """The reference's models/ops Python package (functions/, modules/) from its staged copy
+    oracle/_ref, with OUR MultiScaleDeformableAttention module standing in for the compiled one."""
     import importlib
     import os
     import sys
     sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools"))
     import ref_import
     if not ref_import.available():
-        pytest.skip("no reference tree (neither /root/reference nor baseline/_ref)")
+        pytest.skip("no reference tree (oracle/_ref is staged by build() from a reference checkout)")
     mod = sys.modules.get("MultiScaleDeformableAttention")
     if mod is None or not hasattr(mod, "ms_deform_attn_forward"):
         sys.modules.pop("MultiScaleDeformableAttention", None)
@@ -357,7 +357,7 @@ def _reference_ops_package():
 def test_reference_msdeformattnfunction_binds_to_this_library():
     """models/ops/test.py replayed with the reference's OWN autograd Function and checker, unmodified
     (functions/ms_deform_attn_func.py:23-50): `import MultiScaleDeformableAttention as MSDA` resolves to the drop-in
-    module, forward and backward run on the sm_100a kernels."""
+    module, forward and backward run on the sm_90a kernels."""
     Fn, core = _reference_ops_package()
     N, M, D, Lq, L, P = 1, 2, 2, 2, 2, 2                                   # test.py:27-31
     shapes = torch.as_tensor([(6, 4), (3, 2)], dtype=torch.long).cuda()

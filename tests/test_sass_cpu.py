@@ -1,5 +1,5 @@
-"""The shipped library really takes the Blackwell path: SASS mnemonic counts per kernel (cuobjdump, no GPU needed).
-UTCHMMA = tcgen05.mma, UTMALDG = TMA tensor load, UBLKCP = cp.async.bulk, LDTM / STTM = tcgen05.ld / st, HMMA = legacy mma.sync."""
+"""The shipped library really takes the Hopper path: SASS mnemonic counts per kernel (cuobjdump, no GPU needed).
+HGMMA = wgmma.mma_async, UTMALDG = TMA tensor load, UBLKCP = cp.async.bulk, HMMA = mma.sync, LDGSTS = cp.async."""
 import os
 import re
 import shutil
@@ -41,31 +41,31 @@ def _sel(table, prefix):
     return {k: v for k, v in table.items() if prefix in k}
 
 
-def test_attention_slot_kernels_are_tcgen05_tma_only(table):
-    ks = _sel(table, "attn_slots_kernel<")
-    assert len(ks) >= 16
+def test_packed_attention_kernels_are_wgmma_tma_only(table):
+    ks = _sel(table, "attn_wg_kernel<")
+    assert len(ks) >= 6                      # head dims 16 / 32 / 64 in fp16 and bf16
     for name, c in ks.items():
-        assert c["UTCHMMA"] > 0 and c["UTMALDG"] > 0 and c["LDTM"] > 0 and c["STTM"] > 0, name
+        assert c["HGMMA"] > 0 and c["UTMALDG"] > 0 and c["SYNCS"] > 0, name
         assert c["HMMA"] == 0 and c["LDGSTS"] == 0, name
 
 
-def test_gemm_family_is_tcgen05_tma(table):
+def test_gemm_family_is_wgmma_tma(table):
     ks = _sel(table, "gemm_tc_kernel<")
     assert len(ks) >= 24
     for name, c in ks.items():
-        assert c["UTCHMMA"] > 0 and c["UTMALDG"] > 0 and c["LDTM"] > 0, name
-        assert c["HMMA"] == 0, name
+        assert c["HGMMA"] > 0 and c["UTMALDG"] > 0 and c["SYNCS"] > 0, name
+        assert c["HMMA"] == 0 and c["LDGSTS"] == 0, name
 
 
 def test_deformable_gather_streams_with_bulk_copies(table):
     ks = _sel(table, "msda_fwd_kernel<")
     assert ks
     for name, c in ks.items():
-        assert c["UBLKCP"] > 0 and c["FFMA2"] > 0, name
+        assert c["UBLKCP"] > 0 and c["SYNCS"] > 0, name
 
 
 def test_legacy_mma_sync_only_where_documented(table):
-    """mma.sync (HMMA) is allowed only in attn.cu's kernels: decoder self-attention, head-dim-64 windows, unpacked q/k/v."""
+    """mma.sync (HMMA) is allowed only in attn.cu's kernels: decoder self-attention, unpacked q/k/v."""
     for name, c in table.items():
         if c["HMMA"] > 0:
             assert name.startswith("attn_kernel<") or name.startswith("attn_short_kernel<"), name

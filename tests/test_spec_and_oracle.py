@@ -1,7 +1,6 @@
 """CPU tests: the state_dict table and the oracle are pinned to the reference.
 
-Goldens (tests/golden/) were produced by tools/make_goldens.py running the UNMODIFIED reference in the
-build container; when /root/reference is present the live comparison runs too."""
+Goldens (tests/golden/) were produced by tools/make_goldens.py running the UNMODIFIED reference."""
 import json
 import os
 import sys
@@ -104,16 +103,14 @@ def test_msda_core_matches_grid_sample_formulation():
     assert torch.allclose(got, ref, rtol=1e-9, atol=1e-12)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/models"), reason="reference tree not present")
 def test_oracle_matches_live_reference_with_forced_topk():
-    import ref_import
+    """The oracle against the reference's forward on a second set of weights / images (seeds 5 / 9); the reference's
+    predictions are stored (tests/golden/ref_tiny_seed5.npz, tools/make_goldens.py make_seed5_golden)."""
     cfg = CONFIGS["tiny"]
-    model, _, _ = ref_import.build_reference(cfg)
     sd = synth_state_dict(cfg, 5)
-    model.load_state_dict(sd, strict=True)
     x = synth_images(2, 9)
-    with torch.no_grad():
-        ref = model(x)
+    g = np.load(os.path.join(GOLD, "ref_tiny_seed5.npz"))
+    ref = {k: torch.from_numpy(g[k]) for k in ("pred_logits", "pred_boxes")}
     out = orc.forward(sd, cfg, x)
     assert (out["pred_logits"] - ref["pred_logits"]).abs().max().item() < 1e-4
     assert (out["pred_boxes"] - ref["pred_boxes"]).abs().max().item() < 1e-5
@@ -124,7 +121,7 @@ def _have_reference():
     return ref_import.available()
 
 
-@pytest.mark.skipif(not _have_reference(), reason="reference tree not present (neither /root/reference nor baseline/_ref)")
+@pytest.mark.skipif(not _have_reference(), reason="reference tree not present (oracle/_ref is staged by build() from a reference checkout)")
 def test_reference_forward_export_is_the_last_layer_tuple():
     """SURVEY.md 8f-4, first half: after LWDETR.export() the reference's forward IS forward_export (lwdetr.py:103-109,
     176-195).  With the decoder in export mode only the last layer's hidden state is returned (transformer.py:406-414),

@@ -2,8 +2,8 @@
 window attention) plus global attention, at the BASELINE configs, through the C ABI.
 
 Timing: CUDA events around each launch, L2 flushed (256 MB write) before every timed launch, median of
-`--iters`; achieved = SURVEY.md 8d algorithmic bytes / time, peak = MEASURED_PEAKS.json HBM copy bandwidth.
-    python tools/bench_kernels.py --out profiles/rNN_kernels.json
+`--iters`; achieved = SURVEY.md 8d algorithmic bytes / time, peak = the H100 SXM data sheet's HBM bandwidth (a ceiling).
+    python tools/bench_kernels.py --out kernels.json
 """
 import argparse
 import json
@@ -22,29 +22,24 @@ from b200.config import CONFIGS  # noqa: E402
 
 
 def peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            m = json.load(f)
-        return m["hbm_gbs"], m["bf16_tflops"], "measured"
-    except Exception:
-        return 6650.0, 1590.0, "fallback"
+    """H100 SXM data sheet (700 W card): HBM3 GB/s, dense 16-bit TFLOP/s - ceilings, not rates this project reached."""
+    return 3350.0, 989.0, "H100 SXM data sheet"
 
 
 FLUSH_MODE = "clean"
 
 
 def timed(fn, iters, flush):
-    """L2 flush before every timed launch.  "dirty": a 256 MB read-modify-write leaves the 126 MB L2 full of DIRTY lines, so
+    """L2 flush before every timed launch.  "dirty": a 256 MB read-modify-write leaves the 50 MB L2 full of DIRTY lines, so
     every line the timed kernel then allocates first evicts a dirty one - the kernel's DRAM reads compete 1:1 with
-    write-backs of the flush buffer, which caps a read-only kernel near half of the copy bandwidth (measured: the same
-    MSDA launch reads 2.9 TB/s "dirty" vs the figure reported here).  "clean" (default): the write pass is followed by a
+    write-backs of the flush buffer, which caps a read-only kernel near half of the copy bandwidth.  "clean" (default): the write pass is followed by a
     256 MB read pass of a second buffer, so the L2 holds clean lines of unrelated data: inputs still come from DRAM, and
     only the kernel's own traffic is on the memory bus.  Both are recorded (`flush` field)."""
     ts = []
     for _ in range(3):
         fn()
     for _ in range(iters):
-        flush[0].add_(1)                                 # 256 MB read+write evicts the 126 MB L2
+        flush[0].add_(1)                                 # 256 MB read+write evicts the 50 MB L2
         if FLUSH_MODE == "clean":
             flush[1].sum()                               # 256 MB read: what stays in L2 is clean
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -105,7 +100,7 @@ def main():
             r = {"kernel": kind, "config": "%s B=%d %s dh=%d" % (name, B, str(dt)[6:], dh), "us_median": med, "us_best": best,
                  "algorithmic_MB": algo / 1e6, "achieved_GBps": algo / med / 1e3, "peak_GBps": hbm, "hbm_frac": algo / med / 1e3 / hbm,
                  "gflop": flops / 1e9, "achieved_TFLOPs": flops / med / 1e6, "tensor_frac": flops / med / 1e6 / tflops,
-                 "gexp_per_s": exps / med / 1e3, "exp_frac_of_mufu_peak": exps / med / 1e3 / (16 * 148 * 1.965)}
+                 "gexp_per_s": exps / med / 1e3, "exp_frac_of_mufu_peak": exps / med / 1e3 / (16 * 132 * 1.98)}
             r["bound"] = "hbm" if kind == "window_attention" else "tensor (nominal) / exp"
             r["frac"] = r["hbm_frac"] if kind == "window_attention" else r["tensor_frac"]
             res.append(r)

@@ -1,7 +1,6 @@
 """Build liblwdetr_b200.so (CUDA kernels + C-ABI) and the CPU oracle helpers.
 
-nvcc cross-compiles for sm_100a without a GPU, so this runs in the build container as well as on
-the GPU box.  Objects are cached by source mtime under lw-detr_b200/build/.
+nvcc cross-compiles for sm_90a without a GPU, so this runs on a machine without a GPU as well.  Objects are cached by source mtime under lw-detr_b200/build/.
 """
 import concurrent.futures as cf
 import os
@@ -16,7 +15,7 @@ LIB = os.path.join(PKG, "lib", "liblwdetr_b200.so")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "-I", os.path.join(ROOT, "include"), "-I", CSRC,
 ]
 
@@ -55,7 +54,7 @@ def build(verbose=False, force=False):
         for f in futs:
             objs.append(f.result())
     if _stale(LIB, objs):
-        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
         if verbose:
             print(" ".join(cmd), flush=True)
         r = subprocess.run(cmd, capture_output=True, text=True)

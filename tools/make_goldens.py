@@ -1,7 +1,8 @@
-"""Generate tests/golden/*.npz by running the UNMODIFIED reference (imported from /root/reference via
-tools/ref_import.py) on the deterministic synthetic weights/inputs of b200/synth.py.
+"""Generate tests/golden/*.npz by running the UNMODIFIED reference (imported via tools/ref_import.py from the
+checkout named by $LWDETR_REFERENCE_SRC or staged under oracle/_ref) on the deterministic synthetic weights/inputs of
+b200/synth.py.
 
-Run in the build container only:  python tools/make_goldens.py
+    python tools/make_goldens.py [--postprocess-only | --padded-only | --seed5-only]
 Each fixture holds the reference's final outputs and strided samples of its intermediates (captured
 with forward hooks), plus the state_dict names/shapes (tests/golden/state_dict_<cfg>.json).
 """
@@ -85,9 +86,25 @@ def make_padded_golden():
     print("padded", out["pred_logits"].shape)
 
 
+def make_seed5_golden():
+    """Reference forward of LW-DETR-tiny on a second set of weights / images (seeds 5 / 9, batch 2): the final predictions
+    the oracle is compared with in tests/test_spec_and_oracle.py::test_oracle_matches_live_reference_with_forced_topk."""
+    cfg = CONFIGS["tiny"]
+    model, _, _ = ref_import.build_reference(cfg)
+    model.load_state_dict(synth_state_dict(cfg, 5), strict=True)
+    with torch.no_grad():
+        out = model(synth_images(2, 9))
+    np.savez_compressed(os.path.join(GOLD, "ref_tiny_seed5.npz"), pred_logits=out["pred_logits"].numpy(),
+                        pred_boxes=out["pred_boxes"].numpy(), meta=np.array([2, 5, 9], dtype=np.int64))
+    print("seed5", out["pred_logits"].shape)
+
+
 def main():
     torch.set_num_threads(os.cpu_count())
     os.makedirs(GOLD, exist_ok=True)
+    if "--seed5-only" in sys.argv:
+        make_seed5_golden()
+        return
     if "--postprocess-only" in sys.argv:
         make_postprocess_goldens()
         return
@@ -132,6 +149,7 @@ def main():
         print(name, "B=%d" % B, {k: v.shape for k, v in rec.items() if k.startswith("pred")})
     make_postprocess_goldens()
     make_padded_golden()
+    make_seed5_golden()
 
 
 if __name__ == "__main__":

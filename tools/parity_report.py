@@ -1,7 +1,7 @@
 """Parity ladder: CUDA engine (fp16 / bf16) vs the CPU oracle (fp32) on identical synthetic weights/inputs.
 
 Prints / returns per-stage errors (SURVEY.md 8c tiers T1 pre-top-k tensors, T2 forced indices,
-T3 free-running).  Runs on the GPU box:  python tools/parity_report.py small --batch 2 --dtype fp16
+T3 free-running).  Needs a GPU:  python tools/parity_report.py small --batch 2 --dtype fp16
 """
 import argparse
 import json

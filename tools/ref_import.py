@@ -1,8 +1,8 @@
-"""Import the UNMODIFIED reference (Atten4Vis/LW-DETR at /root/reference) in the build container.
+"""Import the UNMODIFIED reference (Atten4Vis/LW-DETR): the checkout named by $LWDETR_REFERENCE_SRC, else the byte-identical
+copy staged under oracle/_ref/ by oracle/vendor_reference.py (git-ignored).
 
-Used by the golden-vector generator (tools/make_goldens.py), by CPU tests that are skipped when no
-reference tree is available, and by bench.py's reference arm / cpu_baseline leg, which on the GPU box import
-the byte-identical copy staged under baseline/_ref/ by tools/vendor_reference.py (git-ignored).  Three third-party modules the
+Used by the golden-vector generator (tools/make_goldens.py), by tests that are skipped when no reference tree is
+available, and by bench.py's reference arm / cpu_baseline leg.  Three third-party modules the
 reference imports are missing offline and are shimmed (SURVEY.md section 8c):
   * timm.models.layers: DropPath (identity at eval), Mlp (fc1 -> GELU(erf) -> fc2), trunc_normal_
   * fairscale.nn.checkpoint.checkpoint_wrapper (never invoked: use_act_checkpoint=False)
@@ -14,9 +14,8 @@ import os
 import sys
 import types
 
-_VENDORED = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "baseline", "_ref")
-# /root/reference in the build container; on the GPU box the unmodified copy staged by tools/vendor_reference.py
-REF = os.environ.get("LWDETR_REFERENCE") or ("/root/reference" if os.path.isdir("/root/reference/models") else _VENDORED)
+_VENDORED = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref")
+REF = os.environ.get("LWDETR_REFERENCE_SRC") or _VENDORED
 
 
 def available():

@@ -1,8 +1,8 @@
 """Per-kernel counts of the SASS mnemonics that prove which hardware path a kernel takes, from `cuobjdump -sass` of the
 shipped library (runs without a GPU).
-    python tools/sass_proof.py [lib] > profiles/rNN_sass_proof.txt
+    python tools/sass_proof.py [lib]
 A function's block runs from its "Function : <mangled>" line to the next one; every instruction line of the block is counted
-(the round-1 generator stopped at the first blank line, which truncated long kernels and reported zeros for them)."""
+(a block does not end at its first blank line: long kernels contain several)."""
 import collections
 import os
 import re
@@ -10,7 +10,7 @@ import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-COLS = ["UTCHMMA", "UTCBAR", "UTCATOMSWS", "LDTM", "STTM", "UTMALDG", "UBLKCP", "HMMA", "MUFU.EX2", "LDGSTS", "LDSM", "SYNCS", "FFMA2"]
+COLS = ["HGMMA", "UTMALDG", "UBLKCP", "HMMA", "MUFU.EX2", "LDGSTS", "LDSM", "SYNCS"]
 
 
 def main(lib):
@@ -36,9 +36,9 @@ def main(lib):
         for c in COLS:
             if op == c or op.startswith(c + "."):
                 counts[cur][c] += 1
-    print("# cuobjdump -sass %s (sm_100a): per-kernel counts of the SASS mnemonics that prove the path" % os.path.relpath(lib, ROOT))
-    print("# UTCHMMA = tcgen05.mma, UTCBAR = tcgen05.commit, UTCATOMSWS = tcgen05.alloc, LDTM/STTM = tcgen05.ld/st, UTMALDG = TMA tensor load,")
-    print("# UBLKCP = cp.async.bulk (1-D bulk copy), HMMA = legacy mma.sync, LDGSTS = cp.async, FFMA2 = packed fp32x2 FMA")
+    print("# cuobjdump -sass %s (sm_90a): per-kernel counts of the SASS mnemonics that prove the path" % os.path.relpath(lib, ROOT))
+    print("# HGMMA = wgmma.mma_async, UTMALDG = TMA tensor load, UBLKCP = cp.async.bulk (1-D bulk copy), HMMA = mma.sync,")
+    print("# LDGSTS = cp.async, LDSM = ldmatrix, SYNCS = mbarrier operations")
     w = max(len(n) for n in order) + 2
     print("%-*s" % (w, "kernel") + "".join("%11s" % c for c in COLS))
     for n in sorted(order):

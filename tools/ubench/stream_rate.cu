@@ -3,8 +3,8 @@
 //          the stages (chunk size x ring depth sweep, 1 or 2 CTAs per SM)
 //   ldg  : every thread issues 16-byte ld.global.nc loads (8 in flight per thread), 1024 / 2048 threads per SM
 // The buffer (1 GiB) is larger than the L2; every byte is read once.  Motivation: msda.cu stages 51 KB value slabs with
-// bulk copies and reached only ~2 TB/s - is that the TMA path's limit or the kernel's?
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tools/ubench/stream_rate tools/ubench/stream_rate.cu
+// bulk copies - is its rate the TMA path's limit or the kernel's?
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/ubench/stream_rate tools/ubench/stream_rate.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -63,6 +63,9 @@ __global__ void __launch_bounds__(1024) k_ldg(const uint4* src, size_t n16, unsi
 
 int main() {
   const size_t total = 1ull << 30;
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+  if (sms <= 0) { fprintf(stderr, "no CUDA device\n"); return 1; }
   uint8_t* buf;
   unsigned long long* sink;
   cudaMalloc(&buf, total);
@@ -78,7 +81,7 @@ int main() {
     const size_t smem = (size_t)c.chunk * c.stages + 16 * c.stages + 64;
     for (int rep = 0; rep < 3; ++rep) {
       cudaEventRecord(e0);
-      k_bulk<<<148 * c.ctas_per_sm, 160, smem>>>(buf, total, c.chunk, c.stages, sink);
+      k_bulk<<<sms * c.ctas_per_sm, 160, smem>>>(buf, total, c.chunk, c.stages, sink);
       cudaEventRecord(e1);
       cudaEventSynchronize(e1);
       float ms;
@@ -92,7 +95,7 @@ int main() {
       if (tpb * cps > 2048) continue;
       for (int rep = 0; rep < 3; ++rep) {
         cudaEventRecord(e0);
-        k_ldg<<<148 * cps, tpb>>>(reinterpret_cast<const uint4*>(buf), total / 16, sink);
+        k_ldg<<<sms * cps, tpb>>>(reinterpret_cast<const uint4*>(buf), total / 16, sink);
         cudaEventRecord(e1);
         cudaEventSynchronize(e1);
         float ms;
