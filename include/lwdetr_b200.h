@@ -114,7 +114,7 @@ LWDETR_API int lwdetr_msda_forward(int dtype, const void* value_hm, int64_t v_im
                                    const int32_t* level_start_host, void* stream);
 
 /* torch.topk(score, k, dim=1)[1] for fp32 score [B, S] -> int32 idx [B, k], sorted, ties -> lower index
- * (transformer.py:246). */
+ * (transformer.py:246).  Any S >= k; above S = 16384 (large inputs) a radix select that streams the row, with k <= 4096. */
 LWDETR_API int lwdetr_topk(const float* score, int B, int S, int k, int32_t* idx, void* stream);
 
 /* PostProcess.forward (lwdetr.py:515-544) fused on the device: per image the top `num_select` of
@@ -130,6 +130,9 @@ LWDETR_API int lwdetr_postprocess(const float* pred_logits, const float* pred_bo
 /* Host helper (no GPU): bicubic, align_corners=False resize of a channels-last [n_in, n_in, C] fp32 grid
  * to [n_out, n_out, C] - the absolute position embedding resize of vit.py:26-54, done once at load. */
 LWDETR_API int lwdetr_host_bicubic(const float* src, int n_in, int C, int n_out, float* dst);
+/* The same resize to a non-square [out_h, out_w, C] grid: the position table of a non-square input (vit.py:26-54 with
+ * hw = (H/16, W/16)). */
+LWDETR_API int lwdetr_host_bicubic_hw(const float* src, int n_in, int C, int out_h, int out_w, float* dst);
 
 /* ------------------------------------------------------------------------------------------------
  * Model-level API: what models.lwdetr.LWDETR.forward (lwdetr.py:111-174) binds to.
@@ -190,10 +193,20 @@ typedef struct {
 LWDETR_API int lwdetr_forward_ex(lwdetr_handle* h, const lwdetr_input* input, int B, float* pred_logits, float* pred_boxes,
                                  const lwdetr_aux_out* aux, const int32_t* topk_override, void* stream);
 
+/* lwdetr_forward_ex at any supported input size: images [B, 3, height, width] (fp32 / compute dtype) or [B, height, width, 3]
+ * (uint8), padding_mask [B, height, width].  height and width are multiples of 64 in [128, 1344] (4x4 windows of 16-pixel
+ * patches, vit.py:353-358); the position embedding is resized to the (height/16, width/16) token grid (vit.py:26-54) and
+ * every feature level takes its shape from that grid.  The memory length (tokens over all levels) must be at least
+ * num_queries.  lwdetr_forward_ex is this call with height = width = img_size.  A (B, height, width) different from the
+ * previous call re-plans the schedule and drops its CUDA graphs (one plan is kept at a time). */
+LWDETR_API int lwdetr_forward_hw(lwdetr_handle* h, const lwdetr_input* input, int B, int height, int width, float* pred_logits,
+                                 float* pred_boxes, const lwdetr_aux_out* aux, const int32_t* topk_override, void* stream);
+
 /* Multi-GPU init (SURVEY.md 8e): ONE ncclBroadcast of the packed weight arena from rank `root`, stream-ordered on
  * `stream`; the only collective of the path (images shard across ranks as independent replicas, nothing on the hot path).
  * Every rank first calls lwdetr_load_weights with tensors of the right shapes (any values on the non-root ranks): that
  * fixes the arena layout, which is a function of (config, dtype) only; the call verifies that the arena sizes agree.
+ * The arena holds the raw pos_embed too, so position tables planned for other input sizes follow the root's weights.
  * `nccl_comm` is an ncclComm_t of a communicator the caller created (one rank per GPU); NCCL is resolved at run time
  * from the libnccl already loaded in the process (or dlopen("libnccl.so.2")), the library does not link it. */
 LWDETR_API int lwdetr_broadcast_weights(lwdetr_handle* h, void* nccl_comm, int root, void* stream);

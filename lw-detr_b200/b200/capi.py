@@ -29,6 +29,7 @@ _SIGNATURES = {
     "lwdetr_topk": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "lwdetr_postprocess": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_host_bicubic": (_i, [_vp, _i, _i, _i, _vp]),
+    "lwdetr_host_bicubic_hw": (_i, [_vp, _i, _i, _i, _i, _vp]),
     "lwdetr_create": (_i, [_vp, _i, _vp]),
     "lwdetr_destroy": (None, [_vp]),
     "lwdetr_load_weights": (_i, [_vp, _i, _vp, _vp, _vp]),
@@ -36,6 +37,7 @@ _SIGNATURES = {
     "lwdetr_broadcast_weights": (_i, [_vp, _vp, _i, _vp]),
     "lwdetr_weight_arena_bytes": (_i64, [_vp]),
     "lwdetr_forward_ex": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
+    "lwdetr_forward_hw": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_set_option": (_i, [_vp, ctypes.c_char_p, _i]),
     "lwdetr_add_capture": (_i, [_vp, ctypes.c_char_p, _vp, _i64]),
     "lwdetr_capture_result": (_i64, [_vp, _i]),
@@ -232,6 +234,15 @@ def host_bicubic(src, n_out):
     return dst
 
 
+def host_bicubic_hw(src, out_h, out_w):
+    """src: CPU fp32 [n, n, C] -> [out_h, out_w, C] (no GPU involved)."""
+    import torch
+    src = src.contiguous().float()
+    dst = torch.empty(out_h, out_w, src.shape[2], dtype=torch.float32)
+    check(lib().lwdetr_host_bicubic_hw(ptr(src), src.shape[0], src.shape[2], out_h, out_w, ptr(dst)), "lwdetr_host_bicubic_hw")
+    return dst
+
+
 class ConfigStruct(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in ("vit_dim", "vit_depth", "vit_heads", "window_block_mask", "n_taps")] + \
                [("taps", ctypes.c_int32 * 4), ("n_levels", ctypes.c_int32), ("level_scale_log2", ctypes.c_int32 * 2)] + \
@@ -321,32 +332,37 @@ class Engine:
         check(lib().lwdetr_set_option(self._h, name.encode(), int(value)), "lwdetr_set_option")
 
     def forward(self, images, want_aux=True, topk_override=None, mask=None, mean=IMAGENET_MEAN, std=IMAGENET_STD):
-        """images: CUDA [B,3,S,S] fp32 / compute dtype, or CUDA uint8 [B,S,S,3] (HWC, normalised on the fly with mean/std);
-        mask: CUDA bool [B,S,S] (True = padded pixel) or None.  Returns the reference's output dict (fp32 CUDA tensors)."""
+        """images: CUDA [B,3,H,W] fp32 / compute dtype, or CUDA uint8 [B,H,W,3] (HWC, normalised on the fly with mean/std);
+        mask: CUDA bool [B,H,W] (True = padded pixel) or None.  H and W: multiples of 64 in [128, 1344] (b200.config.
+        check_input_size); a size other than the previous call's re-plans the engine.  Returns the reference's output dict
+        (fp32 CUDA tensors)."""
         import torch
+        from .config import check_input_size
         if images.device.type != "cuda":
             raise RuntimeError("lwdetr_b200: images must be CUDA tensors")
         if images.device != self.device:
             raise RuntimeError("lwdetr_b200: images are on %s but the engine lives on %s" % (images.device, self.device))
-        S = self.cfg.img_size
         desc = InputDesc()
         if images.dtype == torch.uint8:
-            if images.dim() != 4 or tuple(images.shape[1:]) != (S, S, 3):
-                raise RuntimeError("lwdetr_b200: uint8 images must be [B, %d, %d, 3] (HWC), got %s" % (S, S, tuple(images.shape)))
+            if images.dim() != 4 or images.shape[3] != 3:
+                raise RuntimeError("lwdetr_b200: uint8 images must be [B, H, W, 3] (HWC), got %s" % (tuple(images.shape),))
+            H, W = int(images.shape[1]), int(images.shape[2])
             desc.format = IN_U8_NHWC
             for c in range(3):
                 desc.mean[c], desc.std[c] = float(mean[c]), float(std[c])
         else:
-            if images.dim() != 4 or images.shape[1] != 3 or images.shape[2] != S or images.shape[3] != S:
-                raise RuntimeError("lwdetr_b200: expected images [B, 3, %d, %d], got %s" % (S, S, tuple(images.shape)))
+            if images.dim() != 4 or images.shape[1] != 3:
+                raise RuntimeError("lwdetr_b200: expected images [B, 3, H, W], got %s" % (tuple(images.shape),))
+            H, W = int(images.shape[2]), int(images.shape[3])
             if images.dtype not in (torch.float32, self.dtype):
                 images = images.float()
             desc.format = IN_F32_NCHW if images.dtype == torch.float32 else IN_16_NCHW
+        check_input_size(self.cfg, H, W)
         images = images.contiguous()
         mk = None
         if mask is not None:
-            if tuple(mask.shape) != (images.shape[0], S, S):
-                raise RuntimeError("lwdetr_b200: mask must be [B, %d, %d], got %s" % (S, S, tuple(mask.shape)))
+            if tuple(mask.shape) != (images.shape[0], H, W):
+                raise RuntimeError("lwdetr_b200: mask must be [B, %d, %d], got %s" % (H, W, tuple(mask.shape)))
             mk = mask.to(device=self.device, dtype=torch.bool).contiguous()
         desc.images = images.data_ptr()
         desc.padding_mask = mk.data_ptr() if mk is not None else None
@@ -371,8 +387,8 @@ class Engine:
         ov = None
         if topk_override is not None:
             ov = topk_override.to(device=dev, dtype=torch.int32).contiguous()
-        check(lib().lwdetr_forward_ex(self._h, ctypes.byref(desc), B, ptr(logits), ptr(boxes),
-                                      ctypes.byref(aux) if aux is not None else None, ptr(ov), stream_ptr(self.device)), "lwdetr_forward_ex")
+        check(lib().lwdetr_forward_hw(self._h, ctypes.byref(desc), B, H, W, ptr(logits), ptr(boxes),
+                                      ctypes.byref(aux) if aux is not None else None, ptr(ov), stream_ptr(self.device)), "lwdetr_forward_hw")
         self._last_inputs = (images, ov, mk)    # keep alive until the stream has consumed them
         return res
 

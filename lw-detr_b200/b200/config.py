@@ -57,6 +57,40 @@ class LWDETRConfig:
     def taps(self):
         return tuple(sorted(i if i >= 0 else i + self.vit_depth for i in self.out_feature_indexes))
 
+    def level_shapes_at(self, height, width):
+        """Feature-level shapes of an input of height x width pixels: P3 = 2x, P4 = 1x, P5 = 1/2 of the (H/16, W/16) token grid."""
+        gh, gw = height // self.patch, width // self.patch
+        f = {"P3": 2.0, "P4": 1.0, "P5": 0.5}
+        return tuple((int(gh * f[p]), int(gw * f[p])) for p in self.projector_scale)
+
+    def memory_len_at(self, height, width):
+        return sum(h * w for h, w in self.level_shapes_at(height, width))
+
+
+# Input sizes the CUDA path runs: both sides multiples of 64 (4x4 windows of 16-pixel patches, vit.py:353-358) in
+# [MIN_SIDE, MAX_SIDE], and at least num_queries memory tokens (torch.topk over the memory, transformer.py:246).
+SIDE_STEP, MIN_SIDE, MAX_SIDE = 64, 128, 1344
+
+
+def check_input_size(cfg, height, width):
+    """Raise RuntimeError unless a height x width input is one the CUDA path runs."""
+    if height % SIDE_STEP or width % SIDE_STEP or not (MIN_SIDE <= height <= MAX_SIDE and MIN_SIDE <= width <= MAX_SIDE):
+        raise RuntimeError("lwdetr_b200: input %dx%d is not supported: height and width must be multiples of %d in [%d, %d]"
+                           % (height, width, SIDE_STEP, MIN_SIDE, MAX_SIDE))
+    if cfg.memory_len_at(height, width) < cfg.num_queries:
+        raise RuntimeError("lwdetr_b200: a %dx%d input has %d memory tokens, fewer than num_queries = %d"
+                           % (height, width, cfg.memory_len_at(height, width), cfg.num_queries))
+
+
+def run_size(cfg, height, width):
+    """The (H, W) a batch whose largest image is height x width runs at: each side rounded up to a multiple of 64 and never
+    below img_size (smaller batches are padded to the configured size, as before), bottom / right padding carried by the
+    NestedTensor mask.  800x1333 -> 832x1344.  RuntimeError when the result is not a supported input size."""
+    up = lambda v: -(-int(v) // SIDE_STEP) * SIDE_STEP
+    H, W = max(cfg.img_size, up(height)), max(cfg.img_size, up(width))
+    check_input_size(cfg, H, W)
+    return H, W
+
 
 _W10 = (0, 1, 3, 6, 7, 9)
 _T10 = (2, 4, 5, 9)

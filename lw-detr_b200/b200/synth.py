@@ -82,6 +82,8 @@ def synth_state_dict(cfg, seed=1):
 
 
 def synth_images(batch, seed=0, size=640):
-    """ImageNet-normalised-looking input: N(0, 1) pixels, [B, 3, size, size] fp32 (demo.py:146-159)."""
+    """ImageNet-normalised-looking input: N(0, 1) pixels, [B, 3, size, size] fp32 (demo.py:146-159); size may also be a
+    (height, width) pair."""
     g = torch.Generator().manual_seed(int(seed))
-    return torch.randn((batch, 3, size, size), generator=g)
+    h, w = (size, size) if isinstance(size, int) else (int(size[0]), int(size[1]))
+    return torch.randn((batch, 3, h, w), generator=g)

@@ -138,7 +138,7 @@ int lwdetr_msda_forward(int dtype, const void* value_hm, int64_t v_image_stride,
   a.value = value_hm; a.v_b_stride = v_image_stride; a.offs_logits = offs_logits; a.ld_ol = ld_ol; a.ref = ref; a.valid_ratio = valid_ratio;
   a.out = out; a.ld_out = ld_out; a.batch = B; a.nq = Lq; a.heads = M; a.levels = L; a.points = P; a.S = S;
   for (int l = 0; l < L; ++l) { a.lvl_h[l] = spatial_shapes_host[2 * l]; a.lvl_w[l] = spatial_shapes_host[2 * l + 1]; a.lvl_start[l] = level_start_host[l]; }
-  if (lwb::msda_plan(&a)) return fail("lwdetr_msda_forward: a feature level is wider than 840 tokens, larger than 8192 tokens, or there are too many bands");
+  if (lwb::msda_plan(&a)) return fail("lwdetr_msda_forward: invalid level table (a level is empty or extends past S)");
   int e = lwb::msda_launch(dtype, a, static_cast<cudaStream_t>(stream));
   if (e == -2) return fail("lwdetr_msda_forward: unsupported (levels, points) combination");
   if (e) return cuda_fail(e, "lwdetr_msda_forward launch");
@@ -148,7 +148,7 @@ int lwdetr_msda_forward(int dtype, const void* value_hm, int64_t v_image_stride,
 int lwdetr_topk(const float* score, int B, int S, int k, int32_t* idx, void* stream) {
   if (!score || !idx) return fail("lwdetr_topk: null pointer");
   int e = lwb::topk_launch(score, B, S, k, idx, static_cast<cudaStream_t>(stream));
-  if (e == -2) return fail("lwdetr_topk: need k <= S <= 16384");
+  if (e == -2) return fail("lwdetr_topk: need k <= S, and k <= 4096 when S > 16384");
   if (e) return cuda_fail(e, "lwdetr_topk launch");
   return 0;
 }
@@ -167,6 +167,12 @@ int lwdetr_postprocess(const float* pred_logits, const float* pred_boxes, const 
 int lwdetr_host_bicubic(const float* src, int n_in, int C, int n_out, float* dst) {
   if (!src || !dst || n_in < 1 || n_out < 1 || C < 1) return fail("lwdetr_host_bicubic: bad arguments");
   lwb::bicubic_resize_chlast(src, n_in, C, n_out, dst);
+  return 0;
+}
+
+int lwdetr_host_bicubic_hw(const float* src, int n_in, int C, int out_h, int out_w, float* dst) {
+  if (!src || !dst || n_in < 1 || out_h < 1 || out_w < 1 || C < 1) return fail("lwdetr_host_bicubic_hw: bad arguments");
+  lwb::bicubic_resize_chlast_hw(src, n_in, C, out_h, out_w, dst);
   return 0;
 }
 
@@ -214,25 +220,38 @@ int lwdetr_forward(lwdetr_handle* h, const void* images, int images_fp32, int B,
   std::string err;
   lwb::ForwardIn in;
   in.images = images; in.kind = images_fp32 ? lwb::IN_F32_NCHW : lwb::IN_16_NCHW;
-  if (h->eng->forward(in, B, pred_logits, pred_boxes, aux, topk_override, static_cast<cudaStream_t>(stream), &err))
+  const int S = h->eng->config().img_size;
+  if (h->eng->forward(in, B, S, S, pred_logits, pred_boxes, aux, topk_override, static_cast<cudaStream_t>(stream), &err))
     return fail(err);
+  return 0;
+}
+
+static int forward_input(const char* fn, lwdetr_handle* h, const lwdetr_input* input, int B, int height, int width, float* pred_logits,
+                         float* pred_boxes, const lwdetr_aux_out* aux, const int32_t* topk_override, void* stream) {
+  if (!h || !input || !input->images) return fail(std::string(fn) + ": null pointer");
+  if (input->format != LWDETR_IN_F32_NCHW && input->format != LWDETR_IN_16_NCHW && input->format != LWDETR_IN_U8_NHWC)
+    return fail(std::string(fn) + ": format must be LWDETR_IN_F32_NCHW, LWDETR_IN_16_NCHW or LWDETR_IN_U8_NHWC");
+  lwb::ForwardIn in;
+  in.images = input->images; in.kind = input->format; in.mask = input->padding_mask;
+  for (int c = 0; c < 3; ++c) {
+    in.mean[c] = input->mean[c]; in.stdv[c] = input->std[c];
+    if (input->format == LWDETR_IN_U8_NHWC && !(input->std[c] > 0.f)) return fail(std::string(fn) + ": std must be positive");
+  }
+  std::string err;
+  if (h->eng->forward(in, B, height, width, pred_logits, pred_boxes, aux, topk_override, static_cast<cudaStream_t>(stream), &err)) return fail(err);
   return 0;
 }
 
 int lwdetr_forward_ex(lwdetr_handle* h, const lwdetr_input* input, int B, float* pred_logits, float* pred_boxes,
                       const lwdetr_aux_out* aux, const int32_t* topk_override, void* stream) {
-  if (!h || !input || !input->images) return fail("lwdetr_forward_ex: null pointer");
-  if (input->format != LWDETR_IN_F32_NCHW && input->format != LWDETR_IN_16_NCHW && input->format != LWDETR_IN_U8_NHWC)
-    return fail("lwdetr_forward_ex: format must be LWDETR_IN_F32_NCHW, LWDETR_IN_16_NCHW or LWDETR_IN_U8_NHWC");
-  lwb::ForwardIn in;
-  in.images = input->images; in.kind = input->format; in.mask = input->padding_mask;
-  for (int c = 0; c < 3; ++c) {
-    in.mean[c] = input->mean[c]; in.stdv[c] = input->std[c];
-    if (input->format == LWDETR_IN_U8_NHWC && !(input->std[c] > 0.f)) return fail("lwdetr_forward_ex: std must be positive");
-  }
-  std::string err;
-  if (h->eng->forward(in, B, pred_logits, pred_boxes, aux, topk_override, static_cast<cudaStream_t>(stream), &err)) return fail(err);
-  return 0;
+  if (!h) return fail("lwdetr_forward_ex: null pointer");
+  const int S = h->eng->config().img_size;
+  return forward_input("lwdetr_forward_ex", h, input, B, S, S, pred_logits, pred_boxes, aux, topk_override, stream);
+}
+
+int lwdetr_forward_hw(lwdetr_handle* h, const lwdetr_input* input, int B, int height, int width, float* pred_logits, float* pred_boxes,
+                      const lwdetr_aux_out* aux, const int32_t* topk_override, void* stream) {
+  return forward_input("lwdetr_forward_hw", h, input, B, height, width, pred_logits, pred_boxes, aux, topk_override, stream);
 }
 
 // One ncclBroadcast of the packed weight arena (SURVEY.md 8b / 8e).  NCCL is not linked: the symbol is taken from the

@@ -43,27 +43,49 @@ static void cubic_coeffs(float t, float w[4]) {
   w[2] = c1(1.f - t);
   w[3] = c2(2.f - t);
 }
-void bicubic_resize_chlast(const float* src, int n_in, int C, int n_out, float* dst) {
+// source taps and weights of one output axis (F.interpolate's scale = n_in / n_out, border clamped)
+static void cubic_axis(int n_in, int n_out, std::vector<int>* idx, std::vector<float>* wts) {
   const float scale = static_cast<float>(n_in) / static_cast<float>(n_out);
-  std::vector<int> idx(static_cast<size_t>(n_out) * 4);
-  std::vector<float> wts(static_cast<size_t>(n_out) * 4);
+  idx->assign(static_cast<size_t>(n_out) * 4, 0);
+  wts->assign(static_cast<size_t>(n_out) * 4, 0.f);
   for (int o = 0; o < n_out; ++o) {
     const float s = (o + 0.5f) * scale - 0.5f;
     const float f = std::floor(s);
-    cubic_coeffs(s - f, &wts[o * 4]);
-    for (int k = 0; k < 4; ++k) idx[o * 4 + k] = std::min(std::max(static_cast<int>(f) - 1 + k, 0), n_in - 1);
+    cubic_coeffs(s - f, &(*wts)[o * 4]);
+    for (int k = 0; k < 4; ++k) (*idx)[o * 4 + k] = std::min(std::max(static_cast<int>(f) - 1 + k, 0), n_in - 1);
   }
-  for (int oy = 0; oy < n_out; ++oy)
-    for (int ox = 0; ox < n_out; ++ox) {
-      float* d = dst + (static_cast<size_t>(oy) * n_out + ox) * C;
+}
+void bicubic_resize_chlast_hw(const float* src, int n_in, int C, int out_h, int out_w, float* dst) {
+  std::vector<int> iy, ix;
+  std::vector<float> wy, wx;
+  cubic_axis(n_in, out_h, &iy, &wy);
+  cubic_axis(n_in, out_w, &ix, &wx);
+  for (int oy = 0; oy < out_h; ++oy)
+    for (int ox = 0; ox < out_w; ++ox) {
+      float* d = dst + (static_cast<size_t>(oy) * out_w + ox) * C;
       for (int c = 0; c < C; ++c) d[c] = 0.f;
       for (int ky = 0; ky < 4; ++ky)
         for (int kx = 0; kx < 4; ++kx) {
-          const float w = wts[oy * 4 + ky] * wts[ox * 4 + kx];
-          const float* s = src + (static_cast<size_t>(idx[oy * 4 + ky]) * n_in + idx[ox * 4 + kx]) * C;
+          const float w = wy[oy * 4 + ky] * wx[ox * 4 + kx];
+          const float* s = src + (static_cast<size_t>(iy[oy * 4 + ky]) * n_in + ix[ox * 4 + kx]) * C;
           for (int c = 0; c < C; ++c) d[c] += w * s[c];
         }
     }
+}
+void bicubic_resize_chlast(const float* src, int n_in, int C, int n_out, float* dst) { bicubic_resize_chlast_hw(src, n_in, C, n_out, n_out, dst); }
+
+// The ViT's position table at a GH x GW token grid: the 14x14 pretraining grid of pos_embed [197, C] (cls slot first)
+// resized bicubically (vit.py:26-54) and laid out in window-major token order (vit.py:353-358), fp32.
+static std::vector<float> window_major_pos(const float* pos_embed, int C, int GH, int GW) {
+  const int T = GH * GW, wh = GH / 4, ww = GW / 4, wsz = wh * ww;
+  std::vector<float> grid(static_cast<size_t>(T) * C), wm(static_cast<size_t>(T) * C);
+  bicubic_resize_chlast_hw(pos_embed + C, 14, C, GH, GW, grid.data());   // drop the cls slot (vit.py:39-40)
+  for (int r = 0; r < T; ++r) {   // window-major row r -> spatial (y, x)
+    const int win = r / wsz, t = r % wsz;
+    const int y = (win >> 2) * wh + t / ww, x = (win & 3) * ww + t % ww;
+    std::memcpy(&wm[static_cast<size_t>(r) * C], &grid[(static_cast<size_t>(y) * GW + x) * C], C * sizeof(float));
+  }
+  return wm;
 }
 
 // ------------------------------------------------------------------------------- Engine basics
@@ -110,9 +132,7 @@ void* Engine::salloc(size_t bytes) {
   return p;
 }
 
-void* Engine::upload16(const std::vector<float>& v) {
-  void* d = walloc(v.size() * 2);
-  if (!d) return nullptr;
+std::vector<uint16_t> Engine::to16(const std::vector<float>& v) const {
   std::vector<uint16_t> h(v.size());
   if (dtype_ == DT_BF16) {
     for (size_t i = 0; i < v.size(); ++i) {
@@ -125,6 +145,12 @@ void* Engine::upload16(const std::vector<float>& v) {
       std::memcpy(&h[i], &b, 2);
     }
   }
+  return h;
+}
+void* Engine::upload16(const std::vector<float>& v) {
+  void* d = walloc(v.size() * 2);
+  if (!d) return nullptr;
+  const std::vector<uint16_t> h = to16(v);
   cudaMemcpy(d, h.data(), h.size() * 2, cudaMemcpyHostToDevice);
   return d;
 }
@@ -139,7 +165,7 @@ int Engine::set_option(const char* name, int value) {
   if (std::strcmp(name, "fuse_layernorm") == 0) {
     fuse_ln_ = value;
     drop_graphs();
-    planned_B_ = 0;
+    planned_B_ = planned_H_ = planned_W_ = 0;
     return 0;
   }
   if (std::strcmp(name, "cuda_graph") == 0) {
@@ -160,10 +186,10 @@ int Engine::load_weights(const std::map<std::string, HostTensor>& w, std::string
   DeviceGuard guard(device_);
   // Whatever happens below, the old packing is gone: a failed load must not leave a schedule pointing into a freed arena.
   weights_loaded_ = false;
-  planned_B_ = 0;
+  planned_B_ = planned_H_ = planned_W_ = 0;
   ops_.clear();
   const int C = cfg_.vit_dim, d = cfg_.hidden_dim, nq = cfg_.num_queries, ncls = cfg_.num_classes;
-  const int G = cfg_.img_size / 16, T = G * G, ntap = cfg_.n_taps, c2 = d / 2;
+  const int G = cfg_.img_size / 16, ntap = cfg_.n_taps, c2 = d / 2;
   const int M = cfg_.ca_heads, L = cfg_.n_levels, P = cfg_.dec_points, ff = cfg_.dim_feedforward;
   bool missing = false;
   auto get = [&](const std::string& name, long long numel) -> const float* {
@@ -242,18 +268,8 @@ int Engine::load_weights(const std::map<std::string, HostTensor>& w, std::string
   const std::string E = "backbone.0.encoder.";
   put16("patch.w", vec(E + "patch_embed.proj.weight", 1LL * C * 768));
   put32("patch.b", vec(E + "patch_embed.proj.bias", C));
-  {
-    auto pe = vec(E + "pos_embed", 197LL * C);
-    std::vector<float> grid(static_cast<size_t>(T) * C), wm(static_cast<size_t>(T) * C);
-    bicubic_resize_chlast(pe.data() + C, 14, C, G, grid.data());   // drop the cls slot (vit.py:39-40)
-    const int wh = G / 4, wsz = wh * wh;
-    for (int r = 0; r < T; ++r) {   // window-major row r -> spatial (y, x)   (vit.py:353-358)
-      const int win = r / wsz, t = r % wsz;
-      const int y = (win >> 2) * wh + t / wh, x = (win & 3) * wh + t % wh;
-      std::memcpy(&wm[static_cast<size_t>(r) * C], &grid[(static_cast<size_t>(y) * G + x) * C], C * sizeof(float));
-    }
-    put16("pos", wm);
-  }
+  const std::vector<float> pos_embed = vec(E + "pos_embed", 197LL * C);
+  put16("pos", window_major_pos(pos_embed.data(), C, G, G));   // the table at the configured resolution
   for (int i = 0; i < cfg_.vit_depth; ++i) {
     const std::string b = E + "blocks." + std::to_string(i) + ".", k = "blk" + std::to_string(i) + ".";
     put_norm(k + "ln1", b + "norm1", C);
@@ -381,39 +397,66 @@ int Engine::load_weights(const std::map<std::string, HostTensor>& w, std::string
   put_norm("dec_norm", TR + "decoder.norm", d);
   put_linear("cls", "class_embed", ncls, d);
   for (int i = 0; i < 3; ++i) put_linear("box" + std::to_string(i), "bbox_embed.layers." + std::to_string(i), i == 2 ? 4 : d, d);
+  // the raw pos_embed (fp32, after every other entry): plan() derives the table of any other input size from the ARENA copy,
+  // which lwdetr_broadcast_weights fills on every rank
+  put32("pos_raw", pos_embed);
   if (missing) return -1;
   if (oom) { *err = "weight arena exhausted"; return -1; }
   if (cudaDeviceSynchronize() != cudaSuccess) { *err = "CUDA error while uploading weights"; return -1; }
   weights_loaded_ = true;
-  planned_B_ = 0;   // pointers changed: re-plan
+  planned_B_ = planned_H_ = planned_W_ = 0;   // pointers changed: re-plan
   return 0;
 }
 
 // ------------------------------------------------------------------------------- schedule
-int Engine::plan(int B, std::string* err) {
+int Engine::plan(int B, int IH, int IW, std::string* err) {
   const int C = cfg_.vit_dim, d = cfg_.hidden_dim, nq = cfg_.num_queries, ncls = cfg_.num_classes;
-  const int G = cfg_.img_size / 16, T = G * G, ntap = cfg_.n_taps, c2 = d / 2, heads = cfg_.vit_heads;
+  const int GH = IH / 16, GW = IW / 16, T = GH * GW, ntap = cfg_.n_taps, c2 = d / 2, heads = cfg_.vit_heads;
   const int M = cfg_.ca_heads, L = cfg_.n_levels, P = cfg_.dec_points, ff = cfg_.dim_feedforward, NL = cfg_.dec_layers;
   const long long BT = 1LL * B * T;
-  int lvl_hw[2] = {0, 0}, lvl_start[2] = {0, 0}, S = 0;
-  for (int l = 0; l < L; ++l) {
+  int lvl_h[2] = {0, 0}, lvl_w[2] = {0, 0}, lvl_start[2] = {0, 0}, S = 0;
+  for (int l = 0; l < L; ++l) {   // P3 = 2x the token grid, P4 = the grid, P5 = half of it (projector.py:165-193)
     const int sc = cfg_.level_scale_log2[l];
-    lvl_hw[l] = sc == 1 ? 2 * G : (sc == -1 ? G / 2 : G);
+    lvl_h[l] = sc == 1 ? 2 * GH : (sc == -1 ? GH / 2 : GH);
+    lvl_w[l] = sc == 1 ? 2 * GW : (sc == -1 ? GW / 2 : GW);
     lvl_start[l] = S;
-    S += lvl_hw[l] * lvl_hw[l];
+    S += lvl_h[l] * lvl_w[l];
   }
   const long long BS = 1LL * B * S, BQ = 1LL * B * nq;
   const int ldc = static_cast<int>(align_up(static_cast<size_t>(ncls), 32));   // row pitch of the fp32 class-logit buffers
   ldc_ = ldc;
   if (d / M != 16) { *err = "deformable attention head dim must be 16"; return -1; }
   if (C / heads != 16 && C / heads != 32 && C / heads != 64) { *err = "unsupported ViT head dim"; return -1; }
+  if (S < nq) {
+    *err = "lwdetr_forward: a " + std::to_string(IH) + "x" + std::to_string(IW) + " input has " + std::to_string(S) +
+           " memory tokens, fewer than num_queries = " + std::to_string(nq);
+    return -1;
+  }
+  // position table of this token grid: the packed table at the configured size, else resized from the arena's raw pos_embed
+  const bool own_pos = !(GH == cfg_.img_size / 16 && GW == cfg_.img_size / 16);
+  std::vector<uint16_t> pos_host;
+  if (own_pos) {
+    std::vector<float> pe(static_cast<size_t>(197) * C);
+    const float* raw = F_.count("pos_raw") ? F_["pos_raw"] : nullptr;
+    // the arena may just have been filled by a stream-ordered broadcast: the whole device is synchronised first
+    if (!raw || cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(pe.data(), raw, pe.size() * 4, cudaMemcpyDeviceToHost) != cudaSuccess) {
+      *err = "lwdetr_forward: reading pos_embed from the weight arena failed";
+      return -1;
+    }
+    pos_host = to16(window_major_pos(pe.data(), C, GH, GW));
+  }
 
   for (int pass = 0; pass < 2; ++pass) {   // pass 0 sizes the workspace, pass 1 builds the ops
     soff_ = 0;
     ops_.clear();
     bool fail = false;
-    auto buf16 = [&](long long rows, int cols) { return Mat{salloc(static_cast<size_t>(rows) * cols * 2), cols}; };
-    auto buf32 = [&](long long n) { return static_cast<float*>(salloc(static_cast<size_t>(n) * 4)); };
+    // every kernel indexes a buffer's elements / a GEMM's rows with 32-bit integers somewhere: no buffer may exceed that range
+    auto fits = [&](long long n) {
+      if (n > 2147483647LL && !fail) { fail = true; *err = "lwdetr_forward: batch " + std::to_string(B) + " at " + std::to_string(IH) + "x" + std::to_string(IW) + " needs a workspace buffer of more than 2^31-1 elements"; }
+      return n <= 2147483647LL;
+    };
+    auto buf16 = [&](long long rows, int cols) { fits(rows * cols); return Mat{salloc(static_cast<size_t>(rows) * cols * 2), cols}; };
+    auto buf32 = [&](long long n) { fits(n); return static_cast<float*>(salloc(static_cast<size_t>(n) * 4)); };
     auto col = [&](Mat m, int c) { return Mat{cptr(m.p) + static_cast<size_t>(c) * 2, m.ld}; };
     auto w16 = [&](const std::string& k) -> void* { auto it = W_.find(k); if (it == W_.end()) { fail = true; *err = "internal: weight " + k; return nullptr; } return it->second; };
     auto w32 = [&](const std::string& k) -> float* { auto it = F_.find(k); if (it == F_.end()) { fail = true; *err = "internal: vector " + k; return nullptr; } return it->second; };
@@ -428,7 +471,7 @@ int Engine::plan(int B, std::string* err) {
     int stats_parts = 0;   // partial (sum, sumsq) pairs per row written by the N = C producer GEMMs
     auto add_gemm = [&](const std::string& label, Mat A, long long Mrows, int K, const std::string& wkey, int N, void* out, int ld_out,
                         const GemmOpt& o, long long out_rows = -1) {
-      if (pass == 0) return;
+      if (!fits(Mrows) || pass == 0) return;
       GemmDesc g;
       g.dtype = dtype_; g.A = A.p; g.lda = A.ld; g.M = static_cast<int>(Mrows); g.N = N; g.K = K;
       g.W = w16(wkey + ".w"); g.bias = F_.count(wkey + ".b") ? F_[wkey + ".b"] : nullptr;
@@ -503,11 +546,10 @@ int Engine::plan(int B, std::string* err) {
     uint8_t* invalid_b = static_cast<uint8_t*>(salloc(static_cast<size_t>(BS)));
     uint8_t* pad_b = static_cast<uint8_t*>(salloc(static_cast<size_t>(BS)));
     {
-      const int img = cfg_.img_size;
-      const int lh0 = lvl_hw[0], lh1 = lvl_hw[1], ls0 = lvl_start[0], ls1 = lvl_start[1];
-      add_op("mask_setup", [this, B, img, L, S, lh0, lh1, ls0, ls1, prop_b, invalid_b, pad_b, vr_b](cudaStream_t st) {
-        const int lh[2] = {lh0, lh1}, ls[2] = {ls0, ls1};
-        return mask_setup_launch(in_.mask, B, img, img, L, S, lh, lh, ls, prop_b, invalid_b, pad_b, vr_b, st);
+      const int lh0 = lvl_h[0], lh1 = lvl_h[1], lw0 = lvl_w[0], lw1 = lvl_w[1], ls0 = lvl_start[0], ls1 = lvl_start[1];
+      add_op("mask_setup", [this, B, IH, IW, L, S, lh0, lh1, lw0, lw1, ls0, ls1, prop_b, invalid_b, pad_b, vr_b](cudaStream_t st) {
+        const int lh[2] = {lh0, lh1}, lw[2] = {lw0, lw1}, ls[2] = {ls0, ls1};
+        return mask_setup_launch(in_.mask, B, IH, IW, L, S, lh, lw, ls, prop_b, invalid_b, pad_b, vr_b, st);
       }, prop_b, BS, 4, 4, 1, 24.0 * BS);
       if (pass) ops_.back().reads_input = true;
     }
@@ -518,20 +560,24 @@ int Engine::plan(int B, std::string* err) {
     Mat qkv = buf16(BT, 3 * C), att = buf16(BT, C), hid = buf16(BT, 4 * C);
     {
       void* a0p = a0.p;
-      const int img = cfg_.img_size;
-      add_op("patch_gather", [this, a0p, B, img, dt](cudaStream_t st) {
-               if (in_.kind == IN_U8_NHWC) return patch_gather_u8_launch(dt, in_.images, in_.mean, in_.stdv, a0p, B, img, st);
-               return patch_gather_launch(dt, in_.images, in_.kind == IN_F32_NCHW ? 1 : 0, a0p, B, img, st);
+      add_op("patch_gather", [this, a0p, B, IH, IW, dt](cudaStream_t st) {
+               if (in_.kind == IN_U8_NHWC) return patch_gather_u8_launch(dt, in_.images, in_.mean, in_.stdv, a0p, B, IH, IW, st);
+               return patch_gather_launch(dt, in_.images, in_.kind == IN_F32_NCHW ? 1 : 0, a0p, B, IH, IW, st);
              },
-             a0.p, BT, 768, 768, 0, 1.0 * B * 3 * img * img * 4 + 2.0 * BT * 768);
+             a0.p, BT, 768, 768, 0, 1.0 * B * 3 * IH * IW * 4 + 2.0 * BT * 768);
       if (pass) ops_.back().reads_input = true;
     }
     float2* stats_x = static_cast<float2*>(salloc(static_cast<size_t>(BT) * 48 * sizeof(float2)));   // row stats of x (block input)
     float2* stats_m = static_cast<float2*>(salloc(static_cast<size_t>(BT) * 48 * sizeof(float2)));   // row stats of x + attn
     const bool fuse = fuse_ln_ != 0;
     Mat xcur = xa;
+    void* pos_tab = own_pos ? salloc(pos_host.size() * 2) : nullptr;
+    if (own_pos && pass == 1 && cudaMemcpy(pos_tab, pos_host.data(), pos_host.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) {
+      *err = "lwdetr_forward: position table upload failed";
+      return -1;
+    }
     {
-      GemmOpt o; o.resid = Mat{pass ? w16("pos") : nullptr, C}; o.resid_mod = T;
+      GemmOpt o; o.resid = Mat{pass ? (own_pos ? pos_tab : w16("pos")) : nullptr, C}; o.resid_mod = T;
       if (fuse) o.stats_out = stats_x;
       add_gemm("patch_embed", a0, BT, 768, "patch", C, xcur.p, xcur.ld, o);
     }
@@ -570,12 +616,12 @@ int Engine::plan(int B, std::string* err) {
     // ================================================================ projector -> decoder memory [B, S, d]
     Mat memory = buf16(BS, d);
     for (int l = 0; l < L; ++l) {
-      const int sc = cfg_.level_scale_log2[l], H = lvl_hw[l];
-      const long long rows = 1LL * B * H * H;
+      const int sc = cfg_.level_scale_log2[l], H = lvl_h[l], W = lvl_w[l];
+      const long long rows = 1LL * B * H * W;
       const std::string k = "lvl" + std::to_string(l) + ".", lb = "level" + std::to_string(l);
       Mat c2f = buf16(rows, 5 * c2), tmp = buf16(rows, c2), pout = buf16(rows, d);
       if (sc == 0) {
-        GemmOpt o; o.act = ACT_SILU; o.rows_in = ROWS_WINDOW_MAJOR; o.remap = 1; o.IH = G; o.IW = G;
+        GemmOpt o; o.act = ACT_SILU; o.rows_in = ROWS_WINDOW_MAJOR; o.remap = 1; o.IH = GH; o.IW = GW;
         add_gemm(lb + ".cv1", tapbuf, BT, ntap * C, k + "cv1", 2 * c2, c2f.p, c2f.ld, o);
       } else if (sc == 1) {
         const int cs = C > 512 ? C / 4 : C / 2;
@@ -590,7 +636,7 @@ int Engine::plan(int B, std::string* err) {
             add_gemm(lb + ".pre" + std::to_string(t), src, BT, C, ks + ".pre", C / 2, pre.p, pre.ld, o);
             src = pre; kin = C / 2;
           }
-          GemmOpt o; o.rows_in = ROWS_WINDOW_MAJOR; o.shuffle = cs; o.IH = G; o.IW = G;
+          GemmOpt o; o.rows_in = ROWS_WINDOW_MAJOR; o.shuffle = cs; o.IH = GH; o.IW = GW;
           Mat dst = col(samp, t * cs);
           add_gemm(lb + ".up" + std::to_string(t), src, BT, kin, ks + ".up", 4 * cs, dst.p, dst.ld, o);
         }
@@ -600,11 +646,11 @@ int Engine::plan(int B, std::string* err) {
         Mat spat = buf16(BT, ntap * C), samp = buf16(rows, ntap * C);
         {
           void* sp = tapbuf.p; void* dp = spat.p; const int ldx = ntap * C;
-          add_op(lb + ".unwindow", [sp, dp, ldx, BT, G, dt](cudaStream_t st) { return unwindow_launch(dt, sp, ldx, dp, ldx, BT, ldx, G, st); },
+          add_op(lb + ".unwindow", [sp, dp, ldx, BT, GH, GW, dt](cudaStream_t st) { return unwindow_launch(dt, sp, ldx, dp, ldx, BT, ldx, GH, GW, st); },
                  spat.p, BT, ldx, ldx, 0, 4.0 * BT * ldx);
         }
         for (int t = 0; t < ntap; ++t) {
-          GemmOpt o; o.act = ACT_RELU; o.conv = 2; o.cB = B; o.cOH = H; o.cOW = H;
+          GemmOpt o; o.act = ACT_RELU; o.conv = 2; o.cB = B; o.cOH = H; o.cOW = W;
           Mat src = col(spat, t * C), dst = col(samp, t * C);
           add_gemm(lb + ".down" + std::to_string(t), src, rows, 9 * C, k + "samp" + std::to_string(t) + ".down", C, dst.p, dst.ld, o);
         }
@@ -612,13 +658,13 @@ int Engine::plan(int B, std::string* err) {
         add_gemm(lb + ".cv1", samp, rows, ntap * C, k + "cv1", 2 * c2, c2f.p, c2f.ld, o);
       }
       for (int j = 0; j < 3; ++j) {
-        GemmOpt o; o.act = ACT_SILU; o.conv = 1; o.cB = B; o.cOH = H; o.cOW = H;
+        GemmOpt o; o.act = ACT_SILU; o.conv = 1; o.cB = B; o.cOH = H; o.cOW = W;
         Mat src = col(c2f, (1 + j) * c2), dst = col(c2f, (2 + j) * c2);
         add_gemm(lb + ".m" + std::to_string(j) + "a", src, rows, 9 * c2, k + "m" + std::to_string(j) + "a", c2, tmp.p, tmp.ld, o);
         add_gemm(lb + ".m" + std::to_string(j) + "b", tmp, rows, 9 * c2, k + "m" + std::to_string(j) + "b", c2, dst.p, dst.ld, o);
       }
       { GemmOpt o; o.act = ACT_SILU; add_gemm(lb + ".cv2", c2f, rows, 5 * c2, k + "cv2", d, pout.p, pout.ld, o); }
-      add_ln(lb, pout, memory, k + "ln", 1e-6f, rows, d, nullptr, 0, nullptr, Mat{nullptr, 0}, Mat{nullptr, 0}, 1LL * H * H, S, lvl_start[l], BS);
+      add_ln(lb, pout, memory, k + "ln", 1e-6f, rows, d, nullptr, 0, nullptr, Mat{nullptr, 0}, Mat{nullptr, 0}, 1LL * H * W, S, lvl_start[l], BS);
     }
 
     // ================================================================ two-stage query selection
@@ -675,8 +721,8 @@ int Engine::plan(int B, std::string* err) {
     std::memset(&mbase, 0, sizeof mbase);
     mbase.v_b_stride = 1LL * NL * M * S * MSDA_D; mbase.valid_ratio = vr_b; mbase.offs_logits = oa.p; mbase.ld_ol = oa.ld; mbase.ref = refpoint; mbase.out = ms.p; mbase.ld_out = ms.ld;
     mbase.batch = B; mbase.nq = nq; mbase.heads = M; mbase.levels = L; mbase.points = P; mbase.S = S;
-    for (int l = 0; l < L; ++l) { mbase.lvl_h[l] = lvl_hw[l]; mbase.lvl_w[l] = lvl_hw[l]; mbase.lvl_start[l] = lvl_start[l]; }
-    if (msda_plan(&mbase)) { *err = "deformable attention: a feature level is too wide to stage"; return -1; }
+    for (int l = 0; l < L; ++l) { mbase.lvl_h[l] = lvl_h[l]; mbase.lvl_w[l] = lvl_w[l]; mbase.lvl_start[l] = lvl_start[l]; }
+    if (msda_plan(&mbase)) { *err = "deformable attention: invalid level table"; return -1; }   // nbands = 0: direct-gather kernel
     Mat cur = tgt;
     for (int i = 0; i < NL; ++i) {
       const std::string k = "dec" + std::to_string(i) + ".", lb = "dec" + std::to_string(i);
@@ -715,6 +761,7 @@ int Engine::plan(int B, std::string* err) {
     out_logits_ = logits; out_boxes_ = boxes; out_enc_logits_ = enc_logits; out_enc_boxes_ = enc_boxes; topk_idx_ = topk_idx;
 
     if (pass == 0) {
+      if (fail) return -1;
       const size_t need = soff_ + 4096;
       if (need > sarena_.bytes) {
         if (sarena_.p) cudaFree(sarena_.p);
@@ -729,6 +776,8 @@ int Engine::plan(int B, std::string* err) {
   drop_graphs();
   eager_runs_ = 0;
   planned_B_ = B;
+  planned_H_ = IH;
+  planned_W_ = IW;
   return 0;
 }
 
@@ -749,12 +798,21 @@ int Engine::do_capture(const Op& op, cudaStream_t st) {
   return 0;
 }
 
-int Engine::forward(const ForwardIn& in, int B, float* pred_logits, float* pred_boxes, const lwdetr_aux_out* aux,
+int Engine::forward(const ForwardIn& in, int B, int H, int W, float* pred_logits, float* pred_boxes, const lwdetr_aux_out* aux,
                     const int32_t* topk_override, cudaStream_t st, std::string* err) {
   DeviceGuard guard(device_);
   if (!weights_loaded_) { *err = "lwdetr_forward: weights not loaded"; return -1; }
   if (B <= 0) { *err = "lwdetr_forward: batch must be positive"; return -1; }
-  if (B != planned_B_ && plan(B, err)) return -1;
+  if (H % 64 || W % 64 || H < kMinSide || W < kMinSide || H > kMaxSide || W > kMaxSide) {
+    *err = "lwdetr_forward: input " + std::to_string(H) + "x" + std::to_string(W) + " is not supported: height and width must be multiples of 64 in [" +
+           std::to_string(kMinSide) + ", " + std::to_string(kMaxSide) + "] (4x4 windows of 16-pixel patches)";
+    return -1;
+  }
+  if ((B != planned_B_ || H != planned_H_ || W != planned_W_) && plan(B, H, W, err)) {
+    planned_B_ = planned_H_ = planned_W_ = 0;   // a failed plan leaves no schedule behind
+    ops_.clear();
+    return -1;
+  }
   if (!in.images) { *err = "lwdetr_forward: null images"; return -1; }
   in_ = in; in_topk_override_ = topk_override;
   // The first forward of a plan always runs eagerly (it also performs the one-time cudaFuncSetAttribute calls).

@@ -1,5 +1,5 @@
 // LW-DETR forward engine: weight packing (folding, layout changes, 16-bit conversion) and the fixed
-// kernel schedule for one batch size.  Host-only interface; see engine.cpp.
+// kernel schedule for one (batch size, input height, input width).  Host-only interface; see engine.cpp.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -39,18 +39,21 @@ struct Op {
 // One forward's input: the image batch in one of three encodings plus the optional NestedTensor padding mask.
 enum : int { IN_F32_NCHW = 0, IN_16_NCHW = 1, IN_U8_NHWC = 2 };
 struct ForwardIn {
-  const void* images = nullptr;   // DEVICE [B,3,S,S] fp32 / compute dtype, or [B,S,S,3] uint8
+  const void* images = nullptr;   // DEVICE [B,3,H,W] fp32 / compute dtype, or [B,H,W,3] uint8
   int kind = IN_F32_NCHW;
-  const uint8_t* mask = nullptr;  // DEVICE bool [B,S,S] (True = padded pixel) or null
+  const uint8_t* mask = nullptr;  // DEVICE bool [B,H,W] (True = padded pixel) or null
   float mean[3] = {0.f, 0.f, 0.f}, stdv[3] = {1.f, 1.f, 1.f};   // IN_U8_NHWC: (x/255 - mean) / std
 };
 
 class Engine {
  public:
+  // supported input sides (pixels, multiples of 64: 4x4 windows of 16-pixel patches)
+  static constexpr int kMinSide = 128, kMaxSide = 1344;
   Engine(const lwdetr_config& cfg, int dtype);
   ~Engine();
   int load_weights(const std::map<std::string, HostTensor>& w, std::string* err);
-  int forward(const ForwardIn& in, int B, float* pred_logits, float* pred_boxes,
+  // input [B, 3, H, W] (or [B, H, W, 3] uint8); a (B, H, W) other than the last one re-plans and drops the graphs
+  int forward(const ForwardIn& in, int B, int H, int W, float* pred_logits, float* pred_boxes,
               const lwdetr_aux_out* aux, const int32_t* topk_override, cudaStream_t st, std::string* err);
   void add_capture(const char* label, float* dst, long long cap) { captures_.push_back({label, dst, cap, -1}); }
   void clear_captures() { captures_.clear(); }
@@ -69,9 +72,10 @@ class Engine {
 
  private:
   struct DevBuf { void* p = nullptr; size_t bytes = 0; };
-  int plan(int B, std::string* err);
+  int plan(int B, int H, int W, std::string* err);
   void* walloc(size_t bytes);      // weight arena (bump)
   void* salloc(size_t bytes);      // workspace arena (bump)
+  std::vector<uint16_t> to16(const std::vector<float>& v) const;   // round to the compute dtype
   void* upload16(const std::vector<float>& v);
   float* upload32(const std::vector<float>& v);
   int do_capture(const Op& op, cudaStream_t st);
@@ -79,13 +83,13 @@ class Engine {
   lwdetr_config cfg_;
   int dtype_;
   int device_ = 0;    // CUDA device the engine was created on; every entry point switches to it (one handle per device)
-  int planned_B_ = 0;
+  int planned_B_ = 0, planned_H_ = 0, planned_W_ = 0;   // shape of the current schedule (0: none)
   bool weights_loaded_ = false;
   int use_graph_ = 0;
   int fuse_ln_ = 1;   // ViT LayerNorms folded into the consuming GEMM's epilogue (option "fuse_layernorm")
   // CUDA graphs: the two ops that read caller-owned memory (mask tables, patch gather) are launched eagerly on the
   // caller's stream; everything behind them only touches engine-owned buffers and is ONE executable graph per planned
-  // batch size - whatever tensor, input encoding or mask the caller passes.  (The test-only top-k override pointer is
+  // (batch size, height, width) - whatever tensor, input encoding or mask the caller passes.  (The test-only top-k override pointer is
   // the one caller pointer left inside, hence the key.)  Captured on an internal stream: the caller's stream may be the
   // legacy default stream, which cannot be captured.
   struct GraphKey { const void* topk; bool operator<(const GraphKey& o) const { return topk < o.topk; } };
@@ -117,5 +121,6 @@ class Engine {
 
 // host helpers exposed for CPU tests
 void bicubic_resize_chlast(const float* src, int n_in, int C, int n_out, float* dst);   // [n_in,n_in,C] -> [n_out,n_out,C]
+void bicubic_resize_chlast_hw(const float* src, int n_in, int C, int out_h, int out_w, float* dst);   // [n_in,n_in,C] -> [out_h,out_w,C]
 
 }  // namespace lwb

@@ -2,7 +2,7 @@
 // ms_deform_im2col_cuda.cuh:33-84 bilinear, :237-299 kernel, launcher :923-954; host glue
 // ms_deform_attn_cuda.cu:20-80; module math ops/modules/ms_deform_attn.py:118-131).
 //
-// Two kernels, both HBM-bound byte movers without tensor cores:
+// Three kernels, all HBM-bound byte movers without tensor cores:
 //
 // 1. msda_fwd_kernel - the model path.  The reference gathers 32-byte head slices from a token-major value tensor:
 //    every bilinear corner is a random DRAM sector.  Here value_proj writes the value tensor HEAD-MAJOR
@@ -17,7 +17,10 @@
 //    A P3 level (80x80 = 205 KB per head) does not fit a stage: it is cut into bands of 21 rows (one halo row), each
 //    sample is handled by the band that holds both of its rows.
 //
-// 2. msda_op_kernel - the reference operator's own interface (token-major value [B,S,M,D], explicit sampling
+// 2. msda_gather_kernel - the model path when a level set does not fit the staged kernel's tables (large inputs, see
+//    msda_plan): the same fused contract, bilinear corners gathered from global memory instead of a staged slab.
+//
+// 3. msda_op_kernel - the reference operator's own interface (token-major value [B,S,M,D], explicit sampling
 //    locations and attention weights, fp32 / fp16 / bf16, any D % 8 == 0): a direct gather, one thread = 8 (16-bit)
 //    or 4 (fp32) channels of one (query, head), 16-byte read-only loads, all L*P*4 corner loads issued before use.
 #include "msda.h"
@@ -40,6 +43,11 @@ static constexpr int MS_SMEM = MS_STAGES * MS_STAGE_BYTES + 128;
 __device__ __forceinline__ U4 lds16(uint32_t addr) {
   U4 r;
   asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(addr));
+  return r;
+}
+__device__ __forceinline__ U4 ldg_nc16(const void* p) {
+  U4 r;
+  asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
   return r;
 }
 // one 32-bit word = two 16-bit values -> packed fp32 pair (low element first), on the ALU pipe (the FMA pipe is the busy one)
@@ -283,18 +291,22 @@ __global__ void __launch_bounds__(MS_THREADS, 1) msda_fwd_kernel(const __grid_co
 
 int msda_plan(MsdaArgs* a) {
   a->nbands = 0;
+  for (int l = 0; l < a->levels; ++l)
+    if (a->lvl_h[l] < 1 || a->lvl_w[l] < 1 || a->lvl_start[l] < 0 || 1LL * a->lvl_h[l] * a->lvl_w[l] + a->lvl_start[l] > a->S) return -2;
   for (int l = 0; l < a->levels; ++l) {
     const int H = a->lvl_h[l], W = a->lvl_w[l];
-    if (H < 1 || W < 1 || 2 * W > MS_STAGE_TOKENS || H * W > 8192 || H > 0xfff0) return -2;   // token / row fields of the packed sample info
+    // a level the staged kernel cannot hold (row wider than half a stage, more tokens than the 13-bit token field of the packed
+    // sample info, or more bands than the table): the whole level set goes to the direct-gather kernel (nbands = 0)
+    if (2 * W > MS_STAGE_TOKENS || H * W > 8192 || H > 0xfff0) { a->nbands = 0; return 0; }
     const int rows_max = MS_STAGE_TOKENS / W;                    // rows a stage holds
     if (H <= rows_max) {
-      if (a->nbands >= MSDA_MAX_BANDS) return -2;
+      if (a->nbands >= MSDA_MAX_BANDS) { a->nbands = 0; return 0; }
       a->bands[a->nbands++] = MsdaBand{l, 0, -1, H - 1, a->lvl_start[l], H * W * MSDA_D * 2};
       continue;
     }
     const int own = rows_max - 1;                                // one halo row per band
     for (int r0 = 0; r0 < H; r0 += own) {
-      if (a->nbands >= MSDA_MAX_BANDS) return -2;
+      if (a->nbands >= MSDA_MAX_BANDS) { a->nbands = 0; return 0; }
       const int r1 = std::min(r0 + own, H - 1);                  // last staged row (halo included)
       const bool last = r0 + own >= H;
       a->bands[a->nbands++] = MsdaBand{l, r0, r0 == 0 ? -1 : r0, last ? H - 1 : r0 + own - 1, a->lvl_start[l] + r0 * W, (r1 - r0 + 1) * W * MSDA_D * 2};
@@ -303,8 +315,111 @@ int msda_plan(MsdaArgs* a) {
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// 3. msda_gather_kernel - the model path for level sets the staged kernel cannot hold (nbands == 0: P3 levels from 96x128
+//    on).  Same contract as msda_fwd_kernel (raw offsets and logits in; softmax, location math and valid ratios in
+//    registers; head-major value), but the bilinear corners come straight from global memory: one thread per
+//    (image, query, head), two 16-byte loads per corner (D = 16, 32 bytes per token), all four corners of a sample issued
+//    before they are combined.  It reads at most B*nq*M*L*P*4*32 bytes, far less than streaming B*M*S*32 bytes of slabs
+//    when the levels are large.
+template <typename T, int NL, int NP>
+__global__ void __launch_bounds__(256) msda_gather_kernel(const __grid_constant__ MsdaArgs p) {
+  constexpr int LP = NL * NP;
+  pdl_sync();   // programmatic dependent launch: release the successor, wait for the predecessor (launch.h)
+  const long long gid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (gid >= static_cast<long long>(p.batch) * p.nq * p.heads) return;
+  const int m = static_cast<int>(gid % p.heads);
+  const long long row = gid / p.heads;                          // b * nq + q
+  const int b = static_cast<int>(row / p.nq);
+  const T* oa = reinterpret_cast<const T*>(p.offs_logits) + row * p.ld_ol;
+  const uint32_t* o32 = reinterpret_cast<const uint32_t*>(oa + m * (2 * LP));
+  const uint32_t* l32 = reinterpret_cast<const uint32_t*>(oa + p.heads * (2 * LP) + m * LP);
+  float lg[LP];
+  float mx = -INFINITY;
+#pragma unroll
+  for (int i = 0; i < LP / 2; ++i) {
+    const float2 f = Cvt<T>::unpack(__ldg(l32 + i));
+    lg[2 * i] = f.x;
+    lg[2 * i + 1] = f.y;
+    mx = fmaxf(mx, fmaxf(f.x, f.y));
+  }
+  float sum = 0.f;
+#pragma unroll
+  for (int i = 0; i < LP; ++i) {
+    lg[i] = __expf(lg[i] - mx);
+    sum += lg[i];
+  }
+  const float inv = __fdividef(1.f, sum);
+  const float4 ref = __ldg(reinterpret_cast<const float4*>(p.ref) + row);
+  const float sx = ref.z * (0.5f / NP), sy = ref.w * (0.5f / NP);
+  const T* vhead = reinterpret_cast<const T*>(p.value) + static_cast<long long>(b) * p.v_b_stride + static_cast<long long>(m) * p.S * MSDA_D;
+  float acc[MSDA_D];
+#pragma unroll
+  for (int c = 0; c < MSDA_D; ++c) acc[c] = 0.f;
+#pragma unroll
+  for (int l = 0; l < NL; ++l) {
+    const int H = p.lvl_h[l], W = p.lvl_w[l];
+    const T* vl = vhead + static_cast<long long>(p.lvl_start[l]) * MSDA_D;
+    const float vrx = p.valid_ratio != nullptr ? __ldg(p.valid_ratio + (b * NL + l) * 2) : 1.f;
+    const float vry = p.valid_ratio != nullptr ? __ldg(p.valid_ratio + (b * NL + l) * 2 + 1) : 1.f;
+#pragma unroll
+    for (int pt = 0; pt < NP; ++pt) {
+      const int i = l * NP + pt;
+      const float2 o = Cvt<T>::unpack(__ldg(o32 + i));
+      float lx = ref.x + o.x * sx, ly = ref.y + o.y * sy;             // ms_deform_attn.py:125-127
+      if (p.valid_ratio != nullptr) {                                  // transformer.py:352-353
+        lx *= vrx;
+        ly *= vry;
+      }
+      const float px = lx * W - 0.5f, py = ly * H - 0.5f;              // cuh:285-286
+      if (!(py > -1.f && px > -1.f && py < H && px < W)) continue;     // cuh:288
+      const float w = lg[i] * inv;
+      const float yf = floorf(py), xf = floorf(px);
+      const int y0 = static_cast<int>(yf), x0 = static_cast<int>(xf);
+      const float fy = py - yf, fx = px - xf;
+      // clamped corner tokens (always readable), zero weight for the corners outside the level (cuh:58-84)
+      const int ya = max(y0, 0), yb = min(y0 + 1, H - 1), xa = max(x0, 0), xb = min(x0 + 1, W - 1);
+      const float wy0 = y0 >= 0 ? w - w * fy : 0.f, wy1 = y0 + 1 < H ? w * fy : 0.f;
+      const float wx0 = x0 >= 0 ? 1.f - fx : 0.f, wx1 = x0 + 1 < W ? fx : 0.f;
+      const float wc[4] = {wy0 * wx0, wy0 * wx1, wy1 * wx0, wy1 * wx1};
+      const long long tok[4] = {1LL * ya * W + xa, 1LL * ya * W + xb, 1LL * yb * W + xa, 1LL * yb * W + xb};
+      U4 v[4][2];
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        v[c][0] = ldg_nc16(vl + tok[c] * MSDA_D);
+        v[c][1] = ldg_nc16(vl + tok[c] * MSDA_D + 8);
+      }
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const uint32_t uu[4] = {v[c][hh].x, v[c][hh].y, v[c][hh].z, v[c][hh].w};
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const float2 f = Cvt<T>::unpack(uu[j]);
+            acc[hh * 8 + 2 * j] = fmaf(wc[c], f.x, acc[hh * 8 + 2 * j]);
+            acc[hh * 8 + 2 * j + 1] = fmaf(wc[c], f.y, acc[hh * 8 + 2 * j + 1]);
+          }
+        }
+    }
+  }
+  T* out = reinterpret_cast<T*>(p.out) + row * p.ld_out + m * MSDA_D;
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    U4 o;
+    o.x = Cvt<T>::pack(acc[hh * 8 + 0], acc[hh * 8 + 1]); o.y = Cvt<T>::pack(acc[hh * 8 + 2], acc[hh * 8 + 3]);
+    o.z = Cvt<T>::pack(acc[hh * 8 + 4], acc[hh * 8 + 5]); o.w = Cvt<T>::pack(acc[hh * 8 + 6], acc[hh * 8 + 7]);
+    *reinterpret_cast<U4*>(out + hh * 8) = o;
+  }
+}
+
 template <typename T, int NL, int NP>
 static int launch_fwd(const MsdaArgs& a, cudaStream_t st) {
+  if (a.nbands == 0) {
+    const long long threads = static_cast<long long>(a.batch) * a.nq * a.heads;
+    launch_k(msda_gather_kernel<T, NL, NP>, dim3(static_cast<unsigned>((threads + 255) / 256)), dim3(256), 0, st, a);
+    return static_cast<int>(cudaGetLastError());
+  }
   int e = ensure_max_dyn_smem(reinterpret_cast<const void*>(msda_fwd_kernel<T, NL, NP>), MS_SMEM);
   if (e) return e;
   const int items = a.batch * a.heads;
@@ -324,7 +439,7 @@ static int dispatch(const MsdaArgs& a, cudaStream_t st) {
 }
 
 int msda_launch(int dtype, const MsdaArgs& a, cudaStream_t st) {
-  if (a.nbands < 1 || a.batch < 1 || a.nq < 1) return -2;
+  if (a.nbands < 0 || a.batch < 1 || a.nq < 1) return -2;
   return dtype == DT_BF16 ? dispatch<__nv_bfloat16>(a, st) : dispatch<__half>(a, st);
 }
 
@@ -367,12 +482,6 @@ template <> struct Elt<__nv_bfloat16> {
     *reinterpret_cast<U4*>(p) = o;
   }
 };
-
-__device__ __forceinline__ U4 ldg_nc16(const void* p) {
-  U4 r;
-  asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
-  return r;
-}
 
 template <typename T>
 __global__ void __launch_bounds__(256) msda_op_kernel(const MsdaOpArgs p) {

@@ -34,7 +34,9 @@ struct MsdaArgs {
   MsdaBand bands[MSDA_MAX_BANDS];
 };
 
-// fills nbands / bands from the level table; returns -2 when a level cannot be staged (row wider than a stage)
+// fills nbands / bands from the level table; nbands = 0 when a level cannot be staged (row wider than half a stage, more
+// than 8192 tokens, more than MSDA_MAX_BANDS bands): msda_launch then takes the direct-gather kernel.  Returns -2 for an
+// invalid level table.
 int msda_plan(MsdaArgs* a);
 int msda_launch(int dtype, const MsdaArgs& a, cudaStream_t st);
 

@@ -192,13 +192,21 @@ int layernorm_launch(int dtype, const LayerNormArgs& a, cudaStream_t st) {
 }
 
 // ----------------------------------------------------------------------------------- patch gather
-// Image [B,3,S,S] (fp32 or 16-bit, NCHW) -> A [B*G*G, 3*256] 16-bit with rows in WINDOW-MAJOR token
+// Image [B,3,H,W] (fp32 or 16-bit, NCHW) -> A [B*GH*GW, 3*256] 16-bit with rows in WINDOW-MAJOR token
 // order and k = c*256 + py*16 + px, so that the 16x16/s16 patch-embedding conv (vit.py:79-83)
-// becomes one wgmma GEMM whose output is already in the layout of vit.py:353-358.
+// becomes one wgmma GEMM whose output is already in the layout of vit.py:353-358: 4x4 windows of
+// (GH/4) x (GW/4) tokens, windows enumerated row-major.
+__device__ __forceinline__ void window_token_yx(int rem, int GH, int GW, int* Y, int* X) {
+  const int wh = GH / 4, ww = GW / 4, wsz = wh * ww;
+  const int win = rem / wsz, t = rem % wsz;
+  *Y = (win >> 2) * wh + t / ww;
+  *X = (win & 3) * ww + t % ww;
+}
+
 template <typename T, typename TIn>
-__global__ void __launch_bounds__(256) patch_gather_kernel(const TIn* __restrict__ img, T* __restrict__ A, int B, int S) {
+__global__ void __launch_bounds__(256) patch_gather_kernel(const TIn* __restrict__ img, T* __restrict__ A, int B, int H, int W) {
   pdl_sync();   // programmatic dependent launch: release the successor, wait for the predecessor (launch.h)
-  const int G = S / 16, T_ = G * G;
+  const int GH = H / 16, GW = W / 16, T_ = GH * GW;
   const long long total = static_cast<long long>(B) * T_ * 48;      // (row, c, py)
   const long long id = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (id >= total) return;
@@ -207,10 +215,9 @@ __global__ void __launch_bounds__(256) patch_gather_kernel(const TIn* __restrict
   const int cp = static_cast<int>(id / rows);
   const int c = cp / 16, py = cp % 16;
   const int b = static_cast<int>(r / T_), rem = static_cast<int>(r % T_);
-  const int wh = G / 4, wsz = wh * wh;
-  const int win = rem / wsz, t = rem % wsz;
-  const int Y = (win >> 2) * wh + t / wh, X = (win & 3) * wh + t % wh;
-  const TIn* src = img + ((static_cast<long long>(b) * 3 + c) * S + (Y * 16 + py)) * S + X * 16;
+  int Y, X;
+  window_token_yx(rem, GH, GW, &Y, &X);
+  const TIn* src = img + ((static_cast<long long>(b) * 3 + c) * H + (Y * 16 + py)) * W + X * 16;
   float f[16];
   if constexpr (sizeof(TIn) == 4) {
 #pragma unroll
@@ -228,16 +235,16 @@ __global__ void __launch_bounds__(256) patch_gather_kernel(const TIn* __restrict
   stg256(A + r * 768 + c * 256 + py * 16, o);
 }
 
-int patch_gather_launch(int dtype, const void* img, int img_is_fp32, void* A, int B, int S, cudaStream_t st) {
-  if (S % 64 != 0) return -2;
-  const long long total = static_cast<long long>(B) * (S / 16) * (S / 16) * 48;
+int patch_gather_launch(int dtype, const void* img, int img_is_fp32, void* A, int B, int H, int W, cudaStream_t st) {
+  if (H % 64 != 0 || W % 64 != 0 || H < 64 || W < 64) return -2;
+  const long long total = static_cast<long long>(B) * (H / 16) * (W / 16) * 48;
   const unsigned grid = static_cast<unsigned>((total + 255) / 256);
   if (dtype == DT_BF16) {
-    if (img_is_fp32) launch_k(patch_gather_kernel<__nv_bfloat16, float>, dim3(grid), dim3(256), 0, st, static_cast<const float*>(img), static_cast<__nv_bfloat16*>(A), B, S);
-    else launch_k(patch_gather_kernel<__nv_bfloat16, __nv_bfloat16>, dim3(grid), dim3(256), 0, st, static_cast<const __nv_bfloat16*>(img), static_cast<__nv_bfloat16*>(A), B, S);
+    if (img_is_fp32) launch_k(patch_gather_kernel<__nv_bfloat16, float>, dim3(grid), dim3(256), 0, st, static_cast<const float*>(img), static_cast<__nv_bfloat16*>(A), B, H, W);
+    else launch_k(patch_gather_kernel<__nv_bfloat16, __nv_bfloat16>, dim3(grid), dim3(256), 0, st, static_cast<const __nv_bfloat16*>(img), static_cast<__nv_bfloat16*>(A), B, H, W);
   } else {
-    if (img_is_fp32) launch_k(patch_gather_kernel<__half, float>, dim3(grid), dim3(256), 0, st, static_cast<const float*>(img), static_cast<__half*>(A), B, S);
-    else launch_k(patch_gather_kernel<__half, __half>, dim3(grid), dim3(256), 0, st, static_cast<const __half*>(img), static_cast<__half*>(A), B, S);
+    if (img_is_fp32) launch_k(patch_gather_kernel<__half, float>, dim3(grid), dim3(256), 0, st, static_cast<const float*>(img), static_cast<__half*>(A), B, H, W);
+    else launch_k(patch_gather_kernel<__half, __half>, dim3(grid), dim3(256), 0, st, static_cast<const __half*>(img), static_cast<__half*>(A), B, H, W);
   }
   return static_cast<int>(cudaGetLastError());
 }
@@ -250,19 +257,18 @@ struct NormParams {
   float mean[3], stdv[3];
 };
 template <typename T>
-__global__ void __launch_bounds__(256) patch_gather_u8_kernel(const uint8_t* __restrict__ img, T* __restrict__ A, int B, int S, const NormParams np) {
+__global__ void __launch_bounds__(256) patch_gather_u8_kernel(const uint8_t* __restrict__ img, T* __restrict__ A, int B, int H, int W, const NormParams np) {
   pdl_sync();
-  const int G = S / 16, T_ = G * G;
+  const int GH = H / 16, GW = W / 16, T_ = GH * GW;
   const long long rows = static_cast<long long>(B) * T_;
   const long long id = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;      // (py, row): row fastest
   if (id >= rows * 16) return;
   const long long r = id % rows;
   const int py = static_cast<int>(id / rows);
   const int b = static_cast<int>(r / T_), rem = static_cast<int>(r % T_);
-  const int wh = G / 4, wsz = wh * wh;
-  const int win = rem / wsz, t = rem % wsz;
-  const int Y = (win >> 2) * wh + t / wh, X = (win & 3) * wh + t % wh;
-  const uint8_t* src = img + ((static_cast<long long>(b) * S + (Y * 16 + py)) * S + X * 16) * 3;
+  int Y, X;
+  window_token_yx(rem, GH, GW, &Y, &X);
+  const uint8_t* src = img + ((static_cast<long long>(b) * H + (Y * 16 + py)) * W + X * 16) * 3;
   uint32_t w[12];
 #pragma unroll
   for (int j = 0; j < 3; ++j) {
@@ -285,14 +291,14 @@ __global__ void __launch_bounds__(256) patch_gather_u8_kernel(const uint8_t* __r
   }
 }
 
-int patch_gather_u8_launch(int dtype, const void* img, const float* mean, const float* stdv, void* A, int B, int S, cudaStream_t st) {
-  if (S % 64 != 0) return -2;
+int patch_gather_u8_launch(int dtype, const void* img, const float* mean, const float* stdv, void* A, int B, int H, int W, cudaStream_t st) {
+  if (H % 64 != 0 || W % 64 != 0 || H < 64 || W < 64) return -2;
   NormParams np;
   for (int c = 0; c < 3; ++c) { np.mean[c] = mean[c]; np.stdv[c] = stdv[c]; }
-  const long long total = static_cast<long long>(B) * (S / 16) * (S / 16) * 16;
+  const long long total = static_cast<long long>(B) * (H / 16) * (W / 16) * 16;
   const unsigned grid = static_cast<unsigned>((total + 255) / 256);
-  if (dtype == DT_BF16) launch_k(patch_gather_u8_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, st, static_cast<const uint8_t*>(img), static_cast<__nv_bfloat16*>(A), B, S, np);
-  else launch_k(patch_gather_u8_kernel<__half>, dim3(grid), dim3(256), 0, st, static_cast<const uint8_t*>(img), static_cast<__half*>(A), B, S, np);
+  if (dtype == DT_BF16) launch_k(patch_gather_u8_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, st, static_cast<const uint8_t*>(img), static_cast<__nv_bfloat16*>(A), B, H, W, np);
+  else launch_k(patch_gather_u8_kernel<__half>, dim3(grid), dim3(256), 0, st, static_cast<const uint8_t*>(img), static_cast<__half*>(A), B, H, W, np);
   return static_cast<int>(cudaGetLastError());
 }
 
@@ -360,28 +366,29 @@ int mask_setup_launch(const uint8_t* mask, int B, int Himg, int Wimg, int L, int
 }
 
 // ----------------------------------------------------------------------------------- window-major -> spatial copy
+// rows of a GH x GW token grid per image, window-major (vit.py:353-358) -> row-major (b, y, x)
 template <typename T>
 __global__ void __launch_bounds__(256) unwindow_kernel(const T* __restrict__ src, int lds, T* __restrict__ dst, int ldd,
-                                                       long long rows, int C, int G) {
+                                                       long long rows, int C, int GH, int GW) {
   pdl_sync();   // programmatic dependent launch: release the successor, wait for the predecessor (launch.h)
   const int cpr = C / 8;
   const long long id = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (id >= rows * cpr) return;
   const long long r = id / cpr;
   const int c = static_cast<int>(id % cpr);
-  const int T_ = G * G, wh = G / 4, wsz = wh * wh;
+  const int T_ = GH * GW;
   const long long b = r / T_;
-  const int rem = static_cast<int>(r % T_);
-  const int win = rem / wsz, t = rem % wsz;
-  const int y = (win >> 2) * wh + t / wh, x = (win & 3) * wh + t % wh;
+  int y, x;
+  window_token_yx(static_cast<int>(r % T_), GH, GW, &y, &x);
   const U4 v = *reinterpret_cast<const U4*>(src + r * lds + c * 8);
-  *reinterpret_cast<U4*>(dst + (b * T_ + y * G + x) * ldd + c * 8) = v;
+  *reinterpret_cast<U4*>(dst + (b * T_ + y * GW + x) * ldd + c * 8) = v;
 }
-int unwindow_launch(int dtype, const void* src, int lds, void* dst, int ldd, long long rows, int C, int G, cudaStream_t st) {
+int unwindow_launch(int dtype, const void* src, int lds, void* dst, int ldd, long long rows, int C, int GH, int GW, cudaStream_t st) {
+  if (GH % 4 != 0 || GW % 4 != 0 || GH < 4 || GW < 4 || C % 8 != 0 || rows % (static_cast<long long>(GH) * GW) != 0) return -2;
   const long long n = rows * (C / 8);
   const unsigned grid = static_cast<unsigned>((n + 255) / 256);
-  if (dtype == DT_BF16) launch_k(unwindow_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, st, static_cast<const __nv_bfloat16*>(src), lds, static_cast<__nv_bfloat16*>(dst), ldd, rows, C, G);
-  else launch_k(unwindow_kernel<__half>, dim3(grid), dim3(256), 0, st, static_cast<const __half*>(src), lds, static_cast<__half*>(dst), ldd, rows, C, G);
+  if (dtype == DT_BF16) launch_k(unwindow_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, st, static_cast<const __nv_bfloat16*>(src), lds, static_cast<__nv_bfloat16*>(dst), ldd, rows, C, GH, GW);
+  else launch_k(unwindow_kernel<__half>, dim3(grid), dim3(256), 0, st, static_cast<const __half*>(src), lds, static_cast<__half*>(dst), ldd, rows, C, GH, GW);
   return static_cast<int>(cudaGetLastError());
 }
 
@@ -477,13 +484,115 @@ __global__ void __launch_bounds__(1024) topk_kernel(const float* __restrict__ sc
   bitonic_sort_desc(key, val, np2);
   for (int i = threadIdx.x; i < k; i += blockDim.x) idx_out[static_cast<long long>(b) * k + i] = val[i];
 }
+// Rows longer than a shared-memory sort holds (S > 16384: the P3 level of the two-level configs from 1024x1024 on).
+// One CTA per image; the score row is streamed from global memory / L2 and never held on chip:
+//   1. radix select on order-preserving uint32 keys, 8 bits per pass (four passes, a 256-bin shared histogram each):
+//      finds the k-th largest key `thr` and how many of the k winners equal it (`need`);
+//   2. one ordered pass compacts the <= k winners: every key > thr (any slot order) and the `need` LOWEST indices whose
+//      key equals thr (a block-wide prefix count over index order) - torch.topk's tie rule;
+//   3. the k survivors are sorted by (score desc, index asc) in shared memory.
+// Same result as topk_kernel (and torch.topk): descending, ties to the lower index.  -0.0 counts as +0.0, as a float
+// comparison does.
+__device__ __forceinline__ uint32_t topk_key(float f) {
+  const uint32_t u = f == 0.f ? 0u : __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+__global__ void __launch_bounds__(1024) topk_radix_kernel(const float* __restrict__ score, int S, int k, int np2k, int* __restrict__ idx_out) {
+  pdl_sync();   // programmatic dependent launch: release the successor, wait for the predecessor (launch.h)
+  extern __shared__ uint8_t sm_topk[];
+  float* ckey = reinterpret_cast<float*>(sm_topk);
+  int* cval = reinterpret_cast<int*>(ckey + np2k);
+  __shared__ int hist[256];
+  __shared__ int warp_excl[32];
+  __shared__ uint32_t s_prefix;
+  __shared__ int s_need, s_gt, s_eq_base, s_eq_tile;
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
+  const float* row = score + static_cast<long long>(b) * S;
+  if (tid == 0) { s_prefix = 0u; s_need = k; s_gt = 0; s_eq_base = 0; }
+  uint32_t mask = 0u;
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    for (int i = tid; i < 256; i += blockDim.x) hist[i] = 0;
+    __syncthreads();
+    const uint32_t prefix = s_prefix;
+    for (int i = tid; i < S; i += blockDim.x) {
+      const uint32_t key = topk_key(__ldg(row + i));
+      if ((key & mask) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1);
+    }
+    __syncthreads();
+    if (tid == 0) {                     // the bin holding the need-th largest key of the candidates
+      int cum = 0, need = s_need, bin = 255;
+      for (; bin > 0; --bin) {
+        if (cum + hist[bin] >= need) break;
+        cum += hist[bin];
+      }
+      s_need = need - cum;
+      s_prefix = prefix | (static_cast<uint32_t>(bin) << shift);
+    }
+    mask |= 255u << shift;
+    __syncthreads();
+  }
+  const uint32_t thr = s_prefix;
+  const int need = s_need, n_gt = k - need;
+  // ---- ordered compaction, one tile of blockDim indices at a time
+  for (int base = 0; base < S; base += blockDim.x) {
+    const int i = base + tid;
+    const float f = i < S ? __ldg(row + i) : 0.f;
+    const uint32_t key = i < S ? topk_key(f) : 0u;
+    const bool gt = i < S && key > thr, eq = i < S && key == thr;
+    if (gt) {
+      const int slot = atomicAdd(&s_gt, 1);
+      ckey[slot] = f;
+      cval[slot] = i;
+    }
+    const unsigned bal = __ballot_sync(0xffffffffu, eq);
+    if (lane == 0) warp_excl[warp] = __popc(bal);
+    __syncthreads();
+    if (warp == 0) {
+      const int v = lane < nwarps ? warp_excl[lane] : 0;
+      int incl = v;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+      }
+      if (lane < nwarps) warp_excl[lane] = incl - v;
+      if (lane == 31) s_eq_tile = incl;
+    }
+    __syncthreads();
+    const int rank = s_eq_base + warp_excl[warp] + __popc(bal & ((1u << lane) - 1u));
+    if (eq && rank < need) {
+      ckey[n_gt + rank] = f;
+      cval[n_gt + rank] = i;
+    }
+    __syncthreads();
+    if (tid == 0) s_eq_base += s_eq_tile;
+  }
+  for (int i = k + tid; i < np2k; i += blockDim.x) {
+    ckey[i] = -CUDART_INF_F;
+    cval[i] = 0x7fffffff;
+  }
+  __syncthreads();
+  bitonic_sort_desc(ckey, cval, np2k);
+  for (int i = tid; i < k; i += blockDim.x) idx_out[static_cast<long long>(b) * k + i] = cval[i];
+}
+
 int topk_launch(const float* score, int B, int S, int k, int* idx_out, cudaStream_t st) {
+  if (k > S) return -2;
   int np2 = 1;
   while (np2 < S) np2 <<= 1;
-  if (np2 > 16384 || k > S) return -2;
-  const size_t smem = static_cast<size_t>(np2) * 8;
-  if (int e = ensure_max_dyn_smem(reinterpret_cast<const void*>(topk_kernel), 16384 * 8)) return e;
-  launch_k(topk_kernel, dim3(B), dim3(1024), smem, st, score, S, np2, k, idx_out);
+  if (np2 <= 16384) {
+    const size_t smem = static_cast<size_t>(np2) * 8;
+    if (int e = ensure_max_dyn_smem(reinterpret_cast<const void*>(topk_kernel), 16384 * 8)) return e;
+    launch_k(topk_kernel, dim3(B), dim3(1024), smem, st, score, S, np2, k, idx_out);
+    return static_cast<int>(cudaGetLastError());
+  }
+  if (k < 1) return 0;
+  int np2k = 1;
+  while (np2k < k) np2k <<= 1;
+  if (np2k > 4096) return -2;
+  const size_t smem = static_cast<size_t>(np2k) * 8;
+  launch_k(topk_radix_kernel, dim3(B), dim3(1024), smem, st, score, S, k, np2k, idx_out);
   return static_cast<int>(cudaGetLastError());
 }
 

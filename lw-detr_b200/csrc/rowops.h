@@ -20,16 +20,20 @@ struct LayerNormArgs {
 };
 int layernorm_launch(int dtype, const LayerNormArgs& a, cudaStream_t st);
 
-int patch_gather_launch(int dtype, const void* img, int img_is_fp32, void* A, int B, int S, cudaStream_t st);
-// uint8 HWC [B,S,S,3] with fused (x/255 - mean) / std
-int patch_gather_u8_launch(int dtype, const void* img, const float* mean, const float* stdv, void* A, int B, int S, cudaStream_t st);
+// image [B,3,H,W] -> window-major patch matrix [B*(H/16)*(W/16), 768]; H, W multiples of 64
+int patch_gather_launch(int dtype, const void* img, int img_is_fp32, void* A, int B, int H, int W, cudaStream_t st);
+// uint8 HWC [B,H,W,3] with fused (x/255 - mean) / std
+int patch_gather_u8_launch(int dtype, const void* img, const float* mean, const float* stdv, void* A, int B, int H, int W, cudaStream_t st);
 // padding-mask tables of a (possibly) padded batch; mask == nullptr: no padding
 int mask_setup_launch(const uint8_t* mask, int B, int Himg, int Wimg, int L, int S, const int* lvl_h, const int* lvl_w, const int* lvl_start,
                       float* proposals, uint8_t* invalid, uint8_t* pad, float* valid_ratio, cudaStream_t st);
-int unwindow_launch(int dtype, const void* src, int lds, void* dst, int ldd, long long rows, int C, int G, cudaStream_t st);
+// window-major rows of a GH x GW token grid -> row-major (b, y, x); GH, GW multiples of 4
+int unwindow_launch(int dtype, const void* src, int lds, void* dst, int ldd, long long rows, int C, int GH, int GW, cudaStream_t st);
 int add_rows_launch(int dtype, const void* a, int lda, long long amod, const void* b, int ldb, void* out, int ldo,
                     long long rows, int C, cudaStream_t st);
 int rowmax_launch(const float* x, int ld, int n, float* out, long long rows, cudaStream_t st);
+// per-image top-k indices, descending, ties to the lower index: shared-memory bitonic sort up to S = 16384, radix select
+// streaming the row from global memory above (then k <= 4096)
 int topk_launch(const float* score, int B, int S, int k, int* idx_out, cudaStream_t st);
 // work: B * ceil(nq*ncls / 16384) * k ints
 int postprocess_launch(const float* logits, const float* boxes, const float* target_sizes, int B, int nq, int ncls, int k,

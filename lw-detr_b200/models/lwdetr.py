@@ -10,7 +10,7 @@ import torch
 from torch import nn
 
 from b200 import capi
-from b200.config import config_from_args
+from b200.config import config_from_args, run_size
 from b200.spec import param_spec
 from util.misc import NestedTensor, nested_tensor_from_tensor_list
 
@@ -102,11 +102,15 @@ class LWDETR(nn.Module):
         if self.training:
             raise RuntimeError("lwdetr_b200 implements the inference forward only; call model.eval()")
         if isinstance(samples, torch.Tensor) and samples.dtype == torch.uint8:
-            # raw camera / decoder frames [B, S, S, 3] (HWC, RGB, 0..255): the reference's host-side pre-processing
-            # (demo.py:146-159: /255, Normalize(mean, std), HWC -> CHW) is fused into the patch-embed load on the device
+            # raw camera / decoder frames [B, H, W, 3] (HWC, RGB, 0..255): the reference's host-side pre-processing
+            # (demo.py:146-159: /255, Normalize(mean, std), HWC -> CHW) is fused into the patch-embed load on the device.
+            # H and W are multiples of 64, not smaller than img_size (frames are not padded)
             dev = next(self.parameters()).device
             if dev.type != "cuda":
                 raise RuntimeError("lwdetr_b200: move the model to a CUDA device (no CPU fallback)")
+            S = self.cfg.img_size
+            if samples.dim() != 4 or samples.shape[3] != 3 or samples.shape[1] < S or samples.shape[2] < S:
+                raise RuntimeError("lwdetr_b200: uint8 frames must be [B, H, W, 3] (HWC) with H, W >= %d, got %s" % (S, tuple(samples.shape)))
             out = self.engine().forward(samples.to(dev), want_aux=True)
             return self._pack_outputs(out)
         if isinstance(samples, (list, torch.Tensor)):
@@ -115,15 +119,17 @@ class LWDETR(nn.Module):
         dev = next(self.parameters()).device
         if dev.type != "cuda":
             raise RuntimeError("lwdetr_b200: move the model to a CUDA device (no CPU fallback)")
-        S = self.cfg.img_size
-        if x.dim() != 4 or x.shape[-1] > S or x.shape[-2] > S:
-            raise RuntimeError("lwdetr_b200: images larger than the configured %dx%d are not supported, got %s" % (S, S, tuple(x.shape)))
-        if x.shape[-1] != S or x.shape[-2] != S:
-            # a batch whose largest image is smaller than the model's input: pad to the configured size (bottom / right,
-            # exactly what nested_tensor_from_tensor_list does between the images of a batch) and extend the mask
-            xp = x.new_zeros((x.shape[0], x.shape[1], S, S))
+        if x.dim() != 4:
+            raise RuntimeError("lwdetr_b200: expected a [B, 3, H, W] batch, got %s" % (tuple(x.shape),))
+        # the batch runs at (max(img_size, ceil64(H)), max(img_size, ceil64(W))): sides of at most img_size keep the
+        # configured input size, larger or non-square batches run at their own 64-aligned size (b200.config.run_size)
+        H, W = run_size(self.cfg, x.shape[-2], x.shape[-1])
+        if x.shape[-2] != H or x.shape[-1] != W:
+            # pad to the run size (bottom / right, exactly what nested_tensor_from_tensor_list does between the images of a
+            # batch) and extend the mask
+            xp = x.new_zeros((x.shape[0], x.shape[1], H, W))
             xp[:, :, : x.shape[-2], : x.shape[-1]] = x
-            mp = torch.ones((x.shape[0], S, S), dtype=torch.bool, device=x.device)
+            mp = torch.ones((x.shape[0], H, W), dtype=torch.bool, device=x.device)
             mp[:, : x.shape[-2], : x.shape[-1]] = mask if mask is not None else False
             x, mask = xp, mp
         x = x.to(dev)

@@ -2,10 +2,11 @@
 checkout named by $LWDETR_REFERENCE_SRC or staged under oracle/_ref) on the deterministic synthetic weights/inputs of
 b200/synth.py.
 
-    python tools/make_goldens.py [--postprocess-only | --padded-only | --seed5-only]
+    python tools/make_goldens.py [--postprocess-only | --padded-only | --seed5-only | --resolution-only]
 Each fixture holds the reference's final outputs and strided samples of its intermediates (captured
 with forward hooks), plus the state_dict names/shapes (tests/golden/state_dict_<cfg>.json).
 """
+import dataclasses
 import json
 import os
 import sys
@@ -99,9 +100,63 @@ def make_seed5_golden():
     print("seed5", out["pred_logits"].shape)
 
 
+# Inputs other than 640x640 (the reference's ViT resizes pos_embed to any token grid, vit.py:26-54, 343-358):
+# (config, img_size, batch, height, width).  large at 1024x1024 takes the streaming top-k (S = 17408 > 16384) and the
+# direct-gather deformable attention (P3 = 128x128 tokens); tiny at 512 runs natively with img_size = 512.
+RES_CASES = [("tiny", 512, 2, 512, 512), ("small", 640, 1, 448, 768), ("large", 640, 1, 1024, 1024), ("xlarge", 640, 1, 768, 1344)]
+RES_PADDED = ("tiny", 640, 832, 1344, [(800, 1333), (832, 1100)])   # COCO-style sizes (coco.py:111, max_size 1333), padded to 64
+RES_IMAGE_SEED = 21
+
+
+def res_golden_name(name, h, w, padded=False):
+    return "ref_res_%s_%dx%d%s.npz" % (name, h, w, "_padded" if padded else "")
+
+
+def res_padded_inputs():
+    """Two differently sized images at the bottom / right of an 832x1344 canvas, with the NestedTensor mask."""
+    name, _, H, W, sizes = RES_PADDED
+    x = torch.zeros(len(sizes), 3, H, W)
+    mask = torch.ones(len(sizes), H, W, dtype=torch.bool)
+    for b, (h, w) in enumerate(sizes):
+        x[b, :, :h, :w] = synth_images(1, RES_IMAGE_SEED + b, (h, w))[0]
+        mask[b, :h, :w] = False
+    return x, mask
+
+
+def make_resolution_goldens():
+    """Reference forward at input sizes other than 640x640, synthetic weights (seed WEIGHT_SEED) and images (seed
+    RES_IMAGE_SEED): pins the oracle's grid, windows, position table and level shapes, and through it the device path."""
+    for name, img_size, B, H, W in RES_CASES:
+        cfg = dataclasses.replace(CONFIGS[name], img_size=img_size)
+        model, _, _ = ref_import.build_reference(cfg)
+        model.load_state_dict(synth_state_dict(cfg, WEIGHT_SEED), strict=True)
+        with torch.no_grad():
+            out = model(synth_images(B, RES_IMAGE_SEED, (H, W)))
+        np.savez_compressed(os.path.join(GOLD, res_golden_name(name, H, W)), pred_logits=out["pred_logits"].numpy(),
+                            pred_boxes=out["pred_boxes"].numpy(), enc_logits=out["enc_outputs"]["pred_logits"].numpy(),
+                            enc_boxes=out["enc_outputs"]["pred_boxes"].numpy(),
+                            meta=np.array([B, WEIGHT_SEED, RES_IMAGE_SEED, H, W, img_size], dtype=np.int64))
+        print("resolution", name, H, W, out["pred_logits"].shape, flush=True)
+    name, img_size, H, W, sizes = RES_PADDED
+    cfg = dataclasses.replace(CONFIGS[name], img_size=img_size)
+    model, _, _ = ref_import.build_reference(cfg)
+    model.load_state_dict(synth_state_dict(cfg, WEIGHT_SEED), strict=True)
+    x, mask = res_padded_inputs()
+    with torch.no_grad():
+        out = model(sys.modules["_ref_util.misc"].NestedTensor(x, mask))
+    np.savez_compressed(os.path.join(GOLD, res_golden_name(name, H, W, padded=True)), pred_logits=out["pred_logits"].numpy(),
+                        pred_boxes=out["pred_boxes"].numpy(), enc_boxes=out["enc_outputs"]["pred_boxes"].numpy(),
+                        valid=np.array(sizes, dtype=np.int64),
+                        meta=np.array([len(sizes), WEIGHT_SEED, RES_IMAGE_SEED, H, W, img_size], dtype=np.int64))
+    print("resolution padded", name, H, W, out["pred_logits"].shape, flush=True)
+
+
 def main():
     torch.set_num_threads(os.cpu_count())
     os.makedirs(GOLD, exist_ok=True)
+    if "--resolution-only" in sys.argv:
+        make_resolution_goldens()
+        return
     if "--seed5-only" in sys.argv:
         make_seed5_golden()
         return
@@ -150,6 +205,7 @@ def main():
     make_postprocess_goldens()
     make_padded_golden()
     make_seed5_golden()
+    make_resolution_goldens()
 
 
 if __name__ == "__main__":

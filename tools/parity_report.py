@@ -19,23 +19,27 @@ from b200.config import CONFIGS  # noqa: E402
 from b200.synth import synth_images, synth_state_dict  # noqa: E402
 from oracle import lwdetr_oracle as orc  # noqa: E402
 
+import oracle_hw  # noqa: E402  (tools/: the oracle at any input size)
+
 
 def rel_l2(a, b):
     return ((a - b).norm() / (b.norm() + 1e-12)).item()
 
 
-def ladder(name, batch, dtype, wseed=1, iseed=0, eng=None):
+def ladder(name, batch, dtype, wseed=1, iseed=0, eng=None, hw=None):
+    """hw: (height, width) of the synthetic input, default the config's img_size square."""
     cfg = CONFIGS[name]
+    H, W = (cfg.img_size, cfg.img_size) if hw is None else (int(hw[0]), int(hw[1]))
     sd = synth_state_dict(cfg, wseed)
-    x = synth_images(batch, iseed)
+    x = synth_images(batch, iseed, (H, W))
     inter = {}
-    ref = orc.forward(sd, cfg, x, inter=inter)
+    ref = oracle_hw.forward(sd, cfg, x, inter=inter)     # = orc.forward at the configured size
     own = eng is None
     if own:
         eng = capi.Engine(cfg, dtype)
         eng.load_state_dict(sd)
     xg = x.cuda()
-    BT, C, d, S, nq = batch * cfg.tokens, cfg.vit_dim, cfg.hidden_dim, cfg.memory_len, cfg.num_queries
+    BT, C, d, S, nq = batch * (H // cfg.patch) * (W // cfg.patch), cfg.vit_dim, cfg.hidden_dim, cfg.memory_len_at(H, W), cfg.num_queries
     caps = {"patch_embed": BT * C}
     for i in range(cfg.vit_depth):
         caps["block%d" % i] = BT * C
@@ -52,7 +56,7 @@ def ladder(name, batch, dtype, wseed=1, iseed=0, eng=None):
     torch.cuda.synchronize()
     got = eng.capture_results()
     eng.clear_captures()
-    rep = {"config": name, "batch": batch, "dtype": str(dtype).replace("torch.", "")}
+    rep = {"config": name, "batch": batch, "dtype": str(dtype).replace("torch.", ""), "hw": [H, W]}
     t1 = {}
     t1["patch_embed"] = rel_l2(got["patch_embed"].reshape(BT, C), inter["patch"].reshape(BT, C))
     for i in range(cfg.vit_depth):
@@ -60,7 +64,7 @@ def ladder(name, batch, dtype, wseed=1, iseed=0, eng=None):
     mem = got["level%d" % (cfg.n_levels - 1)].reshape(batch, S, d)
     t1["memory"] = rel_l2(mem, inter["memory"])
     start = 0
-    for l, (h, w) in enumerate(cfg.level_shapes):
+    for l, (h, w) in enumerate(cfg.level_shapes_at(H, W)):
         t1["level%d" % l] = rel_l2(mem[:, start:start + h * w], inter["level%d" % l])
         start += h * w
     t1["enc_score_maxabs"] = (got["enc_score"].reshape(batch, S) - inter["enc_score"]).abs().max().item()
