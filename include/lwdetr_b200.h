@@ -202,6 +202,40 @@ LWDETR_API int lwdetr_forward_ex(lwdetr_handle* h, const lwdetr_input* input, in
 LWDETR_API int lwdetr_forward_hw(lwdetr_handle* h, const lwdetr_input* input, int B, int height, int width, float* pred_logits,
                                  float* pred_boxes, const lwdetr_aux_out* aux, const int32_t* topk_override, void* stream);
 
+/* Raw camera / decoder frames of any size (SURVEY.md 8f rank 2: the resize in front of the uint8 path).  One frame is a
+ * DEVICE uint8 HWC RGB image of height x width pixels, rows pitch_bytes >= 3 * width apart; `data` and `pitch_bytes` need
+ * no alignment (decoder surfaces, crops of a larger surface).  The frame is resized on the device to dst_h x dst_w by
+ * antialiased bilinear interpolation - the separable triangle filter of PIL.Image.resize(BILINEAR) and
+ * F.interpolate(mode="bilinear", antialias=True): per axis scale = n_in / n_out, support = max(scale, 1), output o has
+ * centre c = (o + 0.5) * scale, taps x in [max(int(c - support + 0.5), 0), min(int(c + support + 0.5), n_in)), weight
+ * max(0, 1 - |x - c + 0.5| / support) over the sum of the weights; horizontal then vertical in fp32, rounded half up to an
+ * integer level and clamped to [0, 255] - so the result is the uint8 image a host resize hands to LWDETR_IN_U8_NHWC, within
+ * one level of PIL (which also rounds between the passes).  Then (v / 255 - mean[c]) / std[c] as for LWDETR_IN_U8_NHWC.
+ * Limits: source sides in [8, 8192]; n_in / dst <= 16 per axis; any upscale; dst sides in [1, run side]. */
+typedef struct {
+  const uint8_t* data;
+  int32_t height, width;
+  int64_t pitch_bytes;
+  int32_t dst_h, dst_w;
+} lwdetr_frame;
+
+/* lwdetr_forward_hw on B frames, each with its own size: frame b is resized to its (dst_h, dst_w) and placed top-left on
+ * the height x width canvas the batch runs at (height, width as lwdetr_forward_hw requires).  The rest of the canvas is 0
+ * after normalisation and, when any frame leaves some, carries a padding mask made on the device (as util/misc.py:317-339
+ * builds it).  The resize is fused into the patch gather: no resized and no fp32 image exists in device memory.  `frames`
+ * is a HOST array of B descriptors with DEVICE data pointers; the caller may reuse it as soon as the call returns.  Same
+ * outputs and stream ordering as lwdetr_forward_hw; asynchronous; nothing is allocated per call.  Source sizes, pointers
+ * and dst sizes are not part of the plan: only a change of (B, height, width) re-plans. */
+LWDETR_API int lwdetr_forward_frames(lwdetr_handle* h, const lwdetr_frame* frames, const float mean[3], const float std[3], int B,
+                                     int height, int width, float* pred_logits, float* pred_boxes, const lwdetr_aux_out* aux,
+                                     const int32_t* topk_override, void* stream);
+
+/* The kernel behind it, without a model: frames -> A, the 16-bit window-major patch matrix [B * (height/16) * (width/16), 768]
+ * (k = c*256 + py*16 + px) that the patch-embedding GEMM reads, and (mask != NULL) the padding mask uint8 [B, height, width],
+ * 1 = outside the frame.  height and width multiples of 64. */
+LWDETR_API int lwdetr_resize_patches(int dtype, const lwdetr_frame* frames, int B, int height, int width, const float mean[3],
+                                     const float std[3], void* A, uint8_t* mask, void* stream);
+
 /* Multi-GPU init (SURVEY.md 8e): ONE ncclBroadcast of the packed weight arena from rank `root`, stream-ordered on
  * `stream`; the only collective of the path (images shard across ranks as independent replicas, nothing on the hot path).
  * Every rank first calls lwdetr_load_weights with tensors of the right shapes (any values on the non-root ranks): that

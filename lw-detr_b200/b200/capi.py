@@ -38,6 +38,8 @@ _SIGNATURES = {
     "lwdetr_weight_arena_bytes": (_i64, [_vp]),
     "lwdetr_forward_ex": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_forward_hw": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "lwdetr_forward_frames": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "lwdetr_resize_patches": (_i, [_i, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_set_option": (_i, [_vp, ctypes.c_char_p, _i]),
     "lwdetr_add_capture": (_i, [_vp, ctypes.c_char_p, _vp, _i64]),
     "lwdetr_capture_result": (_i64, [_vp, _i]),
@@ -258,6 +260,63 @@ IN_F32_NCHW, IN_16_NCHW, IN_U8_NHWC = 0, 1, 2
 IMAGENET_MEAN, IMAGENET_STD = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)      # demo/demo.py:150-153, datasets/coco.py
 
 
+class FrameStruct(ctypes.Structure):
+    _fields_ = [("data", _vp), ("height", ctypes.c_int32), ("width", ctypes.c_int32), ("pitch_bytes", ctypes.c_int64),
+                ("dst_h", ctypes.c_int32), ("dst_w", ctypes.c_int32)]
+
+
+def frame_list(frames, device=None):
+    """Raw frames as a list of CUDA uint8 [h, w, 3] tensors: takes that list or one [B, h, w, 3] tensor.  A frame may be a
+    view (a crop of a larger surface) as long as its pixels are packed RGB: stride(2) == 1 and stride(1) == 3."""
+    import torch
+    if isinstance(frames, torch.Tensor):
+        if frames.dim() != 4:
+            raise RuntimeError("lwdetr_b200: a frame batch must be [B, h, w, 3], got %s" % (tuple(frames.shape),))
+        frames = list(frames.unbind(0))
+    frames = list(frames)
+    if not frames:
+        raise RuntimeError("lwdetr_b200: no frames")
+    for i, f in enumerate(frames):
+        if not isinstance(f, torch.Tensor) or f.dtype != torch.uint8:
+            raise RuntimeError("lwdetr_b200: frame %d must be a uint8 tensor, got %s" % (i, getattr(f, "dtype", type(f))))
+        if f.dim() != 3 or f.shape[2] != 3:
+            raise RuntimeError("lwdetr_b200: frame %d must be [h, w, 3] (HWC), got %s" % (i, tuple(f.shape)))
+        if f.device.type != "cuda" or (device is not None and f.device != device):
+            raise RuntimeError("lwdetr_b200: frame %d is on %s; frames must be CUDA tensors%s"
+                               % (i, f.device, "" if device is None else " on %s" % (device,)))
+        if f.stride(2) != 1 or f.stride(1) != 3 or f.stride(0) < 3 * f.shape[1]:
+            raise RuntimeError("lwdetr_b200: frame %d has strides %s; packed RGB pixels are required: stride(2) == 1, "
+                               "stride(1) == 3, stride(0) >= 3 * width" % (i, tuple(f.stride())))
+    return frames
+
+
+def frame_descs(frames, dsts):
+    """HOST array of lwdetr_frame for frame_list() tensors and their (dst_h, dst_w)."""
+    arr = (FrameStruct * len(frames))()
+    for d, f, (dh, dw) in zip(arr, frames, dsts):
+        d.data, d.height, d.width, d.pitch_bytes, d.dst_h, d.dst_w = f.data_ptr(), f.shape[0], f.shape[1], f.stride(0), int(dh), int(dw)
+    return arr
+
+
+def _norm3(v):
+    return (ctypes.c_float * 3)(*[float(x) for x in v])
+
+
+def resize_patches(frames, dsts, size, dtype, mean=None, std=None, want_mask=False):
+    """lwdetr_resize_patches: frames resized to their dsts on an (H, W) = size canvas -> (window-major patch matrix
+    [B*(H/16)*(W/16), 768] in `dtype`, padding mask bool [B, H, W] or None)."""
+    import torch
+    frames = frame_list(frames)
+    H, W = int(size[0]), int(size[1])
+    dev, B = frames[0].device, len(frames)
+    mean, std = IMAGENET_MEAN if mean is None else mean, IMAGENET_STD if std is None else std
+    A = torch.empty(max(B * (H // 16) * (W // 16), 1), 768, device=dev, dtype=dtype)
+    mask = torch.empty(B, H, W, device=dev, dtype=torch.bool) if want_mask else None
+    check(lib().lwdetr_resize_patches(dtype_code(dtype), ctypes.cast(frame_descs(frames, dsts), _vp), B, H, W, ctypes.cast(_norm3(mean), _vp),
+                                      ctypes.cast(_norm3(std), _vp), ptr(A), ptr(mask), stream_ptr(dev)), "lwdetr_resize_patches")
+    return A, mask
+
+
 class AuxOut(ctypes.Structure):
     _fields_ = [(n, _vp) for n in ("aux_logits", "aux_boxes", "enc_logits", "enc_boxes", "topk_index")]
 
@@ -366,8 +425,20 @@ class Engine:
             mk = mask.to(device=self.device, dtype=torch.bool).contiguous()
         desc.images = images.data_ptr()
         desc.padding_mask = mk.data_ptr() if mk is not None else None
-        B, nq, nc, nl = images.shape[0], self.cfg.num_queries, self.cfg.num_classes, self.cfg.dec_layers
-        dev = images.device
+        B, dev = images.shape[0], images.device
+        res, logits, boxes, aux = self._outputs(B, dev, want_aux)
+        ov = None
+        if topk_override is not None:
+            ov = topk_override.to(device=dev, dtype=torch.int32).contiguous()
+        check(lib().lwdetr_forward_hw(self._h, ctypes.byref(desc), B, H, W, ptr(logits), ptr(boxes),
+                                      ctypes.byref(aux) if aux is not None else None, ptr(ov), stream_ptr(self.device)), "lwdetr_forward_hw")
+        self._last_inputs = (images, ov, mk)    # keep alive until the stream has consumed them
+        return res
+
+    def _outputs(self, B, dev, want_aux):
+        """Output tensors of one forward: (result dict, pred_logits, pred_boxes, AuxOut or None)."""
+        import torch
+        nq, nc, nl = self.cfg.num_queries, self.cfg.num_classes, self.cfg.dec_layers
         logits = torch.empty(B, nq, nc, device=dev, dtype=torch.float32)
         boxes = torch.empty(B, nq, 4, device=dev, dtype=torch.float32)
         aux = None
@@ -384,12 +455,32 @@ class Engine:
             res["aux_outputs"] = [{"pred_logits": al[i], "pred_boxes": ab[i]} for i in range(nl - 1)]
             res["enc_outputs"] = {"pred_logits": el, "pred_boxes": eb}
             res["topk_index"] = ti
+        return res, logits, boxes, aux
+
+    def forward_frames(self, frames, size=None, fit="stretch", short_side=None, max_side=None, want_aux=True, topk_override=None,
+                       mean=IMAGENET_MEAN, std=IMAGENET_STD):
+        """Raw camera / decoder frames of any size: a list of CUDA uint8 [h, w, 3] tensors (each its own size; views with
+        packed RGB pixels are fine) or one [B, h, w, 3] tensor.  Every frame is resized on the device (antialiased bilinear,
+        fused into the patch gather) and normalised with mean / std.  fit="stretch": to `size` = (H, W), default (img_size,
+        img_size).  fit="keep_aspect": to the reference's resize(size=short_side, max_size=max_side), frames top-left on the
+        run size (`size`, or run_size of the largest resized frame), the rest padded with a mask made on the device
+        (b200.config.frame_sizes).  Source sizes are not part of the plan: only a new (B, H, W) re-plans.  Returns the
+        dict of forward(), plus "frame_sizes": the (dst_h, dst_w) of each frame."""
+        import torch
+        from .config import frame_sizes
+        frames = frame_list(frames, self.device)
+        (H, W), dsts = frame_sizes(self.cfg, [(f.shape[0], f.shape[1]) for f in frames], size, fit, short_side, max_side)
+        B = len(frames)
+        res, logits, boxes, aux = self._outputs(B, self.device, want_aux)
         ov = None
         if topk_override is not None:
-            ov = topk_override.to(device=dev, dtype=torch.int32).contiguous()
-        check(lib().lwdetr_forward_hw(self._h, ctypes.byref(desc), B, H, W, ptr(logits), ptr(boxes),
-                                      ctypes.byref(aux) if aux is not None else None, ptr(ov), stream_ptr(self.device)), "lwdetr_forward_hw")
-        self._last_inputs = (images, ov, mk)    # keep alive until the stream has consumed them
+            ov = topk_override.to(device=self.device, dtype=torch.int32).contiguous()
+        check(lib().lwdetr_forward_frames(self._h, ctypes.cast(frame_descs(frames, dsts), _vp), ctypes.cast(_norm3(mean), _vp),
+                                          ctypes.cast(_norm3(std), _vp), B, H, W, ptr(logits), ptr(boxes),
+                                          ctypes.byref(aux) if aux is not None else None, ptr(ov), stream_ptr(self.device)),
+              "lwdetr_forward_frames")
+        self._last_inputs = (frames, ov, None)    # keep alive until the stream has consumed them
+        res["frame_sizes"] = dsts
         return res
 
     # ---- debug captures -------------------------------------------------------------------------

@@ -92,6 +92,49 @@ def run_size(cfg, height, width):
     return H, W
 
 
+def keep_aspect_size(height, width, short_side, max_side=None):
+    """(dst_h, dst_w) of the reference's resize(image, target, size, max_size) for a height x width image
+    (datasets/transforms.py:97-115, the same int() / round() calls): the shorter side goes to short_side, unless the longer
+    side would then exceed max_side, in which case the longer side goes to (about) max_side."""
+    w, h, size = int(width), int(height), int(short_side)
+    if max_side is not None:
+        mn, mx = float(min(w, h)), float(max(w, h))
+        if mx / mn * size > max_side:
+            size = int(round(max_side * mn / mx))
+    if (w <= h and w == size) or (h <= w and h == size):
+        return h, w
+    if w < h:
+        return int(size * h / w), size
+    return size, int(size * w / h)
+
+
+def frame_sizes(cfg, shapes, size=None, fit="stretch", short_side=None, max_side=None):
+    """Run size (H, W) and per-frame (dst_h, dst_w) of a batch of raw frames with the given (h, w) shapes.
+    fit="stretch": every frame fills `size` (default img_size x img_size): transforms.Resize([H, W]), what demo.py and the
+    square-resize evaluation do.  fit="keep_aspect": each frame takes keep_aspect_size(h, w, short_side, max_side); without
+    `size` the batch runs at run_size(cfg, max dst_h, max dst_w), frames top-left, the rest padded."""
+    if fit == "stretch":
+        if short_side is not None or max_side is not None:
+            raise RuntimeError("lwdetr_b200: short_side / max_side belong to fit='keep_aspect'")
+        H, W = (cfg.img_size, cfg.img_size) if size is None else (int(size[0]), int(size[1]))
+        check_input_size(cfg, H, W)
+        return (H, W), [(H, W)] * len(shapes)
+    if fit != "keep_aspect":
+        raise RuntimeError("lwdetr_b200: fit must be 'stretch' or 'keep_aspect', got %r" % (fit,))
+    if short_side is None:
+        raise RuntimeError("lwdetr_b200: fit='keep_aspect' needs short_side")
+    dsts = [keep_aspect_size(h, w, short_side, max_side) for h, w in shapes]
+    mh, mw = max(d[0] for d in dsts), max(d[1] for d in dsts)
+    if size is None:
+        H, W = run_size(cfg, mh, mw)
+    else:
+        H, W = int(size[0]), int(size[1])
+        check_input_size(cfg, H, W)
+        if mh > H or mw > W:
+            raise RuntimeError("lwdetr_b200: a frame resized to %dx%d does not fit the run size %dx%d" % (mh, mw, H, W))
+    return (H, W), dsts
+
+
 _W10 = (0, 1, 3, 6, 7, 9)
 _T10 = (2, 4, 5, 9)
 CONFIGS = {

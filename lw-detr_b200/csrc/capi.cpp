@@ -15,6 +15,7 @@
 #include "engine.h"
 #include "gemm_tc.h"
 #include "msda.h"
+#include "resize.h"
 #include "rowops.h"
 
 
@@ -252,6 +253,38 @@ int lwdetr_forward_ex(lwdetr_handle* h, const lwdetr_input* input, int B, float*
 int lwdetr_forward_hw(lwdetr_handle* h, const lwdetr_input* input, int B, int height, int width, float* pred_logits, float* pred_boxes,
                       const lwdetr_aux_out* aux, const int32_t* topk_override, void* stream) {
   return forward_input("lwdetr_forward_hw", h, input, B, height, width, pred_logits, pred_boxes, aux, topk_override, stream);
+}
+
+int lwdetr_forward_frames(lwdetr_handle* h, const lwdetr_frame* frames, const float mean[3], const float std[3], int B, int height,
+                          int width, float* pred_logits, float* pred_boxes, const lwdetr_aux_out* aux, const int32_t* topk_override,
+                          void* stream) {
+  if (!h || !frames || !mean || !std) return fail("lwdetr_forward_frames: null pointer");
+  if (B <= 0) return fail("lwdetr_forward_frames: batch must be positive");
+  lwb::ForwardIn in;
+  in.kind = lwb::IN_FRAMES; in.frames = frames;
+  for (int c = 0; c < 3; ++c) {
+    in.mean[c] = mean[c]; in.stdv[c] = std[c];
+    if (!(std[c] > 0.f)) return fail("lwdetr_forward_frames: std must be positive");
+  }
+  std::string err;
+  if (lwb::frames_check(frames, B, height, width, &err)) return fail("lwdetr_forward_frames: " + err);
+  if (h->eng->forward(in, B, height, width, pred_logits, pred_boxes, aux, topk_override, static_cast<cudaStream_t>(stream), &err)) return fail(err);
+  return 0;
+}
+
+int lwdetr_resize_patches(int dtype, const lwdetr_frame* frames, int B, int height, int width, const float mean[3], const float std[3],
+                          void* A, uint8_t* mask, void* stream) {
+  if (!frames || !mean || !std || !A) return fail("lwdetr_resize_patches: null pointer");
+  if (dtype != LWDETR_F16 && dtype != LWDETR_BF16) return fail("lwdetr_resize_patches: dtype must be LWDETR_F16 or LWDETR_BF16");
+  if (B <= 0 || height < 64 || width < 64 || height % 64 || width % 64) return fail("lwdetr_resize_patches: batch must be positive, height and width multiples of 64");
+  for (int c = 0; c < 3; ++c)
+    if (!(std[c] > 0.f)) return fail("lwdetr_resize_patches: std must be positive");
+  std::string err;
+  if (lwb::frames_check(frames, B, height, width, &err)) return fail("lwdetr_resize_patches: " + err);
+  int e = mask ? lwb::frame_mask_launch(frames, B, height, width, mask, static_cast<cudaStream_t>(stream)) : 0;
+  if (!e) e = lwb::resize_patches_launch(dtype, frames, B, height, width, mean, std, A, static_cast<cudaStream_t>(stream));
+  if (e) return cuda_fail(e, "lwdetr_resize_patches launch");
+  return 0;
 }
 
 // One ncclBroadcast of the packed weight arena (SURVEY.md 8b / 8e).  NCCL is not linked: the symbol is taken from the

@@ -18,6 +18,7 @@
 #include "attn.h"
 #include "gemm_tc.h"
 #include "msda.h"
+#include "resize.h"
 #include "rowops.h"
 
 namespace lwb {
@@ -545,11 +546,17 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
     float* vr_b = buf32(static_cast<long long>(B) * L * 2 + 4);
     uint8_t* invalid_b = static_cast<uint8_t*>(salloc(static_cast<size_t>(BS)));
     uint8_t* pad_b = static_cast<uint8_t*>(salloc(static_cast<size_t>(BS)));
+    uint8_t* fmask_b = static_cast<uint8_t*>(salloc(static_cast<size_t>(B) * IH * IW));   // padding mask of a batch of raw frames
     {
       const int lh0 = lvl_h[0], lh1 = lvl_h[1], lw0 = lvl_w[0], lw1 = lvl_w[1], ls0 = lvl_start[0], ls1 = lvl_start[1];
-      add_op("mask_setup", [this, B, IH, IW, L, S, lh0, lh1, lw0, lw1, ls0, ls1, prop_b, invalid_b, pad_b, vr_b](cudaStream_t st) {
+      add_op("mask_setup", [this, B, IH, IW, L, S, lh0, lh1, lw0, lw1, ls0, ls1, prop_b, invalid_b, pad_b, vr_b, fmask_b](cudaStream_t st) {
         const int lh[2] = {lh0, lh1}, lw[2] = {lw0, lw1}, ls[2] = {ls0, ls1};
-        return mask_setup_launch(in_.mask, B, IH, IW, L, S, lh, lw, ls, prop_b, invalid_b, pad_b, vr_b, st);
+        const uint8_t* mask = in_.mask;
+        if (in_.kind == IN_FRAMES) {      // raw frames: the mask follows from their dst sizes and is made on the device
+          mask = frames_padded_ ? fmask_b : nullptr;
+          if (frames_padded_) { const int rc = frame_mask_launch(in_.frames, B, IH, IW, fmask_b, st); if (rc) return rc; }
+        }
+        return mask_setup_launch(mask, B, IH, IW, L, S, lh, lw, ls, prop_b, invalid_b, pad_b, vr_b, st);
       }, prop_b, BS, 4, 4, 1, 24.0 * BS);
       if (pass) ops_.back().reads_input = true;
     }
@@ -561,6 +568,7 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
     {
       void* a0p = a0.p;
       add_op("patch_gather", [this, a0p, B, IH, IW, dt](cudaStream_t st) {
+               if (in_.kind == IN_FRAMES) return resize_patches_launch(dt, in_.frames, B, IH, IW, in_.mean, in_.stdv, a0p, st);
                if (in_.kind == IN_U8_NHWC) return patch_gather_u8_launch(dt, in_.images, in_.mean, in_.stdv, a0p, B, IH, IW, st);
                return patch_gather_launch(dt, in_.images, in_.kind == IN_F32_NCHW ? 1 : 0, a0p, B, IH, IW, st);
              },
@@ -813,8 +821,13 @@ int Engine::forward(const ForwardIn& in, int B, int H, int W, float* pred_logits
     ops_.clear();
     return -1;
   }
-  if (!in.images) { *err = "lwdetr_forward: null images"; return -1; }
+  if (in.kind == IN_FRAMES ? !in.frames : !in.images) { *err = "lwdetr_forward: null images"; return -1; }
   in_ = in; in_topk_override_ = topk_override;
+  if (in.kind == IN_FRAMES) {   // the schedule (and profile_ops, later) reads the engine's copy: the caller's array is free on return
+    frames_.assign(in.frames, in.frames + B);
+    in_.frames = frames_.data();
+    frames_padded_ = frames_padded(in.frames, B, H, W);
+  }
   // The first forward of a plan always runs eagerly (it also performs the one-time cudaFuncSetAttribute calls).
   const bool graph_ok = use_graph_ && captures_.empty() && eager_runs_ > 0;
   if (graph_ok) {

@@ -138,6 +138,33 @@ class LWDETR(nn.Module):
         out = self.engine().forward(x, want_aux=True, mask=mask)
         return self._pack_outputs(out)
 
+    @torch.no_grad()
+    def forward_frames(self, frames, size=None, fit="stretch", short_side=None, max_side=None):
+        """Raw camera / decoder frames of ANY size: a list of CUDA uint8 [h, w, 3] tensors (RGB, each its own size) or one
+        [B, h, w, 3] tensor.  The reference's host-side transforms.Resize (demo.py:146-159; datasets/transforms.py:97-134
+        for fit="keep_aspect" with short_side / max_side) runs on the device, fused into the patch-embed load together with
+        /255 and Normalize (capi.Engine.forward_frames).  Returns the output dict of forward()."""
+        if self.training:
+            raise RuntimeError("lwdetr_b200 implements the inference forward only; call model.eval()")
+        if next(self.parameters()).device.type != "cuda":
+            raise RuntimeError("lwdetr_b200: move the model to a CUDA device (no CPU fallback)")
+        out = self.engine().forward_frames(frames, size=size, fit=fit, short_side=short_side, max_side=max_side, want_aux=True)
+        return self._pack_outputs(out)
+
+    @torch.no_grad()
+    def detect(self, frames, size=None, fit="stretch", short_side=None, max_side=None, num_select=None):
+        """forward_frames + PostProcess: per frame {"scores", "labels", "boxes"} with xyxy boxes in the frame's ORIGINAL
+        pixel coordinates (for fit="keep_aspect" the predicted boxes are relative to the frame's valid region, which the
+        valid ratios of the padded batch already provide).  num_select defaults to num_queries."""
+        frames = capi.frame_list(frames, next(self.parameters()).device)
+        export, self._export = self._export, False
+        try:
+            out = self.forward_frames(frames, size=size, fit=fit, short_side=short_side, max_side=max_side)
+        finally:
+            self._export = export
+        sizes = torch.tensor([[f.shape[0], f.shape[1]] for f in frames], dtype=torch.float32, device=out["pred_logits"].device)
+        return PostProcess(self.num_queries if num_select is None else num_select)(out, sizes)
+
     def _pack_outputs(self, out):
         if self._export:
             return out["pred_boxes"], out["pred_logits"]      # forward_export tuple (lwdetr.py:176-195)
