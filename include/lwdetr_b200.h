@@ -21,7 +21,18 @@ extern "C" {
 
 #define LWDETR_API __attribute__((visibility("default")))
 
-enum { LWDETR_F16 = 0, LWDETR_BF16 = 1 };
+/* Compute modes of lwdetr_create.  LWDETR_F16_E4M3 is LWDETR_F16 with the ViT encoder's qkv and fc1 GEMMs on the FP8
+ * tensor cores (e4m3 x e4m3 -> fp32), with dynamic per-token and static per-channel scales.  Per block, for the fp16
+ * residual row x, the LayerNorm (w, b, eps 1e-6) and the linear (W [N, C], bias beta; qkv: beta = [q_bias, 0, v_bias]):
+ *   activations, per row m: x^ = (x - mean) * rstd in fp32 (affine not applied), a_m = max_k |x^_mk|,
+ *     s_a[m] = a_m / 448, q_a = e4m3(x^ * 448 / a_m) (round to nearest even, saturating; a_m = 0: both factors 1);
+ *   weights, per output channel n, packed once by lwdetr_load_weights: W' = W diag(w), s_w[n] = max_k |W'_nk| / 448
+ *     (0 -> 1), q_w = e4m3(W'_nk * 448 / max_k |W'_nk|), beta'[n] = beta[n] + sum_k b_k W_nk;
+ *   y = s_a[m] * s_w[n] * sum_k q_a q_w + beta'[n] (fp32 accumulation on the tensor cores, which keep fewer than 32 bits
+ *     of the running sum): qkv stores y, fc1 stores gelu(y), both fp16.
+ * Everything else (attention, proj, fc2, the projector, the decoder, every input path) is LWDETR_F16.  The option
+ * "fuse_layernorm" has no effect on the encoder in this mode. */
+enum { LWDETR_F16 = 0, LWDETR_BF16 = 1, LWDETR_F16_E4M3 = 2 };
 enum { LWDETR_ACT_NONE = 0, LWDETR_ACT_RELU = 1, LWDETR_ACT_GELU = 2, LWDETR_ACT_SILU = 3 };
 
 LWDETR_API const char* lwdetr_last_error(void);
@@ -127,6 +138,22 @@ LWDETR_API int lwdetr_postprocess(const float* pred_logits, const float* pred_bo
                                   int num_classes, int num_select, int32_t* work, float* scores, int32_t* labels, float* boxes,
                                   void* stream);
 
+/* The LWDETR_F16_E4M3 mode's two kernels.
+ * lwdetr_layernorm_e4m3: fp16 rows x [rows, ldx] -> e4m3 codes q [rows, ldq] (uint8) and fp32 row_scale [rows], as the mode's
+ *   activation contract above (x^ without the LayerNorm affine, eps as given).  C % 8 == 0, C <= 1024, ldx and ldq
+ *   multiples of 8.
+ * lwdetr_gemm_e4m3: out[m, n] = act(a_scale[m] * w_scale[n] * sum_k A[m,k] W[n,k] + bias[n]) in fp16; A e4m3 [M, lda]
+ *   (lda bytes, a multiple of 16), W e4m3 [N, K], a_scale fp32 [M], w_scale fp32 [N], bias fp32 [N] or NULL,
+ *   act LWDETR_ACT_NONE or LWDETR_ACT_GELU (exact-erf GELU, as the fp16 fc1), out fp16 [M, ld_out].  K % 64 == 0. */
+LWDETR_API int lwdetr_layernorm_e4m3(const void* x, int ldx, int64_t rows, int C, float eps, uint8_t* q, int ldq, float* row_scale,
+                                     void* stream);
+LWDETR_API int lwdetr_gemm_e4m3(const void* A, int lda, const float* a_scale, int M, int K, const void* W, const float* w_scale, int N,
+                                const float* bias, int act, void* out, int ld_out, void* stream);
+/* Host helper (no GPU): the weight quantiser lwdetr_load_weights uses in the LWDETR_F16_E4M3 mode.  Per row r of src
+ * fp32 [rows, K]: scale[r] = max_k |src[r,k]| / 448 (0 -> 1) and q[r,k] = e4m3(src[r,k] * 448 / max_k |src[r,k]|) as a
+ * uint8 code (round to nearest even, saturating to +-448). */
+LWDETR_API int lwdetr_host_quant_e4m3_rows(const float* src, int64_t rows, int K, uint8_t* q, float* scale);
+
 /* Host helper (no GPU): bicubic, align_corners=False resize of a channels-last [n_in, n_in, C] fp32 grid
  * to [n_out, n_out, C] - the absolute position embedding resize of vit.py:26-54, done once at load. */
 LWDETR_API int lwdetr_host_bicubic(const float* src, int n_in, int C, int n_out, float* dst);
@@ -156,7 +183,8 @@ typedef struct {
   int32_t* topk_index; /* [B, nq] two-stage selection (token index per query slot) or NULL */
 } lwdetr_aux_out;
 
-/* One handle per (device, config, compute dtype); not thread-safe per handle.  The handle binds to the CUDA device
+/* dtype: LWDETR_F16, LWDETR_BF16 or LWDETR_F16_E4M3 (see above).
+ * One handle per (device, config, compute dtype); not thread-safe per handle.  The handle binds to the CUDA device
  * that is current at creation; every later call switches to that device for its duration. */
 LWDETR_API int lwdetr_create(const lwdetr_config* cfg, int dtype, lwdetr_handle** out);
 LWDETR_API void lwdetr_destroy(lwdetr_handle* h);

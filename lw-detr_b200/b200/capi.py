@@ -9,7 +9,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), "lib", "liblwdetr_b200.so")
 
-F16, BF16 = 0, 1
+F16, BF16, F16_E4M3 = 0, 1, 2
 ACT_NONE, ACT_RELU, ACT_GELU, ACT_SILU = 0, 1, 2, 3
 
 _lib = None
@@ -28,6 +28,9 @@ _SIGNATURES = {
     "lwdetr_msda_forward": (_i, [_i, _vp, _i64, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "lwdetr_topk": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "lwdetr_postprocess": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "lwdetr_layernorm_e4m3": (_i, [_vp, _i, _i64, _i, _f, _vp, _i, _vp, _vp]),
+    "lwdetr_gemm_e4m3": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _i, _vp]),
+    "lwdetr_host_quant_e4m3_rows": (_i, [_vp, _i64, _i, _vp, _vp]),
     "lwdetr_host_bicubic": (_i, [_vp, _i, _i, _i, _vp]),
     "lwdetr_host_bicubic_hw": (_i, [_vp, _i, _i, _i, _i, _vp]),
     "lwdetr_create": (_i, [_vp, _i, _vp]),
@@ -82,12 +85,30 @@ def ptr(t):
 
 
 def dtype_code(torch_dtype):
+    """Engine compute mode of a torch dtype: float16, bfloat16, or float8_e4m3fn for the fp16 engine whose encoder qkv / fc1
+    GEMMs run in e4m3 (LWDETR_F16_E4M3)."""
     import torch
     if torch_dtype == torch.float16:
         return F16
     if torch_dtype == torch.bfloat16:
         return BF16
-    raise RuntimeError("lwdetr_b200 computes in float16 or bfloat16, got %s" % torch_dtype)
+    if torch_dtype == torch.float8_e4m3fn:
+        return F16_E4M3
+    raise RuntimeError("lwdetr_b200 computes in float16, bfloat16 or float8_e4m3fn (e4m3 encoder mode), got %s" % torch_dtype)
+
+
+def kernel_dtype_code(torch_dtype):
+    """dtype code of the 16-bit kernel-level entry points (tensors in float16 or bfloat16 only)."""
+    code = dtype_code(torch_dtype)
+    if code not in (F16, BF16):
+        raise RuntimeError("lwdetr_b200 kernels take float16 or bfloat16 tensors, got %s" % torch_dtype)
+    return code
+
+
+def io_dtype(torch_dtype):
+    """The 16-bit type of an engine's activations (and of 16-bit images it takes): float16 in the e4m3 mode."""
+    import torch
+    return torch.float16 if torch_dtype == torch.float8_e4m3fn else torch_dtype
 
 
 def stream_ptr(device=None):
@@ -102,7 +123,7 @@ def gemm(A, W, out, bias=None, gamma=None, resid=None, resid_mod=0, act=ACT_NONE
     M = A.shape[0] if M is None else M
     K = A.shape[1] if K is None else K
     N = W.shape[0] if N is None else N
-    check(lib().lwdetr_gemm(dtype_code(A.dtype), ptr(A), A.stride(0), M, K, ptr(W), N, ptr(bias), ptr(gamma),
+    check(lib().lwdetr_gemm(kernel_dtype_code(A.dtype), ptr(A), A.stride(0), M, K, ptr(W), N, ptr(bias), ptr(gamma),
                             ptr(resid), 0 if resid is None else resid.stride(0), resid_mod, act, ptr(out),
                             out.stride(0), 1 if out.dtype == torch.float32 else 0, rows_in, remap_rows,
                             shuffle_cout, IH, IW, stream_ptr()), "lwdetr_gemm")
@@ -111,7 +132,7 @@ def gemm(A, W, out, bias=None, gamma=None, resid=None, resid_mod=0, act=ACT_NONE
 
 def conv3x3(X, Wk, out, B, OH, OW, stride, Cin, bias=None, act=ACT_NONE):
     """X NHWC [B, s*OH, s*OW, ldx] (uses channels [0, Cin)), Wk [N, 9*Cin], out [B*OH*OW, ld_out]."""
-    check(lib().lwdetr_conv3x3(dtype_code(X.dtype), ptr(X), X.stride(2), B, OH, OW, stride, Cin, ptr(Wk),
+    check(lib().lwdetr_conv3x3(kernel_dtype_code(X.dtype), ptr(X), X.stride(2), B, OH, OW, stride, Cin, ptr(Wk),
                                Wk.shape[0], ptr(bias), act, ptr(out), out.stride(0), stream_ptr()),
           "lwdetr_conv3x3")
     return out
@@ -120,14 +141,14 @@ def conv3x3(X, Wk, out, B, OH, OW, stride, Cin, bias=None, act=ACT_NONE):
 def layernorm(x, y, w, b, eps, rows=None, C=None):
     rows = x.shape[0] if rows is None else rows
     C = x.shape[1] if C is None else C
-    check(lib().lwdetr_layernorm(dtype_code(x.dtype), ptr(x), x.stride(0), ptr(y), y.stride(0), ptr(w), ptr(b), eps,
+    check(lib().lwdetr_layernorm(kernel_dtype_code(x.dtype), ptr(x), x.stride(0), ptr(y), y.stride(0), ptr(w), ptr(b), eps,
                                  rows, C, stream_ptr()), "lwdetr_layernorm")
     return y
 
 
 def attention(q, k, v, out, nseq, seqlen, heads, dh, scale):
     """q/k/v/out: 2-D views [nseq*seqlen, heads*dh] (any row stride)."""
-    check(lib().lwdetr_attention(dtype_code(q.dtype), ptr(q), q.stride(0), ptr(k), k.stride(0), ptr(v), v.stride(0),
+    check(lib().lwdetr_attention(kernel_dtype_code(q.dtype), ptr(q), q.stride(0), ptr(k), k.stride(0), ptr(v), v.stride(0),
                                  ptr(out), out.stride(0), nseq, seqlen, heads, dh, scale, stream_ptr()),
           "lwdetr_attention")
     return out
@@ -147,7 +168,7 @@ def msda_forward(value_hm, offs_logits, ref, out, B, S, Lq, M, L, P, shapes, val
         acc += h * w
     st = (ctypes.c_int32 * L)(*starts)
     stride = M * S * 16 if v_image_stride is None else v_image_stride
-    check(lib().lwdetr_msda_forward(dtype_code(value_hm.dtype), ptr(value_hm), stride, ptr(offs_logits),
+    check(lib().lwdetr_msda_forward(kernel_dtype_code(value_hm.dtype), ptr(value_hm), stride, ptr(offs_logits),
                                     offs_logits.stride(0), ptr(ref), ptr(valid_ratio), ptr(out), out.stride(0), B, S, Lq, M, L, P,
                                     ctypes.cast(sh, _vp), ctypes.cast(st, _vp), stream_ptr()), "lwdetr_msda_forward")
     return out
@@ -225,6 +246,44 @@ def postprocess(pred_logits, pred_boxes, target_sizes, num_select):
     check(lib().lwdetr_postprocess(ptr(logits), ptr(boxes), ptr(ts), B, nq, ncls, num_select, ptr(work), ptr(scores), ptr(labels),
                                    ptr(out), stream_ptr()), "lwdetr_postprocess")
     return scores, labels, out
+
+
+def layernorm_e4m3(x, eps=1e-6):
+    """x: CUDA fp16 [rows, C] (any row stride) -> (e4m3 codes uint8 [rows, C], fp32 row scales [rows]); see
+    lwdetr_layernorm_e4m3."""
+    import torch
+    if x.dtype != torch.float16:
+        raise RuntimeError("layernorm_e4m3: x must be float16, got %s" % x.dtype)
+    rows, C = x.shape
+    q = torch.empty(rows, C, device=x.device, dtype=torch.uint8)
+    s = torch.empty(rows, device=x.device, dtype=torch.float32)
+    check(lib().lwdetr_layernorm_e4m3(ptr(x), x.stride(0), rows, C, float(eps), ptr(q), q.stride(0), ptr(s), stream_ptr(x.device)),
+          "lwdetr_layernorm_e4m3")
+    return q, s
+
+
+def gemm_e4m3(A, a_scale, W, w_scale, bias=None, act=ACT_NONE, out=None):
+    """out fp16 [M, N] = act(a_scale[m] * w_scale[n] * (A @ W.T) + bias); A uint8 e4m3 codes [M, K] (row stride a multiple of
+    16), W uint8 [N, K] contiguous, scales / bias fp32 (lwdetr_gemm_e4m3)."""
+    import torch
+    M, K = A.shape
+    N = W.shape[0]
+    if out is None:
+        out = torch.empty(M, N, device=A.device, dtype=torch.float16)
+    check(lib().lwdetr_gemm_e4m3(ptr(A), A.stride(0), ptr(a_scale), M, K, ptr(W), ptr(w_scale), N, ptr(bias), act, ptr(out),
+                                 out.stride(0), stream_ptr(A.device)), "lwdetr_gemm_e4m3")
+    return out
+
+
+def host_quant_e4m3_rows(src):
+    """src: CPU fp32 [rows, K] -> (e4m3 codes uint8 [rows, K], fp32 scales [rows]), the weight quantiser of the e4m3 mode."""
+    import torch
+    src = src.detach().to("cpu", torch.float32).contiguous()
+    rows, K = src.shape
+    q = torch.empty(rows, K, dtype=torch.uint8)
+    s = torch.empty(rows, dtype=torch.float32)
+    check(lib().lwdetr_host_quant_e4m3_rows(ptr(src), rows, K, ptr(q), ptr(s)), "lwdetr_host_quant_e4m3_rows")
+    return q, s
 
 
 def host_bicubic(src, n_out):
@@ -312,7 +371,7 @@ def resize_patches(frames, dsts, size, dtype, mean=None, std=None, want_mask=Fal
     mean, std = IMAGENET_MEAN if mean is None else mean, IMAGENET_STD if std is None else std
     A = torch.empty(max(B * (H // 16) * (W // 16), 1), 768, device=dev, dtype=dtype)
     mask = torch.empty(B, H, W, device=dev, dtype=torch.bool) if want_mask else None
-    check(lib().lwdetr_resize_patches(dtype_code(dtype), ctypes.cast(frame_descs(frames, dsts), _vp), B, H, W, ctypes.cast(_norm3(mean), _vp),
+    check(lib().lwdetr_resize_patches(kernel_dtype_code(dtype), ctypes.cast(frame_descs(frames, dsts), _vp), B, H, W, ctypes.cast(_norm3(mean), _vp),
                                       ctypes.cast(_norm3(std), _vp), ptr(A), ptr(mask), stream_ptr(dev)), "lwdetr_resize_patches")
     return A, mask
 
@@ -342,6 +401,8 @@ class Engine:
     """Owns one lwdetr_handle: packed weights + kernel schedule on the current CUDA device."""
 
     def __init__(self, cfg, dtype, device=None):
+        """dtype: torch.float16, torch.bfloat16, or torch.float8_e4m3fn for the fp16 engine with the encoder's qkv / fc1 in
+        e4m3 (outputs are the same fp32 dict in every mode)."""
         import torch
         if not torch.cuda.is_available():
             raise RuntimeError("lwdetr_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
@@ -413,7 +474,7 @@ class Engine:
             if images.dim() != 4 or images.shape[1] != 3:
                 raise RuntimeError("lwdetr_b200: expected images [B, 3, H, W], got %s" % (tuple(images.shape),))
             H, W = int(images.shape[2]), int(images.shape[3])
-            if images.dtype not in (torch.float32, self.dtype):
+            if images.dtype not in (torch.float32, io_dtype(self.dtype)):
                 images = images.float()
             desc.format = IN_F32_NCHW if images.dtype == torch.float32 else IN_16_NCHW
         check_input_size(self.cfg, H, W)

@@ -165,6 +165,33 @@ int lwdetr_postprocess(const float* pred_logits, const float* pred_boxes, const 
   return 0;
 }
 
+int lwdetr_layernorm_e4m3(const void* x, int ldx, int64_t rows, int C, float eps, uint8_t* q, int ldq, float* row_scale, void* stream) {
+  if (!x || !q || !row_scale) return fail("lwdetr_layernorm_e4m3: null pointer");
+  int e = lwb::layernorm_e4m3_launch(x, ldx, rows, C, eps, q, ldq, row_scale, static_cast<cudaStream_t>(stream));
+  if (e == -2) return fail("lwdetr_layernorm_e4m3: need rows >= 1, C % 8 == 0, 8 <= C <= 1024, ldx and ldq multiples of 8 and >= C");
+  if (e) return cuda_fail(e, "lwdetr_layernorm_e4m3 launch");
+  return 0;
+}
+
+int lwdetr_gemm_e4m3(const void* A, int lda, const float* a_scale, int M, int K, const void* W, const float* w_scale, int N,
+                     const float* bias, int act, void* out, int ld_out, void* stream) {
+  lwb::GemmE4m3Desc d;
+  d.A = A; d.lda = lda; d.a_scale = a_scale; d.M = M; d.K = K; d.W = W; d.w_scale = w_scale; d.N = N; d.bias = bias;
+  d.act = act; d.out = out; d.ld_out = ld_out;
+  lwb::GemmOp op;
+  std::string err;
+  if (lwb::gemm_e4m3_build(d, &op, &err)) return fail("lwdetr_gemm_e4m3: " + err);
+  int e = lwb::gemm_launch(op, static_cast<cudaStream_t>(stream));
+  if (e) return cuda_fail(e, "lwdetr_gemm_e4m3 launch");
+  return 0;
+}
+
+int lwdetr_host_quant_e4m3_rows(const float* src, int64_t rows, int K, uint8_t* q, float* scale) {
+  if (!src || !q || !scale || rows < 0 || K < 1) return fail("lwdetr_host_quant_e4m3_rows: bad arguments");
+  lwb::host_quant_e4m3_rows(src, rows, K, q, scale);
+  return 0;
+}
+
 int lwdetr_host_bicubic(const float* src, int n_in, int C, int n_out, float* dst) {
   if (!src || !dst || n_in < 1 || n_out < 1 || C < 1) return fail("lwdetr_host_bicubic: bad arguments");
   lwb::bicubic_resize_chlast(src, n_in, C, n_out, dst);
@@ -184,7 +211,8 @@ struct lwdetr_handle {
 
 int lwdetr_create(const lwdetr_config* cfg, int dtype, lwdetr_handle** out) {
   if (!cfg || !out) return fail("lwdetr_create: null pointer");
-  if (dtype != LWDETR_F16 && dtype != LWDETR_BF16) return fail("lwdetr_create: dtype must be LWDETR_F16 or LWDETR_BF16");
+  if (dtype != LWDETR_F16 && dtype != LWDETR_BF16 && dtype != LWDETR_F16_E4M3)
+    return fail("lwdetr_create: dtype must be LWDETR_F16, LWDETR_BF16 or LWDETR_F16_E4M3");
   if (cfg->n_taps < 1 || cfg->n_taps > 4 || cfg->n_levels < 1 || cfg->n_levels > 2 || cfg->vit_depth < 1 || cfg->vit_depth > 31)
     return fail("lwdetr_create: unsupported configuration");
   if (cfg->img_size % 64 != 0 || cfg->vit_dim % 64 != 0 || cfg->hidden_dim % 128 != 0)

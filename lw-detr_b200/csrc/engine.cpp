@@ -75,6 +75,33 @@ void bicubic_resize_chlast_hw(const float* src, int n_in, int C, int out_h, int 
 }
 void bicubic_resize_chlast(const float* src, int n_in, int C, int n_out, float* dst) { bicubic_resize_chlast_hw(src, n_in, C, n_out, n_out, dst); }
 
+// fp32 -> e4m3 (OCP E4M3, "fn": no infinities, 0x7F is NaN) code, round to nearest even, saturating to +-448: what
+// cvt.rn.satfinite.e4m3x2.f32 computes on the device and torch's float8_e4m3fn conversion after a clamp to +-448.
+static uint8_t e4m3_code(float v) {
+  const uint8_t sign = std::signbit(v) ? 0x80 : 0x00;
+  const float a = std::fabs(v);
+  if (!(a < 448.f)) return sign | 0x7E;                        // saturate (and +-448 itself)
+  if (a < 0.015625f) return sign | static_cast<uint8_t>(std::nearbyint(a * 512.f));   // subnormal steps of 2^-9 (8 -> 2^-6)
+  int e;
+  const float f = std::frexp(a, &e);                            // a = f * 2^e, f in [0.5, 1)
+  int m = static_cast<int>(std::nearbyint((f * 2.f - 1.f) * 8.f));
+  int be = e - 1 + 7;
+  if (m == 8) { m = 0; ++be; }
+  const int code = (be << 3) | m;
+  return sign | static_cast<uint8_t>(code > 0x7E ? 0x7E : code);
+}
+
+void host_quant_e4m3_rows(const float* src, long long rows, int K, uint8_t* q, float* scale) {
+  for (long long r = 0; r < rows; ++r) {
+    const float* x = src + r * K;
+    float m = 0.f;
+    for (int k = 0; k < K; ++k) m = std::max(m, std::fabs(x[k]));
+    const float inv = m > 0.f ? 448.f / m : 1.f;
+    scale[r] = m > 0.f ? m / 448.f : 1.f;
+    for (int k = 0; k < K; ++k) q[r * K + k] = e4m3_code(x[k] * inv);
+  }
+}
+
 // The ViT's position table at a GH x GW token grid: the 14x14 pretraining grid of pos_embed [197, C] (cls slot first)
 // resized bicubically (vit.py:26-54) and laid out in window-major token order (vit.py:353-358), fp32.
 static std::vector<float> window_major_pos(const float* pos_embed, int C, int GH, int GW) {
@@ -90,7 +117,10 @@ static std::vector<float> window_major_pos(const float* pos_embed, int C, int GH
 }
 
 // ------------------------------------------------------------------------------- Engine basics
-Engine::Engine(const lwdetr_config& cfg, int dtype) : cfg_(cfg), dtype_(dtype) { cudaGetDevice(&device_); }
+// LWDETR_F16_E4M3 is the fp16 engine with the encoder's qkv / fc1 (and their LayerNorms) in e4m3
+Engine::Engine(const lwdetr_config& cfg, int dtype) : cfg_(cfg), dtype_(dtype == LWDETR_F16_E4M3 ? DT_F16 : dtype), e4m3_(dtype == LWDETR_F16_E4M3) {
+  cudaGetDevice(&device_);
+}
 
 namespace {
 // Switches to the engine's device for the duration of a call (the caller's current device is restored afterwards).
@@ -153,6 +183,12 @@ void* Engine::upload16(const std::vector<float>& v) {
   if (!d) return nullptr;
   const std::vector<uint16_t> h = to16(v);
   cudaMemcpy(d, h.data(), h.size() * 2, cudaMemcpyHostToDevice);
+  return d;
+}
+void* Engine::upload8(const std::vector<uint8_t>& v) {
+  void* d = walloc(v.size());
+  if (!d) return nullptr;
+  cudaMemcpy(d, v.data(), v.size(), cudaMemcpyHostToDevice);
   return d;
 }
 float* Engine::upload32(const std::vector<float>& v) {
@@ -273,6 +309,42 @@ int Engine::load_weights(const std::map<std::string, HostTensor>& w, std::string
   put16("pos", window_major_pos(pos_embed.data(), C, G, G));   // the table at the configured resolution
   for (int i = 0; i < cfg_.vit_depth; ++i) {
     const std::string b = E + "blocks." + std::to_string(i) + ".", k = "blk" + std::to_string(i) + ".";
+    if (e4m3_) {
+      // e4m3 mode: qkv and fc1 only as e4m3 weights with the LayerNorm affine folded in (see lwdetr_b200.h LWDETR_F16_E4M3):
+      //   W' = W diag(ln_w), per output channel n: w_scale[n] = max_k |W'[n,k]| / 448, codes e4m3(W'[n,k] * 448 / max),
+      //   bias'[n] = bias[n] + sum_k ln_b[k] W[n,k] (double)
+      auto put_e4m3 = [&](const std::string& key, const std::vector<float>& Wm, const std::vector<float>& bias, const std::string& ln, int n_out) {
+        auto lw = vec(ln + ".weight", C), lb = vec(ln + ".bias", C);
+        std::vector<float> Wf(Wm.size()), bf(n_out), sw(n_out);
+        for (int n = 0; n < n_out; ++n) {
+          double acc_b = bias[n];
+          for (int kk = 0; kk < C; ++kk) {
+            const float wv = Wm[static_cast<size_t>(n) * C + kk];
+            Wf[static_cast<size_t>(n) * C + kk] = wv * lw[kk];
+            acc_b += static_cast<double>(lb[kk]) * wv;
+          }
+          bf[n] = static_cast<float>(acc_b);
+        }
+        std::vector<uint8_t> q(Wf.size());
+        host_quant_e4m3_rows(Wf.data(), n_out, C, q.data(), sw.data());
+        void* p = upload8(q);
+        if (!p) oom = true;
+        W_[key + ".w"] = p;
+        put32(key + ".b", bf);
+        put32(key + ".s", sw);
+      };
+      auto qb = vec(b + "attn.q_bias", C), vb = vec(b + "attn.v_bias", C);
+      std::vector<float> bias(static_cast<size_t>(3) * C, 0.f);     // [q_bias, 0, v_bias]  (vit.py:123-125)
+      std::copy(qb.begin(), qb.end(), bias.begin());
+      std::copy(vb.begin(), vb.end(), bias.begin() + 2 * C);
+      put_e4m3(k + "qkv_q", vec(b + "attn.qkv.weight", 3LL * C * C), bias, b + "norm1", 3 * C);
+      put_e4m3(k + "fc1_q", vec(b + "mlp.fc1.weight", 4LL * C * C), vec(b + "mlp.fc1.bias", 4LL * C), b + "norm2", 4 * C);
+      put_linear(k + "proj", b + "attn.proj", C, C);
+      put32(k + "g1", vec(b + "gamma_1", C));
+      put_linear(k + "fc2", b + "mlp.fc2", C, 4 * C);
+      put32(k + "g2", vec(b + "gamma_2", C));
+      continue;
+    }
     put_norm(k + "ln1", b + "norm1", C);
     put16(k + "qkv.w", vec(b + "attn.qkv.weight", 3LL * C * C));
     {
@@ -577,7 +649,36 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
     }
     float2* stats_x = static_cast<float2*>(salloc(static_cast<size_t>(BT) * 48 * sizeof(float2)));   // row stats of x (block input)
     float2* stats_m = static_cast<float2*>(salloc(static_cast<size_t>(BT) * 48 * sizeof(float2)));   // row stats of x + attn
-    const bool fuse = fuse_ln_ != 0;
+    const bool fuse = fuse_ln_ != 0 && !e4m3_;   // the e4m3 mode has its own LayerNorm -> e4m3 pass in front of qkv / fc1
+    // e4m3 mode: the LayerNorm output as e4m3 codes + per-row scales, shared by qkv and fc1
+    uint8_t* lnq = e4m3_ ? static_cast<uint8_t*>(salloc(static_cast<size_t>(BT) * C)) : nullptr;
+    float* lns = e4m3_ ? buf32(BT) : nullptr;
+    auto add_ln_e4m3 = [&](const std::string& label, Mat x) {
+      if (pass == 0) return;
+      const void* xp = x.p; const int ldx = x.ld;
+      Op P_;
+      P_.label = label;
+      P_.run = [xp, ldx, BT, C, lnq, lns](cudaStream_t st) { return layernorm_e4m3_launch(xp, ldx, BT, C, 1e-6f, lnq, C, lns, st); };
+      P_.out = lns; P_.rows = BT; P_.cols = 1; P_.ld = 1; P_.fp32 = 1;   // a capture returns the row scales
+      P_.bytes = 2.0 * BT * C + 1.0 * BT * C + 4.0 * BT;
+      ops_.push_back(P_);
+    };
+    auto add_gemm_e4m3 = [&](const std::string& label, const std::string& wkey, int N, int act, Mat out) {
+      if (pass == 0) return;
+      GemmE4m3Desc g;
+      g.A = lnq; g.lda = C; g.a_scale = lns; g.M = static_cast<int>(BT); g.K = C; g.N = N;
+      g.W = w16(wkey + ".w"); g.w_scale = w32(wkey + ".s"); g.bias = w32(wkey + ".b"); g.act = act; g.out = out.p; g.ld_out = out.ld;
+      GemmOp op;
+      std::string e;
+      if (fail || gemm_e4m3_build(g, &op, &e)) { if (!fail) *err = label + ": " + e; fail = true; return; }
+      Op P_;
+      P_.label = label;
+      P_.run = [op](cudaStream_t st) { return gemm_launch(op, st); };
+      P_.out = out.p; P_.rows = BT; P_.cols = N; P_.ld = out.ld;
+      P_.flops = op.flops;
+      P_.bytes = 1.0 * (static_cast<double>(BT) * C + static_cast<double>(N) * C) + 4.0 * BT + 8.0 * N + 2.0 * BT * N;   // 1-byte operands
+      ops_.push_back(P_);
+    };
     Mat xcur = xa;
     void* pos_tab = own_pos ? salloc(pos_host.size() * 2) : nullptr;
     if (own_pos && pass == 1 && cudaMemcpy(pos_tab, pos_host.data(), pos_host.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) {
@@ -593,7 +694,10 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
     for (int i = 0; i < cfg_.vit_depth; ++i) {
       const std::string k = "blk" + std::to_string(i) + ".", lb = "block" + std::to_string(i);
       const bool window = (cfg_.window_block_mask >> i) & 1;
-      if (fuse) {
+      if (e4m3_) {
+        add_ln_e4m3(lb + ".ln1", xcur);
+        add_gemm_e4m3(lb + ".qkv", k + "qkv_q", 3 * C, ACT_NONE, qkv);
+      } else if (fuse) {
         GemmOpt o; o.stats_in = stats_x; o.ln_C = C; o.ln_eps = 1e-6f;
         add_gemm(lb + ".qkv", xcur, BT, C, k + "qkv_ln", 3 * C, qkv.p, qkv.ld, o);
       } else {
@@ -604,7 +708,10 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
                window ? 16 * B : B, window ? T / 16 : T, heads, C / heads);
       { GemmOpt o; o.gamma = pass ? w32(k + "g1") : nullptr; o.resid = xcur; if (fuse) o.stats_out = stats_m;
         add_gemm(lb + ".proj", att, BT, C, k + "proj", C, xm.p, xm.ld, o); }
-      if (fuse) {
+      if (e4m3_) {
+        add_ln_e4m3(lb + ".ln2", xm);
+        add_gemm_e4m3(lb + ".fc1", k + "fc1_q", 4 * C, ACT_GELU, hid);
+      } else if (fuse) {
         GemmOpt o; o.act = ACT_GELU; o.stats_in = stats_m; o.ln_C = C; o.ln_eps = 1e-6f;
         add_gemm(lb + ".fc1", xm, BT, C, k + "fc1_ln", 4 * C, hid.p, hid.ld, o);
       } else {

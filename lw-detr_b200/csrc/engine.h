@@ -79,15 +79,18 @@ class Engine {
   std::vector<uint16_t> to16(const std::vector<float>& v) const;   // round to the compute dtype
   void* upload16(const std::vector<float>& v);
   float* upload32(const std::vector<float>& v);
+  void* upload8(const std::vector<uint8_t>& v);
   int do_capture(const Op& op, cudaStream_t st);
 
   lwdetr_config cfg_;
   int dtype_;
+  bool e4m3_ = false;   // LWDETR_F16_E4M3: dtype_ is DT_F16; the encoder's LN->qkv and LN->fc1 run in e4m3
   int device_ = 0;    // CUDA device the engine was created on; every entry point switches to it (one handle per device)
   int planned_B_ = 0, planned_H_ = 0, planned_W_ = 0;   // shape of the current schedule (0: none)
   bool weights_loaded_ = false;
   int use_graph_ = 0;
-  int fuse_ln_ = 1;   // ViT LayerNorms folded into the consuming GEMM's epilogue (option "fuse_layernorm")
+  int fuse_ln_ = 1;   // ViT LayerNorms folded into the consuming GEMM's epilogue (option "fuse_layernorm"; no effect on the
+                      // encoder in the e4m3 mode)
   // CUDA graphs: the two ops that read caller-owned memory (mask tables, patch gather) are launched eagerly on the
   // caller's stream; everything behind them only touches engine-owned buffers and is ONE executable graph per planned
   // (batch size, height, width) - whatever tensor, input encoding or mask the caller passes.  (The test-only top-k override pointer is
@@ -125,5 +128,7 @@ class Engine {
 // host helpers exposed for CPU tests
 void bicubic_resize_chlast(const float* src, int n_in, int C, int n_out, float* dst);   // [n_in,n_in,C] -> [n_out,n_out,C]
 void bicubic_resize_chlast_hw(const float* src, int n_in, int C, int out_h, int out_w, float* dst);   // [n_in,n_in,C] -> [out_h,out_w,C]
+// per row: scale = max|x| / 448 (0 -> 1), q = e4m3(x * 448 / max) round to nearest even, saturating (the e4m3 weight packing)
+void host_quant_e4m3_rows(const float* src, long long rows, int K, uint8_t* q, float* scale);
 
 }  // namespace lwb

@@ -482,6 +482,160 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 }
 
 
+
+// ------------------------------------------------------------------------------------------- FP8 (e4m3) GEMM
+// The encoder's qkv and fc1 in the e4m3 compute mode (gemm_tc.h GemmE4m3Desc).  Same tile walk, producer / consumer split,
+// stage ring and accumulator staging as gemm_tc_kernel, with 1-byte operands: a k-block is one 128-byte swizzle row, i.e.
+// 128 elements, and the MMA is m64nBNk32 e4m3 x e4m3 -> fp32.  A k-block past K (K = 192: the second one is half empty)
+// is zero-filled by TMA.  Epilogue: out = act(a_scale[m] * w_scale[n] * acc + bias[n]) -> fp16; no residual, LayerNorm
+// fold, row statistics or row remap.
+static constexpr int BK8 = 128;
+static constexpr int A8_STAGE_BYTES = BM * BK8;
+
+template <int BN, bool GELU>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_e4m3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmArgs p) {
+  constexpr int B_STAGE_BYTES = BN * BK8;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const int stages = p.stages;
+  uint8_t* sA = smem;
+  uint8_t* sB = smem + stages * A8_STAGE_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sB + stages * B_STAGE_BYTES);
+  uint64_t* empty_bar = full_bar + MAX_STAGES;
+  float* s_stage = reinterpret_cast<float*>(full_bar + 32);
+  float* s_vec = s_stage + MMA_WARPS * 16 * STG_LD;           // {w_scale | bias}[n_tiles * BN]
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int num_tiles = p.m_tiles * p.n_tiles;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int s = 0; s < stages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], MMA_WARPS);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_sync();
+
+  if (warp < 4) {
+    reg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      uint32_t ring = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const TileCoord tc = decode_tile(p, tile, BN);
+        for (int kb = 0; kb < p.kblocks; ++kb, ++ring) {
+          const int s = ring % stages;
+          mbar_wait(&empty_bar[s], ((ring / stages) & 1) ^ 1);
+          mbar_arrive_expect_tx(&full_bar[s], A8_STAGE_BYTES + B_STAGE_BYTES);
+          tma_load_2d(sA + s * A8_STAGE_BYTES, &tmA, &full_bar[s], kb * BK8, tc.m_tile * BM);
+          tma_load_2d(sB + s * B_STAGE_BYTES, &tmB, &full_bar[s], kb * BK8, tc.n0);
+        }
+      }
+    }
+  } else {
+    reg_inc<232>();
+    const int cw = warp - 4, wg = cw >> 2;
+    const int g = lane >> 2, t4 = lane & 3;
+    const int chalf = lane & 1;
+    const int r = cw * 16 + (lane >> 1);
+    float* stg = s_stage + cw * 16 * STG_LD;
+    const int npad = p.n_tiles * BN;
+    for (int i = threadIdx.x - 128; i < npad; i += 32 * MMA_WARPS) {
+      const bool in = i < p.N;
+      s_vec[i] = in ? __ldg(p.w_scale + i) : 0.f;
+      s_vec[npad + i] = (p.bias != nullptr && in) ? __ldg(p.bias + i) : 0.f;
+    }
+    asm volatile("bar.sync 1, %0;" ::"n"(32 * MMA_WARPS) : "memory");
+
+    uint32_t ring = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const TileCoord tc = decode_tile(p, tile, BN);
+      const int n0 = tc.n0;
+      const int m = tc.m_tile * BM + r;
+      const bool valid = m < p.M;
+      const float sa = valid ? __ldg(p.a_scale + m) : 0.f;   // the load overlaps the MMAs below
+
+      float acc[BN / 2];
+      for (int kb = 0; kb < p.kblocks; ++kb, ++ring) {
+        const int s = ring % stages;
+        mbar_wait(&full_bar[s], (ring / stages) & 1);
+        const uint64_t adesc = wgmma_desc(smem_u32(sA + s * A8_STAGE_BYTES + wg * (64 * BK8)), 128);
+        const uint64_t bdesc = wgmma_desc(smem_u32(sB + s * B_STAGE_BYTES), 128);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK8 / 32; ++k)     // 32 elements (32 B) along K inside the 128 B swizzle row: +2 in 16-byte units
+          WgmmaE4m3<BN>::ss(acc, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        if (kb > 0) {
+          wgmma_wait<1>();
+          if (lane == 0) mbar_arrive(&empty_bar[(ring - 1) % stages]);
+        }
+      }
+      wgmma_wait<0>();
+      fence_regs(acc);
+      if (lane == 0) mbar_arrive(&empty_bar[(ring - 1) % stages]);
+
+      __half* out_row = reinterpret_cast<__half*>(p.out) + static_cast<long long>(m) * p.ld_out;
+      const uint64_t sa2 = f2_pack(sa, sa);
+#pragma unroll
+      for (int pc = 0; pc < BN / 64; ++pc) {
+        __syncwarp();
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int a0 = 4 * (8 * pc + j), col = 8 * j + 2 * t4;
+          *reinterpret_cast<float2*>(stg + g * STG_LD + col) = make_float2(acc[a0], acc[a0 + 1]);
+          *reinterpret_cast<float2*>(stg + (g + 8) * STG_LD + col) = make_float2(acc[a0 + 2], acc[a0 + 3]);
+        }
+        __syncwarp();
+#pragma unroll 1
+        for (int i = 0; i < 2; ++i) {
+          const int c = 4 * pc + 2 * chalf + i;
+          const int n = n0 + c * 16, nrem = p.N - n;
+          if (!valid || nrem <= 0) continue;
+          const float* src = stg + (lane >> 1) * STG_LD + (2 * chalf + i) * 16;
+          const float* sw = s_vec + n;
+          const float* sb = s_vec + npad + n;
+          uint64_t w[8];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const float4 f = lds128(src + 4 * q), w4 = lds128(sw + 4 * q), b4 = lds128(sb + 4 * q);
+            w[2 * q] = f2_fma(f2_mul(sa2, f2_pack(w4.x, w4.y)), f2_pack(f.x, f.y), f2_pack(b4.x, b4.y));
+            w[2 * q + 1] = f2_fma(f2_mul(sa2, f2_pack(w4.z, w4.w)), f2_pack(f.z, f.w), f2_pack(b4.z, b4.w));
+          }
+          if (GELU) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) w[j] = gelu_erf2(w[j]);
+          }
+          __half* op = out_row + n;
+          if (nrem >= 16 && (reinterpret_cast<uintptr_t>(op) & 31) == 0) {
+            U8 o;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              float a, b;
+              f2_unpack(w[j], a, b);
+              o.v[j] = Cvt<__half>::pack(a, b);
+            }
+            stg256(op, o);
+          } else {
+            for (int j = 0; j < 8; ++j) {
+              float a, b;
+              f2_unpack(w[j], a, b);
+              if (2 * j < nrem) op[2 * j] = __float2half_rn(a);
+              if (2 * j + 1 < nrem) op[2 * j + 1] = __float2half_rn(b);
+            }
+          }
+        }
+      }
+    }
+  }
+}
+
+
 // ------------------------------------------------------------------------------------------- host
 static int encode(CUtensorMap* tm, int dtype, int rank, const void* base, const cuuint64_t* dims,
                   const cuuint64_t* strides_bytes, const cuuint32_t* box, std::string* err) {
@@ -515,6 +669,7 @@ static int pick_bn(int N, int m_tiles) {
 
 int gemm_build(const GemmDesc& d, GemmOp* op, std::string* err) {
   std::memset(op, 0, sizeof(*op));
+  if (d.dtype != DT_F16 && d.dtype != DT_BF16) { *err = "gemm: dtype must be fp16 or bf16"; return -1; }
   if (d.K % BK != 0 || d.K <= 0) { *err = "gemm: K must be a positive multiple of 64"; return -1; }
   if (!d.out_fp32 && (d.ld_out % 8) != 0) { *err = "gemm: 16-bit ld_out must be a multiple of 8"; return -1; }
   if ((d.lda % 8) != 0) { *err = "gemm: lda must be a multiple of 8"; return -1; }
@@ -647,7 +802,67 @@ static int launch_ep(const GemmOp& op, cudaStream_t st) {
   }
 }
 
+int gemm_e4m3_build(const GemmE4m3Desc& d, GemmOp* op, std::string* err) {
+  std::memset(op, 0, sizeof(*op));
+  if (!d.A || !d.W || !d.a_scale || !d.w_scale || !d.out) { *err = "gemm_e4m3: null pointer"; return -1; }
+  if (d.M < 1 || d.N < 1 || d.K <= 0 || d.K % 64 != 0) { *err = "gemm_e4m3: M, N must be positive and K a positive multiple of 64"; return -1; }
+  if (d.lda < d.K || d.lda % 16 != 0) { *err = "gemm_e4m3: lda must be >= K and a multiple of 16 bytes"; return -1; }
+  if (d.ld_out < d.N || d.ld_out % 8 != 0) { *err = "gemm_e4m3: ld_out must be >= N and a multiple of 8"; return -1; }
+  if (d.act != ACT_NONE && d.act != ACT_GELU) { *err = "gemm_e4m3: act must be NONE or GELU"; return -1; }
+  GemmArgs& a = op->args;
+  a.M = d.M; a.N = d.N; a.kblocks = (d.K + BK8 - 1) / BK8; a.a_mode = AMODE_PLAIN; a.lda = d.lda;
+  a.bias = d.bias; a.act = d.act; a.out = d.out; a.ld_out = d.ld_out;
+  a.a_scale = d.a_scale; a.w_scale = d.w_scale;
+  op->dtype = DT_E4M3;
+  const int m_tiles = (d.M + BM - 1) / BM;
+  {
+    const cuuint64_t dims[2] = {static_cast<cuuint64_t>(d.K), static_cast<cuuint64_t>(d.M)};
+    const cuuint64_t strides[1] = {static_cast<cuuint64_t>(d.lda)};
+    const cuuint32_t box[2] = {BK8, BM};
+    if (encode(&op->ta, DT_E4M3, 2, d.A, dims, strides, box, err)) return -1;
+  }
+  const int bn = pick_bn(d.N, m_tiles);
+  op->bn = bn;
+  a.n_tiles = (d.N + bn - 1) / bn;
+  {
+    const cuuint64_t dims[2] = {static_cast<cuuint64_t>(d.K), static_cast<cuuint64_t>(d.N)};
+    const cuuint64_t strides[1] = {static_cast<cuuint64_t>(d.K)};
+    const cuuint32_t box[2] = {BK8, static_cast<cuuint32_t>(bn)};
+    if (encode(&op->tb, DT_E4M3, 2, d.W, dims, strides, box, err)) return -1;
+  }
+  const int stage_bytes = A8_STAGE_BYTES + bn * BK8;
+  const size_t vec_bytes = 2 * 4 * static_cast<size_t>(a.n_tiles) * bn;     // w_scale | bias for all n-tiles
+  int stages = static_cast<int>((225 * 1024 - STG_BYTES - vec_bytes) / stage_bytes);
+  stages = std::min(stages, MAX_STAGES);
+  stages = std::max(2, std::min(stages, std::max(2, 2 * a.kblocks)));
+  a.stages = stages;
+  a.m_tiles = m_tiles;
+  op->smem = 1024 + static_cast<size_t>(stages) * stage_bytes + 256 + STG_BYTES + vec_bytes;
+  op->grid = static_cast<unsigned>(std::min<long long>(static_cast<long long>(m_tiles) * a.n_tiles, num_sms()));
+  op->flops = 2.0 * d.M * static_cast<double>(d.N) * d.K;
+  return 0;
+}
+
+template <int BN, bool GELU>
+static int launch_e4m3(const GemmOp& op, cudaStream_t st) {
+  if (int e = ensure_max_dyn_smem(reinterpret_cast<const void*>(gemm_e4m3_kernel<BN, GELU>), 227 * 1024)) return e;
+  launch_k(gemm_e4m3_kernel<BN, GELU>, dim3(op.grid), dim3(GEMM_THREADS), op.smem, st, op.ta, op.tb, op.args);
+  return static_cast<int>(cudaGetLastError());
+}
+
+static int gemm_e4m3_launch(const GemmOp& op, cudaStream_t st) {
+  const bool gelu = op.args.act == ACT_GELU;
+  switch (op.bn) {
+    case 64: return gelu ? launch_e4m3<64, true>(op, st) : launch_e4m3<64, false>(op, st);
+    case 128: return gelu ? launch_e4m3<128, true>(op, st) : launch_e4m3<128, false>(op, st);
+    case 192: return gelu ? launch_e4m3<192, true>(op, st) : launch_e4m3<192, false>(op, st);
+    case 256: return gelu ? launch_e4m3<256, true>(op, st) : launch_e4m3<256, false>(op, st);
+    default: return -1;
+  }
+}
+
 int gemm_launch(const GemmOp& op, cudaStream_t st) {
+  if (op.dtype == DT_E4M3) return gemm_e4m3_launch(op, st);
 #define LWB_BN_SWITCH(T)                                     \
   switch (op.bn) {                                           \
     case 64: return launch_ep<T, 64>(op, st);                \

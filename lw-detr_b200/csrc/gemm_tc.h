@@ -10,7 +10,7 @@
 
 namespace lwb {
 
-enum : int { DT_F16 = 0, DT_BF16 = 1 };
+enum : int { DT_F16 = 0, DT_BF16 = 1, DT_E4M3 = 2 };   // DT_E4M3: 1-byte e4m3 operands (gemm_e4m3_build), fp16 out
 enum : int { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2, ACT_SILU = 3 };
 enum : int { AMODE_PLAIN = 0, AMODE_CONV3_S1 = 1, AMODE_CONV3_S2 = 2 };
 enum : int { ROWS_PLAIN = 0, ROWS_WINDOW_MAJOR = 1 };
@@ -49,6 +49,9 @@ struct GemmArgs {
   int stats_parts_in;
   const float* colsum;      // [N] fp32 (consumer)
   float ln_inv_c, ln_eps;   // 1/C of the normalised dimension, epsilon
+  // e4m3 GEMM only: out = a_scale[m] * w_scale[n] * acc + bias[n]
+  const float* a_scale;     // [M] fp32
+  const float* w_scale;     // [N] fp32
 };
 
 // Host description of one GEMM.
@@ -91,5 +94,23 @@ struct GemmOp {
 // Returns 0 on success; on failure fills *err.
 int gemm_build(const GemmDesc& d, GemmOp* op, std::string* err);
 int gemm_launch(const GemmOp& op, cudaStream_t stream);
+
+// FP8 GEMM (gemm_e4m3_kernel): out[m, n] = act(a_scale[m] * w_scale[n] * sum_k A[m, k] W[n, k] + bias[n]) in fp16, A [M, lda]
+// and W [N, K] e4m3 codes (both K-major), fp32 accumulation on the tensor cores.  act: ACT_NONE or ACT_GELU (the fc1
+// epilogue's GELU).  K % 64 == 0; the last 128-wide k-block may be half empty (TMA fills it with zeros).
+struct GemmE4m3Desc {
+  const void* A = nullptr;
+  int lda = 0;                          // bytes (= elements), multiple of 16
+  const float* a_scale = nullptr;       // [M]
+  int M = 0, N = 0, K = 0;
+  const void* W = nullptr;              // [N, K]
+  const float* w_scale = nullptr;       // [N]
+  const float* bias = nullptr;          // [N] or null
+  int act = ACT_NONE;
+  void* out = nullptr;                  // fp16 [M, ld_out]
+  int ld_out = 0;
+};
+// Fills *op for gemm_launch (op->dtype = DT_E4M3).
+int gemm_e4m3_build(const GemmE4m3Desc& d, GemmOp* op, std::string* err);
 
 }  // namespace lwb

@@ -191,6 +191,101 @@ int layernorm_launch(int dtype, const LayerNormArgs& a, cudaStream_t st) {
   return dtype == DT_BF16 ? ln_dispatch<__nv_bfloat16>(a, st) : ln_dispatch<__half>(a, st);
 }
 
+// ----------------------------------------------------------------------------------- LayerNorm -> e4m3
+// The e4m3 mode's LayerNorm in front of qkv / fc1: per row x^ = (x - mean) * rstd in fp32 with the affine NOT applied (it is
+// folded into the e4m3 weights at load), a = max|x^|, q = e4m3(x^ * (448 / a)) (round to nearest even, saturating) and
+// row_scale = a / 448 (a = 0: both factors 1).  One warp per row, row in registers.  The row is summed SHIFTED by its first
+// value (x - x0 is exact in fp32 for 16-bit x), so a row whose mean is large against its spread keeps its x^ accurate.
+template <int CHUNKS>
+__global__ void __launch_bounds__(256) layernorm_e4m3_kernel(const void* __restrict__ xp, int ldx, long long rows, int C, float eps,
+                                                             uint8_t* __restrict__ q, int ldq, float* __restrict__ row_scale) {
+  pdl_sync();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long row = static_cast<long long>(blockIdx.x) * 8 + warp;
+  if (row >= rows) return;
+  const int nchunk = C >> 3;
+  const __half* x = reinterpret_cast<const __half*>(xp) + row * ldx;
+  const float x0 = __half2float(x[0]);
+  float v[CHUNKS][8];
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < CHUNKS; ++i) {
+    const int c = lane + i * 32;
+    if (c < nchunk) {
+      const U4 u = *reinterpret_cast<const U4*>(x + c * 8);
+      const uint32_t w4[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 f = Cvt<__half>::unpack(w4[j]);
+        v[i][2 * j] = f.x - x0;
+        v[i][2 * j + 1] = f.y - x0;
+      }
+#pragma unroll
+      for (int j = 0; j < 8; ++j) s += v[i][j];
+    } else {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[i][j] = 0.f;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  const float dm = s / C;                      // mean - x0
+  float m2 = 0.f;
+#pragma unroll
+  for (int i = 0; i < CHUNKS; ++i)
+    if (lane + i * 32 < nchunk) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        v[i][j] -= dm;
+        m2 = fmaf(v[i][j], v[i][j], m2);
+      }
+    }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m2 += __shfl_xor_sync(0xffffffffu, m2, o);
+  const float rstd = 1.f / sqrtf(m2 / C + eps);
+  float amax = 0.f;
+#pragma unroll
+  for (int i = 0; i < CHUNKS; ++i)
+    if (lane + i * 32 < nchunk) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        v[i][j] *= rstd;
+        amax = fmaxf(amax, fabsf(v[i][j]));
+      }
+    }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  const float inv = amax > 0.f ? 448.f / amax : 1.f;
+  if (lane == 0) row_scale[row] = amax > 0.f ? amax / 448.f : 1.f;
+  uint8_t* qrow = q + row * ldq;
+#pragma unroll
+  for (int i = 0; i < CHUNKS; ++i) {
+    const int c = lane + i * 32;
+    if (c < nchunk) {
+      uint32_t w2[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        uint16_t lo, hi;
+        asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(lo) : "f"(v[i][4 * h + 1] * inv), "f"(v[i][4 * h] * inv));
+        asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(hi) : "f"(v[i][4 * h + 3] * inv), "f"(v[i][4 * h + 2] * inv));
+        w2[h] = static_cast<uint32_t>(lo) | (static_cast<uint32_t>(hi) << 16);
+      }
+      *reinterpret_cast<uint2*>(qrow + c * 8) = make_uint2(w2[0], w2[1]);
+    }
+  }
+}
+
+int layernorm_e4m3_launch(const void* x, int ldx, long long rows, int C, float eps, uint8_t* q, int ldq, float* row_scale, cudaStream_t st) {
+  if (C % 8 != 0 || C < 8 || C > 1024 || ldx % 8 != 0 || ldq % 8 != 0 || ldx < C || ldq < C || rows < 1) return -2;
+  const int chunks = (C + 255) / 256;
+  const dim3 grid(static_cast<unsigned>((rows + 7) / 8));
+  if (chunks == 1) launch_k(layernorm_e4m3_kernel<1>, grid, dim3(256), 0, st, x, ldx, rows, C, eps, q, ldq, row_scale);
+  else if (chunks == 2) launch_k(layernorm_e4m3_kernel<2>, grid, dim3(256), 0, st, x, ldx, rows, C, eps, q, ldq, row_scale);
+  else if (chunks == 3) launch_k(layernorm_e4m3_kernel<3>, grid, dim3(256), 0, st, x, ldx, rows, C, eps, q, ldq, row_scale);
+  else launch_k(layernorm_e4m3_kernel<4>, grid, dim3(256), 0, st, x, ldx, rows, C, eps, q, ldq, row_scale);
+  return static_cast<int>(cudaGetLastError());
+}
+
 // ----------------------------------------------------------------------------------- patch gather
 // Image [B,3,H,W] (fp32 or 16-bit, NCHW) -> A [B*GH*GW, 3*256] 16-bit with rows in WINDOW-MAJOR token
 // order and k = c*256 + py*16 + px, so that the 16x16/s16 patch-embedding conv (vit.py:79-83)

@@ -19,6 +19,9 @@ struct LayerNormArgs {
   const float* w3; const float* b3; float eps3; void* y3; int ldy3;
 };
 int layernorm_launch(int dtype, const LayerNormArgs& a, cudaStream_t st);
+// the e4m3 mode's LayerNorm (rowops.cu layernorm_e4m3_kernel): fp16 rows [rows, C] -> e4m3 codes [rows, ldq] + fp32
+// row_scale [rows]; C % 8 == 0, C <= 1024, ldx / ldq multiples of 8.  -2: bad sizes
+int layernorm_e4m3_launch(const void* x, int ldx, long long rows, int C, float eps, uint8_t* q, int ldq, float* row_scale, cudaStream_t st);
 
 // image [B,3,H,W] -> window-major patch matrix [B*(H/16)*(W/16), 768]; H, W multiples of 64
 int patch_gather_launch(int dtype, const void* img, int img_is_fp32, void* A, int B, int H, int W, cudaStream_t st);

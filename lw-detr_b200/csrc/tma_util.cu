@@ -74,7 +74,9 @@ int tma_encode(CUtensorMap* tm, int dtype, int rank, const void* base, const cuu
   }
   cuuint32_t estr[5] = {1, 1, 1, 1, 1};
   const CUtensorMapSwizzle swz = swizzle_bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : (swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B);
-  CUresult r = fn(tm, dtype == DT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
+  const CUtensorMapDataType dt = dtype == DT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                 : (dtype == DT_E4M3 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+  CUresult r = fn(tm, dt,
                   static_cast<cuuint32_t>(rank), const_cast<void*>(base), dims, strides_bytes, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

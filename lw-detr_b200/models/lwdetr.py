@@ -19,7 +19,7 @@ from .backbone import build_backbone
 
 
 def _default_dtype():
-    return {"bf16": torch.bfloat16, "fp16": torch.float16}[os.environ.get("LWDETR_B200_DTYPE", "fp16")]
+    return {"bf16": torch.bfloat16, "fp16": torch.float16, "fp8": torch.float8_e4m3fn}[os.environ.get("LWDETR_B200_DTYPE", "fp16")]
 
 
 class LWDETR(nn.Module):
@@ -32,7 +32,9 @@ class LWDETR(nn.Module):
         self.two_stage = True
         self.bbox_reparam = True
         self.lite_refpoint_refine = True
-        self.compute_dtype = compute_dtype       # None: parameters' 16-bit dtype, else LWDETR_B200_DTYPE / fp16
+        # None: parameters' 16-bit dtype, else LWDETR_B200_DTYPE / fp16; torch.float8_e4m3fn: the fp16 engine with the
+        # encoder's qkv / fc1 GEMMs in e4m3 (capi.Engine)
+        self.compute_dtype = compute_dtype
         self.assume_frozen = False               # True: skip the per-forward weight-change check
         entries = [e for e in param_spec(cfg) if not e.name.startswith("backbone.0.")]
         attach_entries(self, entries)

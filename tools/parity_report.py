@@ -26,14 +26,16 @@ def rel_l2(a, b):
     return ((a - b).norm() / (b.norm() + 1e-12)).item()
 
 
-def ladder(name, batch, dtype, wseed=1, iseed=0, eng=None, hw=None):
-    """hw: (height, width) of the synthetic input, default the config's img_size square."""
+def ladder(name, batch, dtype, wseed=1, iseed=0, eng=None, hw=None, oracle=None):
+    """hw: (height, width) of the synthetic input, default the config's img_size square.  oracle: the CPU forward to compare
+    against, with oracle_hw.forward's signature (default: oracle_hw.forward, the fp32 oracle; tools/oracle_fp8.forward for
+    the e4m3 mode's own scheme)."""
     cfg = CONFIGS[name]
     H, W = (cfg.img_size, cfg.img_size) if hw is None else (int(hw[0]), int(hw[1]))
     sd = synth_state_dict(cfg, wseed)
     x = synth_images(batch, iseed, (H, W))
     inter = {}
-    ref = oracle_hw.forward(sd, cfg, x, inter=inter)     # = orc.forward at the configured size
+    ref = (oracle_hw.forward if oracle is None else oracle)(sd, cfg, x, inter=inter)     # oracle_hw = orc.forward at the configured size
     own = eng is None
     if own:
         eng = capi.Engine(cfg, dtype)

@@ -10,7 +10,7 @@ import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-COLS = ["HGMMA", "UTMALDG", "UBLKCP", "HMMA", "MUFU.EX2", "LDGSTS", "LDSM", "SYNCS"]
+COLS = ["HGMMA", "UTMALDG", "UBLKCP", "HMMA", "MUFU.EX2", "LDGSTS", "LDSM", "SYNCS", "QGMMA"]
 
 
 def main(lib):
@@ -38,7 +38,7 @@ def main(lib):
                 counts[cur][c] += 1
     print("# cuobjdump -sass %s (sm_90a): per-kernel counts of the SASS mnemonics that prove the path" % os.path.relpath(lib, ROOT))
     print("# HGMMA = wgmma.mma_async, UTMALDG = TMA tensor load, UBLKCP = cp.async.bulk (1-D bulk copy), HMMA = mma.sync,")
-    print("# LDGSTS = cp.async, LDSM = ldmatrix, SYNCS = mbarrier operations")
+    print("# LDGSTS = cp.async, LDSM = ldmatrix, SYNCS = mbarrier operations, QGMMA = FP8 wgmma.mma_async")
     w = max(len(n) for n in order) + 2
     print("%-*s" % (w, "kernel") + "".join("%11s" % c for c in COLS))
     for n in sorted(order):
