@@ -149,6 +149,17 @@ LWDETR_API int lwdetr_layernorm_e4m3(const void* x, int ldx, int64_t rows, int C
                                      void* stream);
 LWDETR_API int lwdetr_gemm_e4m3(const void* A, int lda, const float* a_scale, int M, int K, const void* W, const float* w_scale, int N,
                                 const float* bias, int act, void* out, int ld_out, void* stream);
+/* The fused ViT MLP of the 192-wide encoder (tiny, small), one kernel in place of the LayerNorm-fused fc1 GEMM and the fc2 GEMM:
+ *   h   = round16(gelu(rstd*(x W1^T) - rstd*mean*colsum1 + b1))    [M, 768], kept on chip
+ *   out = x + gamma * (h W2^T + b2)                                 [M, 192]
+ * dtype LWDETR_F16 / LWDETR_BF16.  x 16-bit [M, ldx] (the raw residual rows, C = 192); stats_in fp32 pairs [M, stats_parts]
+ * with each row's LayerNorm partials (sum, M2) over equal slices of the 192 columns (stats_parts divides 192); W1 16-bit
+ * [768, 192] (the LayerNorm affine folded in), colsum1 / b1 fp32 [768]; W2 16-bit [192, 768], b2 / gamma fp32 [192] or NULL;
+ * out 16-bit [M, ld_out]; stats_out fp32 pairs [M, stats_parts_out] (2 or 6) or NULL: the partials of the rounded output
+ * rows.  ldx and ld_out multiples of 16, x and out 32-byte aligned.  Bit-identical to the two GEMMs it replaces. */
+LWDETR_API int lwdetr_vit_mlp(int dtype, const void* x, int ldx, int M, const float* stats_in, int stats_parts, float eps,
+                              const void* W1, const float* colsum1, const float* b1, const void* W2, const float* b2,
+                              const float* gamma, void* out, int ld_out, float* stats_out, int stats_parts_out, void* stream);
 /* Host helper (no GPU): the weight quantiser lwdetr_load_weights uses in the LWDETR_F16_E4M3 mode.  Per row r of src
  * fp32 [rows, K]: scale[r] = max_k |src[r,k]| / 448 (0 -> 1) and q[r,k] = e4m3(src[r,k] * 448 / max_k |src[r,k]|) as a
  * uint8 code (round to nearest even, saturating to +-448). */

@@ -30,6 +30,7 @@ _SIGNATURES = {
     "lwdetr_postprocess": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_layernorm_e4m3": (_i, [_vp, _i, _i64, _i, _f, _vp, _i, _vp, _vp]),
     "lwdetr_gemm_e4m3": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _i, _vp]),
+    "lwdetr_vit_mlp": (_i, [_i, _vp, _i, _i, _vp, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp]),
     "lwdetr_host_quant_e4m3_rows": (_i, [_vp, _i64, _i, _vp, _vp]),
     "lwdetr_host_bicubic": (_i, [_vp, _i, _i, _i, _vp]),
     "lwdetr_host_bicubic_hw": (_i, [_vp, _i, _i, _i, _i, _vp]),
@@ -272,6 +273,22 @@ def gemm_e4m3(A, a_scale, W, w_scale, bias=None, act=ACT_NONE, out=None):
         out = torch.empty(M, N, device=A.device, dtype=torch.float16)
     check(lib().lwdetr_gemm_e4m3(ptr(A), A.stride(0), ptr(a_scale), M, K, ptr(W), ptr(w_scale), N, ptr(bias), act, ptr(out),
                                  out.stride(0), stream_ptr(A.device)), "lwdetr_gemm_e4m3")
+    return out
+
+
+def vit_mlp(x, stats_in, W1, colsum1, b1, W2, b2=None, gamma=None, eps=1e-6, out=None, stats_out=None):
+    """Fused ViT MLP of the 192-wide encoder (lwdetr_vit_mlp): out = x + gamma * (round16(gelu(LN-fold(x W1^T) + b1)) W2^T + b2).
+    x 16-bit [M, 192] (row stride a multiple of 16), stats_in fp32 [M, parts, 2] LayerNorm partials, W1 [768, 192] and W2
+    [192, 768] contiguous in x's dtype, colsum1 / b1 / b2 / gamma fp32; out [M, 192] (any row stride that is a multiple of
+    16) and stats_out fp32 [M, 2 or 6, 2] optional."""
+    import torch
+    M = x.shape[0]
+    if out is None:
+        out = torch.empty(M, 192, device=x.device, dtype=x.dtype)
+    parts_out = 0 if stats_out is None else stats_out.shape[1]
+    check(lib().lwdetr_vit_mlp(kernel_dtype_code(x.dtype), ptr(x), x.stride(0), M, ptr(stats_in), stats_in.shape[1], float(eps),
+                               ptr(W1), ptr(colsum1), ptr(b1), ptr(W2), ptr(b2), ptr(gamma), ptr(out), out.stride(0),
+                               ptr(stats_out), parts_out, stream_ptr(x.device)), "lwdetr_vit_mlp")
     return out
 
 

@@ -186,6 +186,22 @@ int lwdetr_gemm_e4m3(const void* A, int lda, const float* a_scale, int M, int K,
   return 0;
 }
 
+int lwdetr_vit_mlp(int dtype, const void* x, int ldx, int M, const float* stats_in, int stats_parts, float eps,
+                   const void* W1, const float* colsum1, const float* b1, const void* W2, const float* b2,
+                   const float* gamma, void* out, int ld_out, float* stats_out, int stats_parts_out, void* stream) {
+  lwb::MlpDesc d;
+  d.dtype = dtype; d.x = x; d.ldx = ldx; d.M = M;
+  d.stats_in = reinterpret_cast<const float2*>(stats_in); d.stats_parts_in = stats_parts; d.ln_eps = eps;
+  d.w1 = W1; d.colsum1 = colsum1; d.b1 = b1; d.w2 = W2; d.b2 = b2; d.gamma = gamma;
+  d.out = out; d.ld_out = ld_out; d.stats_out = reinterpret_cast<float2*>(stats_out); d.stats_parts_out = stats_parts_out;
+  lwb::MlpOp op;
+  std::string err;
+  if (lwb::vit_mlp_build(d, &op, &err)) return fail("lwdetr_vit_mlp: " + err);
+  int e = lwb::vit_mlp_launch(op, static_cast<cudaStream_t>(stream));
+  if (e) return cuda_fail(e, "lwdetr_vit_mlp launch");
+  return 0;
+}
+
 int lwdetr_host_quant_e4m3_rows(const float* src, int64_t rows, int K, uint8_t* q, float* scale) {
   if (!src || !q || !scale || rows < 0 || K < 1) return fail("lwdetr_host_quant_e4m3_rows: bad arguments");
   lwb::host_quant_e4m3_rows(src, rows, K, q, scale);

@@ -636,7 +636,11 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
     Mat a0 = buf16(BT, 768);
     Mat xa = buf16(BT, C), xb = buf16(BT, C), xm = buf16(BT, C), lnb = buf16(BT, C);
     Mat tapbuf = buf16(BT, ntap * C);
-    Mat qkv = buf16(BT, 3 * C), att = buf16(BT, C), hid = buf16(BT, 4 * C);
+    // the 192-wide encoder (tiny, small) runs each block's LN2 -> fc1 -> GELU -> fc2 as one kernel (mlp.cu): no hidden buffer.
+    // Only when its 128-row tiles cover every SM: below that (batch 1 - 10 at 640x640) the two GEMMs, whose narrower n-tiles
+    // spread the work over more SMs, are faster.  Both paths give the same bits.
+    const bool fused_mlp = fuse_ln_ != 0 && !e4m3_ && C == MLP_C && (BT + 127) / 128 >= current_device_sms();
+    Mat qkv = buf16(BT, 3 * C), att = buf16(BT, C), hid = fused_mlp ? Mat{nullptr, 4 * C} : buf16(BT, 4 * C);
     {
       void* a0p = a0.p;
       add_op("patch_gather", [this, a0p, B, IH, IW, dt](cudaStream_t st) {
@@ -679,6 +683,27 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
       P_.bytes = 1.0 * (static_cast<double>(BT) * C + static_cast<double>(N) * C) + 4.0 * BT + 8.0 * N + 2.0 * BT * N;   // 1-byte operands
       ops_.push_back(P_);
     };
+    // fused MLP (vit_mlp_kernel): LN2 statistics from stats_m, folded fc1, GELU, fc2, layer-scale and residual; writes the next
+    // block's LayerNorm partials in the layout the fc2 GEMM would have used (stats_parts per row)
+    auto add_mlp = [&](const std::string& label, Mat x, const std::string& k, float2* st_out, Mat out) {
+      if (pass == 0) return;
+      MlpDesc g;
+      g.dtype = dtype_; g.x = x.p; g.ldx = x.ld; g.M = static_cast<int>(BT);
+      g.stats_in = stats_m; g.stats_parts_in = stats_parts; g.ln_eps = 1e-6f;
+      g.w1 = w16(k + "fc1_ln.w"); g.colsum1 = w32(k + "fc1_ln.cs"); g.b1 = w32(k + "fc1_ln.b");
+      g.w2 = w16(k + "fc2.w"); g.b2 = w32(k + "fc2.b"); g.gamma = w32(k + "g2");
+      g.out = out.p; g.ld_out = out.ld; g.stats_out = st_out; g.stats_parts_out = stats_parts;
+      MlpOp op;
+      std::string e;
+      if (fail || vit_mlp_build(g, &op, &e)) { if (!fail) *err = label + ": " + e; fail = true; return; }
+      Op P_;
+      P_.label = label;
+      P_.run = [op](cudaStream_t st) { return vit_mlp_launch(op, st); };
+      P_.out = out.p; P_.rows = BT; P_.cols = C; P_.ld = out.ld;
+      P_.flops = op.flops;
+      P_.bytes = 2.0 * 3.0 * BT * C + 2.0 * 2.0 * (4.0 * C) * C;   // x (operand and residual), out, both weights
+      ops_.push_back(P_);
+    };
     Mat xcur = xa;
     void* pos_tab = own_pos ? salloc(pos_host.size() * 2) : nullptr;
     if (own_pos && pass == 1 && cudaMemcpy(pos_tab, pos_host.data(), pos_host.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) {
@@ -708,7 +733,9 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
                window ? 16 * B : B, window ? T / 16 : T, heads, C / heads);
       { GemmOpt o; o.gamma = pass ? w32(k + "g1") : nullptr; o.resid = xcur; if (fuse) o.stats_out = stats_m;
         add_gemm(lb + ".proj", att, BT, C, k + "proj", C, xm.p, xm.ld, o); }
-      if (e4m3_) {
+      if (fused_mlp) {
+        // fc1 + fc2 in one op under the fc2 label (block taps and captures stay where they were)
+      } else if (e4m3_) {
         add_ln_e4m3(lb + ".ln2", xm);
         add_gemm_e4m3(lb + ".fc1", k + "fc1_q", 4 * C, ACT_GELU, hid);
       } else if (fuse) {
@@ -723,8 +750,12 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
       for (int t = 0; t < ntap; ++t) is_tap = is_tap || cfg_.taps[t] == i;
       if (is_tap) xnext = col(tapbuf, (tap_slot++) * C);
       else xnext = (xcur.p == xa.p) ? xb : xa;
-      { GemmOpt o; o.gamma = pass ? w32(k + "g2") : nullptr; o.resid = xm; if (fuse && i + 1 < cfg_.vit_depth) o.stats_out = stats_x;
-        add_gemm(lb, hid, BT, 4 * C, k + "fc2", C, xnext.p, xnext.ld, o); }
+      if (fused_mlp) {
+        add_mlp(lb, xm, k, i + 1 < cfg_.vit_depth ? stats_x : nullptr, xnext);
+      } else {
+        GemmOpt o; o.gamma = pass ? w32(k + "g2") : nullptr; o.resid = xm; if (fuse && i + 1 < cfg_.vit_depth) o.stats_out = stats_x;
+        add_gemm(lb, hid, BT, 4 * C, k + "fc2", C, xnext.p, xnext.ld, o);
+      }
       xcur = xnext;
     }
 

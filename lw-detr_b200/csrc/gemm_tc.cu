@@ -13,6 +13,7 @@
 // SURVEY.md appendix B (reference: models/backbone/vit.py:120-140,206-220, projector.py:85-132,
 // transformer.py:27-39,466-517, ops/modules/ms_deform_attn.py:112-143, lwdetr.py:149-159).
 #include "gemm_tc.h"
+#include "epilogue.cuh"
 #include "launch.h"
 #include "ptx.cuh"
 #include "tma_util.h"
@@ -35,46 +36,6 @@ static constexpr int STG_LD = 68;                         // floats per staged a
 static constexpr int STG_BYTES = MMA_WARPS * 16 * STG_LD * 4;
 
 
-// Exact (erf) GELU, nn.GELU() default used by timm's Mlp (vit.py:184).  gelu(x) = x*Phi(x) with
-// Phi(-|x|) = 0.5*erfc(|x|/sqrt2) from Abramowitz-Stegun 7.1.26 (|erf error| <= 1.5e-7):
-//   gelu(x) = max(x, 0) - |x| * [0.5 * poly(t) * exp(-x^2/2)],  t = 1 / (1 + p|x|/sqrt2)
-// 14 instructions incl. 2 MUFU instead of ~30 for erff(); max abs deviation from the erff form 2.2e-7.
-__device__ __forceinline__ float gelu_erf(float x) {
-  const float ax = fabsf(x);
-  float t, e;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t) : "f"(fmaf(0.2316418882f, ax, 1.0f)));       // 0.3275911 / sqrt(2)
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(x * x * -0.72134752044448170f));        // exp(-x^2/2)
-  float p = fmaf(0.5307027145f, t, -0.7265760135f);                                          // 0.5 * A&S coefficients
-  p = fmaf(p, t, 0.7107068705f);
-  p = fmaf(p, t, -0.142248368f);
-  p = fmaf(p, t, 0.127414796f);
-  return fmaf(-ax * t, p * e, fmaxf(x, 0.f));
-}
-
-// The same exact-erf GELU for a PAIR of values (ptx.cuh f2_*), without the MUFU: gelu(x) = x * (0.5 + xc * q(xc^2)), xc = x
-// clamped to [-4.5, 4.5], q a degree-9 polynomial fitted to erf(x/sqrt2) / (2x) (weighted least squares at Chebyshev nodes;
-// fp32 Horner: max |error| 7.4e-5 at |x| ~ 4.46 where gelu ~ 4.46, < 1e-5 for |x| < 3 (tests/test_numerics_cpu.py); beyond the clamp Phi(-4.5) = 3.4e-6
-// multiplies x).  FMA pipe only, where gelu_erf spends two MUFU operations per element.
-__device__ __forceinline__ uint64_t gelu_erf2(uint64_t x2) {
-  float x0, x1;
-  f2_unpack(x2, x0, x1);
-  const uint64_t xc = f2_pack(fminf(fmaxf(x0, -4.5f), 4.5f), fminf(fmaxf(x1, -4.5f), 4.5f));
-  const uint64_t u = f2_mul(xc, xc);
-#define LWB_K2(v) f2_pack(v, v)
-  uint64_t q = f2_fma(LWB_K2(-1.3369040159e-12f), u, LWB_K2(1.6336444415e-10f));
-  q = f2_fma(q, u, LWB_K2(-8.9213697499e-09f));
-  q = f2_fma(q, u, LWB_K2(2.8944761772e-07f));
-  q = f2_fma(q, u, LWB_K2(-6.2733902842e-06f));
-  q = f2_fma(q, u, LWB_K2(9.7063541348e-05f));
-  q = f2_fma(q, u, LWB_K2(-1.1183810776e-03f));
-  q = f2_fma(q, u, LWB_K2(9.8202145566e-03f));
-  q = f2_fma(q, u, LWB_K2(-6.6317755718e-02f));
-  q = f2_fma(q, u, LWB_K2(3.9887377948e-01f));
-  const uint64_t t = f2_fma(xc, q, LWB_K2(0.5f));
-#undef LWB_K2
-  return f2_mul(x2, t);
-}
-
 struct TileCoord {
   int m_tile, n_tile, n0, cb, cy0, cx0;
 };
@@ -95,12 +56,6 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmArgs& p, int tile, in
   return t;
 }
 
-// keeps the compiler from moving uses of the accumulators across the asynchronous MMAs' wait
-template <int N> __device__ __forceinline__ void fence_regs(float (&d)[N]) {
-#pragma unroll
-  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
-}
-
 // EP (epilogue specialisation): EP_GENERIC keeps every feature behind runtime flags; the others compile the
 // features of the hot GEMMs in or out so the per-element instruction count stays minimal:
 //   EP_BIAS      out = acc + bias                     (16-bit out, plain rows, no LN / residual / activation)
@@ -109,12 +64,6 @@ template <int N> __device__ __forceinline__ void fence_regs(float (&d)[N]) {
 //   EP_LN_GELU   out = gelu(LN-fold(acc) + bias)      (fc1)
 //   EP_RESID     out = resid + gamma*(acc + bias), optional row statistics (proj, fc2, patch embed, decoder)
 enum : int { EP_GENERIC = 0, EP_BIAS = 1, EP_BIAS_ACT = 2, EP_LN = 3, EP_LN_GELU = 4, EP_RESID = 5 };
-
-__device__ __forceinline__ float4 lds128(const float* p) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(smem_u32(p)));
-  return v;
-}
 
 template <typename T, int BN, int EP>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
@@ -211,15 +160,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const float part_n = p.stats_parts_in > 0 ? 1.f / (p.ln_inv_c * p.stats_parts_in) : 1.f, part_inv_n = 1.f / part_n;
 
     auto stats_of = [&](long long mrow, float& mean, float& rstd) {
-      float s1 = 0.f, m2 = 0.f;
-      for (int i = 0; i < p.stats_parts_in; ++i) s1 += __ldg(p.stats_in + mrow * p.stats_parts_in + i).x;
-      mean = s1 * p.ln_inv_c;
-      for (int i = 0; i < p.stats_parts_in; ++i) {
-        const float2 q = __ldg(p.stats_in + mrow * p.stats_parts_in + i);
-        const float dm = q.x * part_inv_n - mean;
-        m2 += q.y + part_n * dm * dm;
-      }
-      rstd = rsqrtf(m2 * p.ln_inv_c + p.ln_eps);
+      ln_row_stats(p.stats_in + mrow * p.stats_parts_in, p.stats_parts_in, part_n, part_inv_n, p.ln_inv_c, p.ln_eps, mean, rstd);
     };
     uint32_t ring = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {

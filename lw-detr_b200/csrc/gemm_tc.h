@@ -113,4 +113,57 @@ struct GemmE4m3Desc {
 // Fills *op for gemm_launch (op->dtype = DT_E4M3).
 int gemm_e4m3_build(const GemmE4m3Desc& d, GemmOp* op, std::string* err);
 
+// Fused ViT MLP of the 192-wide encoder (mlp.cu vit_mlp_kernel), the LayerNorm-fused fc1 GEMM and the fc2 GEMM in one kernel:
+//   h = T(gelu(rstd * (x W1'^T) - rstd * mean * colsum1 + b1))        [M, 768], never stored
+//   out = x + gamma * (h W2^T + b2)                                     [M, 192] in the compute dtype T
+// x: the raw residual rows [M, ldx]; (mean, rstd) combined from the row partials stats_in (as the LN-fused GEMMs do); W1' the
+// fc1 weight [768, 192] with the LayerNorm affine folded in, colsum1 its row sums, b1 its folded bias; W2 the fc2 weight
+// [192, 768].  stats_out (optional) receives the LayerNorm partials of the rounded output rows, stats_parts_out = 2 or 6
+// per row, laid out as the fc2 GEMM at BN = 192 or 64 writes them.  The result equals gemm_tc fc1 -> fc2 bit for bit.
+static constexpr int MLP_C = 192;
+struct MlpArgs {
+  int M, m_tiles;
+  const void* x;
+  int ldx;
+  const float2* stats_in;
+  int stats_parts_in;
+  float ln_inv_c, ln_eps;
+  const float* b1;          // [768]
+  const float* colsum1;     // [768]
+  const float* b2;          // [192] or null
+  const float* gamma;       // [192] or null
+  void* out;
+  int ld_out;
+  float2* stats_out;        // [M, stats_parts_out] or null
+  int stats_parts_out;
+};
+struct MlpDesc {
+  int dtype = DT_F16;
+  const void* x = nullptr;
+  int ldx = 0, M = 0;
+  const float2* stats_in = nullptr;
+  int stats_parts_in = 0;
+  float ln_eps = 0.f;
+  const void* w1 = nullptr;
+  const float* colsum1 = nullptr;
+  const float* b1 = nullptr;
+  const void* w2 = nullptr;
+  const float* b2 = nullptr;
+  const float* gamma = nullptr;
+  void* out = nullptr;
+  int ld_out = 0;
+  float2* stats_out = nullptr;
+  int stats_parts_out = 2;
+};
+struct MlpOp {
+  CUtensorMap tx, tw1, tw2;
+  MlpArgs args;
+  int dtype;
+  unsigned grid;
+  size_t smem;
+  double flops;
+};
+int vit_mlp_build(const MlpDesc& d, MlpOp* op, std::string* err);
+int vit_mlp_launch(const MlpOp& op, cudaStream_t stream);
+
 }  // namespace lwb
