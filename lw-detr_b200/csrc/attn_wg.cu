@@ -12,8 +12,9 @@
 //               A warpgroup whose 64 rows lie beyond the sequence (100-token windows use 100 of 128 rows, the last tile
 //               of a 1600-token sequence 64) exits at once.
 //   warp 8    : TMA producer (one elected lane).
-// The kernel keeps no cross-chunk overlap inside a warpgroup; latency is hidden by the second warpgroup and by two to
-// five resident CTAs per SM (20-80 KB of shared memory each).
+// The kernel keeps no cross-chunk overlap inside a warpgroup; latency is hidden by the second warpgroup and by the other
+// resident CTAs of the SM: 3 at head dim 16 (at most 72 registers), 2 at 32 and 64.  The last chunk of a sequence masks the keys
+// beyond its end; one of at most 40 keys (the second chunk of a 100-token window) computes only 5 of the 8 n-tiles.
 #include "attn.h"
 #include "launch.h"
 #include "ptx.cuh"
@@ -40,12 +41,91 @@ __device__ __forceinline__ float ex2(float x) {
   return y;
 }
 
+// Keys [kbase, kbase + 8 NT) of one K / V stage for the warpgroup's 64 query rows: S = Q K^T, online softmax on the
+// fragments, O += P V.
+//   NT   : 8-key n-tiles computed - 8 = the whole stage; 5 = keys 0..39 of it (the second stage of a 100-token window:
+//          no scores, exponentials or P V steps are spent on keys that cannot exist).
+//   MASK : keys at or beyond seqlen become -inf (the sequence's last stage).
+template <typename T, int DH, int NT, bool MASK>
+__device__ __forceinline__ void attend_chunk(uint64_t qdesc, uint64_t kdesc, uint64_t vdesc, int kbase, int seqlen, float c, int t4,
+                                             float (&m_run)[2], float (&lsum)[2], float (&o)[DH / 2]) {
+  constexpr bool BF = Cvt<T>::is_bf16;
+  constexpr uint32_t PITCH = DH * 2;
+  constexpr int NTP = (NT + 1) & ~1;                             // P V runs 16 keys per step
+  float sc[NT * 4];
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < DH / 16; ++kk) Wgmma<BF, NT * 8>::ss(sc, qdesc + 2 * kk, kdesc + 2 * kk, kk != 0 ? 1u : 0u);
+  wgmma_commit();
+  wgmma_wait<0>();
+  fence_regs(sc);
+  if (MASK) {
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+      for (int e = 0; e < 4; ++e)
+        if (kbase + nt * 8 + t4 * 2 + (e & 1) >= seqlen) sc[4 * nt + e] = -INFINITY;
+  }
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int nt = 0; nt < NT; ++nt) {
+    mx[0] = fmaxf(mx[0], fmaxf(sc[4 * nt], sc[4 * nt + 1]));
+    mx[1] = fmaxf(mx[1], fmaxf(sc[4 * nt + 2], sc[4 * nt + 3]));
+  }
+  float alpha[2], msc[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+    mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+    const float m_new = fmaxf(m_run[h], mx[h]);                  // running max of the RAW scores (finite: key kbase is valid)
+    alpha[h] = ex2((m_run[h] - m_new) * c);
+    m_run[h] = m_new;
+    msc[h] = m_new * c;
+    lsum[h] *= alpha[h];
+  }
+  uint32_t pf[NTP / 2][4];                                       // C fragments of n-tiles (2k, 2k+1) form the A fragment of key-step k
+#pragma unroll
+  for (int nt = 0; nt < NTP; ++nt) {
+    if (nt >= NT) {                                              // padding half of the last 16-key step
+      pf[nt >> 1][(nt & 1) * 2 + 0] = 0u;
+      pf[nt >> 1][(nt & 1) * 2 + 1] = 0u;
+      continue;
+    }
+    const float p0 = ex2(fmaf(sc[4 * nt], c, -msc[0])), p1 = ex2(fmaf(sc[4 * nt + 1], c, -msc[0]));
+    const float p2 = ex2(fmaf(sc[4 * nt + 2], c, -msc[1])), p3 = ex2(fmaf(sc[4 * nt + 3], c, -msc[1]));
+    lsum[0] += p0 + p1;
+    lsum[1] += p2 + p3;
+    pf[nt >> 1][(nt & 1) * 2 + 0] = Cvt<T>::pack(p0, p1);
+    pf[nt >> 1][(nt & 1) * 2 + 1] = Cvt<T>::pack(p2, p3);
+  }
+#pragma unroll
+  for (int dt = 0; dt < DH / 8; ++dt) {
+    o[4 * dt] *= alpha[0];
+    o[4 * dt + 1] *= alpha[0];
+    o[4 * dt + 2] *= alpha[1];
+    o[4 * dt + 3] *= alpha[1];
+  }
+  // ---- O += P V: 16 keys per MMA, B advances 16 rows of the MN-major V chunk
+  fence_regs(o);
+  wgmma_fence();
+#pragma unroll
+  for (int kt = 0; kt < NTP / 2; ++kt) Wgmma<BF, DH>::rs_tb(o, pf[kt], vdesc + ((16 * PITCH) >> 4) * kt, 1u);
+  wgmma_commit();
+  wgmma_wait<0>();
+  fence_regs(o);
+}
+
+// Resident CTAs per SM the register budget is cut for.  Each warpgroup runs S -> softmax -> P V one after another, so
+// only the other warpgroups on the SM cover its MMA round trips: at head dim 16 the kernel is cut to 72 registers for 3
+// CTAs (small's global attention: 427 us with 2, 380 us with 3, on an H100 80GB HBM3 at 700 W).  At 32, 72 registers
+// would spill; 64 is held to 2 by shared memory.
+template <int DH> constexpr int kMinCtas = DH == 16 ? 3 : 2;
+
 template <typename T, int DH>
-__global__ void __launch_bounds__(THREADS, 2) attn_wg_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
-                                                              const AttnArgs p, int C) {
+__global__ void __launch_bounds__(THREADS, kMinCtas<DH>) attn_wg_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
+                                                                          const AttnArgs p, int C) {
   constexpr uint32_t PITCH = DH * 2;                           // bytes per row = swizzle span
   constexpr int Q_BYTES = BM * DH * 2, KV_BYTES = BK * DH * 2;
-  constexpr bool BF = Cvt<T>::is_bf16;
   extern __shared__ uint8_t wg_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(wg_smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
@@ -105,63 +185,11 @@ __global__ void __launch_bounds__(THREADS, 2) attn_wg_kernel(const __grid_consta
     mbar_wait(&kv_full[s], (j / STAGES) & 1);
     const uint64_t kdesc = wgmma_desc(smem_u32(sKV + s * 2 * KV_BYTES), PITCH);
     const uint64_t vdesc = wgmma_desc(smem_u32(sKV + s * 2 * KV_BYTES + KV_BYTES), PITCH);
-    float sc[BK / 2];
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < DH / 16; ++kk) Wgmma<BF, BK>::ss(sc, qdesc + 2 * kk, kdesc + 2 * kk, kk != 0 ? 1u : 0u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(sc);
-    // ---- online softmax on the fragments: keys beyond the sequence (next sequence's rows / zero fill) are masked
-    if (j * BK + BK > p.seqlen) {
-#pragma unroll
-      for (int nt = 0; nt < BK / 8; ++nt)
-#pragma unroll
-        for (int e = 0; e < 4; ++e)
-          if (j * BK + nt * 8 + t4 * 2 + (e & 1) >= p.seqlen) sc[4 * nt + e] = -INFINITY;
-    }
-    float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int nt = 0; nt < BK / 8; ++nt) {
-      mx[0] = fmaxf(mx[0], fmaxf(sc[4 * nt], sc[4 * nt + 1]));
-      mx[1] = fmaxf(mx[1], fmaxf(sc[4 * nt + 2], sc[4 * nt + 3]));
-    }
-    float alpha[2], msc[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
-      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
-      const float m_new = fmaxf(m_run[h], mx[h]);              // running max of the RAW scores (finite: key j*BK is valid)
-      alpha[h] = ex2((m_run[h] - m_new) * c);
-      m_run[h] = m_new;
-      msc[h] = m_new * c;
-      lsum[h] *= alpha[h];
-    }
-    uint32_t pf[BK / 16][4];                                     // C fragments of n-tiles (2k, 2k+1) form the A fragment of key-step k
-#pragma unroll
-    for (int nt = 0; nt < BK / 8; ++nt) {
-      const float p0 = ex2(fmaf(sc[4 * nt], c, -msc[0])), p1 = ex2(fmaf(sc[4 * nt + 1], c, -msc[0]));
-      const float p2 = ex2(fmaf(sc[4 * nt + 2], c, -msc[1])), p3 = ex2(fmaf(sc[4 * nt + 3], c, -msc[1]));
-      lsum[0] += p0 + p1;
-      lsum[1] += p2 + p3;
-      pf[nt >> 1][(nt & 1) * 2 + 0] = Cvt<T>::pack(p0, p1);
-      pf[nt >> 1][(nt & 1) * 2 + 1] = Cvt<T>::pack(p2, p3);
-    }
-#pragma unroll
-    for (int dt = 0; dt < DH / 8; ++dt) {
-      o[4 * dt] *= alpha[0];
-      o[4 * dt + 1] *= alpha[0];
-      o[4 * dt + 2] *= alpha[1];
-      o[4 * dt + 3] *= alpha[1];
-    }
-    // ---- O += P V: 16 keys per MMA, B advances 16 rows of the MN-major V chunk
-    fence_regs(o);
-    wgmma_fence();
-#pragma unroll
-    for (int kt = 0; kt < BK / 16; ++kt) Wgmma<BF, DH>::rs_tb(o, pf[kt], vdesc + ((16 * PITCH) >> 4) * kt, 1u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(o);
+    // keys beyond the sequence (the next sequence's rows / zero fill) are masked in the last chunk
+    const int rem = p.seqlen - j * BK;
+    if (rem >= BK) attend_chunk<T, DH, BK / 8, false>(qdesc, kdesc, vdesc, j * BK, p.seqlen, c, t4, m_run, lsum, o);
+    else if (rem <= 40) attend_chunk<T, DH, 5, true>(qdesc, kdesc, vdesc, j * BK, p.seqlen, c, t4, m_run, lsum, o);
+    else attend_chunk<T, DH, BK / 8, true>(qdesc, kdesc, vdesc, j * BK, p.seqlen, c, t4, m_run, lsum, o);
     __syncwarp();
     if (lane == 0) mbar_arrive(&kv_empty[s]);
   }

@@ -9,6 +9,7 @@ import argparse
 import json
 import os
 import statistics
+import subprocess
 import sys
 
 import torch
@@ -24,6 +25,17 @@ from b200.config import CONFIGS  # noqa: E402
 def peaks():
     """H100 SXM data sheet (700 W card): HBM3 GB/s, dense 16-bit TFLOP/s - ceilings, not rates this project reached."""
     return 3350.0, 989.0, "H100 SXM data sheet"
+
+
+def sm_clock_ghz():
+    """SM clock of the current device now (nvidia-smi), in GHz; NaN when it cannot be read.  Read right after a timed
+    kernel, it sets that kernel's MUFU ceiling: 16 ex2 per clock per SM."""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=clocks.sm", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, check=True).stdout
+        return float(out.strip().splitlines()[0]) / 1e3
+    except (OSError, subprocess.CalledProcessError, ValueError, IndexError):
+        return float("nan")
 
 
 FLUSH_MODE = "clean"
@@ -64,6 +76,7 @@ def main():
     FLUSH_MODE = a.flush
     flush = [torch.zeros(64 * 1024 * 1024, device="cuda", dtype=torch.float32) for _ in range(2)]
     res = []
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
     g = torch.Generator(device="cuda").manual_seed(0)
     cases = [("small", 32, torch.float16), ("medium", 64, torch.bfloat16), ("large", 32, torch.float16), ("xlarge", 16, torch.float16)]
     only = set(a.only.split(",")) if a.only else None
@@ -94,13 +107,14 @@ def main():
                 continue
             fn = lambda: capi.attention(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], att, nseq, seqlen, heads, dh, dh ** -0.5)
             med, best = timed(fn, a.iters, flush)
+            clk = sm_clock_ghz()
             algo = B * T * 4 * C * elt
             flops = 4.0 * nseq * seqlen * seqlen * C
             exps = nseq * heads * seqlen * seqlen
             r = {"kernel": kind, "config": "%s B=%d %s dh=%d" % (name, B, str(dt)[6:], dh), "us_median": med, "us_best": best,
                  "algorithmic_MB": algo / 1e6, "achieved_GBps": algo / med / 1e3, "peak_GBps": hbm, "hbm_frac": algo / med / 1e3 / hbm,
                  "gflop": flops / 1e9, "achieved_TFLOPs": flops / med / 1e6, "tensor_frac": flops / med / 1e6 / tflops,
-                 "gexp_per_s": exps / med / 1e3, "exp_frac_of_mufu_peak": exps / med / 1e3 / (16 * 132 * 1.98)}
+                 "gexp_per_s": exps / med / 1e3, "sm_clock_ghz": clk, "exp_frac_of_mufu_peak": exps / med / 1e3 / (16 * sms * clk)}
             r["bound"] = "hbm" if kind == "window_attention" else "tensor (nominal) / exp"
             r["frac"] = r["hbm_frac"] if kind == "window_attention" else r["tensor_frac"]
             res.append(r)
