@@ -275,6 +275,40 @@ LWDETR_API int lwdetr_forward_frames(lwdetr_handle* h, const lwdetr_frame* frame
 LWDETR_API int lwdetr_resize_patches(int dtype, const lwdetr_frame* frames, int B, int height, int width, const float mean[3],
                                      const float std[3], void* A, uint8_t* mask, void* stream);
 
+/* NV12 (YUV 4:2:0) frames, the output of video decoders and camera pipelines: a luma plane of height rows of width bytes,
+ * rows luma_pitch >= width apart, and an interleaved chroma plane of ceil(height/2) rows of ceil(width/2) (U, V) byte pairs,
+ * rows chroma_pitch >= 2 * ceil(width/2) apart.  No pointer or pitch needs any alignment; odd sizes are allowed.
+ * Each source pixel (y, x) is converted to an RGB uint8 triple from Y at (y, x) and the chroma pair at (y >> 1, x >> 1)
+ * (replicated, not filtered), and from there on the frame is exactly an lwdetr_frame of that RGB image: the same resize,
+ * rounding, normalisation, gather, padding and mask.  The conversion is int32 and exact (>> is an arithmetic shift):
+ *   u = U - 128, v = V - 128;  y' = max(Y - 16, 0) * cY (the _LIMITED rows)  or  Y * cY (the _FULL rows)
+ *   R = clamp((y' + cRv * v + 2^19) >> 20, 0, 255)
+ *   G = clamp((y' + cGu * u + cGv * v + 2^19) >> 20, 0, 255)
+ *   B = clamp((y' + cBu * u + 2^19) >> 20, 0, 255)
+ *   colorspace               cY        cRv       cGu       cGv       cBu
+ *   LWDETR_CSC_BT601_LIMITED 1220542   1673527   -409993   -852492   2116026   (bit-identical to OpenCV's COLOR_YUV2RGB_NV12)
+ *   LWDETR_CSC_BT709_LIMITED 1220945   1879825   -223607   -558796   2215014
+ *   LWDETR_CSC_BT601_FULL    1048576   1470104   -360853   -748826   1858077
+ *   LWDETR_CSC_BT709_FULL    1048576   1651297   -196424   -490864   1945738
+ * The first row is OpenCV's 3-decimal table times 2^20; the others are round(2^20 c) of the exact BT.601 / BT.709
+ * coefficients, with 255/219 luma and 255/224 chroma scaling for limited range.  Every row is within one level of the
+ * float64 conversion.  Limits as lwdetr_frame. */
+enum { LWDETR_CSC_BT601_LIMITED = 0, LWDETR_CSC_BT709_LIMITED = 1, LWDETR_CSC_BT601_FULL = 2, LWDETR_CSC_BT709_FULL = 3 };
+typedef struct {
+  const uint8_t* luma;   int64_t luma_pitch;    /* height rows of width bytes */
+  const uint8_t* chroma; int64_t chroma_pitch;  /* ceil(height/2) rows of ceil(width/2) (U, V) byte pairs */
+  int32_t height, width, dst_h, dst_w;
+  int32_t colorspace;                           /* per frame: cameras of one batch may differ */
+} lwdetr_frame_nv12;
+
+/* lwdetr_forward_frames on NV12 frames.  RGB and NV12 batches of one (B, height, width) share the plan and its CUDA graphs. */
+LWDETR_API int lwdetr_forward_frames_nv12(lwdetr_handle* h, const lwdetr_frame_nv12* frames, const float mean[3], const float std[3],
+                                          int B, int height, int width, float* pred_logits, float* pred_boxes,
+                                          const lwdetr_aux_out* aux, const int32_t* topk_override, void* stream);
+/* lwdetr_resize_patches on NV12 frames. */
+LWDETR_API int lwdetr_resize_patches_nv12(int dtype, const lwdetr_frame_nv12* frames, int B, int height, int width,
+                                          const float mean[3], const float std[3], void* A, uint8_t* mask, void* stream);
+
 /* Multi-GPU init (SURVEY.md 8e): ONE ncclBroadcast of the packed weight arena from rank `root`, stream-ordered on
  * `stream`; the only collective of the path (images shard across ranks as independent replicas, nothing on the hot path).
  * Every rank first calls lwdetr_load_weights with tensors of the right shapes (any values on the non-root ranks): that

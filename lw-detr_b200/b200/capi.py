@@ -44,6 +44,8 @@ _SIGNATURES = {
     "lwdetr_forward_hw": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_forward_frames": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_resize_patches": (_i, [_i, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "lwdetr_forward_frames_nv12": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "lwdetr_resize_patches_nv12": (_i, [_i, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_set_option": (_i, [_vp, ctypes.c_char_p, _i]),
     "lwdetr_add_capture": (_i, [_vp, ctypes.c_char_p, _vp, _i64]),
     "lwdetr_capture_result": (_i64, [_vp, _i]),
@@ -374,22 +376,134 @@ def frame_descs(frames, dsts):
     return arr
 
 
+class FrameNV12Struct(ctypes.Structure):
+    _fields_ = [("luma", _vp), ("luma_pitch", ctypes.c_int64), ("chroma", _vp), ("chroma_pitch", ctypes.c_int64),
+                ("height", ctypes.c_int32), ("width", ctypes.c_int32), ("dst_h", ctypes.c_int32), ("dst_w", ctypes.c_int32),
+                ("colorspace", ctypes.c_int32)]
+
+
+# colorspace names of NV12 frames -> LWDETR_CSC_* (include/lwdetr_b200.h): limited (studio) range unless "_full"
+COLORSPACES = {"bt601": 0, "bt709": 1, "bt601_full": 2, "bt709_full": 3}
+
+
+def _is_nv12(f):
+    import torch
+    return isinstance(f, (tuple, list)) or (isinstance(f, torch.Tensor) and f.dim() == 2)
+
+
+def _check_plane(i, name, t, rows, row_bytes, device):
+    import torch
+    if not isinstance(t, torch.Tensor) or t.dtype != torch.uint8 or t.dim() != 2:
+        raise RuntimeError("lwdetr_b200: NV12 frame %d: %s must be a 2-D uint8 tensor, got %s" % (i, name, getattr(t, "dtype", type(t))))
+    if tuple(t.shape) != (rows, row_bytes):
+        raise RuntimeError("lwdetr_b200: NV12 frame %d: %s must be [%d, %d], got %s" % (i, name, rows, row_bytes, tuple(t.shape)))
+    if t.stride(1) != 1 or (rows > 1 and t.stride(0) < row_bytes):
+        raise RuntimeError("lwdetr_b200: NV12 frame %d: %s has strides %s; stride(1) == 1 and stride(0) >= %d are required"
+                           % (i, name, tuple(t.stride()), row_bytes))
+    if t.device.type != "cuda" or (device is not None and t.device != device):
+        raise RuntimeError("lwdetr_b200: NV12 frame %d: %s is on %s; frames must be CUDA tensors%s"
+                           % (i, name, t.device, "" if device is None else " on %s" % (device,)))
+
+
+def nv12_list(frames, device=None):
+    """NV12 frames as a list of (luma [h, w], chroma [ceil(h/2), 2 * ceil(w/2)]) CUDA uint8 pairs (each plane any row stride,
+    stride(1) == 1).  Takes that list, packed NV12 frames [3h/2, w] (h and w even; split into their two planes here) in the
+    list, or one packed [B, 3h/2, w] tensor."""
+    import torch
+    if isinstance(frames, torch.Tensor):
+        frames = list(frames.unbind(0))
+    pairs = []
+    for i, f in enumerate(frames):
+        if isinstance(f, torch.Tensor):
+            rows, w = f.shape
+            h = rows * 2 // 3
+            if rows % 3 or h % 2 or w % 2:
+                raise RuntimeError("lwdetr_b200: packed NV12 frame %d is %s; [3h/2, w] with h and w even is required (odd sizes: pass "
+                                   "the (luma, chroma) planes)" % (i, tuple(f.shape)))
+            f = (f[:h], f[h:])
+        if len(f) != 2:
+            raise RuntimeError("lwdetr_b200: NV12 frame %d must be a (luma, chroma) pair" % i)
+        luma, chroma = f
+        if not isinstance(luma, torch.Tensor) or luma.dim() != 2:
+            raise RuntimeError("lwdetr_b200: NV12 frame %d: luma must be a 2-D uint8 tensor [h, w]" % i)
+        h, w = luma.shape
+        _check_plane(i, "luma", luma, h, w, device)
+        _check_plane(i, "chroma", chroma, (h + 1) // 2, 2 * ((w + 1) // 2), luma.device)
+        pairs.append((luma, chroma))
+    return pairs
+
+
+def colorspace_codes(colorspace, B):
+    """LWDETR_CSC_* code of each of B NV12 frames from one name or one name per frame."""
+    if colorspace is None:
+        raise RuntimeError("lwdetr_b200: NV12 frames need colorspace= (one of %s, or one per frame): there is no safe default, a "
+                           "wrong matrix shifts every colour" % ", ".join(COLORSPACES))
+    names = [colorspace] * B if isinstance(colorspace, str) else list(colorspace)
+    if len(names) != B:
+        raise RuntimeError("lwdetr_b200: %d colorspaces for %d frames" % (len(names), B))
+    for n in names:
+        if n not in COLORSPACES:
+            raise RuntimeError("lwdetr_b200: unknown colorspace %r; one of %s" % (n, ", ".join(COLORSPACES)))
+    return [COLORSPACES[n] for n in names]
+
+
+class Frames:
+    """One batch of raw frames, RGB (frame_list) or NV12 (nv12_list), told apart by their form.  colorspace is required for
+    NV12 frames and rejected for RGB ones.  .sizes: each frame's (h, w); .descs(dsts): the HOST descriptor array of the C ABI."""
+
+    def __init__(self, frames, device=None, colorspace=None):
+        import torch
+        if isinstance(frames, Frames):
+            self.__dict__.update(frames.__dict__)
+            return
+        if isinstance(frames, torch.Tensor):
+            self.nv12 = frames.dim() == 3 and frames.shape[2] != 3      # [B, 3h/2, w]; [h, w, 3] is an RGB frame without its batch axis
+        else:
+            frames = list(frames)
+            kinds = {_is_nv12(f) for f in frames}
+            if len(kinds) > 1:
+                raise RuntimeError("lwdetr_b200: one call takes RGB or NV12 frames, not a mix of both")
+            self.nv12 = kinds == {True}
+        if self.nv12:
+            self.codes = colorspace_codes(colorspace, len(frames))
+            self.items = nv12_list(frames, device)
+            self.sizes = [(y.shape[0], y.shape[1]) for y, _ in self.items]
+        else:
+            if colorspace is not None:
+                raise RuntimeError("lwdetr_b200: colorspace applies to NV12 frames only; these frames are RGB")
+            self.items = frame_list(frames, device)
+            self.sizes = [(f.shape[0], f.shape[1]) for f in self.items]
+        self.device = self.items[0][0].device if self.nv12 else self.items[0].device
+
+    def descs(self, dsts):
+        """ctypes pointer to the HOST array of lwdetr_frame / lwdetr_frame_nv12 for these frames and their (dst_h, dst_w)."""
+        if not self.nv12:
+            return ctypes.cast(frame_descs(self.items, dsts), _vp)
+        arr = (FrameNV12Struct * len(self.items))()
+        self._arr = arr
+        for d, (y, c), cs, (dh, dw) in zip(arr, self.items, self.codes, dsts):
+            d.luma, d.luma_pitch, d.chroma, d.chroma_pitch = y.data_ptr(), y.stride(0), c.data_ptr(), c.stride(0)
+            d.height, d.width, d.dst_h, d.dst_w, d.colorspace = y.shape[0], y.shape[1], int(dh), int(dw), cs
+        return ctypes.cast(arr, _vp)
+
+
 def _norm3(v):
     return (ctypes.c_float * 3)(*[float(x) for x in v])
 
 
-def resize_patches(frames, dsts, size, dtype, mean=None, std=None, want_mask=False):
-    """lwdetr_resize_patches: frames resized to their dsts on an (H, W) = size canvas -> (window-major patch matrix
-    [B*(H/16)*(W/16), 768] in `dtype`, padding mask bool [B, H, W] or None)."""
+def resize_patches(frames, dsts, size, dtype, mean=None, std=None, want_mask=False, colorspace=None):
+    """lwdetr_resize_patches(_nv12): frames (RGB or NV12, see Frames) resized to their dsts on an (H, W) = size canvas ->
+    (window-major patch matrix [B*(H/16)*(W/16), 768] in `dtype`, padding mask bool [B, H, W] or None)."""
     import torch
-    frames = frame_list(frames)
+    fb = Frames(frames, colorspace=colorspace)
     H, W = int(size[0]), int(size[1])
-    dev, B = frames[0].device, len(frames)
+    dev, B = fb.device, len(fb.items)
     mean, std = IMAGENET_MEAN if mean is None else mean, IMAGENET_STD if std is None else std
     A = torch.empty(max(B * (H // 16) * (W // 16), 1), 768, device=dev, dtype=dtype)
     mask = torch.empty(B, H, W, device=dev, dtype=torch.bool) if want_mask else None
-    check(lib().lwdetr_resize_patches(kernel_dtype_code(dtype), ctypes.cast(frame_descs(frames, dsts), _vp), B, H, W, ctypes.cast(_norm3(mean), _vp),
-                                      ctypes.cast(_norm3(std), _vp), ptr(A), ptr(mask), stream_ptr(dev)), "lwdetr_resize_patches")
+    name = "lwdetr_resize_patches_nv12" if fb.nv12 else "lwdetr_resize_patches"
+    check(getattr(lib(), name)(kernel_dtype_code(dtype), fb.descs(dsts), B, H, W, ctypes.cast(_norm3(mean), _vp),
+                               ctypes.cast(_norm3(std), _vp), ptr(A), ptr(mask), stream_ptr(dev)), name)
     return A, mask
 
 
@@ -536,28 +650,34 @@ class Engine:
         return res, logits, boxes, aux
 
     def forward_frames(self, frames, size=None, fit="stretch", short_side=None, max_side=None, want_aux=True, topk_override=None,
-                       mean=IMAGENET_MEAN, std=IMAGENET_STD):
-        """Raw camera / decoder frames of any size: a list of CUDA uint8 [h, w, 3] tensors (each its own size; views with
-        packed RGB pixels are fine) or one [B, h, w, 3] tensor.  Every frame is resized on the device (antialiased bilinear,
-        fused into the patch gather) and normalised with mean / std.  fit="stretch": to `size` = (H, W), default (img_size,
-        img_size).  fit="keep_aspect": to the reference's resize(size=short_side, max_size=max_side), frames top-left on the
-        run size (`size`, or run_size of the largest resized frame), the rest padded with a mask made on the device
-        (b200.config.frame_sizes).  Source sizes are not part of the plan: only a new (B, H, W) re-plans.  Returns the
-        dict of forward(), plus "frame_sizes": the (dst_h, dst_w) of each frame."""
+                       mean=IMAGENET_MEAN, std=IMAGENET_STD, colorspace=None):
+        """Raw camera / decoder frames of any size, RGB or NV12 (told apart by their form):
+          RGB: a list of CUDA uint8 [h, w, 3] tensors (each its own size; views with packed RGB pixels are fine) or one
+            [B, h, w, 3] tensor;
+          NV12: a list of (luma [h, w], chroma [ceil(h/2), 2 * ceil(w/2)]) CUDA uint8 pairs (any row stride), of packed
+            [3h/2, w] tensors (h, w even), or one packed [B, 3h/2, w] tensor; colorspace= "bt601", "bt709", "bt601_full" or
+            "bt709_full" (one, or one per frame) is required, and each pixel is converted to RGB on the device
+            (include/lwdetr_b200.h) as the frame is read.
+        Every frame is resized on the device (antialiased bilinear, fused into the patch gather) and normalised with mean / std.
+        fit="stretch": to `size` = (H, W), default (img_size, img_size).  fit="keep_aspect": to the reference's
+        resize(size=short_side, max_size=max_side), frames top-left on the run size (`size`, or run_size of the largest resized
+        frame), the rest padded with a mask made on the device (b200.config.frame_sizes).  Source sizes and the frame format
+        are not part of the plan: only a new (B, H, W) re-plans.  Returns the dict of forward(), plus "frame_sizes": the
+        (dst_h, dst_w) of each frame."""
         import torch
         from .config import frame_sizes
-        frames = frame_list(frames, self.device)
-        (H, W), dsts = frame_sizes(self.cfg, [(f.shape[0], f.shape[1]) for f in frames], size, fit, short_side, max_side)
-        B = len(frames)
+        fb = Frames(frames, self.device, colorspace)
+        (H, W), dsts = frame_sizes(self.cfg, fb.sizes, size, fit, short_side, max_side)
+        B = len(fb.items)
         res, logits, boxes, aux = self._outputs(B, self.device, want_aux)
         ov = None
         if topk_override is not None:
             ov = topk_override.to(device=self.device, dtype=torch.int32).contiguous()
-        check(lib().lwdetr_forward_frames(self._h, ctypes.cast(frame_descs(frames, dsts), _vp), ctypes.cast(_norm3(mean), _vp),
-                                          ctypes.cast(_norm3(std), _vp), B, H, W, ptr(logits), ptr(boxes),
-                                          ctypes.byref(aux) if aux is not None else None, ptr(ov), stream_ptr(self.device)),
-              "lwdetr_forward_frames")
-        self._last_inputs = (frames, ov, None)    # keep alive until the stream has consumed them
+        name = "lwdetr_forward_frames_nv12" if fb.nv12 else "lwdetr_forward_frames"
+        check(getattr(lib(), name)(self._h, fb.descs(dsts), ctypes.cast(_norm3(mean), _vp), ctypes.cast(_norm3(std), _vp), B, H, W,
+                                   ptr(logits), ptr(boxes), ctypes.byref(aux) if aux is not None else None, ptr(ov),
+                                   stream_ptr(self.device)), name)
+        self._last_inputs = (fb.items, ov, None)    # keep alive until the stream has consumed them
         res["frame_sizes"] = dsts
         return res
 

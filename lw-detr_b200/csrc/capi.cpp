@@ -9,6 +9,7 @@
 
 #include <map>
 #include <new>
+#include <type_traits>
 #include <vector>
 
 #include "attn.h"
@@ -299,36 +300,68 @@ int lwdetr_forward_hw(lwdetr_handle* h, const lwdetr_input* input, int B, int he
   return forward_input("lwdetr_forward_hw", h, input, B, height, width, pred_logits, pred_boxes, aux, topk_override, stream);
 }
 
-int lwdetr_forward_frames(lwdetr_handle* h, const lwdetr_frame* frames, const float mean[3], const float std[3], int B, int height,
+}  // extern "C"
+
+// the frame entry points of both source formats (lwdetr_frame, lwdetr_frame_nv12)
+template <typename F>
+static int forward_frames(const char* fn, lwdetr_handle* h, const F* frames, const float mean[3], const float std[3], int B, int height,
                           int width, float* pred_logits, float* pred_boxes, const lwdetr_aux_out* aux, const int32_t* topk_override,
                           void* stream) {
-  if (!h || !frames || !mean || !std) return fail("lwdetr_forward_frames: null pointer");
-  if (B <= 0) return fail("lwdetr_forward_frames: batch must be positive");
+  if (!h || !frames || !mean || !std) return fail(std::string(fn) + ": null pointer");
+  if (B <= 0) return fail(std::string(fn) + ": batch must be positive");
   lwb::ForwardIn in;
-  in.kind = lwb::IN_FRAMES; in.frames = frames;
+  if constexpr (std::is_same<F, lwdetr_frame_nv12>::value) { in.kind = lwb::IN_FRAMES_NV12; in.frames_nv12 = frames; }
+  else { in.kind = lwb::IN_FRAMES; in.frames = frames; }
   for (int c = 0; c < 3; ++c) {
     in.mean[c] = mean[c]; in.stdv[c] = std[c];
-    if (!(std[c] > 0.f)) return fail("lwdetr_forward_frames: std must be positive");
+    if (!(std[c] > 0.f)) return fail(std::string(fn) + ": std must be positive");
   }
   std::string err;
-  if (lwb::frames_check(frames, B, height, width, &err)) return fail("lwdetr_forward_frames: " + err);
+  if (lwb::frames_check(frames, B, height, width, &err)) return fail(std::string(fn) + ": " + err);
   if (h->eng->forward(in, B, height, width, pred_logits, pred_boxes, aux, topk_override, static_cast<cudaStream_t>(stream), &err)) return fail(err);
   return 0;
 }
 
-int lwdetr_resize_patches(int dtype, const lwdetr_frame* frames, int B, int height, int width, const float mean[3], const float std[3],
+template <typename F>
+static int resize_patches(const char* fn, int dtype, const F* frames, int B, int height, int width, const float mean[3], const float std[3],
                           void* A, uint8_t* mask, void* stream) {
-  if (!frames || !mean || !std || !A) return fail("lwdetr_resize_patches: null pointer");
-  if (dtype != LWDETR_F16 && dtype != LWDETR_BF16) return fail("lwdetr_resize_patches: dtype must be LWDETR_F16 or LWDETR_BF16");
-  if (B <= 0 || height < 64 || width < 64 || height % 64 || width % 64) return fail("lwdetr_resize_patches: batch must be positive, height and width multiples of 64");
+  const std::string f(fn);
+  if (!frames || !mean || !std || !A) return fail(f + ": null pointer");
+  if (dtype != LWDETR_F16 && dtype != LWDETR_BF16) return fail(f + ": dtype must be LWDETR_F16 or LWDETR_BF16");
+  if (B <= 0 || height < 64 || width < 64 || height % 64 || width % 64) return fail(f + ": batch must be positive, height and width multiples of 64");
   for (int c = 0; c < 3; ++c)
-    if (!(std[c] > 0.f)) return fail("lwdetr_resize_patches: std must be positive");
+    if (!(std[c] > 0.f)) return fail(f + ": std must be positive");
   std::string err;
-  if (lwb::frames_check(frames, B, height, width, &err)) return fail("lwdetr_resize_patches: " + err);
+  if (lwb::frames_check(frames, B, height, width, &err)) return fail(f + ": " + err);
   int e = mask ? lwb::frame_mask_launch(frames, B, height, width, mask, static_cast<cudaStream_t>(stream)) : 0;
   if (!e) e = lwb::resize_patches_launch(dtype, frames, B, height, width, mean, std, A, static_cast<cudaStream_t>(stream));
-  if (e) return cuda_fail(e, "lwdetr_resize_patches launch");
+  if (e) return cuda_fail(e, (f + " launch").c_str());
   return 0;
+}
+
+extern "C" {
+
+int lwdetr_forward_frames(lwdetr_handle* h, const lwdetr_frame* frames, const float mean[3], const float std[3], int B, int height,
+                          int width, float* pred_logits, float* pred_boxes, const lwdetr_aux_out* aux, const int32_t* topk_override,
+                          void* stream) {
+  return forward_frames("lwdetr_forward_frames", h, frames, mean, std, B, height, width, pred_logits, pred_boxes, aux, topk_override, stream);
+}
+
+int lwdetr_forward_frames_nv12(lwdetr_handle* h, const lwdetr_frame_nv12* frames, const float mean[3], const float std[3], int B, int height,
+                               int width, float* pred_logits, float* pred_boxes, const lwdetr_aux_out* aux, const int32_t* topk_override,
+                               void* stream) {
+  return forward_frames("lwdetr_forward_frames_nv12", h, frames, mean, std, B, height, width, pred_logits, pred_boxes, aux, topk_override,
+                        stream);
+}
+
+int lwdetr_resize_patches(int dtype, const lwdetr_frame* frames, int B, int height, int width, const float mean[3], const float std[3],
+                          void* A, uint8_t* mask, void* stream) {
+  return resize_patches("lwdetr_resize_patches", dtype, frames, B, height, width, mean, std, A, mask, stream);
+}
+
+int lwdetr_resize_patches_nv12(int dtype, const lwdetr_frame_nv12* frames, int B, int height, int width, const float mean[3],
+                               const float std[3], void* A, uint8_t* mask, void* stream) {
+  return resize_patches("lwdetr_resize_patches_nv12", dtype, frames, B, height, width, mean, std, A, mask, stream);
 }
 
 // One ncclBroadcast of the packed weight arena (SURVEY.md 8b / 8e).  NCCL is not linked: the symbol is taken from the

@@ -624,9 +624,13 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
       add_op("mask_setup", [this, B, IH, IW, L, S, lh0, lh1, lw0, lw1, ls0, ls1, prop_b, invalid_b, pad_b, vr_b, fmask_b](cudaStream_t st) {
         const int lh[2] = {lh0, lh1}, lw[2] = {lw0, lw1}, ls[2] = {ls0, ls1};
         const uint8_t* mask = in_.mask;
-        if (in_.kind == IN_FRAMES) {      // raw frames: the mask follows from their dst sizes and is made on the device
+        if (in_.kind == IN_FRAMES || in_.kind == IN_FRAMES_NV12) {   // raw frames: the mask follows from their dst sizes, made on the device
           mask = frames_padded_ ? fmask_b : nullptr;
-          if (frames_padded_) { const int rc = frame_mask_launch(in_.frames, B, IH, IW, fmask_b, st); if (rc) return rc; }
+          if (frames_padded_) {
+            const int rc = in_.kind == IN_FRAMES ? frame_mask_launch(in_.frames, B, IH, IW, fmask_b, st)
+                                                 : frame_mask_launch(in_.frames_nv12, B, IH, IW, fmask_b, st);
+            if (rc) return rc;
+          }
         }
         return mask_setup_launch(mask, B, IH, IW, L, S, lh, lw, ls, prop_b, invalid_b, pad_b, vr_b, st);
       }, prop_b, BS, 4, 4, 1, 24.0 * BS);
@@ -645,6 +649,7 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
       void* a0p = a0.p;
       add_op("patch_gather", [this, a0p, B, IH, IW, dt](cudaStream_t st) {
                if (in_.kind == IN_FRAMES) return resize_patches_launch(dt, in_.frames, B, IH, IW, in_.mean, in_.stdv, a0p, st);
+               if (in_.kind == IN_FRAMES_NV12) return resize_patches_launch(dt, in_.frames_nv12, B, IH, IW, in_.mean, in_.stdv, a0p, st);
                if (in_.kind == IN_U8_NHWC) return patch_gather_u8_launch(dt, in_.images, in_.mean, in_.stdv, a0p, B, IH, IW, st);
                return patch_gather_launch(dt, in_.images, in_.kind == IN_F32_NCHW ? 1 : 0, a0p, B, IH, IW, st);
              },
@@ -959,12 +964,18 @@ int Engine::forward(const ForwardIn& in, int B, int H, int W, float* pred_logits
     ops_.clear();
     return -1;
   }
-  if (in.kind == IN_FRAMES ? !in.frames : !in.images) { *err = "lwdetr_forward: null images"; return -1; }
+  if (in.kind == IN_FRAMES ? !in.frames : in.kind == IN_FRAMES_NV12 ? !in.frames_nv12 : !in.images) { *err = "lwdetr_forward: null images"; return -1; }
   in_ = in; in_topk_override_ = topk_override;
-  if (in.kind == IN_FRAMES) {   // the schedule (and profile_ops, later) reads the engine's copy: the caller's array is free on return
+  // the schedule (and profile_ops, later) reads the engine's copy: the caller's array is free on return.  Neither the source
+  // format nor the descriptors are part of the plan or the graphs: the input ops run eagerly in front of them
+  if (in.kind == IN_FRAMES) {
     frames_.assign(in.frames, in.frames + B);
     in_.frames = frames_.data();
     frames_padded_ = frames_padded(in.frames, B, H, W);
+  } else if (in.kind == IN_FRAMES_NV12) {
+    frames_nv12_.assign(in.frames_nv12, in.frames_nv12 + B);
+    in_.frames_nv12 = frames_nv12_.data();
+    frames_padded_ = frames_padded(in.frames_nv12, B, H, W);
   }
   // The first forward of a plan always runs eagerly (it also performs the one-time cudaFuncSetAttribute calls).
   const bool graph_ok = use_graph_ && captures_.empty() && eager_runs_ > 0;

@@ -37,10 +37,11 @@ struct Op {
 };
 
 // One forward's input: the image batch in one of three encodings plus the optional NestedTensor padding mask.
-enum : int { IN_F32_NCHW = 0, IN_16_NCHW = 1, IN_U8_NHWC = 2, IN_FRAMES = 3 };
+enum : int { IN_F32_NCHW = 0, IN_16_NCHW = 1, IN_U8_NHWC = 2, IN_FRAMES = 3, IN_FRAMES_NV12 = 4 };
 struct ForwardIn {
   const void* images = nullptr;   // DEVICE [B,3,H,W] fp32 / compute dtype, or [B,H,W,3] uint8
   const lwdetr_frame* frames = nullptr;   // IN_FRAMES: HOST array of B checked descriptors (resize.h); mean / stdv apply
+  const lwdetr_frame_nv12* frames_nv12 = nullptr;   // IN_FRAMES_NV12: the same for NV12 frames
   int kind = IN_F32_NCHW;
   const uint8_t* mask = nullptr;  // DEVICE bool [B,H,W] (True = padded pixel) or null
   float mean[3] = {0.f, 0.f, 0.f}, stdv[3] = {1.f, 1.f, 1.f};   // IN_U8_NHWC: (x/255 - mean) / std
@@ -114,6 +115,7 @@ class Engine {
   // live I/O pointers patched into the schedule at forward() time
   ForwardIn in_;
   std::vector<lwdetr_frame> frames_;   // the engine's copy of an IN_FRAMES batch's descriptors (in_.frames points here)
+  std::vector<lwdetr_frame_nv12> frames_nv12_;   // the same for IN_FRAMES_NV12 (in_.frames_nv12 points here)
   bool frames_padded_ = false;         // some frame leaves part of the canvas unfilled: mask_setup takes the device-made mask
   const int32_t* in_topk_override_ = nullptr;
   // result buffers (engine owned)

@@ -19,12 +19,17 @@
 // and the row pitch carry no alignment), the horizontal pass writes R x 3 x 64 fp32 values to shared memory, and the
 // vertical pass accumulates them into 16 registers per thread (thread = one (token, channel, patch row), the unit of a
 // 32-byte store).  Frames up to ~4x downscale take one chunk.
+//
+// NV12 frames (lwdetr_frame_nv12) take the same kernel: per chunk the luma span and the chroma pairs under it are staged the
+// same way and converted once per CTA into the interleaved RGB rows the horizontal pass reads, so the NV12 result is the RGB
+// result of the converted frame by construction.  tools/yuv_spec.py restates the conversion.
 #include "resize.h"
 #include "gemm_tc.h"
 #include "launch.h"
 #include "ptx.cuh"
 
 #include <algorithm>
+#include <type_traits>
 
 namespace lwb {
 
@@ -34,15 +39,34 @@ constexpr int HROW = 3 * TILE_W;                              // fp32 values of 
 constexpr int GROUP = 64;                                     // frames per launch (descriptors are kernel parameters)
 constexpr int SMEM_BUDGET = 64 * 1024;                        // dynamic shared memory of one CTA, at most
 
+template <typename F>
 struct FrameGroup {
-  lwdetr_frame f[GROUP];
+  F f[GROUP];
+};
+// the padding mask depends on the dst sizes only: one kernel for every source format
+struct DstGroup {
+  int h[GROUP], w[GROUP];
 };
 struct ResizeNorm {
   float mean[3], stdv[3];
 };
+static_assert(sizeof(FrameGroup<lwdetr_frame_nv12>) + sizeof(ResizeNorm) + 64 <= 4096, "NV12 group exceeds 4 KB of kernel parameters");
+
+// NV12 -> RGB rows of include/lwdetr_b200.h: cY, cRv, cGu, cGv, cBu per colorspace; codes 0 and 1 are limited range
+__constant__ int kCsc[4][5] = {{1220542, 1673527, -409993, -852492, 2116026},
+                               {1220945, 1879825, -223607, -558796, 2215014},
+                               {1048576, 1470104, -360853, -748826, 1858077},
+                               {1048576, 1651297, -196424, -490864, 1945738}};
 
 // bytes of one staged source row: the 16-byte aligned global span covering `nbytes` from any start address
 __host__ __device__ inline int staged_row_bytes(int nbytes) { return ((nbytes + 15) & ~15) + 16; }
+// shared bytes per source row of a chunk that spans `ncols` source columns.  RGB: the staged row, then the horizontal pass's
+// fp32 row.  NV12: the converted RGB row, the staged luma row, one staged chroma row (a chunk of R luma rows touches at most
+// R chroma rows) and the fp32 row.
+__host__ __device__ inline int rgb_row_bytes(int ncols) { return staged_row_bytes(ncols * 3) + HROW * 4; }
+__host__ __device__ inline int nv12_row_bytes(int ncols, int nchroma_bytes) {
+  return ((ncols * 3 + 15) & ~15) + staged_row_bytes(ncols) + staged_row_bytes(nchroma_bytes) + HROW * 4;
+}
 
 // upper bound of the source extent that `n_tile` outputs of an axis touch
 inline int extent_bound(int n_tile, int n_in, int n_out) {
@@ -50,21 +74,53 @@ inline int extent_bound(int n_tile, int n_in, int n_out) {
   return std::min(n_in, static_cast<int>(n_tile * scale + 2.0 * support) + 3);
 }
 // dynamic shared memory that lets a frame's tiles run in one chunk, capped at the budget (then they take several)
-inline int frame_smem(const lwdetr_frame& f) {
+template <typename F>
+inline int frame_smem(const F& f) {
   const int rows = extent_bound(TILE_H, f.height, f.dst_h), cols = extent_bound(TILE_W, f.width, f.dst_w);
-  const long long per_row = staged_row_bytes(cols * 3) + HROW * 4;
+  const long long per_row = std::is_same<F, lwdetr_frame_nv12>::value ? nv12_row_bytes(cols, cols + 2) : rgb_row_bytes(cols);
   return static_cast<int>(std::min<long long>(SMEM_BUDGET, per_row * rows));
 }
+
+// stage source rows [y0, y0 + nrows) of a byte span (row y: `nbytes` from col0 + y * pitch) into shared rows `rb` bytes apart.
+// The shared row mirrors the 16-byte aligned global span, so data byte i of row y sits at ((col0 + y * pitch) & 15) + i:
+// 16-byte loads where the global address allows, single bytes at an unaligned head / tail (neither base pointers nor pitches
+// carry alignment)
+__device__ __forceinline__ void stage_rows(uint8_t* raw, int rb, const uint8_t* col0, int y0, long long pitch, int nrows, int nbytes, int tid) {
+  const int nchunk16 = rb >> 4;
+  for (int idx = tid; idx < nrows * nchunk16; idx += NTHREADS) {
+    const int row = idx / nchunk16, j = idx - row * nchunk16;
+    const uint8_t* g = col0 + static_cast<long long>(y0 + row) * pitch;
+    const int lo_b = j * 16 - static_cast<int>(reinterpret_cast<uintptr_t>(g) & 15), hi_b = lo_b + 16;
+    if (lo_b >= nbytes) continue;
+    uint8_t* s = raw + row * rb + j * 16;
+    if (lo_b >= 0 && hi_b <= nbytes) {
+      *reinterpret_cast<uint4*>(s) = __ldg(reinterpret_cast<const uint4*>(g + lo_b));
+    } else {
+      for (int k = max(lo_b, 0); k < min(hi_b, nbytes); ++k) s[k - lo_b] = __ldg(g + k);
+    }
+  }
+}
+// the first staged byte of source column x and the row pitch of the plane the horizontal pass reads from (NV12: luma)
+__device__ __forceinline__ const uint8_t* src_col(const lwdetr_frame& f, int x) { return f.data + static_cast<long long>(x) * 3; }
+__device__ __forceinline__ const uint8_t* src_col(const lwdetr_frame_nv12& f, int x) { return f.luma + x; }
+__device__ __forceinline__ long long src_pitch(const lwdetr_frame& f) { return f.pitch_bytes; }
+__device__ __forceinline__ long long src_pitch(const lwdetr_frame_nv12& f) { return f.luma_pitch; }
+__device__ __forceinline__ int shift20(int v) { return min(max((v + (1 << 19)) >> 20, 0), 255); }
 }  // namespace
 
-template <typename T>
-__global__ void __launch_bounds__(NTHREADS) resize_patches_kernel(const __grid_constant__ FrameGroup fg, int b0, T* __restrict__ A, int H, int W,
+// F: the source format, lwdetr_frame (packed RGB) or lwdetr_frame_nv12.  Only the staging of a chunk's source rows differs:
+// NV12 stages the luma span and the chroma pairs under it and converts each staged pixel once into the interleaved RGB row the
+// horizontal pass reads, so everything from the tap tables on is the same code for both, and an NV12 frame gives exactly the
+// bits of its converted RGB frame.
+template <typename T, typename F>
+__global__ void __launch_bounds__(NTHREADS) resize_patches_kernel(const __grid_constant__ FrameGroup<F> fg, int b0, T* __restrict__ A, int H, int W,
                                                                   const ResizeNorm np, int smem_bytes) {
+  constexpr bool kNV12 = std::is_same<F, lwdetr_frame_nv12>::value;
   pdl_sync();
   extern __shared__ __align__(16) uint8_t smem[];
   __shared__ float s_wx[TILE_W * kResizeMaxTaps], s_wy[TILE_H * kResizeMaxTaps];
   __shared__ int s_xlo[TILE_W], s_xn[TILE_W], s_ylo[TILE_H], s_yn[TILE_H];
-  const lwdetr_frame& f = fg.f[blockIdx.z];
+  const F& f = fg.f[blockIdx.z];
   const int tid = threadIdx.x;
   const int oy0 = blockIdx.y * TILE_H, ox0 = blockIdx.x * TILE_W;
   // this thread's output: token t of the tile, channel c, patch row py -> 16 pixels, one 32-byte store
@@ -104,30 +160,50 @@ __global__ void __launch_bounds__(NTHREADS) resize_patches_kernel(const __grid_c
   // ---- source footprint of the tile (tap ranges are monotone in the output index)
   const int xb0 = s_xlo[0], xb1 = s_xlo[nvx - 1] + s_xn[nvx - 1];
   const int yb0 = s_ylo[0], yb1 = s_ylo[nvy - 1] + s_yn[nvy - 1];
-  const int nbytes = (xb1 - xb0) * 3, rb = staged_row_bytes(nbytes), nchunk16 = rb >> 4;
-  const int R = max(1, min(yb1 - yb0, smem_bytes / (rb + HROW * 4)));
+  const int ncols = xb1 - xb0, xc0 = xb0 >> 1, nchroma = 2 * (((xb1 + 1) >> 1) - xc0);   // chroma: the pairs under [xb0, xb1)
+  // raw: the rows the horizontal pass reads, rb bytes apart (RGB: the staged rows; NV12: the converted rows)
+  const int rb = kNV12 ? (ncols * 3 + 15) & ~15 : staged_row_bytes(ncols * 3);
+  const int R = max(1, min(yb1 - yb0, smem_bytes / (kNV12 ? nv12_row_bytes(ncols, nchroma) : rgb_row_bytes(ncols))));
   uint8_t* raw = smem;
-  float* hbuf = reinterpret_cast<float*>(smem + static_cast<size_t>(R) * rb);
+  const int rbY = staged_row_bytes(ncols), rbC = staged_row_bytes(nchroma);
+  uint8_t* rawY = smem + static_cast<size_t>(R) * rb;                   // NV12 only: staged luma rows,
+  uint8_t* rawC = rawY + static_cast<size_t>(R) * rbY;                  // staged chroma rows
+  float* hbuf = reinterpret_cast<float*>(kNV12 ? rawC + static_cast<size_t>(R) * rbC : smem + static_cast<size_t>(R) * rb);
   const int my_ylo = py < nvy ? s_ylo[py] : 0, my_yhi = py < nvy ? my_ylo + s_yn[py] : 0;
-  const uint8_t* col0 = f.data + static_cast<long long>(xb0) * 3;
+  const uint8_t* col0 = src_col(f, xb0);
   float acc[16];
 #pragma unroll
   for (int j = 0; j < 16; ++j) acc[j] = 0.f;
   for (int yc = yb0; yc < yb1; yc += R) {
     const int rc = min(R, yb1 - yc);
-    // stage rows [yc, yc + rc), bytes [xb0 * 3, xb1 * 3): the shared row mirrors the 16-byte aligned global span, so a data
-    // byte i sits at (address & 15) + i of its row
-    for (int idx = tid; idx < rc * nchunk16; idx += NTHREADS) {
-      const int row = idx / nchunk16, j = idx - row * nchunk16;
-      const uint8_t* g = col0 + static_cast<long long>(yc + row) * f.pitch_bytes;
-      const int lo_b = j * 16 - static_cast<int>(reinterpret_cast<uintptr_t>(g) & 15), hi_b = lo_b + 16;
-      if (lo_b >= nbytes) continue;
-      uint8_t* s = raw + row * rb + j * 16;
-      if (lo_b >= 0 && hi_b <= nbytes) {
-        *reinterpret_cast<uint4*>(s) = __ldg(reinterpret_cast<const uint4*>(g + lo_b));
-      } else {
-        for (int k = max(lo_b, 0); k < min(hi_b, nbytes); ++k) s[k - lo_b] = __ldg(g + k);
+    if constexpr (kNV12) {
+      // luma rows [yc, yc + rc) and the chroma rows under them (a chroma row serves two luma rows and may straddle chunks)
+      const int cy0 = yc >> 1, ncr = ((yc + rc - 1) >> 1) - cy0 + 1;
+      const uint8_t* ccol0 = f.chroma + 2 * xc0;
+      stage_rows(rawY, rbY, col0, yc, f.luma_pitch, rc, ncols, tid);
+      stage_rows(rawC, rbC, ccol0, cy0, f.chroma_pitch, ncr, nchroma, tid);
+      __syncthreads();
+      const int* k = kCsc[f.colorspace];
+      const int cY = k[0], cRv = k[1], cGu = k[2], cGv = k[3], cBu = k[4];
+      const bool limited = f.colorspace < 2;
+      for (int row = 0; row < rc; ++row) {                                // once per staged pixel, row by row
+        const int y = yc + row, cr = y >> 1;
+        const uint8_t* ys = rawY + row * rbY + static_cast<int>(reinterpret_cast<uintptr_t>(col0 + static_cast<long long>(y) * f.luma_pitch) & 15);
+        const uint8_t* uvs = rawC + (cr - cy0) * rbC +
+                             static_cast<int>(reinterpret_cast<uintptr_t>(ccol0 + static_cast<long long>(cr) * f.chroma_pitch) & 15) - 2 * xc0;
+        uint8_t* o = raw + row * rb;
+        for (int i = tid; i < ncols; i += NTHREADS) {
+          const uint8_t* uv = uvs + 2 * ((xb0 + i) >> 1);
+          const int Y = ys[i], u = uv[0] - 128, v = uv[1] - 128;
+          const int yp = (limited ? max(Y - 16, 0) : Y) * cY;
+          o[3 * i] = static_cast<uint8_t>(shift20(yp + cRv * v));
+          o[3 * i + 1] = static_cast<uint8_t>(shift20(yp + cGu * u + cGv * v));
+          o[3 * i + 2] = static_cast<uint8_t>(shift20(yp + cBu * u));
+        }
       }
+    } else {
+      // stage rows [yc, yc + rc), bytes [xb0 * 3, xb1 * 3)
+      stage_rows(raw, rb, col0, yc, f.pitch_bytes, rc, ncols * 3, tid);
     }
     __syncthreads();
     // horizontal pass: hbuf[row][channel][ox]
@@ -135,7 +211,7 @@ __global__ void __launch_bounds__(NTHREADS) resize_patches_kernel(const __grid_c
       const int row = idx / HROW, j = idx - row * HROW, cc = j >> 6, ox = j & 63;
       float v = 0.f;
       if (ox < nvx) {
-        const int sh = static_cast<int>(reinterpret_cast<uintptr_t>(col0 + static_cast<long long>(yc + row) * f.pitch_bytes) & 15);
+        const int sh = kNV12 ? 0 : static_cast<int>(reinterpret_cast<uintptr_t>(col0 + static_cast<long long>(yc + row) * src_pitch(f)) & 15);
         const uint8_t* s = raw + row * rb + sh + (s_xlo[ox] - xb0) * 3 + cc;
         const float* w = s_wx + ox * kResizeMaxTaps;
         const int n = s_xn[ox];
@@ -170,29 +246,47 @@ __global__ void __launch_bounds__(NTHREADS) resize_patches_kernel(const __grid_c
 }
 
 // mask[b, y, x] = 1 outside the frame's dst_h x dst_w (the NestedTensor mask of util/misc.py:317-339), four pixels per thread
-__global__ void __launch_bounds__(256) frame_mask_kernel(const __grid_constant__ FrameGroup fg, int b0, uint8_t* __restrict__ mask, int H, int W) {
+__global__ void __launch_bounds__(256) frame_mask_kernel(const __grid_constant__ DstGroup dg, int b0, uint8_t* __restrict__ mask, int H, int W) {
   pdl_sync();
-  const lwdetr_frame& f = fg.f[blockIdx.y];
+  const int dst_h = dg.h[blockIdx.y], dst_w = dg.w[blockIdx.y];
   const int wq = W / 4, idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= H * wq) return;
   const int y = idx / wq, x = (idx - y * wq) * 4;
   uint32_t v = 0;
 #pragma unroll
-  for (int k = 0; k < 4; ++k) v |= (y >= f.dst_h || x + k >= f.dst_w) ? (1u << (8 * k)) : 0u;
+  for (int k = 0; k < 4; ++k) v |= (y >= dst_h || x + k >= dst_w) ? (1u << (8 * k)) : 0u;
   reinterpret_cast<uint32_t*>(mask + static_cast<long long>(b0 + blockIdx.y) * H * W)[idx] = v;
 }
 
-int frames_check(const lwdetr_frame* frames, int B, int H, int W, std::string* err) {
+namespace {
+// what is wrong with a frame's plane pointers, and (checked after its sides) with its pitches and colour space: "" when nothing
+std::string pointers_error(const lwdetr_frame& f) { return f.data ? "" : "null data pointer"; }
+std::string pointers_error(const lwdetr_frame_nv12& f) { return !f.luma ? "null luma pointer" : !f.chroma ? "null chroma pointer" : ""; }
+std::string layout_error(const lwdetr_frame& f) {
+  if (f.pitch_bytes < 3LL * f.width) return "pitch_bytes " + std::to_string(f.pitch_bytes) + " is smaller than 3 * width";
+  return "";
+}
+std::string layout_error(const lwdetr_frame_nv12& f) {
+  if (f.luma_pitch < f.width) return "luma_pitch " + std::to_string(f.luma_pitch) + " is smaller than width";
+  const long long cw = 2LL * ((f.width + 1) / 2);
+  if (f.chroma_pitch < cw) return "chroma_pitch " + std::to_string(f.chroma_pitch) + " is smaller than 2 * ceil(width / 2) = " + std::to_string(cw);
+  if (f.colorspace < LWDETR_CSC_BT601_LIMITED || f.colorspace > LWDETR_CSC_BT709_FULL)
+    return "unknown colorspace " + std::to_string(f.colorspace) + " (LWDETR_CSC_BT601_LIMITED .. LWDETR_CSC_BT709_FULL)";
+  return "";
+}
+
+template <typename F>
+int frames_check_impl(const F* frames, int B, int H, int W, std::string* err) {
   for (int b = 0; b < B; ++b) {
-    const lwdetr_frame& f = frames[b];
+    const F& f = frames[b];
     const std::string who = "frame " + std::to_string(b) + " (" + std::to_string(f.height) + "x" + std::to_string(f.width) + " -> " +
                             std::to_string(f.dst_h) + "x" + std::to_string(f.dst_w) + ")";
-    if (!f.data) { *err = who + ": null data pointer"; return -1; }
+    if (const std::string e = pointers_error(f); !e.empty()) { *err = who + ": " + e; return -1; }
     if (f.height < kFrameMinSide || f.width < kFrameMinSide || f.height > kFrameMaxSide || f.width > kFrameMaxSide) {
       *err = who + ": source sides must be in [" + std::to_string(kFrameMinSide) + ", " + std::to_string(kFrameMaxSide) + "]";
       return -1;
     }
-    if (f.pitch_bytes < 3LL * f.width) { *err = who + ": pitch_bytes " + std::to_string(f.pitch_bytes) + " is smaller than 3 * width"; return -1; }
+    if (const std::string e = layout_error(f); !e.empty()) { *err = who + ": " + e; return -1; }
     if (f.dst_h < 1 || f.dst_w < 1 || f.dst_h > H || f.dst_w > W) {
       *err = who + ": resized sides must be in [1, run size " + std::to_string(H) + "x" + std::to_string(W) + "]";
       return -1;
@@ -205,43 +299,68 @@ int frames_check(const lwdetr_frame* frames, int B, int H, int W, std::string* e
   return 0;
 }
 
-bool frames_padded(const lwdetr_frame* frames, int B, int H, int W) {
+template <typename F>
+bool frames_padded_impl(const F* frames, int B, int H, int W) {
   for (int b = 0; b < B; ++b)
     if (frames[b].dst_h < H || frames[b].dst_w < W) return true;
   return false;
 }
 
-int resize_patches_launch(int dtype, const lwdetr_frame* frames, int B, int H, int W, const float* mean, const float* stdv, void* A, cudaStream_t st) {
-  if (H % 64 != 0 || W % 64 != 0 || H < 64 || W < 64) return -2;
-  ResizeNorm np;
-  for (int c = 0; c < 3; ++c) { np.mean[c] = mean[c]; np.stdv[c] = stdv[c]; }
-  const void* kern = dtype == DT_BF16 ? reinterpret_cast<const void*>(resize_patches_kernel<__nv_bfloat16>) : reinterpret_cast<const void*>(resize_patches_kernel<__half>);
-  if (const int e = ensure_max_dyn_smem(kern, SMEM_BUDGET)) return e;
+template <typename T, typename F>
+int resize_launch(const F* frames, int B, int H, int W, const ResizeNorm& np, T* A, cudaStream_t st) {
+  if (const int e = ensure_max_dyn_smem(reinterpret_cast<const void*>(resize_patches_kernel<T, F>), SMEM_BUDGET)) return e;
   for (int b0 = 0; b0 < B; b0 += GROUP) {
     const int nb = std::min(GROUP, B - b0);
-    FrameGroup fg = {};
+    FrameGroup<F> fg = {};
     int smem = 0;
     for (int i = 0; i < nb; ++i) { fg.f[i] = frames[b0 + i]; smem = std::max(smem, frame_smem(frames[b0 + i])); }
-    const dim3 grid(W / TILE_W, H / TILE_H, nb);
-    if (dtype == DT_BF16) launch_k(resize_patches_kernel<__nv_bfloat16>, grid, dim3(NTHREADS), smem, st, fg, b0, static_cast<__nv_bfloat16*>(A), H, W, np, smem);
-    else launch_k(resize_patches_kernel<__half>, grid, dim3(NTHREADS), smem, st, fg, b0, static_cast<__half*>(A), H, W, np, smem);
+    launch_k(resize_patches_kernel<T, F>, dim3(W / TILE_W, H / TILE_H, nb), dim3(NTHREADS), smem, st, fg, b0, A, H, W, np, smem);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return static_cast<int>(e);
   }
   return 0;
 }
 
-int frame_mask_launch(const lwdetr_frame* frames, int B, int H, int W, uint8_t* mask, cudaStream_t st) {
+template <typename F>
+int resize_patches_impl(int dtype, const F* frames, int B, int H, int W, const float* mean, const float* stdv, void* A, cudaStream_t st) {
+  if (H % 64 != 0 || W % 64 != 0 || H < 64 || W < 64) return -2;
+  ResizeNorm np;
+  for (int c = 0; c < 3; ++c) { np.mean[c] = mean[c]; np.stdv[c] = stdv[c]; }
+  if (dtype == DT_BF16) return resize_launch(frames, B, H, W, np, static_cast<__nv_bfloat16*>(A), st);
+  return resize_launch(frames, B, H, W, np, static_cast<__half*>(A), st);
+}
+
+template <typename F>
+int frame_mask_impl(const F* frames, int B, int H, int W, uint8_t* mask, cudaStream_t st) {
   if (W % 4 != 0) return -2;
   for (int b0 = 0; b0 < B; b0 += GROUP) {
     const int nb = std::min(GROUP, B - b0);
-    FrameGroup fg = {};
-    for (int i = 0; i < nb; ++i) fg.f[i] = frames[b0 + i];
-    launch_k(frame_mask_kernel, dim3((H * (W / 4) + 255) / 256, nb), dim3(256), 0, st, fg, b0, mask, H, W);
+    DstGroup dg = {};
+    for (int i = 0; i < nb; ++i) { dg.h[i] = frames[b0 + i].dst_h; dg.w[i] = frames[b0 + i].dst_w; }
+    launch_k(frame_mask_kernel, dim3((H * (W / 4) + 255) / 256, nb), dim3(256), 0, st, dg, b0, mask, H, W);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return static_cast<int>(e);
   }
   return 0;
+}
+}  // namespace
+
+int frames_check(const lwdetr_frame* frames, int B, int H, int W, std::string* err) { return frames_check_impl(frames, B, H, W, err); }
+int frames_check(const lwdetr_frame_nv12* frames, int B, int H, int W, std::string* err) { return frames_check_impl(frames, B, H, W, err); }
+bool frames_padded(const lwdetr_frame* frames, int B, int H, int W) { return frames_padded_impl(frames, B, H, W); }
+bool frames_padded(const lwdetr_frame_nv12* frames, int B, int H, int W) { return frames_padded_impl(frames, B, H, W); }
+int resize_patches_launch(int dtype, const lwdetr_frame* frames, int B, int H, int W, const float* mean, const float* stdv, void* A, cudaStream_t st) {
+  return resize_patches_impl(dtype, frames, B, H, W, mean, stdv, A, st);
+}
+int resize_patches_launch(int dtype, const lwdetr_frame_nv12* frames, int B, int H, int W, const float* mean, const float* stdv, void* A,
+                          cudaStream_t st) {
+  return resize_patches_impl(dtype, frames, B, H, W, mean, stdv, A, st);
+}
+int frame_mask_launch(const lwdetr_frame* frames, int B, int H, int W, uint8_t* mask, cudaStream_t st) {
+  return frame_mask_impl(frames, B, H, W, mask, st);
+}
+int frame_mask_launch(const lwdetr_frame_nv12* frames, int B, int H, int W, uint8_t* mask, cudaStream_t st) {
+  return frame_mask_impl(frames, B, H, W, mask, st);
 }
 
 }  // namespace lwb

@@ -141,30 +141,33 @@ class LWDETR(nn.Module):
         return self._pack_outputs(out)
 
     @torch.no_grad()
-    def forward_frames(self, frames, size=None, fit="stretch", short_side=None, max_side=None):
+    def forward_frames(self, frames, size=None, fit="stretch", short_side=None, max_side=None, colorspace=None):
         """Raw camera / decoder frames of ANY size: a list of CUDA uint8 [h, w, 3] tensors (RGB, each its own size) or one
-        [B, h, w, 3] tensor.  The reference's host-side transforms.Resize (demo.py:146-159; datasets/transforms.py:97-134
-        for fit="keep_aspect" with short_side / max_side) runs on the device, fused into the patch-embed load together with
-        /255 and Normalize (capi.Engine.forward_frames).  Returns the output dict of forward()."""
+        [B, h, w, 3] tensor; or NV12 frames, the output of video decoders, as (luma, chroma) pairs or packed [3h/2, w]
+        tensors, with colorspace= "bt601" / "bt709" / "bt601_full" / "bt709_full" (capi.Engine.forward_frames).  The
+        reference's host-side transforms.Resize (demo.py:146-159; datasets/transforms.py:97-134 for fit="keep_aspect" with
+        short_side / max_side) runs on the device, fused into the patch-embed load together with the colour conversion, /255
+        and Normalize.  Returns the output dict of forward()."""
         if self.training:
             raise RuntimeError("lwdetr_b200 implements the inference forward only; call model.eval()")
         if next(self.parameters()).device.type != "cuda":
             raise RuntimeError("lwdetr_b200: move the model to a CUDA device (no CPU fallback)")
-        out = self.engine().forward_frames(frames, size=size, fit=fit, short_side=short_side, max_side=max_side, want_aux=True)
+        out = self.engine().forward_frames(frames, size=size, fit=fit, short_side=short_side, max_side=max_side, want_aux=True,
+                                           colorspace=colorspace)
         return self._pack_outputs(out)
 
     @torch.no_grad()
-    def detect(self, frames, size=None, fit="stretch", short_side=None, max_side=None, num_select=None):
+    def detect(self, frames, size=None, fit="stretch", short_side=None, max_side=None, num_select=None, colorspace=None):
         """forward_frames + PostProcess: per frame {"scores", "labels", "boxes"} with xyxy boxes in the frame's ORIGINAL
-        pixel coordinates (for fit="keep_aspect" the predicted boxes are relative to the frame's valid region, which the
-        valid ratios of the padded batch already provide).  num_select defaults to num_queries."""
-        frames = capi.frame_list(frames, next(self.parameters()).device)
+        pixel coordinates (NV12: those of the luma plane; for fit="keep_aspect" the predicted boxes are relative to the frame's
+        valid region, which the valid ratios of the padded batch already provide).  num_select defaults to num_queries."""
+        frames = capi.Frames(frames, next(self.parameters()).device, colorspace)
         export, self._export = self._export, False
         try:
             out = self.forward_frames(frames, size=size, fit=fit, short_side=short_side, max_side=max_side)
         finally:
             self._export = export
-        sizes = torch.tensor([[f.shape[0], f.shape[1]] for f in frames], dtype=torch.float32, device=out["pred_logits"].device)
+        sizes = torch.tensor(frames.sizes, dtype=torch.float32, device=out["pred_logits"].device)
         return PostProcess(self.num_queries if num_select is None else num_select)(out, sizes)
 
     def _pack_outputs(self, out):

@@ -3,15 +3,18 @@
     python tools/bench_frames.py [--cases small:32,xlarge:16] [--sources 480x640,720x1280,1080x1920] [--dtype fp16]
                                  [--steps 20] [--warmup 5] [--rounds 3] [--out FILE]
 
-Per (config, batch, source size), pinned host uint8 frames going to 640x640, the three paths alternating in one process:
-  frames        forward_frames: H2D copy of the RAW frames + resize fused into the patch gather + forward
+Per (config, batch, source size), pinned host uint8 frames going to 640x640, the four paths alternating in one process:
+  frames        forward_frames: H2D copy of the RAW RGB frames + resize fused into the patch gather + forward
+  frames_nv12   the same from packed NV12 frames [B, 3h/2, w] (1.5 bytes per pixel), colorspace="bt709": the colour
+                conversion is fused into the resize's staging
   u8_ceiling    the existing uint8 path fed frames that are already 640x640 (H2D of those + forward): no resize anywhere
   host_resize   torch's CPU antialias interpolate (all cores) to 640x640, then u8_ceiling's path: what callers do today
 Each is images/s by a host clock around `steps` batches ending in a device synchronise; the median of `rounds` is reported
 with the spread.  Also the resize op's own time (CUDA events around repeated launches of the patch_gather op of the
 schedule, lwdetr_profile_ops) with the bytes it has to move (sum h*w*3 read + B*T*768*2 written) and the time those bytes
 take at the H100 SXM data sheet's 3.35 TB/s, named as a floor, not as something reached; and the H2D copy time of the raw
-frames.  The GPU's name and power limit are read in the same run.  One JSON line per case; --out also writes the list.
+frames.  The same resize-op and copy figures for the NV12 frames (h*w*1.5 bytes read).  The GPU's name and power limit are
+read in the same run.  One JSON line per case; --out also writes the list.
 Needs a GPU.
 """
 import argparse
@@ -51,9 +54,13 @@ def measure(eng, name, batch, h, w, steps, warmup, rounds):
     raw = [torch.randint(0, 256, (batch, h, w, 3), generator=g, dtype=torch.uint8).pin_memory() for _ in range(2)]
     small = [torch.randint(0, 256, (batch, RUN, RUN, 3), generator=g, dtype=torch.uint8).pin_memory() for _ in range(2)]
     staged = torch.empty(batch, RUN, RUN, 3, dtype=torch.uint8).pin_memory()
+    nv12 = [torch.randint(0, 256, (batch, h * 3 // 2, w), generator=g, dtype=torch.uint8).pin_memory() for _ in range(2)]
 
     def frames(i):
         eng.forward_frames(raw[i & 1].cuda(non_blocking=True), want_aux=False)
+
+    def frames_nv12(i):
+        eng.forward_frames(nv12[i & 1].cuda(non_blocking=True), want_aux=False, colorspace="bt709")
 
     def ceiling(i):
         eng.forward(small[i & 1].cuda(non_blocking=True), want_aux=False)
@@ -65,7 +72,7 @@ def measure(eng, name, batch, h, w, steps, warmup, rounds):
         eng.forward(staged.cuda(non_blocking=True), want_aux=False)
         torch.cuda.synchronize()                      # `staged` is reused by the next step
 
-    paths = {"frames": frames, "u8_ceiling": ceiling, "host_resize": host_resize}
+    paths = {"frames": frames, "frames_nv12": frames_nv12, "u8_ceiling": ceiling, "host_resize": host_resize}
     for fn in paths.values():
         for i in range(warmup):
             fn(i)
@@ -88,6 +95,14 @@ def measure(eng, name, batch, h, w, steps, warmup, rounds):
     res["resize_op_GBps"] = round(moved / (op_ms * 1e-3) / 1e9, 1)
     res["resize_op_floor_ms_at_datasheet_3.35TBps"] = round(moved / HBM_DATASHEET_BYTES_PER_S * 1e3, 4)
     res["h2d_raw_frames_ms"] = round(events_ms(lambda i: raw[i & 1].cuda(non_blocking=True), 10) / 10, 4)
+    eng.forward_frames(nv12[0].cuda(), want_aux=False, colorspace="bt709")
+    op_ms = [o[3] for o in eng.profile_ops(iters=20) if o[0] == "patch_gather"][0]
+    moved = batch * h * w * 3 // 2 + batch * (RUN // 16) ** 2 * 768 * 2
+    res["nv12_resize_op_ms"] = round(op_ms, 4)
+    res["nv12_resize_op_bytes"] = moved
+    res["nv12_resize_op_GBps"] = round(moved / (op_ms * 1e-3) / 1e9, 1)
+    res["nv12_resize_op_floor_ms_at_datasheet_3.35TBps"] = round(moved / HBM_DATASHEET_BYTES_PER_S * 1e3, 4)
+    res["h2d_nv12_frames_ms"] = round(events_ms(lambda i: nv12[i & 1].cuda(non_blocking=True), 10) / 10, 4)
     eng.forward(small[0].cuda(), want_aux=False)
     res["u8_gather_op_ms"] = round([o[3] for o in eng.profile_ops(iters=20) if o[0] == "patch_gather"][0], 4)
     return res
