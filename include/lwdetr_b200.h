@@ -57,6 +57,39 @@ LWDETR_API int lwdetr_gemm(int dtype, const void* A, int lda, int M, int K, cons
                            int act, void* out, int ld_out, int out_fp32, int rows_in, int remap_rows,
                            int shuffle_cout, int IH, int IW, void* stream);
 
+/* lwdetr_gemm with every epilogue feature the model schedules (same kernels, same plan as the forward builds).  dtype
+ * LWDETR_F16 or LWDETR_BF16 (the e4m3 GEMM is lwdetr_gemm_e4m3).  Beyond the lwdetr_gemm arguments:
+ *   LayerNorm consumer (stats_in != NULL): A holds the RAW rows [M, K = ln_C]; stats_in fp32 pairs [M, stats_parts_in] are each
+ *     row's partials (sum, M2) over equal slices of its ln_C columns (ln_C % stats_parts_in == 0); colsum fp32 [N];
+ *     out = act(rstd * (acc - mean * colsum[n]) + bias[n]) with mean / rstd = 1 / sqrt(var + ln_eps) combined from the
+ *     partials (W and bias carry the folded LayerNorm affine);
+ *   statistics producer (stats_out != NULL): also writes fp32 pairs [M, stats_parts_out], the partials (sum, M2) of each
+ *     ROUNDED output row, one per (n-tile, column half); N must be a multiple of the tile width bn;
+ *   head-major store (hm_S > 0): element (b*hm_S + s, (slice*hm_heads + head)*16 + c) goes to
+ *     out[(((b*hm_slices + slice)*hm_heads + head)*hm_S + s)*16 + c]; N == hm_slices*hm_heads*16, M % hm_S == 0, ld_out unused;
+ *   row_zero uint8 [M] or NULL: rows flagged non-zero are stored as zeros (forces the generic epilogue).
+ * Reported by the call (also with dry_run != 0, which builds the plan and launches nothing): bn, the n-tile width; epilogue,
+ * the LWDETR_EP_* specialisation that runs; stats_parts_out = 2 * ceil(N / bn). */
+enum { LWDETR_EP_GENERIC = 0, LWDETR_EP_BIAS = 1, LWDETR_EP_BIAS_ACT = 2, LWDETR_EP_LN = 3, LWDETR_EP_LN_GELU = 4, LWDETR_EP_RESID = 5 };
+typedef struct {
+  int32_t dtype;
+  const void* A; int32_t lda, M, K;
+  const void* W; int32_t N;
+  const float* bias; const float* gamma;
+  const void* resid; int32_t ld_resid, resid_mod;
+  int32_t act;
+  void* out; int32_t ld_out, out_fp32;
+  int32_t rows_in, remap_rows, shuffle_cout, IH, IW;
+  const float* stats_in; int32_t stats_parts_in;
+  const float* colsum; int32_t ln_C; float ln_eps;
+  float* stats_out;
+  int32_t hm_S, hm_heads, hm_slices;
+  const uint8_t* row_zero;
+  int32_t dry_run;
+  int32_t bn, epilogue, stats_parts_out;   /* out */
+} lwdetr_gemm_args;
+LWDETR_API int lwdetr_gemm_ex(lwdetr_gemm_args* args, void* stream);
+
 /* 3x3 convolution, padding 1, stride 1 or 2, NHWC, as an implicit GEMM (no im2col buffer):
  * X [B, stride*OH, stride*OW, ldx] (channel slice of width Cin), W [N, 9*Cin] with k = (dy*3+dx)*Cin + c,
  * out [B*OH*OW, ld_out].  Stands in for ConvX (projector.py:85-98) with BN folded into W/bias. */
@@ -68,6 +101,29 @@ LWDETR_API int lwdetr_conv3x3(int dtype, const void* X, int ldx, int B, int OH, 
  * transformer.py norms eps 1e-5).  x/y 16-bit with leading dimensions, w/b fp32 [C], C % 8 == 0, C <= 1024. */
 LWDETR_API int lwdetr_layernorm(int dtype, const void* x, int ldx, void* y, int ldy, const float* w, const float* b,
                                 float eps, int64_t rows, int C, void* stream);
+
+/* lwdetr_layernorm with the extras the decoder and the projector use (one launch, same kernel):
+ *   row_flag uint8 [flag_mod] or NULL: row r with row_flag[r % flag_mod] != 0 normalises override_vec (fp32 [C]) instead of
+ *     its x row (masked two-stage memory rows, transformer.py:116-123);
+ *   y2 (with add_src [rows, ld_add]): y2 = round16(round16(y) + add_src), the sum as a 16-bit consumer of y would form it;
+ *   y_group > 0: row r of y is written to row (r / y_group) * y_group_stride + y_row_off + r % y_group (the memory rows of one
+ *     projector level inside the batch's memory);
+ *   y3 (with w3, b3, eps3): the LayerNorm of the rounded y, exactly what a second call on y would write (decoder norm3 ->
+ *     dec_norm); y3 and y2 rows are NOT regrouped.
+ * Leading dimensions multiples of 8.  rows_per_warp (out) reports the kernel instance that ran: 1, or 4 for C <= 512 once
+ * rows >= 64 * SMs. */
+typedef struct {
+  const void* x; int32_t ldx;
+  void* y; int32_t ldy;
+  const float* w; const float* b; float eps;
+  int64_t rows; int32_t C;
+  const uint8_t* row_flag; int32_t flag_mod; const float* override_vec;
+  const void* add_src; int32_t ld_add; void* y2; int32_t ldy2;
+  int64_t y_group, y_group_stride, y_row_off;
+  const float* w3; const float* b3; float eps3; void* y3; int32_t ldy3;
+  int32_t rows_per_warp;   /* out */
+} lwdetr_layernorm_args;
+LWDETR_API int lwdetr_layernorm_ex(int dtype, lwdetr_layernorm_args* args, void* stream);
 
 /* softmax(Q K^T * scale) V for `nseq` independent sequences of `seqlen` tokens and `heads` heads of
  * width dh in {16, 32, 64}; token (s, t) is matrix row s*seqlen + t, head h occupies columns

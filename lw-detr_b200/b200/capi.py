@@ -20,8 +20,10 @@ _SIGNATURES = {
     "lwdetr_last_error": (ctypes.c_char_p, []),
     "lwdetr_abi_version": (_i, []),
     "lwdetr_gemm": (_i, [_i, _vp, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "lwdetr_gemm_ex": (_i, [_vp, _vp]),
     "lwdetr_conv3x3": (_i, [_i, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp]),
     "lwdetr_layernorm": (_i, [_i, _vp, _i, _vp, _i, _vp, _vp, _f, _i64, _i, _vp]),
+    "lwdetr_layernorm_ex": (_i, [_i, _vp, _vp]),
     "lwdetr_attention": (_i, [_i, _vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _i, _f, _vp]),
     "lwdetr_ms_deform_attn_forward": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "lwdetr_ms_deform_attn_backward": (_i, [_vp] * 9 + [_i] * 8 + [_vp]),
@@ -114,6 +116,11 @@ def io_dtype(torch_dtype):
     return torch.float16 if torch_dtype == torch.float8_e4m3fn else torch_dtype
 
 
+def _addr(t):
+    """Address of a tensor for a pointer field of a ctypes.Structure (None: NULL)."""
+    return None if t is None else t.data_ptr()
+
+
 def stream_ptr(device=None):
     import torch
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
@@ -131,6 +138,73 @@ def gemm(A, W, out, bias=None, gamma=None, resid=None, resid_mod=0, act=ACT_NONE
                             out.stride(0), 1 if out.dtype == torch.float32 else 0, rows_in, remap_rows,
                             shuffle_cout, IH, IW, stream_ptr()), "lwdetr_gemm")
     return out
+
+
+EP_NAMES = {0: "EP_GENERIC", 1: "EP_BIAS", 2: "EP_BIAS_ACT", 3: "EP_LN", 4: "EP_LN_GELU", 5: "EP_RESID"}
+
+
+class GemmArgs(ctypes.Structure):
+    """lwdetr_gemm_args (include/lwdetr_b200.h)."""
+    _fields_ = [("dtype", _i), ("A", _vp), ("lda", _i), ("M", _i), ("K", _i), ("W", _vp), ("N", _i), ("bias", _vp), ("gamma", _vp),
+                ("resid", _vp), ("ld_resid", _i), ("resid_mod", _i), ("act", _i), ("out", _vp), ("ld_out", _i), ("out_fp32", _i),
+                ("rows_in", _i), ("remap_rows", _i), ("shuffle_cout", _i), ("IH", _i), ("IW", _i),
+                ("stats_in", _vp), ("stats_parts_in", _i), ("colsum", _vp), ("ln_C", _i), ("ln_eps", _f), ("stats_out", _vp),
+                ("hm_S", _i), ("hm_heads", _i), ("hm_slices", _i), ("row_zero", _vp), ("dry_run", _i),
+                ("bn", _i), ("epilogue", _i), ("stats_parts_out", _i)]
+
+
+def gemm_ex(A, W, out, bias=None, gamma=None, resid=None, resid_mod=0, act=ACT_NONE, M=None, K=None, N=None,
+            stats_in=None, colsum=None, ln_C=0, ln_eps=0.0, stats_out=None, hm_S=0, hm_heads=0, hm_slices=0, row_zero=None,
+            dry_run=False):
+    """lwdetr_gemm_ex: lwdetr_gemm plus the LayerNorm consumer (stats_in fp32 [M, parts, 2] contiguous, colsum fp32 [N], ln_C,
+    ln_eps), the statistics producer (stats_out fp32 [M, >= parts_out, 2] contiguous), the head-major store (hm_S, hm_heads,
+    hm_slices; out a contiguous buffer) and row_zero (uint8 [M]).  Returns (bn, epilogue name, stats_parts_out) of the plan
+    that ran (dry_run: was built, nothing launched)."""
+    import torch
+    a = GemmArgs()
+    a.dtype = kernel_dtype_code(A.dtype)
+    a.A, a.lda, a.M, a.K = A.data_ptr(), A.stride(0), A.shape[0] if M is None else M, A.shape[1] if K is None else K
+    a.W, a.N = W.data_ptr(), W.shape[0] if N is None else N
+    a.bias, a.gamma = _addr(bias), _addr(gamma)
+    a.resid, a.ld_resid, a.resid_mod = _addr(resid), 0 if resid is None else resid.stride(0), resid_mod
+    a.act, a.out, a.out_fp32 = act, out.data_ptr(), 1 if out.dtype == torch.float32 else 0
+    a.ld_out = 16 if hm_S else out.stride(0)
+    if stats_in is not None:
+        a.stats_in, a.stats_parts_in = stats_in.data_ptr(), stats_in.shape[1]
+    a.colsum, a.ln_C, a.ln_eps = _addr(colsum), ln_C, float(ln_eps)
+    if stats_out is not None:
+        a.stats_out = stats_out.data_ptr()
+    a.hm_S, a.hm_heads, a.hm_slices, a.row_zero = hm_S, hm_heads, hm_slices, _addr(row_zero)
+    a.dry_run = 1 if dry_run else 0
+    check(lib().lwdetr_gemm_ex(ctypes.byref(a), stream_ptr()), "lwdetr_gemm_ex")
+    return a.bn, EP_NAMES[a.epilogue], a.stats_parts_out
+
+
+class LayerNormArgs(ctypes.Structure):
+    """lwdetr_layernorm_args (include/lwdetr_b200.h)."""
+    _fields_ = [("x", _vp), ("ldx", _i), ("y", _vp), ("ldy", _i), ("w", _vp), ("b", _vp), ("eps", _f), ("rows", _i64), ("C", _i),
+                ("row_flag", _vp), ("flag_mod", _i), ("override_vec", _vp), ("add_src", _vp), ("ld_add", _i), ("y2", _vp), ("ldy2", _i),
+                ("y_group", _i64), ("y_group_stride", _i64), ("y_row_off", _i64),
+                ("w3", _vp), ("b3", _vp), ("eps3", _f), ("y3", _vp), ("ldy3", _i), ("rows_per_warp", _i)]
+
+
+def layernorm_ex(x, y, w, b, eps, rows=None, C=None, row_flag=None, override=None, add=None, y2=None,
+                 y_group=0, y_group_stride=0, y_row_off=0, w3=None, b3=None, eps3=0.0, y3=None):
+    """lwdetr_layernorm_ex: y = LN(x) with the optional row flag (uint8 [flag_mod]) + override vector, y2 = y + add, y_group
+    row scatter and chained y3 = LN(y; w3, b3, eps3).  2-D tensors with any row stride.  Returns the rows per warp that ran."""
+    a = LayerNormArgs()
+    a.x, a.ldx, a.y, a.ldy = x.data_ptr(), x.stride(0), y.data_ptr(), y.stride(0)
+    a.w, a.b, a.eps = _addr(w), _addr(b), float(eps)
+    a.rows, a.C = x.shape[0] if rows is None else rows, x.shape[1] if C is None else C
+    if row_flag is not None:
+        a.row_flag, a.flag_mod, a.override_vec = row_flag.data_ptr(), row_flag.numel(), _addr(override)
+    if y2 is not None:
+        a.add_src, a.ld_add, a.y2, a.ldy2 = add.data_ptr(), add.stride(0), y2.data_ptr(), y2.stride(0)
+    a.y_group, a.y_group_stride, a.y_row_off = y_group, y_group_stride, y_row_off
+    if y3 is not None:
+        a.w3, a.b3, a.eps3, a.y3, a.ldy3 = _addr(w3), _addr(b3), float(eps3), y3.data_ptr(), y3.stride(0)
+    check(lib().lwdetr_layernorm_ex(kernel_dtype_code(x.dtype), ctypes.byref(a), stream_ptr()), "lwdetr_layernorm_ex")
+    return a.rows_per_warp
 
 
 def conv3x3(X, Wk, out, B, OH, OW, stride, Cin, bias=None, act=ACT_NONE):

@@ -54,6 +54,33 @@ int lwdetr_gemm(int dtype, const void* A, int lda, int M, int K, const void* W, 
   return 0;
 }
 
+static_assert(LWDETR_EP_GENERIC == lwb::EP_GENERIC && LWDETR_EP_BIAS == lwb::EP_BIAS && LWDETR_EP_BIAS_ACT == lwb::EP_BIAS_ACT &&
+              LWDETR_EP_LN == lwb::EP_LN && LWDETR_EP_LN_GELU == lwb::EP_LN_GELU && LWDETR_EP_RESID == lwb::EP_RESID, "EP codes");
+
+int lwdetr_gemm_ex(lwdetr_gemm_args* a, void* stream) {
+  if (!a || !a->A || !a->W || !a->out) return fail("lwdetr_gemm_ex: null pointer");
+  // 16-bit GEMMs only (the e4m3 GEMM has its own entry point and no epilogue variants), so `epilogue` is always an LWDETR_EP_*
+  if (a->dtype != LWDETR_F16 && a->dtype != LWDETR_BF16) return fail("lwdetr_gemm_ex: dtype must be LWDETR_F16 or LWDETR_BF16");
+  lwb::GemmDesc d;
+  d.dtype = a->dtype; d.A = a->A; d.lda = a->lda; d.M = a->M; d.N = a->N; d.K = a->K; d.W = a->W; d.bias = a->bias; d.gamma = a->gamma;
+  d.resid = a->resid; d.ld_resid = a->ld_resid; d.resid_mod = a->resid_mod; d.act = a->act; d.out = a->out; d.ld_out = a->ld_out;
+  d.out_fp32 = a->out_fp32; d.rows_in = a->rows_in; d.remap_rows = a->remap_rows; d.shuffle_cout = a->shuffle_cout;
+  d.IH = a->IH; d.IW = a->IW;
+  d.stats_in = reinterpret_cast<const float2*>(a->stats_in); d.stats_parts_in = a->stats_parts_in; d.colsum = a->colsum;
+  d.ln_C = a->ln_C; d.ln_eps = a->ln_eps; d.stats_out = reinterpret_cast<float2*>(a->stats_out);
+  d.hm_S = a->hm_S; d.hm_heads = a->hm_heads; d.hm_slices = a->hm_slices; d.row_zero = a->row_zero;
+  lwb::GemmOp op;
+  std::string err;
+  if (lwb::gemm_build(d, &op, &err)) return fail("lwdetr_gemm_ex: " + err);
+  a->bn = op.bn;
+  a->epilogue = lwb::gemm_epilogue(op);
+  a->stats_parts_out = op.args.stats_parts_out;
+  if (a->dry_run) return 0;
+  int e = lwb::gemm_launch(op, static_cast<cudaStream_t>(stream));
+  if (e) return cuda_fail(e, "lwdetr_gemm_ex launch");
+  return 0;
+}
+
 int lwdetr_conv3x3(int dtype, const void* X, int ldx, int B, int OH, int OW, int stride, int Cin, const void* W,
                    int N, const float* bias, int act, void* out, int ld_out, void* stream) {
   if (!X || !W || !out) return fail("lwdetr_conv3x3: null pointer");
@@ -79,6 +106,26 @@ int lwdetr_layernorm(int dtype, const void* x, int ldx, void* y, int ldy, const 
   int e = lwb::layernorm_launch(dtype, a, static_cast<cudaStream_t>(stream));
   if (e == -2) return fail("lwdetr_layernorm: C must be a multiple of 8 and <= 1024");
   if (e) return cuda_fail(e, "lwdetr_layernorm launch");
+  return 0;
+}
+
+int lwdetr_layernorm_ex(int dtype, lwdetr_layernorm_args* p, void* stream) {
+  if (!p || !p->x || !p->y || !p->w || !p->b) return fail("lwdetr_layernorm_ex: null pointer");
+  if (p->row_flag && (!p->override_vec || p->flag_mod < 1)) return fail("lwdetr_layernorm_ex: row_flag needs override_vec and flag_mod >= 1");
+  if (p->y2 && !p->add_src) return fail("lwdetr_layernorm_ex: y2 needs add_src");
+  if (p->y3 && (!p->w3 || !p->b3)) return fail("lwdetr_layernorm_ex: y3 needs w3 and b3");
+  if ((p->ldx | p->ldy | (p->y2 ? p->ld_add | p->ldy2 : 0) | (p->y3 ? p->ldy3 : 0)) % 8) return fail("lwdetr_layernorm_ex: leading dimensions must be multiples of 8");
+  if (p->rows < 1) return fail("lwdetr_layernorm_ex: rows must be positive");
+  lwb::LayerNormArgs a{};
+  a.x = p->x; a.ldx = p->ldx; a.y = p->y; a.ldy = p->ldy; a.w = p->w; a.b = p->b; a.eps = p->eps; a.rows = p->rows; a.C = p->C;
+  a.row_flag = p->row_flag; a.flag_mod = p->row_flag ? p->flag_mod : 1; a.override_vec = p->override_vec;
+  a.add_src = p->add_src; a.ld_add = p->ld_add; a.y2 = p->y2; a.ldy2 = p->ldy2;
+  a.y_group = p->y_group; a.y_group_stride = p->y_group_stride; a.y_row_off = p->y_row_off;
+  a.w3 = p->w3; a.b3 = p->b3; a.eps3 = p->eps3; a.y3 = p->y3; a.ldy3 = p->ldy3;
+  int e = lwb::layernorm_launch(dtype, a, static_cast<cudaStream_t>(stream));
+  if (e == -2) return fail("lwdetr_layernorm_ex: C must be a multiple of 8 and <= 1024");
+  if (e) return cuda_fail(e, "lwdetr_layernorm_ex launch");
+  p->rows_per_warp = lwb::layernorm_rows_per_warp(p->rows, p->C);
   return 0;
 }
 

@@ -63,7 +63,7 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmArgs& p, int tile, in
 //   EP_LN        out = LN-fold(acc) + bias            (qkv)
 //   EP_LN_GELU   out = gelu(LN-fold(acc) + bias)      (fc1)
 //   EP_RESID     out = resid + gamma*(acc + bias), optional row statistics (proj, fc2, patch embed, decoder)
-enum : int { EP_GENERIC = 0, EP_BIAS = 1, EP_BIAS_ACT = 2, EP_LN = 3, EP_LN_GELU = 4, EP_RESID = 5 };
+// (the enum is in gemm_tc.h)
 
 template <typename T, int BN, int EP>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
@@ -730,6 +730,8 @@ static int pick_ep(const GemmArgs& a) {
   if (a.gamma || a.resid || a.stats_out) return a.act == ACT_NONE ? EP_RESID : EP_GENERIC;
   return a.act == ACT_NONE ? EP_BIAS : EP_BIAS_ACT;
 }
+
+int gemm_epilogue(const GemmOp& op) { return op.dtype == DT_E4M3 ? -1 : pick_ep(op.args); }
 
 template <typename T, int BN>
 static int launch_ep(const GemmOp& op, cudaStream_t st) {

@@ -91,9 +91,15 @@ struct GemmOp {
   double flops;
 };
 
+// Epilogue specialisations of gemm_tc_kernel (gemm_tc.cu): EP_GENERIC keeps every feature behind runtime flags, the others
+// compile in only what the hot GEMMs use (bias; bias + activation; LayerNorm fold (+ GELU); residual / layer-scale / statistics).
+enum : int { EP_GENERIC = 0, EP_BIAS = 1, EP_BIAS_ACT = 2, EP_LN = 3, EP_LN_GELU = 4, EP_RESID = 5 };
+
 // Returns 0 on success; on failure fills *err.
 int gemm_build(const GemmDesc& d, GemmOp* op, std::string* err);
 int gemm_launch(const GemmOp& op, cudaStream_t stream);
+// The EP_* specialisation gemm_launch runs for a built 16-bit op (-1 for an e4m3 op).
+int gemm_epilogue(const GemmOp& op);
 
 // FP8 GEMM (gemm_e4m3_kernel): out[m, n] = act(a_scale[m] * w_scale[n] * sum_k A[m, k] W[n, k] + bias[n]) in fp16, A [M, lda]
 // and W [N, K] e4m3 codes (both K-major), fp32 accumulation on the tensor cores.  act: ACT_NONE or ACT_GELU (the fc1

@@ -173,11 +173,15 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const LayerNormArgs p) {
   }
 }
 
+// rows per warp: 4 when there are enough rows to keep every SM busy with a quarter of the warps (and C <= 512), else 1
+int layernorm_rows_per_warp(long long rows, int C) {
+  return (C + 255) / 256 <= 2 && rows >= 8LL * 4 * 2 * current_device_sms() ? 4 : 1;
+}
+
 template <typename T>
 static int ln_dispatch(const LayerNormArgs& a, cudaStream_t st) {
   const int chunks = (a.C + 255) / 256;
-  // rows per warp: 4 when there are enough rows to keep every SM busy with a quarter of the warps, else 1
-  const bool many = a.rows >= 8LL * 4 * 2 * current_device_sms();
+  const bool many = layernorm_rows_per_warp(a.rows, a.C) == 4;
   const unsigned grid4 = static_cast<unsigned>((a.rows + 31) / 32), grid1 = static_cast<unsigned>((a.rows + 7) / 8);
   if (chunks == 1) { if (many) launch_k(layernorm_kernel<T, 1, 4>, dim3(grid4), dim3(256), 0, st, a); else launch_k(layernorm_kernel<T, 1, 1>, dim3(grid1), dim3(256), 0, st, a); }
   else if (chunks == 2) { if (many) launch_k(layernorm_kernel<T, 2, 4>, dim3(grid4), dim3(256), 0, st, a); else launch_k(layernorm_kernel<T, 2, 1>, dim3(grid1), dim3(256), 0, st, a); }

@@ -19,6 +19,8 @@ struct LayerNormArgs {
   const float* w3; const float* b3; float eps3; void* y3; int ldy3;
 };
 int layernorm_launch(int dtype, const LayerNormArgs& a, cudaStream_t st);
+// rows each warp of layernorm_launch's kernel takes for this size (1 or 4)
+int layernorm_rows_per_warp(long long rows, int C);
 // the e4m3 mode's LayerNorm (rowops.cu layernorm_e4m3_kernel): fp16 rows [rows, C] -> e4m3 codes [rows, ldq] + fp32
 // row_scale [rows]; C % 8 == 0, C <= 1024, ldx / ldq multiples of 8.  -2: bad sizes
 int layernorm_e4m3_launch(const void* x, int ldx, long long rows, int C, float eps, uint8_t* q, int ldq, float* row_scale, cudaStream_t st);
