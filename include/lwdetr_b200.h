@@ -96,6 +96,9 @@ LWDETR_API int lwdetr_gemm_ex(lwdetr_gemm_args* args, void* stream);
 LWDETR_API int lwdetr_conv3x3(int dtype, const void* X, int ldx, int B, int OH, int OW, int stride, int Cin,
                               const void* W, int N, const float* bias, int act, void* out, int ld_out,
                               void* stream);
+/* Host query (no device needed): the output tile lwdetr_conv3x3 and the model's 3x3 convolutions use for an OH x OW grid,
+ * either stride.  *tw x *th pixels, tw * th <= 128; the grid is covered by ceil(OW / tw) x ceil(OH / th) tiles. */
+LWDETR_API int lwdetr_conv3x3_plan(int OH, int OW, int32_t* tw, int32_t* th);
 
 /* LayerNorm over the last dimension of rows (vit.py:198,217 eps 1e-6; projector.py:21-47 on NHWC rows;
  * transformer.py norms eps 1e-5).  x/y 16-bit with leading dimensions, w/b fp32 [C], C % 8 == 0, C <= 1024. */
@@ -179,6 +182,14 @@ LWDETR_API int lwdetr_msda_forward(int dtype, const void* value_hm, int64_t v_im
                                    int ld_ol, const float* ref, const float* valid_ratio, void* out, int ld_out, int B,
                                    int S, int Lq, int M, int L, int P, const int32_t* spatial_shapes_host,
                                    const int32_t* level_start_host, void* stream);
+/* Host query (no device needed): the plan lwdetr_msda_forward builds for a level table (same arguments, same validation and
+ * error message).  *nbands = 0: the direct-gather kernel runs.  Otherwise the staged kernel streams *nbands bands (at most
+ * LWDETR_MSDA_MAX_BANDS) of each (image, head) slab; bands, int32 [LWDETR_MSDA_MAX_BANDS, 6], receives one row per band:
+ *   level, row0 (first staged row), own0, own1 (the band samples every location whose floor(y) lies in [own0, own1]),
+ *   tok0 (first staged token inside the slab), bytes (staged bytes, rows * W * 32). */
+enum { LWDETR_MSDA_MAX_BANDS = 16 };
+LWDETR_API int lwdetr_msda_plan(int L, const int32_t* spatial_shapes_host, const int32_t* level_start_host, int S, int32_t* nbands,
+                                int32_t* bands);
 
 /* torch.topk(score, k, dim=1)[1] for fp32 score [B, S] -> int32 idx [B, k], sorted, ties -> lower index
  * (transformer.py:246).  Any S >= k; above S = 16384 (large inputs) a radix select that streams the row, with k <= 4096. */

@@ -28,6 +28,8 @@ _SIGNATURES = {
     "lwdetr_ms_deform_attn_forward": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "lwdetr_ms_deform_attn_backward": (_i, [_vp] * 9 + [_i] * 8 + [_vp]),
     "lwdetr_msda_forward": (_i, [_i, _vp, _i64, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "lwdetr_msda_plan": (_i, [_i, _vp, _vp, _i, _vp, _vp]),
+    "lwdetr_conv3x3_plan": (_i, [_i, _i, _vp, _vp]),
     "lwdetr_topk": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "lwdetr_postprocess": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_layernorm_e4m3": (_i, [_vp, _i, _i64, _i, _f, _vp, _i, _vp, _vp]),
@@ -236,14 +238,40 @@ def value_to_head_major(value, B, S, M):
     return value.reshape(B, S, M, 16).permute(0, 2, 1, 3).contiguous()
 
 
-def msda_forward(value_hm, offs_logits, ref, out, B, S, Lq, M, L, P, shapes, valid_ratio=None, v_image_stride=None):
-    """value_hm head-major [B, M, S, 16], offs_logits [B*Lq, 3*M*L*P], ref fp32 [B*Lq, 4], out [B*Lq, M*16]."""
-    sh = (ctypes.c_int32 * (2 * L))(*[v for hw in shapes for v in hw])
+def _level_table(shapes):
+    """HOST int32 arrays (spatial shapes [L, 2], level starts [L]) of consecutive levels of the given (H, W)."""
     starts, acc = [], 0
     for h, w in shapes:
         starts.append(acc)
         acc += h * w
-    st = (ctypes.c_int32 * L)(*starts)
+    return (ctypes.c_int32 * (2 * len(shapes)))(*[v for hw in shapes for v in hw]), (ctypes.c_int32 * len(shapes))(*starts)
+
+
+MSDA_MAX_BANDS = 16
+
+
+def msda_plan(shapes, S=None):
+    """lwdetr_msda_plan (no device): the bands msda_forward streams for consecutive levels of the given (H, W), S = their
+    token count unless given.  A list of (level, row0, own0, own1, tok0, bytes); empty: the direct-gather kernel runs."""
+    sh, st = _level_table(shapes)
+    S = sum(h * w for h, w in shapes) if S is None else S
+    nb = ctypes.c_int32()
+    rows = (ctypes.c_int32 * (6 * MSDA_MAX_BANDS))()
+    check(lib().lwdetr_msda_plan(len(shapes), ctypes.cast(sh, _vp), ctypes.cast(st, _vp), S, ctypes.byref(nb), ctypes.cast(rows, _vp)),
+          "lwdetr_msda_plan")
+    return [tuple(rows[6 * k:6 * k + 6]) for k in range(nb.value)]
+
+
+def conv3x3_plan(OH, OW):
+    """lwdetr_conv3x3_plan (no device): the (TW, TH) output tile of the implicit-GEMM 3x3 convolution over an OH x OW grid."""
+    tw, th = ctypes.c_int32(), ctypes.c_int32()
+    check(lib().lwdetr_conv3x3_plan(OH, OW, ctypes.byref(tw), ctypes.byref(th)), "lwdetr_conv3x3_plan")
+    return tw.value, th.value
+
+
+def msda_forward(value_hm, offs_logits, ref, out, B, S, Lq, M, L, P, shapes, valid_ratio=None, v_image_stride=None):
+    """value_hm head-major [B, M, S, 16], offs_logits [B*Lq, 3*M*L*P], ref fp32 [B*Lq, 4], out [B*Lq, M*16]."""
+    sh, st = _level_table(shapes)
     stride = M * S * 16 if v_image_stride is None else v_image_stride
     check(lib().lwdetr_msda_forward(kernel_dtype_code(value_hm.dtype), ptr(value_hm), stride, ptr(offs_logits),
                                     offs_logits.stride(0), ptr(ref), ptr(valid_ratio), ptr(out), out.stride(0), B, S, Lq, M, L, P,

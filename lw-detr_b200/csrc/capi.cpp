@@ -97,6 +97,15 @@ int lwdetr_conv3x3(int dtype, const void* X, int ldx, int B, int OH, int OW, int
   return 0;
 }
 
+int lwdetr_conv3x3_plan(int OH, int OW, int32_t* tw, int32_t* th) {
+  if (!tw || !th) return fail("lwdetr_conv3x3_plan: null pointer");
+  if (OH < 1 || OW < 1) return fail("lwdetr_conv3x3_plan: OH and OW must be positive");
+  int w = 0, h = 0;
+  lwb::conv_tile_plan(OH, OW, &w, &h);
+  *tw = w; *th = h;
+  return 0;
+}
+
 
 int lwdetr_layernorm(int dtype, const void* x, int ldx, void* y, int ldy, const float* w, const float* b, float eps,
                      int64_t rows, int C, void* stream) {
@@ -176,6 +185,25 @@ int lwdetr_ms_deform_attn_backward(const float* value, const int64_t* spatial_sh
 }
 
 
+static const char kMsdaBadTable[] = ": invalid level table (a level is empty or extends past S)";
+static_assert(LWDETR_MSDA_MAX_BANDS == lwb::MSDA_MAX_BANDS, "band table size");
+
+int lwdetr_msda_plan(int L, const int32_t* spatial_shapes_host, const int32_t* level_start_host, int S, int32_t* nbands, int32_t* bands) {
+  if (!spatial_shapes_host || !level_start_host || !nbands || !bands) return fail("lwdetr_msda_plan: null pointer");
+  if (L < 1 || L > lwb::MSDA_MAX_LEVELS) return fail("lwdetr_msda_plan: 1..4 levels supported");
+  lwb::MsdaArgs a{};
+  a.levels = L; a.S = S;
+  for (int l = 0; l < L; ++l) { a.lvl_h[l] = spatial_shapes_host[2 * l]; a.lvl_w[l] = spatial_shapes_host[2 * l + 1]; a.lvl_start[l] = level_start_host[l]; }
+  if (lwb::msda_plan(&a)) return fail(std::string("lwdetr_msda_plan") + kMsdaBadTable);
+  *nbands = a.nbands;
+  for (int k = 0; k < a.nbands; ++k) {
+    const lwb::MsdaBand& b = a.bands[k];
+    const int32_t row[6] = {b.level, b.row0, b.own0, b.own1, b.tok0, b.bytes};
+    for (int j = 0; j < 6; ++j) bands[6 * k + j] = row[j];
+  }
+  return 0;
+}
+
 int lwdetr_msda_forward(int dtype, const void* value_hm, int64_t v_image_stride, const void* offs_logits, int ld_ol, const float* ref,
                         const float* valid_ratio, void* out, int ld_out, int B, int S, int Lq, int M, int L, int P,
                         const int32_t* spatial_shapes_host, const int32_t* level_start_host, void* stream) {
@@ -187,7 +215,7 @@ int lwdetr_msda_forward(int dtype, const void* value_hm, int64_t v_image_stride,
   a.value = value_hm; a.v_b_stride = v_image_stride; a.offs_logits = offs_logits; a.ld_ol = ld_ol; a.ref = ref; a.valid_ratio = valid_ratio;
   a.out = out; a.ld_out = ld_out; a.batch = B; a.nq = Lq; a.heads = M; a.levels = L; a.points = P; a.S = S;
   for (int l = 0; l < L; ++l) { a.lvl_h[l] = spatial_shapes_host[2 * l]; a.lvl_w[l] = spatial_shapes_host[2 * l + 1]; a.lvl_start[l] = level_start_host[l]; }
-  if (lwb::msda_plan(&a)) return fail("lwdetr_msda_forward: invalid level table (a level is empty or extends past S)");
+  if (lwb::msda_plan(&a)) return fail(std::string("lwdetr_msda_forward") + kMsdaBadTable);
   int e = lwb::msda_launch(dtype, a, static_cast<cudaStream_t>(stream));
   if (e == -2) return fail("lwdetr_msda_forward: unsupported (levels, points) combination");
   if (e) return cuda_fail(e, "lwdetr_msda_forward launch");

@@ -608,6 +608,18 @@ static int pick_bn(int N, int m_tiles) {
   return bn;
 }
 
+void conv_tile_plan(int OH, int OW, int* tw_out, int* th_out) {
+  // tile = TW x TH output pixels (<= 128): maximise useful rows
+  int best_tw = 1, best_th = 1; double best_u = -1;
+  for (int tw = 1; tw <= std::min(OW, 128); ++tw) {
+    const int th = std::min(128 / tw, OH);
+    const long long tiles = static_cast<long long>((OW + tw - 1) / tw) * ((OH + th - 1) / th);
+    const double u = static_cast<double>(OW) * OH / (tiles * 128.0);
+    if (u > best_u + 1e-9) { best_u = u; best_tw = tw; best_th = th; }
+  }
+  *tw_out = best_tw; *th_out = best_th;
+}
+
 int gemm_build(const GemmDesc& d, GemmOp* op, std::string* err) {
   std::memset(op, 0, sizeof(*op));
   if (d.dtype != DT_F16 && d.dtype != DT_BF16) { *err = "gemm: dtype must be fp16 or bf16"; return -1; }
@@ -653,15 +665,7 @@ int gemm_build(const GemmDesc& d, GemmOp* op, std::string* err) {
     const int cin = d.K / 9;
     a.cin_blocks = cin / BK;
     a.OH = d.OH; a.OW = d.OW;
-    // tile = TW x TH output pixels (<= 128): maximise useful rows
-    int best_tw = 1, best_th = 1; double best_u = -1;
-    for (int tw = 1; tw <= std::min(d.OW, 128); ++tw) {
-      const int th = std::min(128 / tw, d.OH);
-      const long long tiles = static_cast<long long>((d.OW + tw - 1) / tw) * ((d.OH + th - 1) / th);
-      const double u = static_cast<double>(d.OW) * d.OH / (tiles * 128.0);
-      if (u > best_u + 1e-9) { best_u = u; best_tw = tw; best_th = th; }
-    }
-    a.TW = best_tw; a.TH = best_th;
+    conv_tile_plan(d.OH, d.OW, &a.TW, &a.TH);
     a.tiles_x = (d.OW + a.TW - 1) / a.TW;
     a.tiles_y = (d.OH + a.TH - 1) / a.TH;
     m_tiles = d.B * a.tiles_x * a.tiles_y;

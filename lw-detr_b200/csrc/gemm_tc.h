@@ -95,6 +95,10 @@ struct GemmOp {
 // compile in only what the hot GEMMs use (bias; bias + activation; LayerNorm fold (+ GELU); residual / layer-scale / statistics).
 enum : int { EP_GENERIC = 0, EP_BIAS = 1, EP_BIAS_ACT = 2, EP_LN = 3, EP_LN_GELU = 4, EP_RESID = 5 };
 
+// Output tile of the implicit-GEMM 3x3 convolution over an OH x OW grid (OH, OW >= 1): TW x TH pixels, TW * TH <= 128, the
+// pair that maximises the share of useful A rows.  Host only; gemm_build uses it for both strides.
+void conv_tile_plan(int OH, int OW, int* tw, int* th);
+
 // Returns 0 on success; on failure fills *err.
 int gemm_build(const GemmDesc& d, GemmOp* op, std::string* err);
 int gemm_launch(const GemmOp& op, cudaStream_t stream);

@@ -215,6 +215,8 @@ __global__ void __launch_bounds__(MS_THREADS, 1) msda_fwd_kernel(const __grid_co
           const float fy = py - yf, fx = px - xf;
           // clamped corner tokens (always readable), zero weight for the corners outside the image (cuh:58-84)
           const int ya = max(y0, 0), yb = min(y0 + 1, H - 1), xa = max(x0, 0), xb = min(x0 + 1, W - 1);
+          // wy0 reuses the rounded w * fy: exact to 2^-24 w only, all of wy0 when fy -> 1 above the bottom border
+          // (tests/test_geometry_cpu.py msda_bound carries that term; msda_gather_kernel has the same form)
           const float wy0 = y0 >= 0 ? w - w * fy : 0.f, wy1 = y0 + 1 < H ? w * fy : 0.f;
           const float wx0 = x0 >= 0 ? 1.f - fx : 0.f, wx1 = x0 + 1 < W ? fx : 0.f;
           wc[k][0] = wy0 * wx0; wc[k][1] = wy0 * wx1; wc[k][2] = wy1 * wx0; wc[k][3] = wy1 * wx1;
@@ -379,7 +381,7 @@ __global__ void __launch_bounds__(256) msda_gather_kernel(const __grid_constant_
       const float fy = py - yf, fx = px - xf;
       // clamped corner tokens (always readable), zero weight for the corners outside the level (cuh:58-84)
       const int ya = max(y0, 0), yb = min(y0 + 1, H - 1), xa = max(x0, 0), xb = min(x0 + 1, W - 1);
-      const float wy0 = y0 >= 0 ? w - w * fy : 0.f, wy1 = y0 + 1 < H ? w * fy : 0.f;
+      const float wy0 = y0 >= 0 ? w - w * fy : 0.f, wy1 = y0 + 1 < H ? w * fy : 0.f;   // rounding of wy0: see msda_fwd_kernel
       const float wx0 = x0 >= 0 ? 1.f - fx : 0.f, wx1 = x0 + 1 < W ? fx : 0.f;
       const float wc[4] = {wy0 * wx0, wy0 * wx1, wy1 * wx0, wy1 * wx1};
       const long long tok[4] = {1LL * ya * W + xa, 1LL * ya * W + xb, 1LL * yb * W + xa, 1LL * yb * W + xb};

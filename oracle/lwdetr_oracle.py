@@ -202,7 +202,7 @@ def msda_core(value, level_shapes, loc, weight):
       out[b,q,m,:] = sum_{l,p} weight * bilinear(value_l[b,:,m,:], (x*W - .5, y*H - .5)), zero outside."""
     B, S, M, D = value.shape
     Q, P = loc.shape[1], loc.shape[4]
-    out = torch.zeros(B, Q, M, D, dtype=value.dtype)
+    out = torch.zeros(B, Q, M, D, dtype=value.dtype, device=value.device)
     start = 0
     for l, (H, W) in enumerate(level_shapes):
         v = value[:, start:start + H * W].permute(0, 2, 1, 3)                  # [B, M, HW, D]
