@@ -205,6 +205,49 @@ LWDETR_API int lwdetr_postprocess(const float* pred_logits, const float* pred_bo
                                   int num_classes, int num_select, int32_t* work, float* scores, int32_t* labels, float* boxes,
                                   void* stream);
 
+/* Tiled (sliced) detection of high-resolution frames: the detector runs on overlapping full-resolution crops of each frame
+ * plus one downscaled view of the whole frame, and the per-view detections are merged per frame.  Three calls:
+ *   1. lwdetr_forward_frames (or _nv12) on the V crop views, all on one run size H x W (a crop is an lwdetr_frame: device
+ *      pointer of its first pixel, its size, the surface's pitch; NV12 crops need even offsets);
+ *   2. lwdetr_postprocess with k = num_select and target_sizes = each view's crop size (ch, cw): boxes in crop pixels;
+ *   3. lwdetr_tile_merge.
+ * The views (b200.config.tile_views; a host in another language reproduces them from this rule).  Per axis, with n the
+ * frame's side, t the tile side (default: the run side), H the run side, overlap in [0, 0.5]:
+ *   stride s = t - (int)(overlap * t + 0.5);
+ *   starts: [0] if n <= t, else p = 0, s, 2s, ... while p + t < n, then n - t; every start rounded down to even (NV12
+ *     chroma covers 2x2 pixels), duplicates dropped.  When n - t is odd the last tile ends one pixel short of the edge;
+ *   crop side c = min(t, n); destination side H when c == t, else (2 * c * H + t) / (2 * t) (integer division, i.e.
+ *     c * H / t rounded half up) clamped to [1, H], placed top-left on the padded, masked canvas;
+ *   views: per frame the tiles in row-major order, then (optionally) the whole frame stretched to H x W; frames in order.
+ *   every crop side at most 16 times its destination side (the resize's downscale limit): t <= 16 H, and a partial tile's
+ *     rounded destination checked too.
+ * lwdetr_tile_merge: scores fp32 [V, k], labels int32 [V, k], boxes fp32 [V, k, 4] (xyxy in view crop pixels, 16-byte
+ * aligned), all DEVICE, as lwdetr_postprocess writes them; views a HOST array of V {frame, x0, y0} (frames non-decreasing in
+ * [0, num_frames), so each frame's views are contiguous; the caller may reuse it on return).  Per frame:
+ *   candidates: every (view, rank) with score >= score_threshold, box moved to frame pixels by one fp32 add of
+ *     (x0, y0, x0, y0);
+ *   order: score descending, ties to the lower flat index view * k + rank;
+ *   greedy class-aware NMS: a candidate is dropped when an earlier KEPT candidate with the same label overlaps it beyond
+ *     iou_threshold (in [0, 1]).  fp32, each operation rounded on its own (no fused multiply-add):
+ *       ix = max(0, min(ax2, bx2) - max(ax1, bx1)), iy likewise, inter = ix * iy, area = max(0, x2 - x1) * max(0, y2 - y1);
+ *       LWDETR_TILE_IOU: inter > thr * ((area_a + area_b) - inter);  LWDETR_TILE_IOS: inter > thr * min(area_a, area_b).
+ *     A box whose area is not > 0 never suppresses and is never suppressed.  IoS (intersection over the smaller box) is the
+ *     usual choice here: a box cut off at a tile border lies inside the whole-object box of the neighbouring tile or the
+ *     full view, while its IoU with that box can stay below 0.5;
+ *   output: the first max_det kept candidates in that order: out_scores fp32 [num_frames, max_det], out_labels int32,
+ *     out_boxes fp32 [num_frames, max_det, 4] (frame pixels, 16-byte aligned), counts int32 [num_frames]; unused slots get
+ *     score 0, label -1 and a zero box.
+ * Limits: at most 16384 candidates (views * k) and 2048 views per frame, max_det in [1, 1024].  Asynchronous, nothing
+ * allocated per call, no device scratch. */
+enum { LWDETR_TILE_IOU = 0, LWDETR_TILE_IOS = 1 };
+typedef struct {
+  int32_t frame, x0, y0;
+} lwdetr_tile_view;
+LWDETR_API int lwdetr_tile_merge(const float* scores, const int32_t* labels, const float* boxes, int V, int k,
+                                 const lwdetr_tile_view* views, int num_frames, float score_threshold, float iou_threshold,
+                                 int metric, int max_det, float* out_scores, int32_t* out_labels, float* out_boxes,
+                                 int32_t* counts, void* stream);
+
 /* The LWDETR_F16_E4M3 mode's two kernels.
  * lwdetr_layernorm_e4m3: fp16 rows x [rows, ldx] -> e4m3 codes q [rows, ldq] (uint8) and fp32 row_scale [rows], as the mode's
  *   activation contract above (x^ without the LayerNorm affine, eps as given).  C % 8 == 0, C <= 1024, ldx and ldq

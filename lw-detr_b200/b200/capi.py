@@ -32,6 +32,7 @@ _SIGNATURES = {
     "lwdetr_conv3x3_plan": (_i, [_i, _i, _vp, _vp]),
     "lwdetr_topk": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "lwdetr_postprocess": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "lwdetr_tile_merge": (_i, [_vp, _vp, _vp, _i, _i, _vp, _i, _f, _f, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_layernorm_e4m3": (_i, [_vp, _i, _i64, _i, _f, _vp, _i, _vp, _vp]),
     "lwdetr_gemm_e4m3": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _i, _vp]),
     "lwdetr_vit_mlp": (_i, [_i, _vp, _i, _i, _vp, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp]),
@@ -351,6 +352,42 @@ def postprocess(pred_logits, pred_boxes, target_sizes, num_select):
     check(lib().lwdetr_postprocess(ptr(logits), ptr(boxes), ptr(ts), B, nq, ncls, num_select, ptr(work), ptr(scores), ptr(labels),
                                    ptr(out), stream_ptr()), "lwdetr_postprocess")
     return scores, labels, out
+
+
+TILE_METRICS = {"iou": 0, "ios": 1}     # LWDETR_TILE_IOU / LWDETR_TILE_IOS
+
+
+class TileViewStruct(ctypes.Structure):
+    """lwdetr_tile_view (include/lwdetr_b200.h)."""
+    _fields_ = [("frame", ctypes.c_int32), ("x0", ctypes.c_int32), ("y0", ctypes.c_int32)]
+
+
+def tile_merge(scores, labels, boxes, views, num_frames, score_threshold=0.0, iou_threshold=0.5, metric="ios", max_det=300):
+    """lwdetr_tile_merge: the per-view output of postprocess() (scores fp32 [V, k], labels int32 [V, k], xyxy boxes fp32
+    [V, k, 4] in each view's crop pixels, CUDA) and the views as (frame, x0, y0) triples (frames non-decreasing) -> per frame
+    the first max_det survivors of a class-aware greedy NMS over all its views, in frame pixels: (scores fp32 [F, max_det],
+    labels int32 [F, max_det], boxes fp32 [F, max_det, 4], counts int32 [F]), unused slots score 0, label -1, zero box.
+    metric: "ios" (intersection over the smaller box) or "iou".  Stream-ordered, no synchronisation."""
+    import torch
+    if metric not in TILE_METRICS:
+        raise RuntimeError("tile_merge: metric must be one of %s, got %r" % (", ".join(TILE_METRICS), metric))
+    V, k = scores.shape
+    if tuple(labels.shape) != (V, k) or tuple(boxes.shape) != (V, k, 4) or len(views) != V:
+        raise RuntimeError("tile_merge: scores %s, labels %s, boxes %s and %d views do not describe one [V, k] set"
+                           % (tuple(scores.shape), tuple(labels.shape), tuple(boxes.shape), len(views)))
+    if scores.dtype != torch.float32 or labels.dtype != torch.int32 or boxes.dtype != torch.float32:
+        raise RuntimeError("tile_merge: scores / boxes must be float32 and labels int32")
+    scores, labels, boxes = scores.contiguous(), labels.contiguous(), boxes.contiguous()
+    arr = (TileViewStruct * V)(*[TileViewStruct(int(f), int(x0), int(y0)) for f, x0, y0 in views])
+    F, dev = int(num_frames), scores.device
+    out_s = torch.empty(F, max_det, device=dev, dtype=torch.float32)
+    out_l = torch.empty(F, max_det, device=dev, dtype=torch.int32)
+    out_b = torch.empty(F, max_det, 4, device=dev, dtype=torch.float32)
+    counts = torch.empty(F, device=dev, dtype=torch.int32)
+    check(lib().lwdetr_tile_merge(ptr(scores), ptr(labels), ptr(boxes), V, k, ctypes.cast(arr, _vp), F, float(score_threshold),
+                                  float(iou_threshold), TILE_METRICS[metric], int(max_det), ptr(out_s), ptr(out_l), ptr(out_b),
+                                  ptr(counts), stream_ptr(dev)), "lwdetr_tile_merge")
+    return out_s, out_l, out_b, counts
 
 
 def layernorm_e4m3(x, eps=1e-6):
@@ -752,7 +789,7 @@ class Engine:
         return res, logits, boxes, aux
 
     def forward_frames(self, frames, size=None, fit="stretch", short_side=None, max_side=None, want_aux=True, topk_override=None,
-                       mean=IMAGENET_MEAN, std=IMAGENET_STD, colorspace=None):
+                       mean=IMAGENET_MEAN, std=IMAGENET_STD, colorspace=None, dsts=None):
         """Raw camera / decoder frames of any size, RGB or NV12 (told apart by their form):
           RGB: a list of CUDA uint8 [h, w, 3] tensors (each its own size; views with packed RGB pixels are fine) or one
             [B, h, w, 3] tensor;
@@ -764,12 +801,19 @@ class Engine:
         fit="stretch": to `size` = (H, W), default (img_size, img_size).  fit="keep_aspect": to the reference's
         resize(size=short_side, max_size=max_side), frames top-left on the run size (`size`, or run_size of the largest resized
         frame), the rest padded with a mask made on the device (b200.config.frame_sizes).  Source sizes and the frame format
-        are not part of the plan: only a new (B, H, W) re-plans.  Returns the dict of forward(), plus "frame_sizes": the
-        (dst_h, dst_w) of each frame."""
+        are not part of the plan: only a new (B, H, W) re-plans.  dsts: explicit (dst_h, dst_w) per frame, each placed
+        top-left on the run size `size` (default img_size x img_size) with the padding mask (the crop views of tiled
+        detection, b200.config.tile_views); fit / short_side / max_side do not apply then.  Returns the dict of forward(),
+        plus "frame_sizes": the (dst_h, dst_w) of each frame."""
         import torch
-        from .config import frame_sizes
+        from .config import explicit_frame_sizes, frame_sizes
         fb = Frames(frames, self.device, colorspace)
-        (H, W), dsts = frame_sizes(self.cfg, fb.sizes, size, fit, short_side, max_side)
+        if dsts is None:
+            (H, W), dsts = frame_sizes(self.cfg, fb.sizes, size, fit, short_side, max_side)
+        else:
+            if fit != "stretch" or short_side is not None or max_side is not None:
+                raise RuntimeError("lwdetr_b200: dsts= gives every frame's size; fit / short_side / max_side do not combine with it")
+            (H, W), dsts = explicit_frame_sizes(self.cfg, len(fb.items), dsts, size)
         B = len(fb.items)
         res, logits, boxes, aux = self._outputs(B, self.device, want_aux)
         ov = None

@@ -135,6 +135,97 @@ def frame_sizes(cfg, shapes, size=None, fit="stretch", short_side=None, max_side
     return (H, W), dsts
 
 
+def explicit_frame_sizes(cfg, count, dsts, size=None):
+    """Run size (H, W) (`size`, default img_size x img_size) and the given per-frame (dst_h, dst_w), checked: one per frame,
+    each side in [1, run side]."""
+    H, W = (cfg.img_size, cfg.img_size) if size is None else (int(size[0]), int(size[1]))
+    check_input_size(cfg, H, W)
+    dsts = [(int(dh), int(dw)) for dh, dw in dsts]
+    if len(dsts) != count:
+        raise RuntimeError("lwdetr_b200: %d dsts for %d frames" % (len(dsts), count))
+    for dh, dw in dsts:
+        if not (1 <= dh <= H and 1 <= dw <= W):
+            raise RuntimeError("lwdetr_b200: dst %dx%d does not fit the run size %dx%d" % (dh, dw, H, W))
+    return (H, W), dsts
+
+
+# Limits of tiled detection: the resize's downscale factor per axis (include/lwdetr_b200.h, lwdetr_frame) and what
+# lwdetr_tile_merge takes per frame.
+RESIZE_MAX_DOWNSCALE = 16
+TILE_MAX_CANDIDATES, TILE_MAX_VIEWS = 16384, 2048
+
+
+def _tile_starts(n, t, s):
+    if n <= t:
+        return [0]
+    starts, p = [], 0
+    while p + t < n:
+        starts.append(p)
+        p += s
+    starts.append(n - t)
+    out = []
+    for p in starts:
+        p -= p % 2
+        if not out or out[-1] != p:
+            out.append(p)
+    return out
+
+
+def _tile_dst(c, t, run):
+    return run if c == t else min(max((2 * c * run + t) // (2 * t), 1), run)
+
+
+def tile_views(cfg, shapes, tile=None, overlap=0.2, full_frame=True, size=None, per_view=100):
+    """Views of tiled (sliced) detection for frames of the given (h, w) shapes -> ((H, W), views), every view a tuple
+    (frame, y0, x0, ch, cw, dst_h, dst_w): the crop rows [y0, y0 + ch) and columns [x0, x0 + cw) of frame `frame`, resized to
+    dst_h x dst_w top-left on the run size (H, W) = `size` (default img_size x img_size).  The rule, per axis of length n with
+    tile side t (`tile` = (th, tw) or one int, in source pixels, default the run size) and run side R:
+      stride s = t - int(overlap * t + 0.5), overlap in [0, 0.5];
+      starts [0] if n <= t, else p = 0, s, 2s, ... while p + t < n, then n - t; each rounded down to even (one rule for RGB
+        and NV12, whose chroma covers 2x2 pixels: an NV12 crop at even offsets is exact), duplicates dropped.  When n - t is
+        odd, the last tile therefore ends one pixel short of the frame's edge; the full-frame view still sees that strip.
+        Every other pixel is covered whenever the overlap is at least one pixel (s < t);
+      crop side min(t, n); destination R for a full tile (a 1:1 copy when t == R), else the crop scaled as the full tiles
+        are, c * R / t rounded half up and clamped to [1, R] (a partial tile, top-left on the padded, masked canvas).
+    Views come per frame, tiles in row-major order, then (full_frame) the whole frame stretched to (H, W), which is what
+    detect() runs; frames in input order.  RuntimeError for an overlap outside [0, 0.5], a tile more than 16x the run size
+    on an axis, any view whose crop side is more than 16x its destination side (a partial tile, whose rounded destination
+    may be as small as 1; with full_frame, a frame more than 16x the run size), or a frame with more views than
+    lwdetr_tile_merge takes (2048, and views * per_view <= 16384)."""
+    H, W = (cfg.img_size, cfg.img_size) if size is None else (int(size[0]), int(size[1]))
+    check_input_size(cfg, H, W)
+    th, tw = (H, W) if tile is None else ((int(tile), int(tile)) if isinstance(tile, int) else (int(tile[0]), int(tile[1])))
+    if th < 1 or tw < 1:
+        raise RuntimeError("lwdetr_b200: tile %dx%d must have positive sides" % (th, tw))
+    if not (0.0 <= overlap <= 0.5):
+        raise RuntimeError("lwdetr_b200: overlap must be in [0, 0.5], got %r" % (overlap,))
+    if th > RESIZE_MAX_DOWNSCALE * H or tw > RESIZE_MAX_DOWNSCALE * W:
+        raise RuntimeError("lwdetr_b200: tile %dx%d on the run size %dx%d is a downscale factor above %d"
+                           % (th, tw, H, W, RESIZE_MAX_DOWNSCALE))
+    sh, sw = th - int(overlap * th + 0.5), tw - int(overlap * tw + 0.5)
+    views = []
+    for f, (h, w) in enumerate(shapes):
+        h, w = int(h), int(w)
+        ch, cw = min(th, h), min(tw, w)
+        dh, dw = _tile_dst(ch, th, H), _tile_dst(cw, tw, W)
+        if ch > RESIZE_MAX_DOWNSCALE * dh or cw > RESIZE_MAX_DOWNSCALE * dw:
+            # a partial tile's destination is rounded and clamped to >= 1, so its factor can exceed the tile's own
+            raise RuntimeError("lwdetr_b200: frame %d (%dx%d): its %dx%d crop goes to %dx%d, a downscale factor above %d"
+                               % (f, h, w, ch, cw, dh, dw, RESIZE_MAX_DOWNSCALE))
+        mine = [(f, y0, x0, ch, cw, dh, dw) for y0 in _tile_starts(h, th, sh) for x0 in _tile_starts(w, tw, sw)]
+        if full_frame:
+            if h > RESIZE_MAX_DOWNSCALE * H or w > RESIZE_MAX_DOWNSCALE * W:
+                raise RuntimeError("lwdetr_b200: frame %d (%dx%d) on the run size %dx%d is a downscale factor above %d"
+                                   % (f, h, w, H, W, RESIZE_MAX_DOWNSCALE))
+            mine.append((f, 0, 0, h, w, H, W))
+        if len(mine) > TILE_MAX_VIEWS or len(mine) * per_view > TILE_MAX_CANDIDATES:
+            raise RuntimeError("lwdetr_b200: frame %d (%dx%d) makes %d views of %d detections; the merge takes at most %d views "
+                               "and %d candidates per frame (use a larger tile or a smaller per_view)"
+                               % (f, h, w, len(mine), per_view, TILE_MAX_VIEWS, TILE_MAX_CANDIDATES))
+        views += mine
+    return (H, W), views
+
+
 _W10 = (0, 1, 3, 6, 7, 9)
 _T10 = (2, 4, 5, 9)
 CONFIGS = {

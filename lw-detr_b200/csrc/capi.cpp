@@ -18,6 +18,7 @@
 #include "msda.h"
 #include "resize.h"
 #include "rowops.h"
+#include "tiles.h"
 
 
 namespace {
@@ -238,6 +239,36 @@ int lwdetr_postprocess(const float* pred_logits, const float* pred_boxes, const 
                                   static_cast<cudaStream_t>(stream));
   if (e == -2) return fail("lwdetr_postprocess: need num_select <= slice length and slices * num_select <= 16384");
   if (e) return cuda_fail(e, "lwdetr_postprocess launch");
+  return 0;
+}
+
+static_assert(sizeof(lwdetr_tile_view) == sizeof(lwb::TileViewHost) && LWDETR_TILE_IOU == lwb::TILE_IOU &&
+              LWDETR_TILE_IOS == lwb::TILE_IOS, "tile view layout");
+
+int lwdetr_tile_merge(const float* scores, const int32_t* labels, const float* boxes, int V, int k, const lwdetr_tile_view* views,
+                      int num_frames, float score_threshold, float iou_threshold, int metric, int max_det, float* out_scores,
+                      int32_t* out_labels, float* out_boxes, int32_t* counts, void* stream) {
+  if (V < 1 || k < 1 || num_frames < 1) return fail("lwdetr_tile_merge: need V >= 1, k >= 1 and num_frames >= 1");
+  if (max_det < 1 || max_det > lwb::TILE_MAX_DET) return fail("lwdetr_tile_merge: max_det must be in [1, 1024]");
+  if (!scores || !labels || !boxes || !views || !out_scores || !out_labels || !out_boxes || !counts)
+    return fail("lwdetr_tile_merge: null pointer");
+  if (reinterpret_cast<uintptr_t>(boxes) % 16 || reinterpret_cast<uintptr_t>(out_boxes) % 16)
+    return fail("lwdetr_tile_merge: boxes and out_boxes must be 16-byte aligned");
+  if (metric != LWDETR_TILE_IOU && metric != LWDETR_TILE_IOS) return fail("lwdetr_tile_merge: metric must be LWDETR_TILE_IOU or LWDETR_TILE_IOS");
+  if (!(iou_threshold >= 0.f && iou_threshold <= 1.f)) return fail("lwdetr_tile_merge: iou_threshold must be in [0, 1]");
+  if (score_threshold != score_threshold) return fail("lwdetr_tile_merge: score_threshold is NaN");
+  for (int v = 0; v < V; ++v) {
+    if (views[v].frame < 0 || views[v].frame >= num_frames)
+      return fail("lwdetr_tile_merge: view " + std::to_string(v) + " names frame " + std::to_string(views[v].frame) + " outside [0, " +
+                  std::to_string(num_frames) + ")");
+    if (v > 0 && views[v].frame < views[v - 1].frame)
+      return fail("lwdetr_tile_merge: view frames must be non-decreasing (each frame's views contiguous); view " + std::to_string(v) +
+                  " goes back to frame " + std::to_string(views[v].frame));
+  }
+  int e = lwb::tile_merge_launch(scores, labels, boxes, V, k, reinterpret_cast<const lwb::TileViewHost*>(views), num_frames, score_threshold,
+                                 iou_threshold, metric, max_det, out_scores, out_labels, out_boxes, counts, static_cast<cudaStream_t>(stream));
+  if (e == -2) return fail("lwdetr_tile_merge: a frame has more than 16384 candidates (views * k) or more than 2048 views");
+  if (e) return cuda_fail(e, "lwdetr_tile_merge launch");
   return 0;
 }
 

@@ -170,6 +170,40 @@ class LWDETR(nn.Module):
         sizes = torch.tensor(frames.sizes, dtype=torch.float32, device=out["pred_logits"].device)
         return PostProcess(self.num_queries if num_select is None else num_select)(out, sizes)
 
+    @torch.no_grad()
+    def detect_tiled(self, frames, tile=None, overlap=0.2, full_frame=True, size=None, per_view=100, score_threshold=0.0,
+                     iou_threshold=0.5, metric="ios", max_det=300, colorspace=None):
+        """Tiled (sliced) detection for high-resolution frames: the detector runs on overlapping full-resolution crops of
+        every frame (plus, with full_frame, the whole frame stretched to the run size as detect() does), all views of the
+        call in one batch on the run size `size` (default img_size x img_size), and the detections of each frame's views
+        are merged on the device.  Frames are RGB or NV12, taken exactly as detect() takes them; NV12 crops sit at even
+        offsets, so they are exact.  Steps, all on the current stream:
+          b200.config.tile_views (the views: tile = (th, tw) in source pixels, default the run size, and overlap);
+          Engine.forward_frames on the crop views with their dsts (partial tiles top-left on the padded, masked canvas);
+          the fused PostProcess per view (top `per_view`, boxes in crop pixels);
+          capi.tile_merge (boxes moved to frame pixels, score >= score_threshold, class-aware greedy NMS by "ios" or "iou"
+            beyond iou_threshold, the first max_det survivors).
+        Returns detect()'s list: per frame {"scores", "labels", "boxes"} (xyxy in the frame's own pixels, score order), cut to
+        the frame's survivor count; that cut copies the F counts to the host, the call's only synchronisation.  All views of
+        a call share one run size, so a stream of equally sized frames keeps one plan (and its CUDA graphs).  What tiling
+        does to small-object recall depends on the checkpoint and the data and is not measured here."""
+        from b200.config import tile_views
+        if self.training:
+            raise RuntimeError("lwdetr_b200 implements the inference forward only; call model.eval()")
+        dev = next(self.parameters()).device
+        if dev.type != "cuda":
+            raise RuntimeError("lwdetr_b200: move the model to a CUDA device (no CPU fallback)")
+        fb = capi.Frames(frames, dev, colorspace)
+        (H, W), views = tile_views(self.cfg, fb.sizes, tile, overlap, full_frame, size, per_view)
+        crops = tile_crops(fb, views)
+        out = self.engine().forward_frames(crops, size=(H, W), dsts=[(v[5], v[6]) for v in views], want_aux=False)
+        sizes = torch.tensor([(v[3], v[4]) for v in views], dtype=torch.float32, device=dev)
+        scores, labels, boxes = capi.postprocess(out["pred_logits"], out["pred_boxes"], sizes, per_view)
+        s, l, b, counts = capi.tile_merge(scores, labels, boxes, [(v[0], v[2], v[1]) for v in views], len(fb.items),
+                                          score_threshold, iou_threshold, metric, max_det)
+        counts = counts.cpu().tolist()
+        return [{"scores": s[f, :n], "labels": l[f, :n].long(), "boxes": b[f, :n]} for f, n in enumerate(counts)]
+
     def _pack_outputs(self, out):
         if self._export:
             return out["pred_boxes"], out["pred_logits"]      # forward_export tuple (lwdetr.py:176-195)
@@ -178,6 +212,20 @@ class LWDETR(nn.Module):
             res["aux_outputs"] = out["aux_outputs"]
         res["enc_outputs"] = out["enc_outputs"]
         return res
+
+
+def tile_crops(frames, views):
+    """capi.Frames of the crop views (frame, y0, x0, ch, cw, ...) of `frames` (capi.Frames): strided views of the frames'
+    memory, nothing copied.  NV12: the luma rows / columns of the crop and the chroma rows y0/2 .. and bytes x0 .. of its
+    (U, V) pairs, exact because y0 and x0 are even."""
+    if not frames.nv12:
+        return capi.Frames([frames.items[f][y0:y0 + ch, x0:x0 + cw] for f, y0, x0, ch, cw, _, _ in views])
+    if any(y0 % 2 or x0 % 2 for _, y0, x0, _, _, _, _ in views):
+        raise RuntimeError("lwdetr_b200: NV12 crops need even offsets")
+    names = {c: n for n, c in capi.COLORSPACES.items()}
+    pairs = [(frames.items[f][0][y0:y0 + ch, x0:x0 + cw], frames.items[f][1][y0 // 2:y0 // 2 + (ch + 1) // 2, x0:x0 + 2 * ((cw + 1) // 2)])
+             for f, y0, x0, ch, cw, _, _ in views]
+    return capi.Frames(pairs, colorspace=[names[frames.codes[v[0]]] for v in views])
 
 
 class PostProcess(nn.Module):
