@@ -248,6 +248,111 @@ LWDETR_API int lwdetr_tile_merge(const float* scores, const int32_t* labels, con
                                  int metric, int max_det, float* out_scores, int32_t* out_labels, float* out_boxes,
                                  int32_t* counts, void* stream);
 
+/* Multi-object tracking of video streams: ByteTrack (BYTETracker.update of the YOLOX tracker, non-MOT20 settings) per
+ * camera stream on the device.  The usual C composition per batch of frames, one frame per stream:
+ *   1. lwdetr_forward_frames (or _nv12) on the frames;
+ *   2. lwdetr_query_best: one entry per query (its best class), in query order - LW-DETR is NMS-free and lwdetr_postprocess
+ *      ranks (query, class) pairs, so one query can appear there several times with one box; a tracker fed with those makes
+ *      duplicate tracks;
+ *   3. lwdetr_track with k = nq.  Any per-frame entry list works (lwdetr_tile_merge output, with k = max_det, too).
+ * Calls on one tracker must be ordered on one CUDA stream (lwdetr_track reads and writes the tracker's device table).
+ *
+ * lwdetr_query_best: per query, score = max over classes of the fp32 sigmoid of pred_logits (ties to the lower class),
+ * label = that class, box = pred_boxes converted and scaled exactly as lwdetr_postprocess does, so each entry has the bits
+ * lwdetr_postprocess gives the same (query, class) pair.  pred_logits fp32 [B, nq, num_classes], pred_boxes fp32 [B, nq, 4],
+ * target_sizes fp32 [B, 2] (height, width) -> scores fp32 [B, nq], labels int32 [B, nq], boxes fp32 [B, nq, 4]; DEVICE,
+ * boxes 16-byte aligned.
+ *
+ * The tracker contract (tools/track_spec.py is this restatement in numpy).  Parameters (lwdetr_track_params_default fills
+ * ByteTrack's defaults): thresholds are fp32; max_time_lost = (int)(frame_rate / 30.0 * track_buffer).
+ * Entries of a frame: k of them (score fp32, label int32, xyxy fp32 in frame pixels), in input order.  An entry with a
+ * non-finite coordinate, or whose width x2 - x1 or height y2 - y1 (float64) is not > 0, is ignored (ByteTrack would
+ * produce NaN).  High: score > track_thresh; low: low_thresh < score < track_thresh.
+ * Everything below is float64 with every operation rounded on its own (no fused multiply-add), in the order written.
+ * Motion: constant-velocity Kalman filter in xyah.  Its covariance stays four independent 2x2 blocks, so per coordinate
+ * q in (cx, cy, a, h) the state is position p, velocity v and (P, C, V): position variance, covariance, velocity variance.
+ * With wp = 1.0 / 20, wv = 1.0 / 160 and std(w, h, f) = (w * h, w * h, f, w * h) (f for the coordinate a):
+ *   measurement of an entry: w = x2 - x1, h = y2 - y1, z = (x1 + w / 2, y1 + h / 2, w / h, h);
+ *   initiate from z: p = z, v = 0, P = sp * sp with sp = std(2 * wp, z_h, 1e-2), C = 0, V = sv * sv with
+ *     sv = std(10 * wv, z_h, 1e-5);
+ *   predict (h = p_h before the step; a track not in state Tracked first has v_h = 0):
+ *     p = p + v; P = ((P + (C + C)) + V) + sp * sp; C = C + V; V = V + sv * sv, sp = std(wp, h, 1e-2), sv = std(wv, h, 1e-5);
+ *   update with z (h = p_h before the update): S = P + sr * sr, sr = std(wp, h, 1e-1); Kp = P / S; Kv = C / S;
+ *     y = z - p; p = p + Kp * y; v = v + Kv * y; P = P - (Kp * Kp) * S; C = C - (Kp * Kv) * S; V = V - (Kv * Kv) * S;
+ *   box of a track: w = a * h, x1 = cx - w / 2, y1 = cy - h / 2, x2 = x1 + w, y2 = y1 + h.
+ * IoU (no +1 pixel term): ix = max(0, min(ax2, bx2) - max(ax1, bx1)), iy likewise, inter = ix * iy,
+ *   area = max(0, x2 - x1) * max(0, y2 - y1), union = (area_a + area_b) - inter; iou = inter / union, 0 when either area
+ *   or the union is not > 0.  Entry boxes are widened from fp32.
+ * Cost: 1 - iou, or with score fusion 1 - iou * score (score widened).  A pair is admissible iff cost < L (the association's
+ *   threshold, widened) and, with class_aware, the labels agree.
+ * Assignment (rows: tracks in list order, columns: entries in input order): the shortest-augmenting-path Hungarian method
+ *   (classic potentials formulation) on the n x (m + n) matrix [cost | D], inadmissible pairs +inf, D[i][i] = L and +inf
+ *   elsewhere; rows processed in order; each Dijkstra step takes the unused column of least slack, lowest column on ties;
+ *   row i ending on column m + i is unmatched.  This maximises the sum of (L - cost) over matched pairs, which is what
+ *   lap.lapjv(cost, extend_cost=True, cost_limit=L) returns up to ties.
+ * One frame of one stream (frame counts from 1; lists keep ByteTrack's order):
+ *   1. the tracked list splits into unconfirmed (not activated) and confirmed tracks; pool = confirmed, then the lost
+ *      list; the pool is predicted (unconfirmed tracks are not);
+ *   2. pool x high entries at match_thresh, fused if fuse_score: a matched track is updated (a Lost one is re-activated:
+ *      same id and start frame, into the "refound" list);
+ *   3. the pool's unmatched tracks in state Tracked x low entries at second_thresh, never fused: matched ones are updated,
+ *      the others become Lost;
+ *   4. unconfirmed tracks x the high entries left at unconfirmed_thresh, fused if fuse_score: matched ones are updated,
+ *      the others removed;
+ *   5. ageing: a track of the lost list (as it was before this frame) that was not refound and has
+ *      frame - end_frame > max_time_lost is removed;
+ *   6. births: every high entry left with score >= new_track_thresh, in input order, starts a track (initiate; id = the
+ *      stream's next id, from 1; activated at once only on frame 1).  A birth that would take the stream past `capacity`
+ *      tracks (tracked + lost after steps 2-5) is refused and counted in the stream's overflow count; it takes no id;
+ *   7. tracked = previous tracked still Tracked, births, refound; lost = previous lost minus refound and removed, then the
+ *      new lost tracks.  Removed tracks are dropped (ByteTrack keeps them forever);
+ *   8. duplicates: for every (tracked, lost) pair with 1 - iou < duplicate_thresh (and equal labels under class_aware), the
+ *      track with the smaller end_frame - start_frame is dropped, the tracked one on a tie;
+ *   9. output: the activated tracks of the tracked list, in order: id, score and label of the entry that updated or started
+ *      it this frame, xyxy of its state rounded to fp32, and that entry's index.
+ * "Updated" sets the Kalman update with the entry's measurement, state Tracked, activated, end_frame = frame, and the
+ * entry's score, label and index.
+ *
+ * lwdetr_tracker_create: num_streams >= 1 independent streams, params validated (thresholds in [0, 1], the three
+ *   association thresholds in (0, 1], capacity in [1, 1024], track_buffer >= 0, frame_rate >= 1); allocates the device
+ *   table (num_streams * capacity * 2 records) on the current device, every stream at frame 1.  Synchronous.
+ * lwdetr_tracker_reset: the n streams listed (HOST array; ids distinct and in [0, num_streams), else an error and nothing
+ *   happens) back to frame 1, next id 1, empty lists, overflow 0.
+ * lwdetr_track: one frame for each of B streams (stream_ids, HOST; ids distinct and in [0, num_streams), else an error and
+ *   nothing happens; a stream absent from a call does not advance):
+ *   scores fp32 [B, k], labels int32 [B, k], boxes fp32 [B, k, 4] (16-byte aligned), k <= 1024; outputs [B, max_out]:
+ *   out_ids int32, out_scores fp32, out_labels int32, out_boxes fp32 [B, max_out, 4] (16-byte aligned), out_index int32;
+ *   counts int32 [B] = min(output tracks, max_out); unused slots id 0, score 0, label -1, zero box, index -1.  All DEVICE;
+ *   asynchronous, nothing allocated or copied per call, safe to capture in a CUDA graph.
+ * lwdetr_tracker_export: the list state of one stream, synchronous: it waits for the tracker's last lwdetr_track /
+ *   lwdetr_tracker_reset launch (also when that launch was replayed from a CUDA graph) and for nothing else on the device,
+ *   then copies up to cap records (tracked list, then lost list) into host; *count = the stream's record count,
+ *   frame_next_overflow = (frame, next id, overflow). */
+enum { LWDETR_TRACK_TRACKED = 1, LWDETR_TRACK_LOST = 2 };
+typedef struct {
+  float track_thresh, low_thresh, new_track_thresh, match_thresh, second_thresh, unconfirmed_thresh, duplicate_thresh;
+  int32_t track_buffer, frame_rate, fuse_score, class_aware, capacity;
+} lwdetr_track_params;
+typedef struct {
+  int32_t id, state, activated, start_frame, end_frame, label;
+  float score;
+  int32_t index;        /* entry that last updated the track */
+  double mean[8];       /* p (cx, cy, a, h), then v */
+  double cov[12];       /* P[4], C[4], V[4] */
+} lwdetr_track_record;
+typedef struct lwdetr_tracker lwdetr_tracker;
+LWDETR_API void lwdetr_track_params_default(lwdetr_track_params* p);
+LWDETR_API int lwdetr_tracker_create(int num_streams, const lwdetr_track_params* params, lwdetr_tracker** out);
+LWDETR_API void lwdetr_tracker_destroy(lwdetr_tracker* t);
+LWDETR_API int lwdetr_tracker_reset(lwdetr_tracker* t, const int32_t* streams, int n, void* stream);
+LWDETR_API int lwdetr_track(lwdetr_tracker* t, const float* scores, const int32_t* labels, const float* boxes, int B, int k,
+                            const int32_t* stream_ids, int max_out, int32_t* out_ids, float* out_scores, int32_t* out_labels,
+                            float* out_boxes, int32_t* out_index, int32_t* counts, void* stream);
+LWDETR_API int lwdetr_tracker_export(lwdetr_tracker* t, int stream_id, lwdetr_track_record* host, int cap, int32_t* count,
+                                     int32_t frame_next_overflow[3]);
+LWDETR_API int lwdetr_query_best(const float* pred_logits, const float* pred_boxes, const float* target_sizes, int B, int nq, int num_classes,
+                                 float* scores, int32_t* labels, float* boxes, void* stream);
+
 /* The LWDETR_F16_E4M3 mode's two kernels.
  * lwdetr_layernorm_e4m3: fp16 rows x [rows, ldx] -> e4m3 codes q [rows, ldq] (uint8) and fp32 row_scale [rows], as the mode's
  *   activation contract above (x^ without the LayerNorm affine, eps as given).  C % 8 == 0, C <= 1024, ldx and ldq

@@ -33,6 +33,13 @@ _SIGNATURES = {
     "lwdetr_topk": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "lwdetr_postprocess": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_tile_merge": (_i, [_vp, _vp, _vp, _i, _i, _vp, _i, _f, _f, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "lwdetr_track_params_default": (None, [_vp]),
+    "lwdetr_tracker_create": (_i, [_i, _vp, _vp]),
+    "lwdetr_tracker_destroy": (None, [_vp]),
+    "lwdetr_tracker_reset": (_i, [_vp, _vp, _i, _vp]),
+    "lwdetr_track": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "lwdetr_tracker_export": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
+    "lwdetr_query_best": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "lwdetr_layernorm_e4m3": (_i, [_vp, _i, _i64, _i, _f, _vp, _i, _vp, _vp]),
     "lwdetr_gemm_e4m3": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _i, _vp]),
     "lwdetr_vit_mlp": (_i, [_i, _vp, _i, _i, _vp, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp]),
@@ -388,6 +395,127 @@ def tile_merge(scores, labels, boxes, views, num_frames, score_threshold=0.0, io
                                   float(iou_threshold), TILE_METRICS[metric], int(max_det), ptr(out_s), ptr(out_l), ptr(out_b),
                                   ptr(counts), stream_ptr(dev)), "lwdetr_tile_merge")
     return out_s, out_l, out_b, counts
+
+
+def query_best(pred_logits, pred_boxes, target_sizes):
+    """lwdetr_query_best: one detection per query, its best class (CUDA fp32 tensors as for postprocess) -> (scores fp32
+    [B, nq], labels int32 [B, nq], boxes fp32 [B, nq, 4]), each entry with the bits postprocess() gives that (query, class)
+    pair."""
+    import torch
+    B, nq, ncls = pred_logits.shape
+    logits = pred_logits.float().contiguous()
+    boxes = pred_boxes.float().contiguous()
+    dev = logits.device
+    ts = target_sizes.to(device=dev, dtype=torch.float32).contiguous()
+    scores = torch.empty(B, nq, device=dev, dtype=torch.float32)
+    labels = torch.empty(B, nq, device=dev, dtype=torch.int32)
+    out = torch.empty(B, nq, 4, device=dev, dtype=torch.float32)
+    check(lib().lwdetr_query_best(ptr(logits), ptr(boxes), ptr(ts), B, nq, ncls, ptr(scores), ptr(labels), ptr(out), stream_ptr(dev)),
+          "lwdetr_query_best")
+    return scores, labels, out
+
+
+class TrackParams(ctypes.Structure):
+    """lwdetr_track_params (include/lwdetr_b200.h)."""
+    _fields_ = [(n, _f) for n in ("track_thresh", "low_thresh", "new_track_thresh", "match_thresh", "second_thresh",
+                                  "unconfirmed_thresh", "duplicate_thresh")] + \
+               [(n, ctypes.c_int32) for n in ("track_buffer", "frame_rate", "fuse_score", "class_aware", "capacity")]
+
+
+class TrackRecord(ctypes.Structure):
+    """lwdetr_track_record (include/lwdetr_b200.h)."""
+    _fields_ = [(n, ctypes.c_int32) for n in ("id", "state", "activated", "start_frame", "end_frame", "label")] + \
+               [("score", _f), ("index", ctypes.c_int32), ("mean", ctypes.c_double * 8), ("cov", ctypes.c_double * 12)]
+
+
+class Tracker:
+    """ByteTrack on the device for num_streams camera streams (lwdetr_tracker_*, the contract in include/lwdetr_b200.h).
+    Parameters are lwdetr_track_params' fields, ByteTrack's defaults unless given; new_track_thresh defaults to
+    track_thresh + 0.1.  All calls of one tracker must run on one CUDA stream (the current one at each call)."""
+
+    def __init__(self, num_streams, device=None, **params):
+        import torch
+        p = TrackParams()
+        lib().lwdetr_track_params_default(ctypes.byref(p))
+        names = {n for n, _ in TrackParams._fields_}
+        bad = set(params) - names
+        if bad:
+            raise RuntimeError("Tracker: unknown parameters %s" % ", ".join(sorted(bad)))
+        if params.get("new_track_thresh") is None:
+            params["new_track_thresh"] = params.get("track_thresh", 0.5) + 0.1
+        for n, v in params.items():
+            setattr(p, n, v)
+        self.params = p
+        self.num_streams = int(num_streams)
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self._t = _vp()
+        with torch.cuda.device(self.device):
+            check(lib().lwdetr_tracker_create(self.num_streams, ctypes.byref(p), ctypes.byref(self._t)), "lwdetr_tracker_create")
+
+    def close(self):
+        if self._t:
+            lib().lwdetr_tracker_destroy(self._t)
+            self._t = _vp()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @staticmethod
+    def _ids(ids):
+        ids = [int(x) for x in ids]
+        return (ctypes.c_int32 * max(len(ids), 1))(*ids), len(ids)
+
+    def reset(self, streams):
+        """Streams back to frame 1 and id 1 with empty lists (stream-ordered)."""
+        arr, n = self._ids(streams)
+        check(lib().lwdetr_tracker_reset(self._t, ctypes.cast(arr, _vp), n, stream_ptr(self.device)), "lwdetr_tracker_reset")
+
+    def update(self, scores, labels, boxes, stream_ids=None, max_out=None):
+        """One frame for each of B distinct streams: scores fp32 [B, k], labels int [B, k], xyxy boxes fp32 [B, k, 4] (CUDA;
+        stream_ids default range(B)) -> (ids int32 [B, max_out], scores fp32, labels int32, boxes fp32 [B, max_out, 4], index
+        int32 (the entry of each track), counts int32 [B]); unused slots id 0, score 0, label -1, zero box, index -1.
+        max_out defaults to k.  Stream-ordered, no synchronisation."""
+        import torch
+        B, k = scores.shape
+        if tuple(labels.shape) != (B, k) or tuple(boxes.shape) != (B, k, 4):
+            raise RuntimeError("Tracker.update: scores %s, labels %s and boxes %s do not describe one [B, k] set"
+                               % (tuple(scores.shape), tuple(labels.shape), tuple(boxes.shape)))
+        dev = self.device
+        scores = scores.to(device=dev, dtype=torch.float32).contiguous()
+        labels = labels.to(device=dev, dtype=torch.int32).contiguous()
+        boxes = boxes.to(device=dev, dtype=torch.float32).contiguous()
+        ids, n = self._ids(range(B) if stream_ids is None else stream_ids)
+        if n != B:
+            raise RuntimeError("Tracker.update: %d stream ids for %d frames" % (n, B))
+        m = k if max_out is None else int(max_out)
+        o_id = torch.empty(B, m, device=dev, dtype=torch.int32)
+        o_s = torch.empty(B, m, device=dev, dtype=torch.float32)
+        o_l = torch.empty(B, m, device=dev, dtype=torch.int32)
+        o_b = torch.empty(B, m, 4, device=dev, dtype=torch.float32)
+        o_i = torch.empty(B, m, device=dev, dtype=torch.int32)
+        counts = torch.empty(B, device=dev, dtype=torch.int32)
+        check(lib().lwdetr_track(self._t, ptr(scores), ptr(labels), ptr(boxes), B, k, ctypes.cast(ids, _vp), m, ptr(o_id), ptr(o_s),
+                                 ptr(o_l), ptr(o_b), ptr(o_i), ptr(counts), stream_ptr(dev)), "lwdetr_track")
+        return o_id, o_s, o_l, o_b, o_i, counts
+
+    def export(self, stream_id):
+        """Synchronous: (records, (frame, next_id, overflow)) of one stream, records a list of dicts in list order (tracked,
+        then lost) with id, state (1 tracked, 2 lost), activated, start, end, score, label, index, mean (8 float64: cx, cy, a,
+        h, then velocities) and cov (12 float64: P, C, V per coordinate)."""
+        import numpy as np
+        cap = int(self.params.capacity)
+        arr = (TrackRecord * cap)()
+        cnt = ctypes.c_int32()
+        fno = (ctypes.c_int32 * 3)()
+        check(lib().lwdetr_tracker_export(self._t, int(stream_id), ctypes.cast(arr, _vp), cap, ctypes.byref(cnt), ctypes.cast(fno, _vp)),
+              "lwdetr_tracker_export")
+        recs = [dict(id=r.id, state=r.state, activated=r.activated, start=r.start_frame, end=r.end_frame, score=np.float32(r.score),
+                     label=r.label, index=r.index, mean=np.array(r.mean[:], np.float64), cov=np.array(r.cov[:], np.float64))
+                for r in arr[:min(cnt.value, cap)]]
+        return recs, tuple(fno)
 
 
 def layernorm_e4m3(x, eps=1e-6):

@@ -19,6 +19,7 @@
 #include "resize.h"
 #include "rowops.h"
 #include "tiles.h"
+#include "track.h"
 
 
 namespace {
@@ -269,6 +270,188 @@ int lwdetr_tile_merge(const float* scores, const int32_t* labels, const float* b
                                  iou_threshold, metric, max_det, out_scores, out_labels, out_boxes, counts, static_cast<cudaStream_t>(stream));
   if (e == -2) return fail("lwdetr_tile_merge: a frame has more than 16384 candidates (views * k) or more than 2048 views");
   if (e) return cuda_fail(e, "lwdetr_tile_merge launch");
+  return 0;
+}
+
+static_assert(sizeof(lwdetr_track_record) == 192, "track record layout");
+
+struct lwdetr_tracker {
+  lwb::TrackTable table;
+  lwdetr_track_params params;
+  int device;
+  cudaEvent_t done;      // recorded after every launch on the table (an external event node inside a CUDA graph capture)
+  cudaStream_t copy;     // non-blocking: lwdetr_tracker_export waits for `done` only, not for the rest of the device
+};
+
+// marks the tracker's last launch on `stream`, so that lwdetr_tracker_export waits for exactly that work.  Inside a stream
+// capture the record becomes an external event node, so every replay of the graph records it (the flag is accepted only
+// while capturing)
+static int tracker_mark(lwdetr_tracker* t, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  if (cudaError_t e = cudaStreamIsCapturing(st, &cs)) return static_cast<int>(e);
+  return static_cast<int>(cs == cudaStreamCaptureStatusActive ? cudaEventRecordWithFlags(t->done, st, cudaEventRecordExternal)
+                                                              : cudaEventRecord(t->done, st));
+}
+
+void lwdetr_track_params_default(lwdetr_track_params* p) {
+  if (!p) return;
+  p->track_thresh = 0.5f;
+  p->low_thresh = 0.1f;
+  p->new_track_thresh = static_cast<float>(0.5 + 0.1);
+  p->match_thresh = 0.8f;
+  p->second_thresh = 0.5f;
+  p->unconfirmed_thresh = 0.7f;
+  p->duplicate_thresh = 0.15f;
+  p->track_buffer = 30;
+  p->frame_rate = 30;
+  p->fuse_score = 1;
+  p->class_aware = 0;
+  p->capacity = 512;
+}
+
+// Runs a call on the tracker's device and switches back.
+struct DeviceGuard {
+  int prev = -1;
+  explicit DeviceGuard(int dev) {
+    if (cudaGetDevice(&prev) == cudaSuccess && prev != dev) cudaSetDevice(dev);
+  }
+  ~DeviceGuard() {
+    int now = -1;
+    if (prev >= 0 && cudaGetDevice(&now) == cudaSuccess && now != prev) cudaSetDevice(prev);
+  }
+};
+
+int lwdetr_tracker_create(int num_streams, const lwdetr_track_params* params, lwdetr_tracker** out) {
+  if (!params || !out) return fail("lwdetr_tracker_create: null pointer");
+  const lwdetr_track_params& p = *params;
+  if (num_streams < 1) return fail("lwdetr_tracker_create: num_streams must be >= 1");
+  const float th[] = {p.track_thresh, p.low_thresh, p.new_track_thresh, p.duplicate_thresh};
+  for (float v : th)
+    if (!(v >= 0.f && v <= 1.f)) return fail("lwdetr_tracker_create: track_thresh, low_thresh, new_track_thresh and duplicate_thresh must be in [0, 1]");
+  const float lim[] = {p.match_thresh, p.second_thresh, p.unconfirmed_thresh};
+  for (float v : lim)
+    if (!(v > 0.f && v <= 1.f)) return fail("lwdetr_tracker_create: match_thresh, second_thresh and unconfirmed_thresh must be in (0, 1]");
+  if (p.capacity < 1 || p.capacity > lwb::TRACK_MAX) return fail("lwdetr_tracker_create: capacity must be in [1, 1024]");
+  if (p.track_buffer < 0 || p.frame_rate < 1) return fail("lwdetr_tracker_create: need track_buffer >= 0 and frame_rate >= 1");
+  if ((p.fuse_score != 0 && p.fuse_score != 1) || (p.class_aware != 0 && p.class_aware != 1))
+    return fail("lwdetr_tracker_create: fuse_score and class_aware must be 0 or 1");
+  lwdetr_tracker* t = new (std::nothrow) lwdetr_tracker;
+  if (!t) return fail("lwdetr_tracker_create: out of memory");
+  t->params = p;
+  t->table.num_streams = num_streams;
+  t->table.capacity = p.capacity;
+  t->table.head = nullptr;
+  t->table.rec = nullptr;
+  t->done = nullptr;
+  t->copy = nullptr;
+  if (cudaGetDevice(&t->device) != cudaSuccess) { delete t; return fail("lwdetr_tracker_create: no CUDA device (there is no CPU fallback)"); }
+  std::vector<lwb::TrackHead> h(static_cast<size_t>(num_streams));
+  for (auto& x : h) { x = lwb::TrackHead{}; x.frame = 1; x.next_id = 1; }
+  const size_t rec_bytes = static_cast<size_t>(num_streams) * 2 * p.capacity * sizeof(lwdetr_track_record);
+  cudaError_t e = cudaMalloc(&t->table.head, h.size() * sizeof(lwb::TrackHead));
+  if (e == cudaSuccess) e = cudaMalloc(&t->table.rec, rec_bytes);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&t->done, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&t->copy, cudaStreamNonBlocking);
+  if (e == cudaSuccess) e = cudaMemcpy(t->table.head, h.data(), h.size() * sizeof(lwb::TrackHead), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    cudaFree(t->table.head);
+    cudaFree(t->table.rec);
+    if (t->done) cudaEventDestroy(t->done);
+    if (t->copy) cudaStreamDestroy(t->copy);
+    delete t;
+    return cuda_fail(e, "lwdetr_tracker_create");
+  }
+  *out = t;
+  return 0;
+}
+
+void lwdetr_tracker_destroy(lwdetr_tracker* t) {
+  if (!t) return;
+  DeviceGuard g(t->device);
+  cudaStreamSynchronize(t->copy);
+  cudaFree(t->table.head);
+  cudaFree(t->table.rec);
+  cudaEventDestroy(t->done);
+  cudaStreamDestroy(t->copy);
+  delete t;
+}
+
+static std::string check_streams(const lwdetr_tracker* t, const int32_t* ids, int n) {
+  std::vector<char> seen(static_cast<size_t>(t->table.num_streams), 0);
+  for (int i = 0; i < n; ++i) {
+    if (ids[i] < 0 || ids[i] >= t->table.num_streams)
+      return "stream id " + std::to_string(ids[i]) + " outside [0, " + std::to_string(t->table.num_streams) + ")";
+    if (seen[ids[i]]++) return "stream id " + std::to_string(ids[i]) + " appears twice in one call";
+  }
+  return "";
+}
+
+int lwdetr_tracker_reset(lwdetr_tracker* t, const int32_t* streams, int n, void* stream) {
+  if (!t || (n > 0 && !streams)) return fail("lwdetr_tracker_reset: null pointer");
+  if (n < 0) return fail("lwdetr_tracker_reset: n must be >= 0");
+  const std::string err = check_streams(t, streams, n);
+  if (!err.empty()) return fail("lwdetr_tracker_reset: " + err);
+  if (n == 0) return 0;
+  DeviceGuard g(t->device);
+  int e = lwb::track_reset_launch(t->table, streams, n, static_cast<cudaStream_t>(stream));
+  if (!e) e = tracker_mark(t, stream);
+  if (e) return cuda_fail(e, "lwdetr_tracker_reset launch");
+  return 0;
+}
+
+int lwdetr_track(lwdetr_tracker* t, const float* scores, const int32_t* labels, const float* boxes, int B, int k, const int32_t* stream_ids,
+                 int max_out, int32_t* out_ids, float* out_scores, int32_t* out_labels, float* out_boxes, int32_t* out_index,
+                 int32_t* counts, void* stream) {
+  if (!t || !scores || !labels || !boxes || !stream_ids || !out_ids || !out_scores || !out_labels || !out_boxes || !out_index || !counts)
+    return fail("lwdetr_track: null pointer");
+  if (B < 1 || k < 1 || k > lwb::TRACK_MAX || max_out < 1) return fail("lwdetr_track: need B >= 1, k in [1, 1024] and max_out >= 1");
+  if (reinterpret_cast<uintptr_t>(boxes) % 16 || reinterpret_cast<uintptr_t>(out_boxes) % 16)
+    return fail("lwdetr_track: boxes and out_boxes must be 16-byte aligned");
+  const std::string err = check_streams(t, stream_ids, B);
+  if (!err.empty()) return fail("lwdetr_track: " + err);
+  DeviceGuard g(t->device);
+  int e = lwb::track_launch(t->table, t->params, scores, labels, boxes, B, k, stream_ids, max_out, out_ids, out_scores, out_labels,
+                            out_boxes, out_index, counts, static_cast<cudaStream_t>(stream));
+  if (e == -2) return fail("lwdetr_track: a limit is exceeded");
+  if (!e) e = tracker_mark(t, stream);
+  if (e) return cuda_fail(e, "lwdetr_track launch");
+  return 0;
+}
+
+int lwdetr_tracker_export(lwdetr_tracker* t, int stream_id, lwdetr_track_record* host, int cap, int32_t* count, int32_t frame_next_overflow[3]) {
+  if (!t || !count || !frame_next_overflow || (cap > 0 && !host)) return fail("lwdetr_tracker_export: null pointer");
+  if (stream_id < 0 || stream_id >= t->table.num_streams) return fail("lwdetr_tracker_export: stream id outside [0, num_streams)");
+  DeviceGuard g(t->device);
+  lwb::TrackHead h;
+  cudaError_t e = cudaStreamWaitEvent(t->copy, t->done, 0);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&h, t->table.head + stream_id, sizeof(h), cudaMemcpyDeviceToHost, t->copy);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(t->copy);
+  if (e != cudaSuccess) return cuda_fail(e, "lwdetr_tracker_export");
+  const int n = h.n_tracked + h.n_lost;
+  const int m = n < cap ? n : (cap > 0 ? cap : 0);
+  const lwdetr_track_record* src = t->table.rec + (static_cast<size_t>(stream_id) * 2 + h.parity) * t->table.capacity;
+  if (m > 0) {
+    e = cudaMemcpyAsync(host, src, static_cast<size_t>(m) * sizeof(lwdetr_track_record), cudaMemcpyDeviceToHost, t->copy);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(t->copy);
+    if (e != cudaSuccess) return cuda_fail(e, "lwdetr_tracker_export");
+  }
+  *count = n;
+  frame_next_overflow[0] = h.frame;
+  frame_next_overflow[1] = h.next_id;
+  frame_next_overflow[2] = h.overflow;
+  return 0;
+}
+
+int lwdetr_query_best(const float* pred_logits, const float* pred_boxes, const float* target_sizes, int B, int nq, int num_classes,
+                      float* scores, int32_t* labels, float* boxes, void* stream) {
+  if (!pred_logits || !pred_boxes || !target_sizes || !scores || !labels || !boxes) return fail("lwdetr_query_best: null pointer");
+  if (B < 1 || nq < 1 || num_classes < 1) return fail("lwdetr_query_best: bad sizes");
+  if (reinterpret_cast<uintptr_t>(pred_boxes) % 16 || reinterpret_cast<uintptr_t>(boxes) % 16)
+    return fail("lwdetr_query_best: pred_boxes and boxes must be 16-byte aligned");
+  int e = lwb::query_best_launch(pred_logits, pred_boxes, target_sizes, B, nq, num_classes, scores, labels, boxes,
+                                 static_cast<cudaStream_t>(stream));
+  if (e) return cuda_fail(e, "lwdetr_query_best launch");
   return 0;
 }
 

@@ -3,6 +3,7 @@
 // 16/32-byte accesses, one warp per row where a row reduction is needed, and fp32 math throughout.
 #include "rowops.h"
 #include "launch.h"
+#include "postproc.cuh"
 #include "ptx.cuh"
 
 #include <math_constants.h>
@@ -794,8 +795,6 @@ int final_boxes_launch(const float* delta, const float* refpoint, long long rows
 // Two launches: (1) every image's score list is cut into `parts` slices of <= 16384 entries, one CTA sorts a slice
 // (sigmoid computed while loading) and keeps its k best flat indices; (2) one CTA per image merges the parts*k
 // candidates, sorts them again and writes scores / labels / scaled boxes - only [B, k, 6] numbers leave the GPU.
-__device__ __forceinline__ float sigmoid_f32(float x) { return 1.f / (1.f + expf(-x)); }
-
 __global__ void __launch_bounds__(1024) postprocess_part_kernel(const float* __restrict__ logits, int S, int parts, int part_len,
                                                                  int np2, int k, int* __restrict__ cand) {
   pdl_sync();   // programmatic dependent launch: release the successor, wait for the predecessor (launch.h)
@@ -839,12 +838,7 @@ __global__ void __launch_bounds__(1024) postprocess_merge_kernel(const float* __
     const long long o = static_cast<long long>(b) * k + i;
     scores[o] = key[i];
     labels[o] = flat - q * ncls;
-    float4 r;
-    r.x = (bx.x - 0.5f * bx.z) * img_w;
-    r.y = (bx.y - 0.5f * bx.w) * img_h;
-    r.z = (bx.x + 0.5f * bx.z) * img_w;
-    r.w = (bx.y + 0.5f * bx.w) * img_h;
-    *reinterpret_cast<float4*>(out_boxes + o * 4) = r;
+    *reinterpret_cast<float4*>(out_boxes + o * 4) = box_cxcywh_to_xyxy(bx, img_h, img_w);
   }
 }
 

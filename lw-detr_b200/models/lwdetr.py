@@ -204,6 +204,57 @@ class LWDETR(nn.Module):
         counts = counts.cpu().tolist()
         return [{"scores": s[f, :n], "labels": l[f, :n].long(), "boxes": b[f, :n]} for f, n in enumerate(counts)]
 
+    @torch.no_grad()
+    def track(self, frames, tracker, streams=None, size=None, fit="stretch", short_side=None, max_side=None, colorspace=None,
+              max_out=None):
+        """Multi-object tracking of video streams: frames (RGB or NV12, taken exactly as detect() takes them) run as one
+        forward; each query gives one detection, its best class (capi.query_best, boxes in the frame's original pixels);
+        then capi.Tracker `tracker` (ByteTrack on the device, include/lwdetr_b200.h) updates each frame's stream.
+        streams: the stream of each frame, default range(len(frames)).  Several frames of one stream in a call (one video
+        batched offline) are tracked in list order: tracker launch r takes the r-th frame of every stream.
+        Returns per frame {"ids", "scores", "labels", "boxes", "queries"}: the activated tracks in ByteTrack's list order,
+        cut to the frame's count (one read-back for the call), "queries" the query each track took its detection from.
+        max_out (default num_queries) bounds the tracks returned per frame.  How ByteTrack's thresholds (tuned on YOLOX
+        scores) suit LW-DETR's score distribution, in MOTA / IDF1 / HOTA, is not measured here."""
+        if self.training:
+            raise RuntimeError("lwdetr_b200 implements the inference forward only; call model.eval()")
+        dev = next(self.parameters()).device
+        if dev.type != "cuda":
+            raise RuntimeError("lwdetr_b200: move the model to a CUDA device (no CPU fallback)")
+        fb = capi.Frames(frames, dev, colorspace)
+        n = len(fb.items)
+        streams = list(range(n)) if streams is None else [int(s) for s in streams]
+        if len(streams) != n:
+            raise RuntimeError("lwdetr_b200: %d streams for %d frames" % (len(streams), n))
+        out = self.engine().forward_frames(fb, size=size, fit=fit, short_side=short_side, max_side=max_side, want_aux=False)
+        sizes = torch.tensor(fb.sizes, dtype=torch.float32, device=dev)
+        scores, labels, boxes = capi.query_best(out["pred_logits"], out["pred_boxes"], sizes)
+        rounds, seen = [], {}
+        for i, s in enumerate(streams):
+            r = seen.get(s, 0)
+            seen[s] = r + 1
+            if r == len(rounds):
+                rounds.append([])
+            rounds[r].append(i)
+        res, counts = [None] * n, []
+        for rows in rounds:
+            idx = torch.tensor(rows, device=dev)
+            got = tracker.update(scores[idx], labels[idx], boxes[idx], [streams[i] for i in rows],
+                                 self.num_queries if max_out is None else max_out)
+            counts.append(got[5])
+            for j, i in enumerate(rows):
+                res[i] = (got, j)
+        counts = torch.cat(counts).cpu().tolist()
+        order = [i for rows in rounds for i in rows]
+        cnt = {i: c for i, c in zip(order, counts)}
+        dets = []
+        for i in range(n):
+            (ids, sc, lab, bx, q, _), j = res[i]
+            c = cnt[i]
+            dets.append({"ids": ids[j, :c], "scores": sc[j, :c], "labels": lab[j, :c].long(), "boxes": bx[j, :c],
+                         "queries": q[j, :c].long()})
+        return dets
+
     def _pack_outputs(self, out):
         if self._export:
             return out["pred_boxes"], out["pred_logits"]      # forward_export tuple (lwdetr.py:176-195)

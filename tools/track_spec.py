@@ -1,0 +1,453 @@
+"""Multi-object tracking (lwdetr_track in include/lwdetr_b200.h), restated in numpy for the tests: ByteTrack's
+BYTETracker.update (non-MOT20 settings) per camera stream, with the deviations the header states.
+
+Everything is float64 with each operation rounded on its own (numpy does not fuse), in the order the header fixes:
+  Kalman filter in xyah as four independent (position, velocity) pairs with covariance (P, C, V) per coordinate;
+  IoU without the +1 pixel term; costs 1 - iou (or 1 - iou * score with score fusion);
+  assignment by the shortest-augmenting-path Hungarian method on the n x (m + n) matrix whose column m + i is row i's own
+  "unmatched" column of cost L (solve()), which is what lap.lapjv(cost, extend_cost=True, cost_limit=L) returns up to ties.
+
+scene() is a seeded generator of synthetic detection sequences for the tests and the benchmark.
+"""
+import numpy as np
+
+TRACKED, LOST = 1, 2
+WP, WV = 1.0 / 20, 1.0 / 160
+INF = np.inf
+
+DEFAULTS = dict(track_thresh=0.5, low_thresh=0.1, new_track_thresh=None, match_thresh=0.8, second_thresh=0.5,
+                unconfirmed_thresh=0.7, duplicate_thresh=0.15, track_buffer=30, frame_rate=30, fuse_score=1, class_aware=0,
+                capacity=512)
+
+
+def params(**kw):
+    """The parameter block with ByteTrack's defaults; thresholds are float32, as lwdetr_track_params holds them."""
+    bad = set(kw) - set(DEFAULTS)
+    if bad:
+        raise TypeError("unknown tracker parameters: %s" % ", ".join(sorted(bad)))
+    p = dict(DEFAULTS)
+    p.update({k: v for k, v in kw.items()})
+    if p["new_track_thresh"] is None:
+        p["new_track_thresh"] = p["track_thresh"] + 0.1
+    for k in ("track_thresh", "low_thresh", "new_track_thresh", "match_thresh", "second_thresh", "unconfirmed_thresh",
+              "duplicate_thresh"):
+        p[k] = np.float32(p[k])
+    for k in ("track_buffer", "frame_rate", "fuse_score", "class_aware", "capacity"):
+        p[k] = int(p[k])
+    p["max_time_lost"] = int(p["frame_rate"] / 30.0 * p["track_buffer"])
+    return p
+
+
+# ---------------------------------------------------------------------------------------------- Kalman filter (xyah)
+class Track:
+    __slots__ = ("id", "state", "activated", "start", "end", "score", "label", "index", "p", "v", "P", "C", "V")
+
+    def box(self):
+        """xyxy float64 from the state: w = a * h, x1 = cx - w / 2, y1 = cy - h / 2, x2 = x1 + w, y2 = y1 + h."""
+        cx, cy, a, h = self.p
+        w = a * h
+        x1 = cx - w / 2
+        y1 = cy - h / 2
+        return np.array([x1, y1, x1 + w, y1 + h])
+
+
+def measurement(box):
+    """xyah float64 of an xyxy fp32 box: w = x2 - x1, h = y2 - y1, (x1 + w / 2, y1 + h / 2, w / h, h)."""
+    x1, y1, x2, y2 = (np.float64(c) for c in box)
+    w = x2 - x1
+    h = y2 - y1
+    return np.array([x1 + w / 2, y1 + h / 2, w / h, h])
+
+
+def _std(h, w, fixed):
+    """(w * h, w * h, fixed, w * h)."""
+    s = w * h
+    return np.array([s, s, fixed, s])
+
+
+def initiate(t, z):
+    h = z[3]
+    t.p = z.copy()
+    t.v = np.zeros(4)
+    sp = _std(h, 2 * WP, 1e-2)
+    sv = _std(h, 10 * WV, 1e-5)
+    t.P = sp * sp
+    t.C = np.zeros(4)
+    t.V = sv * sv
+
+
+def predict(t):
+    if t.state != TRACKED:
+        t.v[3] = 0.0
+    h = t.p[3]
+    sp = _std(h, WP, 1e-2)
+    sv = _std(h, WV, 1e-5)
+    t.p = t.p + t.v
+    t.P = ((t.P + (t.C + t.C)) + t.V) + sp * sp
+    t.C = t.C + t.V
+    t.V = t.V + sv * sv
+
+
+def kalman_update(t, z):
+    h = t.p[3]
+    sr = _std(h, WP, 1e-1)
+    S = t.P + sr * sr
+    Kp = t.P / S
+    Kv = t.C / S
+    y = z - t.p
+    t.p = t.p + Kp * y
+    t.v = t.v + Kv * y
+    t.P = t.P - (Kp * Kp) * S
+    t.C = t.C - (Kp * Kv) * S
+    t.V = t.V - (Kv * Kv) * S
+
+
+# ---------------------------------------------------------------------------------------------- costs and assignment
+def iou(a, b):
+    """IoU of float64 xyxy boxes a [n, 4] x b [m, 4] -> [n, m]; 0 where either area or the union is not > 0."""
+    a = np.asarray(a, np.float64).reshape(-1, 4)[:, None, :]
+    b = np.asarray(b, np.float64).reshape(-1, 4)[None, :, :]
+    ix = np.fmax(0.0, np.fmin(a[..., 2], b[..., 2]) - np.fmax(a[..., 0], b[..., 0]))
+    iy = np.fmax(0.0, np.fmin(a[..., 3], b[..., 3]) - np.fmax(a[..., 1], b[..., 1]))
+    inter = ix * iy
+    aa = np.fmax(0.0, a[..., 2] - a[..., 0]) * np.fmax(0.0, a[..., 3] - a[..., 1])
+    ab = np.fmax(0.0, b[..., 2] - b[..., 0]) * np.fmax(0.0, b[..., 3] - b[..., 1])
+    union = (aa + ab) - inter
+    ok = (aa > 0) & (ab > 0) & (union > 0)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        return np.where(ok, inter / np.where(ok, union, 1.0), 0.0)
+
+
+def cost_matrix(tboxes, tlabels, dboxes, dscores, dlabels, L, fuse, class_aware):
+    """[n, m] float64: 1 - iou (fuse: 1 - iou * score), +inf where the pair is not admissible (cost >= L, or labels
+    differ under class_aware)."""
+    n, m = len(tboxes), len(dboxes)
+    if n == 0 or m == 0:
+        return np.full((n, m), INF)
+    io = iou(tboxes, np.asarray(dboxes, np.float64))
+    c = 1.0 - io * np.asarray(dscores, np.float32).astype(np.float64)[None, :] if fuse else 1.0 - io
+    ok = c < np.float64(L)
+    if class_aware:
+        ok &= np.asarray(tlabels)[:, None] == np.asarray(dlabels)[None, :]
+    return np.where(ok, c, INF)
+
+
+def solve(cost, L):
+    """Shortest-augmenting-path Hungarian method (the classic potentials formulation) on the n x (m + n) matrix
+    [cost | D], D[i, i] = L and +inf elsewhere; rows in order, each Dijkstra step taking the unused column with the
+    smallest slack, lowest column on ties.  Returns (match [n] int: the column of each row or -1, u [n] and v [m]: the
+    final row and real-column potentials)."""
+    cost = np.asarray(cost, np.float64)
+    n, m = cost.shape
+    match = np.full(n, -1, np.int64)
+    if n == 0 or m == 0:
+        return match, np.zeros(n), np.zeros(m)
+    M = m + n
+    a = np.full((n + 1, M + 1), INF)                  # 1-based, as the classic statement
+    a[1:, 1:m + 1] = cost
+    a[np.arange(1, n + 1), m + np.arange(1, n + 1)] = np.float64(L)
+    u = np.zeros(n + 1)
+    v = np.zeros(M + 1)
+    p = np.zeros(M + 1, np.int64)                     # p[j]: row matched to column j, 0 = free
+    way = np.zeros(M + 1, np.int64)
+    for i in range(1, n + 1):
+        p[0] = i
+        j0 = 0
+        minv = np.full(M + 1, INF)
+        used = np.zeros(M + 1, bool)
+        while True:
+            used[j0] = True
+            i0 = p[j0]
+            free = ~used
+            free[0] = False
+            cur = (a[i0] - u[i0]) - v
+            better = free & (cur < minv)
+            minv[better] = cur[better]
+            way[better] = j0
+            cand = np.where(free, minv, INF)
+            j1 = int(np.argmin(cand))                 # first minimum: lowest column on ties
+            delta = cand[j1]
+            ju = np.nonzero(used)[0]
+            u[p[ju]] += delta                         # distinct rows
+            v[ju] -= delta
+            minv[free] -= delta
+            j0 = j1
+            if p[j0] == 0:
+                break
+        while True:
+            j1 = way[j0]
+            p[j0] = p[j1]
+            j0 = j1
+            if j0 == 0:
+                break
+    for j in range(1, m + 1):
+        if p[j]:
+            match[p[j] - 1] = j - 1
+    return match, u[1:].copy(), v[1:m + 1].copy()
+
+
+def components(cost):
+    """Connected components of the admissible (finite) entries: (list of row index arrays, list of column index arrays),
+    each in ascending order, one pair per component that has a row; columns without an admissible entry are left out."""
+    n, m = cost.shape
+    parent = list(range(n + m))
+
+    def find(x):
+        while parent[x] != x:
+            parent[x] = parent[parent[x]]
+            x = parent[x]
+        return x
+    for i, j in zip(*np.nonzero(np.isfinite(cost))):
+        a, b = find(int(i)), find(n + int(j))
+        if a != b:
+            parent[max(a, b)] = min(a, b)
+    groups = {}
+    for x in range(n + m):
+        groups.setdefault(find(x), []).append(x)
+    rows, cols = [], []
+    for g in sorted(groups):
+        r = [x for x in groups[g] if x < n]
+        if r:
+            rows.append(np.array(r, np.int64))
+            cols.append(np.array([x - n for x in groups[g] if x >= n], np.int64))
+    return rows, cols
+
+
+def solve_by_components(cost, L):
+    """solve() applied to each connected component on its own (rows and columns kept in their global order): the same
+    match, u and v bits as solve() on the whole matrix, because one row's search never leaves its component."""
+    cost = np.asarray(cost, np.float64)
+    n, m = cost.shape
+    match, u, v = np.full(n, -1, np.int64), np.zeros(n), np.zeros(m)
+    for r, c in zip(*components(cost)):
+        if len(c) == 0:                               # a row alone takes its own column: slack L
+            u[r] = np.float64(L)
+            continue
+        mm, uu, vv = solve(cost[np.ix_(r, c)], L)
+        match[r] = np.where(mm >= 0, c[np.maximum(mm, 0)], -1)
+        u[r] = uu
+        v[c] = vv
+    return match, u, v
+
+
+# ---------------------------------------------------------------------------------------------- one stream
+class Stream:
+    """The tracker state of one camera stream: tracked and lost lists in ByteTrack's list order."""
+
+    def __init__(self, p):
+        self.p = p
+        self.reset()
+
+    def reset(self):
+        self.frame, self.next_id, self.overflow = 1, 1, 0
+        self.tracked, self.lost = [], []
+        self.dropped = dict(tracked=0, birth=0, lost=0)       # duplicate removals so far (step 8), for the tests
+
+    def _cost(self, tracks, dets, L, fuse, e):
+        scores, labels, boxes = e
+        tb = np.array([t.box() for t in tracks]).reshape(-1, 4)
+        return cost_matrix(tb, [t.label for t in tracks], boxes[dets].reshape(-1, 4), scores[dets], labels[dets], L, fuse,
+                           self.p["class_aware"])
+
+    def _update(self, t, d, e):
+        scores, labels, boxes = e
+        kalman_update(t, measurement(boxes[d]))
+        t.state, t.activated, t.end = TRACKED, True, self.frame
+        t.score, t.label, t.index = scores[d], labels[d], int(d)
+
+    def update(self, scores, labels, boxes):
+        """One frame: scores fp32 [k], labels int32 [k], boxes fp32 [k, 4] (xyxy) -> the output tracks, a list of
+        (id, score fp32, label, box fp32 [4], index)."""
+        p, frame = self.p, self.frame
+        scores = np.asarray(scores, np.float32).reshape(-1)
+        labels = np.asarray(labels).astype(np.int32).reshape(-1)
+        boxes = np.asarray(boxes, np.float32).reshape(-1, 4)
+        e = (scores, labels, boxes)
+        bd = boxes.astype(np.float64)
+        with np.errstate(invalid="ignore"):
+            valid = np.isfinite(bd).all(1) & (bd[:, 2] - bd[:, 0] > 0) & (bd[:, 3] - bd[:, 1] > 0)
+        high = np.nonzero(valid & (scores > p["track_thresh"]))[0]
+        low = np.nonzero(valid & (scores > p["low_thresh"]) & (scores < p["track_thresh"]))[0]
+
+        unconf = [t for t in self.tracked if not t.activated]
+        pool = [t for t in self.tracked if t.activated] + self.lost
+        for t in pool:
+            predict(t)
+        # 1. pool x high detections
+        m1, _, _ = solve(self._cost(pool, high, p["match_thresh"], p["fuse_score"], e), p["match_thresh"])
+        refound = []
+        for t, c in zip(pool, m1):
+            if c >= 0:
+                if t.state == LOST:
+                    refound.append(t)
+                self._update(t, high[c], e)
+        used = np.zeros(len(high), bool)
+        used[m1[m1 >= 0]] = True
+        rest = high[~used]
+        # 2. the pool's unmatched Tracked tracks x low detections, no score fusion
+        r_tracked = [t for t, c in zip(pool, m1) if c < 0 and t.state == TRACKED]
+        m2, _, _ = solve(self._cost(r_tracked, low, p["second_thresh"], False, e), p["second_thresh"])
+        new_lost = []
+        for t, c in zip(r_tracked, m2):
+            if c >= 0:
+                self._update(t, low[c], e)
+            else:
+                t.state = LOST
+                new_lost.append(t)
+        # 3. unconfirmed tracks x the high detections left
+        m3, _, _ = solve(self._cost(unconf, rest, p["unconfirmed_thresh"], p["fuse_score"], e), p["unconfirmed_thresh"])
+        removed = set()
+        for t, c in zip(unconf, m3):
+            if c >= 0:
+                self._update(t, rest[c], e)
+            else:
+                removed.add(id(t))
+        used = np.zeros(len(rest), bool)
+        used[m3[m3 >= 0]] = True
+        rest = rest[~used]
+        # 6. ageing (counted before births: capacity applies to the lists this frame leaves)
+        ref = {id(t) for t in refound}
+        aged = {id(t) for t in self.lost if id(t) not in ref and frame - t.end > p["max_time_lost"]}
+        live = len(self.tracked) + len(self.lost) - len(removed) - len(aged)
+        # 5. births
+        births = []
+        for d in rest:
+            if scores[d] >= p["new_track_thresh"]:
+                if live + len(births) >= p["capacity"]:
+                    self.overflow += 1
+                    continue
+                t = Track()
+                t.id, self.next_id = self.next_id, self.next_id + 1
+                t.state, t.activated, t.start, t.end = TRACKED, frame == 1, frame, frame
+                t.score, t.label, t.index = scores[d], labels[d], int(d)
+                initiate(t, measurement(boxes[d]))
+                births.append(t)
+        # 7. new lists
+        tracked = [t for t in self.tracked if t.state == TRACKED and id(t) not in removed] + births + refound
+        lost = [t for t in self.lost if id(t) not in ref and id(t) not in aged] + new_lost
+        # 8. duplicates between the two lists
+        if tracked and lost:
+            tb = np.array([t.box() for t in tracked])
+            lb = np.array([t.box() for t in lost])
+            dup = (1.0 - iou(tb, lb)) < np.float64(p["duplicate_thresh"])
+            if p["class_aware"]:
+                dup &= np.array([t.label for t in tracked])[:, None] == np.array([t.label for t in lost])[None, :]
+            da, db = set(), set()
+            for a, b in zip(*np.nonzero(dup)):
+                if tracked[a].end - tracked[a].start > lost[b].end - lost[b].start:
+                    db.add(b)
+                else:
+                    da.add(a)
+            born = {id(t) for t in births}
+            self.dropped["birth"] += sum(id(tracked[a]) in born for a in da)
+            self.dropped["tracked"] += sum(id(tracked[a]) not in born for a in da)
+            self.dropped["lost"] += len(db)
+            tracked = [t for i, t in enumerate(tracked) if i not in da]
+            lost = [t for i, t in enumerate(lost) if i not in db]
+        self.tracked, self.lost = tracked, lost
+        self.frame += 1
+        return [(t.id, np.float32(t.score), int(t.label), t.box().astype(np.float32), t.index) for t in tracked if t.activated]
+
+    def export(self):
+        """Every record in list order (tracked, then lost) as dicts with the float64 state."""
+        return [dict(id=t.id, state=t.state, activated=int(t.activated), start=t.start, end=t.end, score=np.float32(t.score),
+                     label=int(t.label), index=t.index, mean=np.concatenate([t.p, t.v]), cov=np.concatenate([t.P, t.C, t.V]))
+                for t in self.tracked + self.lost]
+
+
+def outputs_array(outs, max_out):
+    """Output tracks of one frame as the kernel's padded arrays: (ids, scores, labels, boxes, index, count), unused slots
+    id 0, score 0, label -1, zero box, index -1; count = min(len, max_out)."""
+    n = min(len(outs), max_out)
+    ids = np.zeros(max_out, np.int32)
+    sc = np.zeros(max_out, np.float32)
+    lab = np.full(max_out, -1, np.int32)
+    bx = np.zeros((max_out, 4), np.float32)
+    ix = np.full(max_out, -1, np.int32)
+    for i, (tid, s, l, b, d) in enumerate(outs[:n]):
+        ids[i], sc[i], lab[i], bx[i], ix[i] = tid, s, l, b, d
+    return ids, sc, lab, bx, ix, n
+
+
+# ---------------------------------------------------------------------------------------------- synthetic scenes
+def scene(seed, frames, objects=20, k=None, ncls=3, size=(1080, 1920), clutter=3, miss=0.05, low_dip=0.1, occlusion=0.02,
+          crossing=True, echo=0.0):
+    """Seeded synthetic detections: `objects` ground-truth boxes alive at a time on average, moving at constant velocity with
+    small accelerations, born and dying over the sequence; per frame each visible object gives a detection with jitter
+    (score mostly high, dipping into the low band with probability low_dip), is missed with probability `miss`, and starts
+    an occlusion (no detection for 1 to 80 frames, around ByteTrack's 30-frame buffer) with probability `occlusion`.  Pairs
+    of objects cross each other (crossing).  `clutter` random boxes per frame on average at low to mid scores.  With
+    probability `echo` per frame an object starts a spell of 2 to 11 frames in which it also gives a second detection a few
+    pixels to the side (IoU about 0.9 with the first): such echoes start tracks on top of tracks, which the duplicate removal
+    between the tracked and the lost list then resolves.  Returns a
+    list of (scores fp32 [k_f], labels int32 [k_f], boxes fp32 [k_f, 4]) in shuffled order, or with k given, padded to k
+    entries (score 0, zero box) or cut to its first k."""
+    rng = np.random.default_rng(seed)
+    H, W = size
+    objs = []
+
+    def spawn(t0):
+        h = rng.uniform(30, 300)
+        w = h * rng.uniform(0.3, 1.2)
+        o = dict(cx=rng.uniform(w, W - w), cy=rng.uniform(h, H - h), w=w, h=h, vx=rng.normal(0, 4), vy=rng.normal(0, 2),
+                 label=int(rng.integers(ncls)), die=t0 + int(rng.integers(40, 4 * frames + 40)), hidden=0)
+        objs.append(o)
+    for _ in range(objects):
+        spawn(0)
+    if crossing and objects >= 2:              # two objects aimed at each other
+        a, b = objs[0], objs[1]
+        a.update(cx=W * 0.3, cy=H * 0.5, vx=6.0, vy=0.0)
+        b.update(cx=W * 0.7, cy=H * 0.5 + 10, vx=-6.0, vy=0.0, h=a["h"] * 1.1, w=a["w"] * 0.9)
+    out = []
+    for f in range(frames):
+        objs = [o for o in objs if o["die"] > f and -o["w"] < o["cx"] < W + o["w"] and -o["h"] < o["cy"] < H + o["h"]]
+        while len(objs) < objects and rng.random() < 0.3:
+            spawn(f)
+        det = []
+        for o in objs:
+            o["vx"] += rng.normal(0, 0.3)
+            o["vy"] += rng.normal(0, 0.2)
+            o["cx"] += o["vx"]
+            o["cy"] += o["vy"]
+            if o["hidden"] > 0:
+                o["hidden"] -= 1
+                continue
+            if rng.random() < occlusion:
+                o["hidden"] = int(rng.integers(1, 80))
+                continue
+            if rng.random() < miss:
+                continue
+            j = 0.03 * o["h"]
+            cx, cy = o["cx"] + rng.normal(0, j), o["cy"] + rng.normal(0, j)
+            w, h = o["w"] * (1 + rng.normal(0, 0.03)), o["h"] * (1 + rng.normal(0, 0.03))
+            s = rng.uniform(0.15, 0.5) if rng.random() < low_dip else rng.uniform(0.55, 0.98)
+            det.append((s, o["label"], cx - w / 2, cy - h / 2, cx + w / 2, cy + h / 2))
+            if echo > 0:
+                if o.get("echo", 0) == 0 and rng.random() < echo:
+                    o["echo"] = int(rng.integers(2, 12))
+                if o.get("echo", 0) > 0:
+                    o["echo"] -= 1
+                    dx = 0.025 * w * (1 + rng.normal(0, 0.1))
+                    ew, eh = w * (1 + rng.normal(0, 0.01)), h * (1 + rng.normal(0, 0.01))     # its own size: no exact IoU ties
+                    det.append((rng.uniform(0.65, 0.98), o["label"], cx + dx - ew / 2, cy - eh / 2, cx + dx + ew / 2, cy + eh / 2))
+        for _ in range(rng.poisson(clutter)):
+            h = rng.uniform(20, 200)
+            w = h * rng.uniform(0.3, 1.5)
+            x, y = rng.uniform(0, W - w), rng.uniform(0, H - h)
+            det.append((rng.uniform(0.05, 0.65), int(rng.integers(ncls)), x, y, x + w, y + h))
+        rng.shuffle(det)
+        a = np.array(det, np.float64).reshape(-1, 6)
+        out.append(pad(a[:, 0].astype(np.float32), a[:, 1].astype(np.int32), a[:, 2:].astype(np.float32), k))
+    return out
+
+
+def pad(scores, labels, boxes, k):
+    """One frame's entries padded with (score 0, label 0, zero box) or cut to k entries (k None: unchanged)."""
+    if k is None:
+        return scores, labels, boxes
+    n = min(len(scores), k)
+    s = np.zeros(k, np.float32)
+    lab = np.zeros(k, np.int32)
+    b = np.zeros((k, 4), np.float32)
+    s[:n], lab[:n], b[:n] = scores[:n], labels[:n], boxes[:n]
+    return s, lab, b
