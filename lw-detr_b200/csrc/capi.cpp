@@ -32,6 +32,18 @@ int cuda_fail(int e, const char* what) {
   g_err = std::string(what) + ": " + cudaGetErrorString(static_cast<cudaError_t>(e));
   return -1;
 }
+// the GEMM both lwdetr_gemm and lwdetr_gemm_ex describe
+lwb::GemmDesc gemm_desc(const lwdetr_gemm_args& a) {
+  lwb::GemmDesc d;
+  d.dtype = a.dtype; d.A = a.A; d.lda = a.lda; d.M = a.M; d.N = a.N; d.K = a.K; d.W = a.W; d.bias = a.bias; d.gamma = a.gamma;
+  d.resid = a.resid; d.ld_resid = a.ld_resid; d.resid_mod = a.resid_mod; d.act = a.act; d.out = a.out; d.ld_out = a.ld_out;
+  d.out_fp32 = a.out_fp32; d.rows_in = a.rows_in; d.remap_rows = a.remap_rows; d.shuffle_cout = a.shuffle_cout;
+  d.IH = a.IH; d.IW = a.IW;
+  d.stats_in = reinterpret_cast<const float2*>(a.stats_in); d.stats_parts_in = a.stats_parts_in; d.colsum = a.colsum;
+  d.ln_C = a.ln_C; d.ln_eps = a.ln_eps; d.stats_out = reinterpret_cast<float2*>(a.stats_out);
+  d.hm_S = a.hm_S; d.hm_heads = a.hm_heads; d.hm_slices = a.hm_slices; d.row_zero = a.row_zero;
+  return d;
+}
 }  // namespace
 
 extern "C" {
@@ -43,14 +55,11 @@ int lwdetr_gemm(int dtype, const void* A, int lda, int M, int K, const void* W, 
                 const float* gamma, const void* resid, int ld_resid, int resid_mod, int act, void* out, int ld_out,
                 int out_fp32, int rows_in, int remap_rows, int shuffle_cout, int IH, int IW, void* stream) {
   if (!A || !W || !out) return fail("lwdetr_gemm: null pointer");
-  lwb::GemmDesc d;
-  d.dtype = dtype; d.A = A; d.lda = lda; d.M = M; d.N = N; d.K = K; d.W = W; d.bias = bias; d.gamma = gamma;
-  d.resid = resid; d.ld_resid = ld_resid; d.resid_mod = resid_mod; d.act = act; d.out = out; d.ld_out = ld_out;
-  d.out_fp32 = out_fp32; d.rows_in = rows_in; d.remap_rows = remap_rows; d.shuffle_cout = shuffle_cout;
-  d.IH = IH; d.IW = IW;
+  const lwdetr_gemm_args a = {dtype, A, lda, M, K, W, N, bias, gamma, resid, ld_resid, resid_mod, act, out, ld_out, out_fp32,
+                              rows_in, remap_rows, shuffle_cout, IH, IW};
   lwb::GemmOp op;
   std::string err;
-  if (lwb::gemm_build(d, &op, &err)) return fail("lwdetr_gemm: " + err);
+  if (lwb::gemm_build(gemm_desc(a), &op, &err)) return fail("lwdetr_gemm: " + err);
   int e = lwb::gemm_launch(op, static_cast<cudaStream_t>(stream));
   if (e) return cuda_fail(e, "lwdetr_gemm launch");
   return 0;
@@ -63,17 +72,9 @@ int lwdetr_gemm_ex(lwdetr_gemm_args* a, void* stream) {
   if (!a || !a->A || !a->W || !a->out) return fail("lwdetr_gemm_ex: null pointer");
   // 16-bit GEMMs only (the e4m3 GEMM has its own entry point and no epilogue variants), so `epilogue` is always an LWDETR_EP_*
   if (a->dtype != LWDETR_F16 && a->dtype != LWDETR_BF16) return fail("lwdetr_gemm_ex: dtype must be LWDETR_F16 or LWDETR_BF16");
-  lwb::GemmDesc d;
-  d.dtype = a->dtype; d.A = a->A; d.lda = a->lda; d.M = a->M; d.N = a->N; d.K = a->K; d.W = a->W; d.bias = a->bias; d.gamma = a->gamma;
-  d.resid = a->resid; d.ld_resid = a->ld_resid; d.resid_mod = a->resid_mod; d.act = a->act; d.out = a->out; d.ld_out = a->ld_out;
-  d.out_fp32 = a->out_fp32; d.rows_in = a->rows_in; d.remap_rows = a->remap_rows; d.shuffle_cout = a->shuffle_cout;
-  d.IH = a->IH; d.IW = a->IW;
-  d.stats_in = reinterpret_cast<const float2*>(a->stats_in); d.stats_parts_in = a->stats_parts_in; d.colsum = a->colsum;
-  d.ln_C = a->ln_C; d.ln_eps = a->ln_eps; d.stats_out = reinterpret_cast<float2*>(a->stats_out);
-  d.hm_S = a->hm_S; d.hm_heads = a->hm_heads; d.hm_slices = a->hm_slices; d.row_zero = a->row_zero;
   lwb::GemmOp op;
   std::string err;
-  if (lwb::gemm_build(d, &op, &err)) return fail("lwdetr_gemm_ex: " + err);
+  if (lwb::gemm_build(gemm_desc(*a), &op, &err)) return fail("lwdetr_gemm_ex: " + err);
   a->bn = op.bn;
   a->epilogue = lwb::gemm_epilogue(op);
   a->stats_parts_out = op.args.stats_parts_out;
@@ -310,18 +311,6 @@ void lwdetr_track_params_default(lwdetr_track_params* p) {
   p->capacity = 512;
 }
 
-// Runs a call on the tracker's device and switches back.
-struct DeviceGuard {
-  int prev = -1;
-  explicit DeviceGuard(int dev) {
-    if (cudaGetDevice(&prev) == cudaSuccess && prev != dev) cudaSetDevice(dev);
-  }
-  ~DeviceGuard() {
-    int now = -1;
-    if (prev >= 0 && cudaGetDevice(&now) == cudaSuccess && now != prev) cudaSetDevice(prev);
-  }
-};
-
 int lwdetr_tracker_create(int num_streams, const lwdetr_track_params* params, lwdetr_tracker** out) {
   if (!params || !out) return fail("lwdetr_tracker_create: null pointer");
   const lwdetr_track_params& p = *params;
@@ -368,7 +357,7 @@ int lwdetr_tracker_create(int num_streams, const lwdetr_track_params* params, lw
 
 void lwdetr_tracker_destroy(lwdetr_tracker* t) {
   if (!t) return;
-  DeviceGuard g(t->device);
+  lwb::DeviceGuard g(t->device);
   cudaStreamSynchronize(t->copy);
   cudaFree(t->table.head);
   cudaFree(t->table.rec);
@@ -393,7 +382,7 @@ int lwdetr_tracker_reset(lwdetr_tracker* t, const int32_t* streams, int n, void*
   const std::string err = check_streams(t, streams, n);
   if (!err.empty()) return fail("lwdetr_tracker_reset: " + err);
   if (n == 0) return 0;
-  DeviceGuard g(t->device);
+  lwb::DeviceGuard g(t->device);
   int e = lwb::track_reset_launch(t->table, streams, n, static_cast<cudaStream_t>(stream));
   if (!e) e = tracker_mark(t, stream);
   if (e) return cuda_fail(e, "lwdetr_tracker_reset launch");
@@ -410,7 +399,7 @@ int lwdetr_track(lwdetr_tracker* t, const float* scores, const int32_t* labels, 
     return fail("lwdetr_track: boxes and out_boxes must be 16-byte aligned");
   const std::string err = check_streams(t, stream_ids, B);
   if (!err.empty()) return fail("lwdetr_track: " + err);
-  DeviceGuard g(t->device);
+  lwb::DeviceGuard g(t->device);
   int e = lwb::track_launch(t->table, t->params, scores, labels, boxes, B, k, stream_ids, max_out, out_ids, out_scores, out_labels,
                             out_boxes, out_index, counts, static_cast<cudaStream_t>(stream));
   if (e == -2) return fail("lwdetr_track: a limit is exceeded");
@@ -422,7 +411,7 @@ int lwdetr_track(lwdetr_tracker* t, const float* scores, const int32_t* labels, 
 int lwdetr_tracker_export(lwdetr_tracker* t, int stream_id, lwdetr_track_record* host, int cap, int32_t* count, int32_t frame_next_overflow[3]) {
   if (!t || !count || !frame_next_overflow || (cap > 0 && !host)) return fail("lwdetr_tracker_export: null pointer");
   if (stream_id < 0 || stream_id >= t->table.num_streams) return fail("lwdetr_tracker_export: stream id outside [0, num_streams)");
-  DeviceGuard g(t->device);
+  lwb::DeviceGuard g(t->device);
   lwb::TrackHead h;
   cudaError_t e = cudaStreamWaitEvent(t->copy, t->done, 0);
   if (e == cudaSuccess) e = cudaMemcpyAsync(&h, t->table.head + stream_id, sizeof(h), cudaMemcpyDeviceToHost, t->copy);
@@ -549,18 +538,6 @@ int lwdetr_load_weights(lwdetr_handle* h, int n, const char* const* names, const
   return 0;
 }
 
-int lwdetr_forward(lwdetr_handle* h, const void* images, int images_fp32, int B, float* pred_logits, float* pred_boxes,
-                   const lwdetr_aux_out* aux, const int32_t* topk_override, void* stream) {
-  if (!h || !images) return fail("lwdetr_forward: null pointer");
-  std::string err;
-  lwb::ForwardIn in;
-  in.images = images; in.kind = images_fp32 ? lwb::IN_F32_NCHW : lwb::IN_16_NCHW;
-  const int S = h->eng->config().img_size;
-  if (h->eng->forward(in, B, S, S, pred_logits, pred_boxes, aux, topk_override, static_cast<cudaStream_t>(stream), &err))
-    return fail(err);
-  return 0;
-}
-
 static int forward_input(const char* fn, lwdetr_handle* h, const lwdetr_input* input, int B, int height, int width, float* pred_logits,
                          float* pred_boxes, const lwdetr_aux_out* aux, const int32_t* topk_override, void* stream) {
   if (!h || !input || !input->images) return fail(std::string(fn) + ": null pointer");
@@ -575,6 +552,14 @@ static int forward_input(const char* fn, lwdetr_handle* h, const lwdetr_input* i
   std::string err;
   if (h->eng->forward(in, B, height, width, pred_logits, pred_boxes, aux, topk_override, static_cast<cudaStream_t>(stream), &err)) return fail(err);
   return 0;
+}
+
+int lwdetr_forward(lwdetr_handle* h, const void* images, int images_fp32, int B, float* pred_logits, float* pred_boxes,
+                   const lwdetr_aux_out* aux, const int32_t* topk_override, void* stream) {
+  if (!h || !images) return fail("lwdetr_forward: null pointer");
+  const lwdetr_input input = {images, images_fp32 ? LWDETR_IN_F32_NCHW : LWDETR_IN_16_NCHW, nullptr, {0.f, 0.f, 0.f}, {1.f, 1.f, 1.f}};
+  const int S = h->eng->config().img_size;
+  return forward_input("lwdetr_forward", h, &input, B, S, S, pred_logits, pred_boxes, aux, topk_override, stream);
 }
 
 int lwdetr_forward_ex(lwdetr_handle* h, const lwdetr_input* input, int B, float* pred_logits, float* pred_boxes,

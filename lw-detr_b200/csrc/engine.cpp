@@ -30,6 +30,147 @@ struct Mat {
 };
 inline char* cptr(void* p) { return static_cast<char*>(p); }
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// What a debug capture of an op copies back: rows x cols of a [*, ld] matrix, fp32 or in the compute dtype.
+struct OutView {
+  const void* p;
+  long long rows;
+  int cols, ld, fp32;
+};
+
+// One pass of Engine::plan.  Pass 0 sizes the workspace: allocations only advance the bump offset (and return null),
+// weight lookups return null and nothing is recorded.  Pass 1 lays the same allocations out from the arena base, resolves
+// the packed weights and records the ops.  The first error is kept.
+class OpBuilder {
+ public:
+  OpBuilder(int pass, int dtype, void* arena, const std::map<std::string, void*>& w16s, const std::map<std::string, float*>& w32s,
+            std::string too_big, std::string* err, std::vector<Op>* ops)
+      : pass_(pass), dtype_(dtype), arena_(pass ? arena : nullptr), w16s_(w16s), w32s_(w32s), too_big_(std::move(too_big)),
+        err_(err), ops_(ops) {}
+
+  bool failed() const { return failed_; }
+  size_t bytes() const { return off_; }
+  void fail(const std::string& m) { if (!failed_) *err_ = m; failed_ = true; }
+  // every kernel indexes a buffer's elements / a GEMM's rows with 32-bit integers somewhere: no buffer may exceed that range
+  bool fits(long long n) { if (n > 2147483647LL) fail(too_big_); return n <= 2147483647LL; }
+  void* alloc(size_t bytes) {
+    off_ = align_up(off_, 1024);
+    void* p = arena_ ? cptr(arena_) + off_ : nullptr;
+    off_ += bytes;
+    return p;
+  }
+  Mat buf16(long long rows, int cols) { fits(rows * cols); return Mat{alloc(static_cast<size_t>(rows) * cols * 2), cols}; }
+  float* buf32(long long n) { fits(n); return static_cast<float*>(alloc(static_cast<size_t>(n) * 4)); }
+  void* w16(const std::string& k) { return lookup(w16s_, k, "internal: weight "); }
+  float* w32(const std::string& k) { return lookup(w32s_, k, "internal: vector "); }
+
+  void record(const std::string& label, std::function<int(cudaStream_t)> run, const OutView& out, double flops, double bytes,
+              bool reads_input) {
+    if (pass_ == 0 || failed_) return;
+    Op op;
+    op.label = label; op.run = std::move(run);
+    op.out = out.p; op.rows = out.rows; op.cols = out.cols; op.ld = out.ld; op.fp32 = out.fp32;
+    op.flops = flops; op.bytes = bytes; op.reads_input = reads_input;
+    ops_->push_back(std::move(op));
+  }
+  void op(const std::string& label, std::function<int(cudaStream_t)> run, const OutView& out, double bytes, bool reads_input = false) {
+    record(label, std::move(run), out, 0.0, bytes, reads_input);
+  }
+  // out = epilogue(A W^T) with W = `wkey`.w, bias `wkey`.b if packed (and colsum `wkey`.cs for a LayerNorm consumer); `g` carries
+  // the A mode and the epilogue, the rest is filled in here
+  void gemm(const std::string& label, GemmDesc g, Mat A, long long M, int K, const std::string& wkey, int N, Mat out) {
+    if (!fits(M) || pass_ == 0) return;
+    g.dtype = dtype_; g.A = A.p; g.lda = A.ld; g.M = static_cast<int>(M); g.N = N; g.K = K;
+    g.W = w16(wkey + ".w"); g.bias = w32s_.count(wkey + ".b") ? w32s_.at(wkey + ".b") : nullptr;
+    g.out = out.p; g.ld_out = out.ld; g.stats_parts_in = stats_parts_;
+    if (g.stats_in) g.colsum = w32(wkey + ".cs");
+    GemmOp op;
+    std::string e;
+    if (failed_ || gemm_build(g, &op, &e)) return fail(label + ": " + e);
+    if (g.stats_out) {   // partial (sum, sumsq) pairs per row written by the N = C producer GEMMs: the same for all of them
+      if (stats_parts_ == 0) stats_parts_ = op.args.stats_parts_out;
+      if (stats_parts_ != op.args.stats_parts_out || stats_parts_ > 48) return fail(label + ": inconsistent LayerNorm partial count");
+    }
+    const long long rows = g.hm_S ? M * g.hm_slices * g.hm_heads : (g.shuffle_cout ? M * 4 : M);
+    const int cols = g.shuffle_cout ? g.shuffle_cout : (g.hm_S ? 16 : N);
+    record(label, [op](cudaStream_t st) { return gemm_launch(op, st); }, {out.p, rows, cols, out.ld, g.out_fp32}, op.flops,
+           2.0 * (static_cast<double>(M) * K + static_cast<double>(N) * K) + (g.out_fp32 ? 4.0 : 2.0) * M * N + (g.resid ? 2.0 * M * N : 0.0),
+           false);
+  }
+  // the e4m3 GEMM: A e4m3 codes [M, K] with per-row scales; W, per-channel scales and bias `wkey`.w / .s / .b
+  void gemm_e4m3(const std::string& label, const void* A, const float* a_scale, long long M, int K, const std::string& wkey, int N, int act,
+                 Mat out) {
+    if (pass_ == 0) return;
+    GemmE4m3Desc g;
+    g.A = A; g.lda = K; g.a_scale = a_scale; g.M = static_cast<int>(M); g.K = K; g.N = N;
+    g.W = w16(wkey + ".w"); g.w_scale = w32(wkey + ".s"); g.bias = w32(wkey + ".b"); g.act = act; g.out = out.p; g.ld_out = out.ld;
+    GemmOp op;
+    std::string e;
+    if (failed_ || gemm_e4m3_build(g, &op, &e)) return fail(label + ": " + e);
+    record(label, [op](cudaStream_t st) { return gemm_launch(op, st); }, {out.p, M, N, out.ld, 0}, op.flops,
+           1.0 * (static_cast<double>(M) * K + static_cast<double>(N) * K) + 4.0 * M + 8.0 * N + 2.0 * M * N, false);   // 1-byte operands
+  }
+  // fused ViT MLP (vit_mlp_kernel) of block `k`: LN2 statistics from stats_in, folded fc1, GELU, fc2, layer-scale and
+  // residual; writes the next block's LayerNorm partials in the layout the fc2 GEMM would have used
+  void mlp(const std::string& label, Mat x, long long M, const float2* stats_in, const std::string& k, float2* stats_out, Mat out) {
+    if (pass_ == 0) return;
+    MlpDesc g;
+    g.dtype = dtype_; g.x = x.p; g.ldx = x.ld; g.M = static_cast<int>(M);
+    g.stats_in = stats_in; g.stats_parts_in = stats_parts_; g.ln_eps = 1e-6f;
+    g.w1 = w16(k + "fc1_ln.w"); g.colsum1 = w32(k + "fc1_ln.cs"); g.b1 = w32(k + "fc1_ln.b");
+    g.w2 = w16(k + "fc2.w"); g.b2 = w32(k + "fc2.b"); g.gamma = w32(k + "g2");
+    g.out = out.p; g.ld_out = out.ld; g.stats_out = stats_out; g.stats_parts_out = stats_parts_;
+    MlpOp op;
+    std::string e;
+    if (failed_ || vit_mlp_build(g, &op, &e)) return fail(label + ": " + e);
+    record(label, [op](cudaStream_t st) { return vit_mlp_launch(op, st); }, {out.p, M, MLP_C, out.ld, 0}, op.flops,
+           2.0 * 3.0 * M * MLP_C + 2.0 * 2.0 * (4.0 * MLP_C) * MLP_C, false);   // x (operand and residual), out, both weights
+  }
+  // y = LN(x; `nkey`.w / .b, eps) over rows x C; `a` carries the optional fields (row flag / override, y2 = y + add_src, grouped
+  // y rows, and the chained y3 = LN(y; `nkey3`.w / .b, eps3)), the rest is filled in here
+  void layernorm(const std::string& label, Mat x, Mat y, const std::string& nkey, float eps, long long rows, int C, LayerNormArgs a = {},
+                 const std::string& nkey3 = std::string()) {
+    if (pass_ == 0) return;
+    if (a.y3) { a.w3 = w32(nkey3 + ".w"); a.b3 = w32(nkey3 + ".b"); }
+    a.x = x.p; a.ldx = x.ld; a.y = y.p; a.ldy = y.ld; a.w = w32(nkey + ".w"); a.b = w32(nkey + ".b"); a.eps = eps;
+    a.rows = rows; a.C = C;
+    if (a.flag_mod < 1) a.flag_mod = 1;
+    const int dt = dtype_;
+    const long long out_rows = a.y_group ? rows / a.y_group * a.y_group_stride : rows;
+    record(label, [a, dt](cudaStream_t st) { return layernorm_launch(dt, a, st); }, {y.p, out_rows, C, y.ld, 0}, 0.0,
+           4.0 * rows * C + (a.y2 ? 4.0 * rows * C : 0.0) + (a.y3 ? 2.0 * rows * C : 0.0), false);
+  }
+  void attention(const std::string& label, Mat q, Mat k, Mat v, Mat o, int nseq, int seqlen, int heads, int dh) {
+    if (pass_ == 0) return;
+    AttnArgs a;
+    a.q = q.p; a.k = k.p; a.v = v.p; a.ldq = q.ld; a.ldk = k.ld; a.ldv = v.ld; a.o = o.p; a.ldo = o.ld;
+    a.seqlen = seqlen; a.nseq = nseq; a.heads = heads;
+    a.scale_log2 = 1.4426950408889634f / std::sqrt(static_cast<float>(dh));
+    const int dt = dtype_;
+    record(label, [a, dt, dh](cudaStream_t st) { return attention_launch(dt, a, dh, st); }, {o.p, 1LL * nseq * seqlen, heads * dh, o.ld, 0},
+           4.0 * nseq * static_cast<double>(seqlen) * seqlen * heads * dh, 2.0 * 4.0 * nseq * seqlen * heads * dh, false);
+  }
+
+ private:
+  template <typename T>
+  T* lookup(const std::map<std::string, T*>& m, const std::string& k, const char* what) {   // packed weights: pass 1 only
+    if (pass_ == 0) return nullptr;
+    auto it = m.find(k);
+    if (it == m.end()) { fail(what + k); return nullptr; }
+    return it->second;
+  }
+
+  const int pass_, dtype_;
+  void* const arena_;
+  const std::map<std::string, void*>& w16s_;
+  const std::map<std::string, float*>& w32s_;
+  const std::string too_big_;
+  std::string* const err_;
+  std::vector<Op>* const ops_;
+  size_t off_ = 0;          // workspace bump offset
+  bool failed_ = false;
+  int stats_parts_ = 0;     // LayerNorm partials per row of the ViT's statistics producers (0 until the first one is built)
+};
 }  // namespace
 
 // ------------------------------------------------------------------------------- host math helpers
@@ -122,26 +263,9 @@ Engine::Engine(const lwdetr_config& cfg, int dtype) : cfg_(cfg), dtype_(dtype ==
   cudaGetDevice(&device_);
 }
 
-namespace {
-// Switches to the engine's device for the duration of a call (the caller's current device is restored afterwards).
-struct DeviceGuard {
-  int prev = -1;
-  explicit DeviceGuard(int dev) {
-    if (cudaGetDevice(&prev) != cudaSuccess) prev = -1;
-    if (prev != dev) cudaSetDevice(dev); else prev = -1;
-  }
-  ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
-};
-}  // namespace
-
-void Engine::drop_graphs() {
-  for (auto& kv : graphs_) cudaGraphExecDestroy(kv.second);
-  graphs_.clear();
-}
-
 Engine::~Engine() {
   DeviceGuard guard(device_);
-  drop_graphs();
+  plan_.reset();
   if (gstream_) cudaStreamDestroy(gstream_);
   if (ev_in_) cudaEventDestroy(ev_in_);
   if (ev_out_) cudaEventDestroy(ev_out_);
@@ -154,12 +278,6 @@ void* Engine::walloc(size_t bytes) {
   if (woff_ + bytes > warena_.bytes) return nullptr;
   void* p = cptr(warena_.p) + woff_;
   woff_ += bytes;
-  return p;
-}
-void* Engine::salloc(size_t bytes) {
-  soff_ = align_up(soff_, 1024);
-  void* p = sarena_.p ? cptr(sarena_.p) + soff_ : nullptr;
-  soff_ += bytes;
   return p;
 }
 
@@ -201,18 +319,17 @@ float* Engine::upload32(const std::vector<float>& v) {
 int Engine::set_option(const char* name, int value) {
   if (std::strcmp(name, "fuse_layernorm") == 0) {
     fuse_ln_ = value;
-    drop_graphs();
-    planned_B_ = planned_H_ = planned_W_ = 0;
+    plan_.reset();
     return 0;
   }
   if (std::strcmp(name, "cuda_graph") == 0) {
     use_graph_ = value;
-    drop_graphs();
+    if (plan_) plan_->clear_graphs();
     return 0;
   }
   if (std::strcmp(name, "pdl") == 0) {                 // programmatic dependent launch of every kernel (launch.h); process-wide
     pdl_enabled() = value ? 1 : 0;
-    drop_graphs();
+    if (plan_) plan_->clear_graphs();
     return 0;
   }
   return -1;
@@ -223,8 +340,7 @@ int Engine::load_weights(const std::map<std::string, HostTensor>& w, std::string
   DeviceGuard guard(device_);
   // Whatever happens below, the old packing is gone: a failed load must not leave a schedule pointing into a freed arena.
   weights_loaded_ = false;
-  planned_B_ = planned_H_ = planned_W_ = 0;
-  ops_.clear();
+  plan_.reset();
   const int C = cfg_.vit_dim, d = cfg_.hidden_dim, nq = cfg_.num_queries, ncls = cfg_.num_classes;
   const int G = cfg_.img_size / 16, ntap = cfg_.n_taps, c2 = d / 2;
   const int M = cfg_.ca_heads, L = cfg_.n_levels, P = cfg_.dec_points, ff = cfg_.dim_feedforward;
@@ -245,7 +361,6 @@ int Engine::load_weights(const std::map<std::string, HostTensor>& w, std::string
   // total parameter bytes bound: every tensor at most once in 16-bit + fp32 vectors + slack
   long long total = 0;
   for (auto& kv : w) total += kv.second.numel;
-  drop_graphs();
   if (warena_.p) { cudaFree(warena_.p); warena_.p = nullptr; }
   warena_.bytes = static_cast<size_t>(total) * 4 + (96u << 20);
   if (cudaMalloc(&warena_.p, warena_.bytes) != cudaSuccess) { *err = "cudaMalloc(weight arena) failed"; return -1; }
@@ -307,86 +422,59 @@ int Engine::load_weights(const std::map<std::string, HostTensor>& w, std::string
   put32("patch.b", vec(E + "patch_embed.proj.bias", C));
   const std::vector<float> pos_embed = vec(E + "pos_embed", 197LL * C);
   put16("pos", window_major_pos(pos_embed.data(), C, G, G));   // the table at the configured resolution
-  for (int i = 0; i < cfg_.vit_depth; ++i) {
-    const std::string b = E + "blocks." + std::to_string(i) + ".", k = "blk" + std::to_string(i) + ".";
+  // The encoder's LayerNorms folded into the consuming GEMM (which then runs on the raw residual stream, see gemm_tc.h):
+  //   W'[n,k] = W[n,k]*ln_w[k] ; bias'[n] = bias[n] + sum_k ln_b[k]*W[n,k] (double).  16-bit: W', bias' and colsum[n] =
+  //   sum_k round16(W'[n,k]).  e4m3 (lwdetr_b200.h LWDETR_F16_E4M3): per output channel n, w_scale[n] = max_k |W'[n,k]| / 448
+  //   and codes e4m3(W'[n,k] * 448 / max), then bias'
+  auto put_folded = [&](const std::string& key, const std::vector<float>& Wm, const std::vector<float>& bias, const std::string& ln, int n_out) {
+    auto lw = vec(ln + ".weight", C), lb = vec(ln + ".bias", C);
+    std::vector<float> Wf(Wm.size()), bf(n_out), per_n(n_out);   // per output channel: w_scale (e4m3) or colsum (16-bit)
+    for (int n = 0; n < n_out; ++n) {
+      double acc_b = bias[n];
+      for (int kk = 0; kk < C; ++kk) {
+        const float wv = Wm[static_cast<size_t>(n) * C + kk];
+        Wf[static_cast<size_t>(n) * C + kk] = wv * lw[kk];
+        acc_b += static_cast<double>(lb[kk]) * wv;
+      }
+      bf[n] = static_cast<float>(acc_b);
+    }
     if (e4m3_) {
-      // e4m3 mode: qkv and fc1 only as e4m3 weights with the LayerNorm affine folded in (see lwdetr_b200.h LWDETR_F16_E4M3):
-      //   W' = W diag(ln_w), per output channel n: w_scale[n] = max_k |W'[n,k]| / 448, codes e4m3(W'[n,k] * 448 / max),
-      //   bias'[n] = bias[n] + sum_k ln_b[k] W[n,k] (double)
-      auto put_e4m3 = [&](const std::string& key, const std::vector<float>& Wm, const std::vector<float>& bias, const std::string& ln, int n_out) {
-        auto lw = vec(ln + ".weight", C), lb = vec(ln + ".bias", C);
-        std::vector<float> Wf(Wm.size()), bf(n_out), sw(n_out);
-        for (int n = 0; n < n_out; ++n) {
-          double acc_b = bias[n];
-          for (int kk = 0; kk < C; ++kk) {
-            const float wv = Wm[static_cast<size_t>(n) * C + kk];
-            Wf[static_cast<size_t>(n) * C + kk] = wv * lw[kk];
-            acc_b += static_cast<double>(lb[kk]) * wv;
-          }
-          bf[n] = static_cast<float>(acc_b);
-        }
-        std::vector<uint8_t> q(Wf.size());
-        host_quant_e4m3_rows(Wf.data(), n_out, C, q.data(), sw.data());
-        void* p = upload8(q);
-        if (!p) oom = true;
-        W_[key + ".w"] = p;
-        put32(key + ".b", bf);
-        put32(key + ".s", sw);
-      };
-      auto qb = vec(b + "attn.q_bias", C), vb = vec(b + "attn.v_bias", C);
-      std::vector<float> bias(static_cast<size_t>(3) * C, 0.f);     // [q_bias, 0, v_bias]  (vit.py:123-125)
-      std::copy(qb.begin(), qb.end(), bias.begin());
-      std::copy(vb.begin(), vb.end(), bias.begin() + 2 * C);
-      put_e4m3(k + "qkv_q", vec(b + "attn.qkv.weight", 3LL * C * C), bias, b + "norm1", 3 * C);
-      put_e4m3(k + "fc1_q", vec(b + "mlp.fc1.weight", 4LL * C * C), vec(b + "mlp.fc1.bias", 4LL * C), b + "norm2", 4 * C);
-      put_linear(k + "proj", b + "attn.proj", C, C);
-      put32(k + "g1", vec(b + "gamma_1", C));
-      put_linear(k + "fc2", b + "mlp.fc2", C, 4 * C);
-      put32(k + "g2", vec(b + "gamma_2", C));
-      continue;
-    }
-    put_norm(k + "ln1", b + "norm1", C);
-    put16(k + "qkv.w", vec(b + "attn.qkv.weight", 3LL * C * C));
-    {
-      auto qb = vec(b + "attn.q_bias", C), vb = vec(b + "attn.v_bias", C);
-      std::vector<float> bias(static_cast<size_t>(3) * C, 0.f);     // [q_bias, 0, v_bias]  (vit.py:123-125)
-      std::copy(qb.begin(), qb.end(), bias.begin());
-      std::copy(vb.begin(), vb.end(), bias.begin() + 2 * C);
-      put32(k + "qkv.b", bias);
-    }
-    // LayerNorm-fused variants (consumer GEMMs run on the raw residual stream, see gemm_tc.h):
-    //   W'[n,k] = W[n,k]*ln_w[k] ; colsum[n] = sum_k round16(W'[n,k]) ; bias'[n] = bias[n] + sum_k ln_b[k]*W[n,k]
-    auto fold_ln = [&](const std::string& key, const std::vector<float>& Wm, const std::vector<float>& bias, const std::string& ln, int n_out) {
-      auto lw = vec(ln + ".weight", C), lb = vec(ln + ".bias", C);
-      std::vector<float> Wf(Wm.size()), cs(n_out), bf(n_out);
+      std::vector<uint8_t> q(Wf.size());
+      host_quant_e4m3_rows(Wf.data(), n_out, C, q.data(), per_n.data());
+      void* p = upload8(q);
+      if (!p) oom = true;
+      W_[key + ".w"] = p;
+    } else {
       for (int n = 0; n < n_out; ++n) {
-        double acc_b = bias[n], acc_c = 0.0;
-        for (int kk = 0; kk < C; ++kk) {
-          const float wv = Wm[static_cast<size_t>(n) * C + kk];
-          const float wf = wv * lw[kk];
-          Wf[static_cast<size_t>(n) * C + kk] = wf;
-          acc_c += round16(wf);
-          acc_b += static_cast<double>(lb[kk]) * wv;
-        }
-        cs[n] = static_cast<float>(acc_c);
-        bf[n] = static_cast<float>(acc_b);
+        double acc_c = 0.0;
+        for (int kk = 0; kk < C; ++kk) acc_c += round16(Wf[static_cast<size_t>(n) * C + kk]);
+        per_n[n] = static_cast<float>(acc_c);
       }
       put16(key + ".w", Wf);
-      put32(key + ".b", bf);
-      put32(key + ".cs", cs);
-    };
-    {
-      auto qb = vec(b + "attn.q_bias", C), vb = vec(b + "attn.v_bias", C);
-      std::vector<float> bias(static_cast<size_t>(3) * C, 0.f);
-      std::copy(qb.begin(), qb.end(), bias.begin());
-      std::copy(vb.begin(), vb.end(), bias.begin() + 2 * C);
-      fold_ln(k + "qkv_ln", vec(b + "attn.qkv.weight", 3LL * C * C), bias, b + "norm1", 3 * C);
-      fold_ln(k + "fc1_ln", vec(b + "mlp.fc1.weight", 4LL * C * C), vec(b + "mlp.fc1.bias", 4LL * C), b + "norm2", 4 * C);
     }
+    put32(key + ".b", bf);
+    put32(key + (e4m3_ ? ".s" : ".cs"), per_n);
+  };
+  for (int i = 0; i < cfg_.vit_depth; ++i) {
+    const std::string b = E + "blocks." + std::to_string(i) + ".", k = "blk" + std::to_string(i) + ".";
+    // the e4m3 mode packs qkv and fc1 only as e4m3 weights with the LayerNorm affine folded in
+    if (!e4m3_) {
+      put_norm(k + "ln1", b + "norm1", C);
+      put16(k + "qkv.w", vec(b + "attn.qkv.weight", 3LL * C * C));
+    }
+    auto qb = vec(b + "attn.q_bias", C), vb = vec(b + "attn.v_bias", C);
+    std::vector<float> qkv_b(static_cast<size_t>(3) * C, 0.f);     // [q_bias, 0, v_bias]  (vit.py:123-125)
+    std::copy(qb.begin(), qb.end(), qkv_b.begin());
+    std::copy(vb.begin(), vb.end(), qkv_b.begin() + 2 * C);
+    if (!e4m3_) put32(k + "qkv.b", qkv_b);
+    put_folded(k + (e4m3_ ? "qkv_q" : "qkv_ln"), vec(b + "attn.qkv.weight", 3LL * C * C), qkv_b, b + "norm1", 3 * C);
+    put_folded(k + (e4m3_ ? "fc1_q" : "fc1_ln"), vec(b + "mlp.fc1.weight", 4LL * C * C), vec(b + "mlp.fc1.bias", 4LL * C), b + "norm2", 4 * C);
     put_linear(k + "proj", b + "attn.proj", C, C);
     put32(k + "g1", vec(b + "gamma_1", C));
-    put_norm(k + "ln2", b + "norm2", C);
-    put_linear(k + "fc1", b + "mlp.fc1", 4 * C, C);
+    if (!e4m3_) {
+      put_norm(k + "ln2", b + "norm2", C);
+      put_linear(k + "fc1", b + "mlp.fc1", 4 * C, C);
+    }
     put_linear(k + "fc2", b + "mlp.fc2", C, 4 * C);
     put32(k + "g2", vec(b + "gamma_2", C));
   }
@@ -477,12 +565,12 @@ int Engine::load_weights(const std::map<std::string, HostTensor>& w, std::string
   if (oom) { *err = "weight arena exhausted"; return -1; }
   if (cudaDeviceSynchronize() != cudaSuccess) { *err = "CUDA error while uploading weights"; return -1; }
   weights_loaded_ = true;
-  planned_B_ = planned_H_ = planned_W_ = 0;   // pointers changed: re-plan
   return 0;
 }
 
 // ------------------------------------------------------------------------------- schedule
 int Engine::plan(int B, int IH, int IW, std::string* err) {
+  plan_.reset();   // its graphs point into the workspace arena, which pass 0 may reallocate; a failed plan leaves none
   const int C = cfg_.vit_dim, d = cfg_.hidden_dim, nq = cfg_.num_queries, ncls = cfg_.num_classes;
   const int GH = IH / 16, GW = IW / 16, T = GH * GW, ntap = cfg_.n_taps, c2 = d / 2, heads = cfg_.vit_heads;
   const int M = cfg_.ca_heads, L = cfg_.n_levels, P = cfg_.dec_points, ff = cfg_.dim_feedforward, NL = cfg_.dec_layers;
@@ -497,7 +585,6 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
   }
   const long long BS = 1LL * B * S, BQ = 1LL * B * nq;
   const int ldc = static_cast<int>(align_up(static_cast<size_t>(ncls), 32));   // row pitch of the fp32 class-logit buffers
-  ldc_ = ldc;
   if (d / M != 16) { *err = "deformable attention head dim must be 16"; return -1; }
   if (C / heads != 16 && C / heads != 32 && C / heads != 64) { *err = "unsupported ViT head dim"; return -1; }
   if (S < nq) {
@@ -518,110 +605,28 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
     }
     pos_host = to16(window_major_pos(pe.data(), C, GH, GW));
   }
+  const std::string too_big = "lwdetr_forward: batch " + std::to_string(B) + " at " + std::to_string(IH) + "x" + std::to_string(IW) +
+                              " needs a workspace buffer of more than 2^31-1 elements";
+  auto p = std::make_unique<Plan>();
+  // GEMM epilogues of the call sites below
+  auto act = [](int a) { GemmDesc g; g.act = a; return g; };
+  auto resid = [](Mat r) { GemmDesc g; g.resid = r.p; g.ld_resid = r.ld; return g; };
+  GemmDesc f32; f32.out_fp32 = 1;
+  auto col = [](Mat m, int c) { return Mat{cptr(m.p) + static_cast<size_t>(c) * 2, m.ld}; };
+  const int dt = dtype_;
 
   for (int pass = 0; pass < 2; ++pass) {   // pass 0 sizes the workspace, pass 1 builds the ops
-    soff_ = 0;
-    ops_.clear();
-    bool fail = false;
-    // every kernel indexes a buffer's elements / a GEMM's rows with 32-bit integers somewhere: no buffer may exceed that range
-    auto fits = [&](long long n) {
-      if (n > 2147483647LL && !fail) { fail = true; *err = "lwdetr_forward: batch " + std::to_string(B) + " at " + std::to_string(IH) + "x" + std::to_string(IW) + " needs a workspace buffer of more than 2^31-1 elements"; }
-      return n <= 2147483647LL;
-    };
-    auto buf16 = [&](long long rows, int cols) { fits(rows * cols); return Mat{salloc(static_cast<size_t>(rows) * cols * 2), cols}; };
-    auto buf32 = [&](long long n) { fits(n); return static_cast<float*>(salloc(static_cast<size_t>(n) * 4)); };
-    auto col = [&](Mat m, int c) { return Mat{cptr(m.p) + static_cast<size_t>(c) * 2, m.ld}; };
-    auto w16 = [&](const std::string& k) -> void* { auto it = W_.find(k); if (it == W_.end()) { fail = true; *err = "internal: weight " + k; return nullptr; } return it->second; };
-    auto w32 = [&](const std::string& k) -> float* { auto it = F_.find(k); if (it == F_.end()) { fail = true; *err = "internal: vector " + k; return nullptr; } return it->second; };
-
-    struct GemmOpt {
-      const float* gamma = nullptr; Mat resid{nullptr, 0}; int resid_mod = 0; int act = ACT_NONE; int out_fp32 = 0;
-      int rows_in = ROWS_PLAIN, remap = 0, shuffle = 0, IH = 0, IW = 0;
-      int conv = 0, cB = 0, cOH = 0, cOW = 0;   // conv: 1 = 3x3 s1, 2 = 3x3 s2
-      int hm_S = 0, hm_heads = 0, hm_slices = 0; const uint8_t* row_zero = nullptr;
-      float2* stats_out = nullptr; const float2* stats_in = nullptr; int ln_C = 0; float ln_eps = 0.f;
-    };
-    int stats_parts = 0;   // partial (sum, sumsq) pairs per row written by the N = C producer GEMMs
-    auto add_gemm = [&](const std::string& label, Mat A, long long Mrows, int K, const std::string& wkey, int N, void* out, int ld_out,
-                        const GemmOpt& o, long long out_rows = -1) {
-      if (!fits(Mrows) || pass == 0) return;
-      GemmDesc g;
-      g.dtype = dtype_; g.A = A.p; g.lda = A.ld; g.M = static_cast<int>(Mrows); g.N = N; g.K = K;
-      g.W = w16(wkey + ".w"); g.bias = F_.count(wkey + ".b") ? F_[wkey + ".b"] : nullptr;
-      g.gamma = o.gamma; g.resid = o.resid.p; g.ld_resid = o.resid.ld; g.resid_mod = o.resid_mod; g.act = o.act;
-      g.out = out; g.ld_out = ld_out; g.out_fp32 = o.out_fp32; g.rows_in = o.rows_in; g.remap_rows = o.remap;
-      g.shuffle_cout = o.shuffle; g.IH = o.IH; g.IW = o.IW;
-      g.hm_S = o.hm_S; g.hm_heads = o.hm_heads; g.hm_slices = o.hm_slices; g.row_zero = o.row_zero;
-      if (o.conv) { g.a_mode = o.conv == 1 ? AMODE_CONV3_S1 : AMODE_CONV3_S2; g.B = o.cB; g.OH = o.cOH; g.OW = o.cOW; }
-      g.stats_out = o.stats_out; g.stats_in = o.stats_in; g.stats_parts_in = stats_parts; g.ln_C = o.ln_C; g.ln_eps = o.ln_eps;
-      if (o.stats_in) g.colsum = w32(wkey + ".cs");
-      GemmOp op;
-      std::string e;
-      if (fail || gemm_build(g, &op, &e)) { if (!fail) *err = label + ": " + e; fail = true; return; }
-      if (o.stats_out) {
-        if (stats_parts == 0) stats_parts = op.args.stats_parts_out;
-        if (stats_parts != op.args.stats_parts_out || stats_parts > 48) { *err = label + ": inconsistent LayerNorm partial count"; fail = true; return; }
-      }
-      Op P_;
-      P_.label = label;
-      P_.run = [op](cudaStream_t st) { return gemm_launch(op, st); };
-      P_.out = out; P_.rows = out_rows >= 0 ? out_rows : (o.shuffle ? Mrows * 4 : Mrows); P_.cols = o.shuffle ? o.shuffle : (o.hm_S ? 16 : N);
-      P_.ld = ld_out; P_.fp32 = o.out_fp32;
-      P_.flops = op.flops;
-      P_.bytes = 2.0 * (static_cast<double>(Mrows) * K + static_cast<double>(N) * K) + (o.out_fp32 ? 4.0 : 2.0) * Mrows * N + (o.resid.p ? 2.0 * Mrows * N : 0.0);
-      ops_.push_back(P_);
-    };
-    auto add_ln = [&](const std::string& label, Mat x, Mat y, const std::string& nkey, float eps, long long rows, int Cn,
-                      const uint8_t* flag = nullptr, int flag_mod = 0, const float* ovr = nullptr, Mat add = Mat{nullptr, 0},
-                      Mat y2 = Mat{nullptr, 0}, long long ygroup = 0, long long ystride = 0, long long yoff = 0, long long out_rows = -1,
-                      const std::string& nkey3 = std::string(), Mat y3 = Mat{nullptr, 0}, float eps3 = 0.f) {
-      if (pass == 0) return;
-      LayerNormArgs a;
-      std::memset(&a, 0, sizeof a);
-      if (y3.p) { a.w3 = w32(nkey3 + ".w"); a.b3 = w32(nkey3 + ".b"); a.eps3 = eps3; a.y3 = y3.p; a.ldy3 = y3.ld; }
-      a.x = x.p; a.ldx = x.ld; a.y = y.p; a.ldy = y.ld; a.w = w32(nkey + ".w"); a.b = w32(nkey + ".b"); a.eps = eps;
-      a.rows = rows; a.C = Cn; a.row_flag = flag; a.flag_mod = flag_mod > 0 ? flag_mod : 1; a.override_vec = ovr;
-      a.add_src = add.p; a.ld_add = add.ld; a.y2 = y2.p; a.ldy2 = y2.ld; a.y_group = ygroup; a.y_group_stride = ystride; a.y_row_off = yoff;
-      const int dt = dtype_;
-      Op P_;
-      P_.label = label;
-      P_.run = [a, dt](cudaStream_t st) { return layernorm_launch(dt, a, st); };
-      P_.out = y.p; P_.rows = out_rows >= 0 ? out_rows : rows; P_.cols = Cn; P_.ld = y.ld;
-      P_.bytes = 4.0 * rows * Cn + (y2.p ? 4.0 * rows * Cn : 0.0) + (y3.p ? 2.0 * rows * Cn : 0.0);
-      ops_.push_back(P_);
-    };
-    auto add_attn = [&](const std::string& label, Mat q, Mat k, Mat v, Mat o, int nseq, int seqlen, int nheads, int dh) {
-      if (pass == 0) return;
-      AttnArgs a;
-      a.q = q.p; a.k = k.p; a.v = v.p; a.ldq = q.ld; a.ldk = k.ld; a.ldv = v.ld; a.o = o.p; a.ldo = o.ld;
-      a.seqlen = seqlen; a.nseq = nseq; a.heads = nheads;
-      a.scale_log2 = 1.4426950408889634f / std::sqrt(static_cast<float>(dh));
-      const int dt = dtype_;
-      Op P_;
-      P_.label = label;
-      P_.run = [a, dt, dh](cudaStream_t st) { return attention_launch(dt, a, dh, st); };
-      P_.out = o.p; P_.rows = 1LL * nseq * seqlen; P_.cols = nheads * dh; P_.ld = o.ld;
-      P_.flops = 4.0 * nseq * static_cast<double>(seqlen) * seqlen * nheads * dh;
-      P_.bytes = 2.0 * 4.0 * nseq * seqlen * nheads * dh;
-      ops_.push_back(P_);
-    };
-    auto add_op = [&](const std::string& label, std::function<int(cudaStream_t)> fn, const void* out, long long rows, int cols, int ld, int fp32, double bytes) {
-      if (pass == 0) return;
-      Op P_;
-      P_.label = label; P_.run = std::move(fn); P_.out = out; P_.rows = rows; P_.cols = cols; P_.ld = ld; P_.fp32 = fp32; P_.bytes = bytes;
-      ops_.push_back(P_);
-    };
-    const int dt = dtype_;
+    OpBuilder b(pass, dtype_, sarena_.p, W_, F_, too_big, err, &p->ops);
 
     // ================================================================ padding-mask tables (constants when the batch is unpadded)
-    float* prop_b = buf32(BS * 4);
-    float* vr_b = buf32(static_cast<long long>(B) * L * 2 + 4);
-    uint8_t* invalid_b = static_cast<uint8_t*>(salloc(static_cast<size_t>(BS)));
-    uint8_t* pad_b = static_cast<uint8_t*>(salloc(static_cast<size_t>(BS)));
-    uint8_t* fmask_b = static_cast<uint8_t*>(salloc(static_cast<size_t>(B) * IH * IW));   // padding mask of a batch of raw frames
+    float* prop_b = b.buf32(BS * 4);
+    float* vr_b = b.buf32(static_cast<long long>(B) * L * 2 + 4);
+    uint8_t* invalid_b = static_cast<uint8_t*>(b.alloc(static_cast<size_t>(BS)));
+    uint8_t* pad_b = static_cast<uint8_t*>(b.alloc(static_cast<size_t>(BS)));
+    uint8_t* fmask_b = static_cast<uint8_t*>(b.alloc(static_cast<size_t>(B) * IH * IW));   // padding mask of a batch of raw frames
     {
       const int lh0 = lvl_h[0], lh1 = lvl_h[1], lw0 = lvl_w[0], lw1 = lvl_w[1], ls0 = lvl_start[0], ls1 = lvl_start[1];
-      add_op("mask_setup", [this, B, IH, IW, L, S, lh0, lh1, lw0, lw1, ls0, ls1, prop_b, invalid_b, pad_b, vr_b, fmask_b](cudaStream_t st) {
+      b.op("mask_setup", [this, B, IH, IW, L, S, lh0, lh1, lw0, lw1, ls0, ls1, prop_b, invalid_b, pad_b, vr_b, fmask_b](cudaStream_t st) {
         const int lh[2] = {lh0, lh1}, lw[2] = {lw0, lw1}, ls[2] = {ls0, ls1};
         const uint8_t* mask = in_.mask;
         if (in_.kind == IN_FRAMES || in_.kind == IN_FRAMES_NV12) {   // raw frames: the mask follows from their dst sizes, made on the device
@@ -633,122 +638,77 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
           }
         }
         return mask_setup_launch(mask, B, IH, IW, L, S, lh, lw, ls, prop_b, invalid_b, pad_b, vr_b, st);
-      }, prop_b, BS, 4, 4, 1, 24.0 * BS);
-      if (pass) ops_.back().reads_input = true;
+      }, {prop_b, BS, 4, 4, 1}, 24.0 * BS, /*reads_input=*/true);
     }
     // ================================================================ ViT encoder
-    Mat a0 = buf16(BT, 768);
-    Mat xa = buf16(BT, C), xb = buf16(BT, C), xm = buf16(BT, C), lnb = buf16(BT, C);
-    Mat tapbuf = buf16(BT, ntap * C);
+    Mat a0 = b.buf16(BT, 768);
+    Mat xa = b.buf16(BT, C), xb = b.buf16(BT, C), xm = b.buf16(BT, C), lnb = b.buf16(BT, C);
+    Mat tapbuf = b.buf16(BT, ntap * C);
     // the 192-wide encoder (tiny, small) runs each block's LN2 -> fc1 -> GELU -> fc2 as one kernel (mlp.cu): no hidden buffer.
     // Only when its 128-row tiles cover every SM: below that (batch 1 - 10 at 640x640) the two GEMMs, whose narrower n-tiles
     // spread the work over more SMs, are faster.  Both paths give the same bits.
     const bool fused_mlp = fuse_ln_ != 0 && !e4m3_ && C == MLP_C && (BT + 127) / 128 >= current_device_sms();
-    Mat qkv = buf16(BT, 3 * C), att = buf16(BT, C), hid = fused_mlp ? Mat{nullptr, 4 * C} : buf16(BT, 4 * C);
+    Mat qkv = b.buf16(BT, 3 * C), att = b.buf16(BT, C), hid = fused_mlp ? Mat{nullptr, 4 * C} : b.buf16(BT, 4 * C);
     {
       void* a0p = a0.p;
-      add_op("patch_gather", [this, a0p, B, IH, IW, dt](cudaStream_t st) {
-               if (in_.kind == IN_FRAMES) return resize_patches_launch(dt, in_.frames, B, IH, IW, in_.mean, in_.stdv, a0p, st);
-               if (in_.kind == IN_FRAMES_NV12) return resize_patches_launch(dt, in_.frames_nv12, B, IH, IW, in_.mean, in_.stdv, a0p, st);
-               if (in_.kind == IN_U8_NHWC) return patch_gather_u8_launch(dt, in_.images, in_.mean, in_.stdv, a0p, B, IH, IW, st);
-               return patch_gather_launch(dt, in_.images, in_.kind == IN_F32_NCHW ? 1 : 0, a0p, B, IH, IW, st);
-             },
-             a0.p, BT, 768, 768, 0, 1.0 * B * 3 * IH * IW * 4 + 2.0 * BT * 768);
-      if (pass) ops_.back().reads_input = true;
+      b.op("patch_gather", [this, a0p, B, IH, IW, dt](cudaStream_t st) {
+             if (in_.kind == IN_FRAMES) return resize_patches_launch(dt, in_.frames, B, IH, IW, in_.mean, in_.stdv, a0p, st);
+             if (in_.kind == IN_FRAMES_NV12) return resize_patches_launch(dt, in_.frames_nv12, B, IH, IW, in_.mean, in_.stdv, a0p, st);
+             if (in_.kind == IN_U8_NHWC) return patch_gather_u8_launch(dt, in_.images, in_.mean, in_.stdv, a0p, B, IH, IW, st);
+             return patch_gather_launch(dt, in_.images, in_.kind == IN_F32_NCHW ? 1 : 0, a0p, B, IH, IW, st);
+           },
+           {a0.p, BT, 768, 768, 0}, 1.0 * B * 3 * IH * IW * 4 + 2.0 * BT * 768, /*reads_input=*/true);
     }
-    float2* stats_x = static_cast<float2*>(salloc(static_cast<size_t>(BT) * 48 * sizeof(float2)));   // row stats of x (block input)
-    float2* stats_m = static_cast<float2*>(salloc(static_cast<size_t>(BT) * 48 * sizeof(float2)));   // row stats of x + attn
+    float2* stats_x = static_cast<float2*>(b.alloc(static_cast<size_t>(BT) * 48 * sizeof(float2)));   // row stats of x (block input)
+    float2* stats_m = static_cast<float2*>(b.alloc(static_cast<size_t>(BT) * 48 * sizeof(float2)));   // row stats of x + attn
     const bool fuse = fuse_ln_ != 0 && !e4m3_;   // the e4m3 mode has its own LayerNorm -> e4m3 pass in front of qkv / fc1
     // e4m3 mode: the LayerNorm output as e4m3 codes + per-row scales, shared by qkv and fc1
-    uint8_t* lnq = e4m3_ ? static_cast<uint8_t*>(salloc(static_cast<size_t>(BT) * C)) : nullptr;
-    float* lns = e4m3_ ? buf32(BT) : nullptr;
-    auto add_ln_e4m3 = [&](const std::string& label, Mat x) {
-      if (pass == 0) return;
+    uint8_t* lnq = e4m3_ ? static_cast<uint8_t*>(b.alloc(static_cast<size_t>(BT) * C)) : nullptr;
+    float* lns = e4m3_ ? b.buf32(BT) : nullptr;
+    auto ln_e4m3 = [&](const std::string& label, Mat x) {   // a capture returns the row scales
       const void* xp = x.p; const int ldx = x.ld;
-      Op P_;
-      P_.label = label;
-      P_.run = [xp, ldx, BT, C, lnq, lns](cudaStream_t st) { return layernorm_e4m3_launch(xp, ldx, BT, C, 1e-6f, lnq, C, lns, st); };
-      P_.out = lns; P_.rows = BT; P_.cols = 1; P_.ld = 1; P_.fp32 = 1;   // a capture returns the row scales
-      P_.bytes = 2.0 * BT * C + 1.0 * BT * C + 4.0 * BT;
-      ops_.push_back(P_);
+      b.op(label, [xp, ldx, BT, C, lnq, lns](cudaStream_t st) { return layernorm_e4m3_launch(xp, ldx, BT, C, 1e-6f, lnq, C, lns, st); },
+           {lns, BT, 1, 1, 1}, 2.0 * BT * C + 1.0 * BT * C + 4.0 * BT);
     };
-    auto add_gemm_e4m3 = [&](const std::string& label, const std::string& wkey, int N, int act, Mat out) {
-      if (pass == 0) return;
-      GemmE4m3Desc g;
-      g.A = lnq; g.lda = C; g.a_scale = lns; g.M = static_cast<int>(BT); g.K = C; g.N = N;
-      g.W = w16(wkey + ".w"); g.w_scale = w32(wkey + ".s"); g.bias = w32(wkey + ".b"); g.act = act; g.out = out.p; g.ld_out = out.ld;
-      GemmOp op;
-      std::string e;
-      if (fail || gemm_e4m3_build(g, &op, &e)) { if (!fail) *err = label + ": " + e; fail = true; return; }
-      Op P_;
-      P_.label = label;
-      P_.run = [op](cudaStream_t st) { return gemm_launch(op, st); };
-      P_.out = out.p; P_.rows = BT; P_.cols = N; P_.ld = out.ld;
-      P_.flops = op.flops;
-      P_.bytes = 1.0 * (static_cast<double>(BT) * C + static_cast<double>(N) * C) + 4.0 * BT + 8.0 * N + 2.0 * BT * N;   // 1-byte operands
-      ops_.push_back(P_);
-    };
-    // fused MLP (vit_mlp_kernel): LN2 statistics from stats_m, folded fc1, GELU, fc2, layer-scale and residual; writes the next
-    // block's LayerNorm partials in the layout the fc2 GEMM would have used (stats_parts per row)
-    auto add_mlp = [&](const std::string& label, Mat x, const std::string& k, float2* st_out, Mat out) {
-      if (pass == 0) return;
-      MlpDesc g;
-      g.dtype = dtype_; g.x = x.p; g.ldx = x.ld; g.M = static_cast<int>(BT);
-      g.stats_in = stats_m; g.stats_parts_in = stats_parts; g.ln_eps = 1e-6f;
-      g.w1 = w16(k + "fc1_ln.w"); g.colsum1 = w32(k + "fc1_ln.cs"); g.b1 = w32(k + "fc1_ln.b");
-      g.w2 = w16(k + "fc2.w"); g.b2 = w32(k + "fc2.b"); g.gamma = w32(k + "g2");
-      g.out = out.p; g.ld_out = out.ld; g.stats_out = st_out; g.stats_parts_out = stats_parts;
-      MlpOp op;
-      std::string e;
-      if (fail || vit_mlp_build(g, &op, &e)) { if (!fail) *err = label + ": " + e; fail = true; return; }
-      Op P_;
-      P_.label = label;
-      P_.run = [op](cudaStream_t st) { return vit_mlp_launch(op, st); };
-      P_.out = out.p; P_.rows = BT; P_.cols = C; P_.ld = out.ld;
-      P_.flops = op.flops;
-      P_.bytes = 2.0 * 3.0 * BT * C + 2.0 * 2.0 * (4.0 * C) * C;   // x (operand and residual), out, both weights
-      ops_.push_back(P_);
-    };
+    // LayerNorm consumers: the GEMM normalises its raw input rows with the statistics the producers wrote
+    auto ln_fold = [&](const float2* stats, int a) { GemmDesc g = act(a); g.stats_in = stats; g.ln_C = C; g.ln_eps = 1e-6f; return g; };
     Mat xcur = xa;
-    void* pos_tab = own_pos ? salloc(pos_host.size() * 2) : nullptr;
+    void* pos_tab = own_pos ? b.alloc(pos_host.size() * 2) : nullptr;
     if (own_pos && pass == 1 && cudaMemcpy(pos_tab, pos_host.data(), pos_host.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) {
       *err = "lwdetr_forward: position table upload failed";
       return -1;
     }
     {
-      GemmOpt o; o.resid = Mat{pass ? (own_pos ? pos_tab : w16("pos")) : nullptr, C}; o.resid_mod = T;
-      if (fuse) o.stats_out = stats_x;
-      add_gemm("patch_embed", a0, BT, 768, "patch", C, xcur.p, xcur.ld, o);
+      GemmDesc g = resid(Mat{own_pos ? pos_tab : b.w16("pos"), C}); g.resid_mod = T; if (fuse) g.stats_out = stats_x;
+      b.gemm("patch_embed", g, a0, BT, 768, "patch", C, xcur);
     }
     int tap_slot = 0;
     for (int i = 0; i < cfg_.vit_depth; ++i) {
       const std::string k = "blk" + std::to_string(i) + ".", lb = "block" + std::to_string(i);
       const bool window = (cfg_.window_block_mask >> i) & 1;
       if (e4m3_) {
-        add_ln_e4m3(lb + ".ln1", xcur);
-        add_gemm_e4m3(lb + ".qkv", k + "qkv_q", 3 * C, ACT_NONE, qkv);
+        ln_e4m3(lb + ".ln1", xcur);
+        b.gemm_e4m3(lb + ".qkv", lnq, lns, BT, C, k + "qkv_q", 3 * C, ACT_NONE, qkv);
       } else if (fuse) {
-        GemmOpt o; o.stats_in = stats_x; o.ln_C = C; o.ln_eps = 1e-6f;
-        add_gemm(lb + ".qkv", xcur, BT, C, k + "qkv_ln", 3 * C, qkv.p, qkv.ld, o);
+        b.gemm(lb + ".qkv", ln_fold(stats_x, ACT_NONE), xcur, BT, C, k + "qkv_ln", 3 * C, qkv);
       } else {
-        add_ln(lb + ".ln1", xcur, lnb, k + "ln1", 1e-6f, BT, C);
-        add_gemm(lb + ".qkv", lnb, BT, C, k + "qkv", 3 * C, qkv.p, qkv.ld, GemmOpt{});
+        b.layernorm(lb + ".ln1", xcur, lnb, k + "ln1", 1e-6f, BT, C);
+        b.gemm(lb + ".qkv", GemmDesc{}, lnb, BT, C, k + "qkv", 3 * C, qkv);
       }
-      add_attn(lb + (window ? ".win_attn" : ".glb_attn"), col(qkv, 0), col(qkv, C), col(qkv, 2 * C), att,
-               window ? 16 * B : B, window ? T / 16 : T, heads, C / heads);
-      { GemmOpt o; o.gamma = pass ? w32(k + "g1") : nullptr; o.resid = xcur; if (fuse) o.stats_out = stats_m;
-        add_gemm(lb + ".proj", att, BT, C, k + "proj", C, xm.p, xm.ld, o); }
+      b.attention(lb + (window ? ".win_attn" : ".glb_attn"), col(qkv, 0), col(qkv, C), col(qkv, 2 * C), att,
+                  window ? 16 * B : B, window ? T / 16 : T, heads, C / heads);
+      { GemmDesc g = resid(xcur); g.gamma = b.w32(k + "g1"); if (fuse) g.stats_out = stats_m;
+        b.gemm(lb + ".proj", g, att, BT, C, k + "proj", C, xm); }
       if (fused_mlp) {
         // fc1 + fc2 in one op under the fc2 label (block taps and captures stay where they were)
       } else if (e4m3_) {
-        add_ln_e4m3(lb + ".ln2", xm);
-        add_gemm_e4m3(lb + ".fc1", k + "fc1_q", 4 * C, ACT_GELU, hid);
+        ln_e4m3(lb + ".ln2", xm);
+        b.gemm_e4m3(lb + ".fc1", lnq, lns, BT, C, k + "fc1_q", 4 * C, ACT_GELU, hid);
       } else if (fuse) {
-        GemmOpt o; o.act = ACT_GELU; o.stats_in = stats_m; o.ln_C = C; o.ln_eps = 1e-6f;
-        add_gemm(lb + ".fc1", xm, BT, C, k + "fc1_ln", 4 * C, hid.p, hid.ld, o);
+        b.gemm(lb + ".fc1", ln_fold(stats_m, ACT_GELU), xm, BT, C, k + "fc1_ln", 4 * C, hid);
       } else {
-        add_ln(lb + ".ln2", xm, lnb, k + "ln2", 1e-6f, BT, C);
-        GemmOpt o; o.act = ACT_GELU; add_gemm(lb + ".fc1", lnb, BT, C, k + "fc1", 4 * C, hid.p, hid.ld, o);
+        b.layernorm(lb + ".ln2", xm, lnb, k + "ln2", 1e-6f, BT, C);
+        b.gemm(lb + ".fc1", act(ACT_GELU), lnb, BT, C, k + "fc1", 4 * C, hid);
       }
       Mat xnext;
       bool is_tap = false;
@@ -756,117 +716,116 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
       if (is_tap) xnext = col(tapbuf, (tap_slot++) * C);
       else xnext = (xcur.p == xa.p) ? xb : xa;
       if (fused_mlp) {
-        add_mlp(lb, xm, k, i + 1 < cfg_.vit_depth ? stats_x : nullptr, xnext);
+        b.mlp(lb, xm, BT, stats_m, k, i + 1 < cfg_.vit_depth ? stats_x : nullptr, xnext);
       } else {
-        GemmOpt o; o.gamma = pass ? w32(k + "g2") : nullptr; o.resid = xm; if (fuse && i + 1 < cfg_.vit_depth) o.stats_out = stats_x;
-        add_gemm(lb, hid, BT, 4 * C, k + "fc2", C, xnext.p, xnext.ld, o);
+        GemmDesc g = resid(xm); g.gamma = b.w32(k + "g2"); if (fuse && i + 1 < cfg_.vit_depth) g.stats_out = stats_x;
+        b.gemm(lb, g, hid, BT, 4 * C, k + "fc2", C, xnext);
       }
       xcur = xnext;
     }
 
     // ================================================================ projector -> decoder memory [B, S, d]
-    Mat memory = buf16(BS, d);
+    Mat memory = b.buf16(BS, d);
     for (int l = 0; l < L; ++l) {
       const int sc = cfg_.level_scale_log2[l], H = lvl_h[l], W = lvl_w[l];
       const long long rows = 1LL * B * H * W;
       const std::string k = "lvl" + std::to_string(l) + ".", lb = "level" + std::to_string(l);
-      Mat c2f = buf16(rows, 5 * c2), tmp = buf16(rows, c2), pout = buf16(rows, d);
+      auto conv3 = [&](int a_mode, int a) { GemmDesc g = act(a); g.a_mode = a_mode; g.B = B; g.OH = H; g.OW = W; return g; };
+      Mat c2f = b.buf16(rows, 5 * c2), tmp = b.buf16(rows, c2), pout = b.buf16(rows, d);
       if (sc == 0) {
-        GemmOpt o; o.act = ACT_SILU; o.rows_in = ROWS_WINDOW_MAJOR; o.remap = 1; o.IH = GH; o.IW = GW;
-        add_gemm(lb + ".cv1", tapbuf, BT, ntap * C, k + "cv1", 2 * c2, c2f.p, c2f.ld, o);
+        GemmDesc g = act(ACT_SILU); g.rows_in = ROWS_WINDOW_MAJOR; g.remap_rows = 1; g.IH = GH; g.IW = GW;
+        b.gemm(lb + ".cv1", g, tapbuf, BT, ntap * C, k + "cv1", 2 * c2, c2f);
       } else if (sc == 1) {
         const int cs = C > 512 ? C / 4 : C / 2;
-        Mat samp = buf16(rows, ntap * cs);
-        Mat pre = C > 512 ? buf16(BT, C / 2) : Mat{nullptr, 0};
+        Mat samp = b.buf16(rows, ntap * cs);
+        Mat pre = C > 512 ? b.buf16(BT, C / 2) : Mat{nullptr, 0};
         for (int t = 0; t < ntap; ++t) {
           const std::string ks = k + "samp" + std::to_string(t);
           Mat src = col(tapbuf, t * C);
           int kin = C;
           if (C > 512) {
-            GemmOpt o; o.act = ACT_RELU;
-            add_gemm(lb + ".pre" + std::to_string(t), src, BT, C, ks + ".pre", C / 2, pre.p, pre.ld, o);
+            b.gemm(lb + ".pre" + std::to_string(t), act(ACT_RELU), src, BT, C, ks + ".pre", C / 2, pre);
             src = pre; kin = C / 2;
           }
-          GemmOpt o; o.rows_in = ROWS_WINDOW_MAJOR; o.shuffle = cs; o.IH = GH; o.IW = GW;
-          Mat dst = col(samp, t * cs);
-          add_gemm(lb + ".up" + std::to_string(t), src, BT, kin, ks + ".up", 4 * cs, dst.p, dst.ld, o);
+          GemmDesc g; g.rows_in = ROWS_WINDOW_MAJOR; g.shuffle_cout = cs; g.IH = GH; g.IW = GW;
+          b.gemm(lb + ".up" + std::to_string(t), g, src, BT, kin, ks + ".up", 4 * cs, col(samp, t * cs));
         }
-        GemmOpt o; o.act = ACT_SILU;
-        add_gemm(lb + ".cv1", samp, rows, ntap * cs, k + "cv1", 2 * c2, c2f.p, c2f.ld, o);
+        b.gemm(lb + ".cv1", act(ACT_SILU), samp, rows, ntap * cs, k + "cv1", 2 * c2, c2f);
       } else {
-        Mat spat = buf16(BT, ntap * C), samp = buf16(rows, ntap * C);
+        Mat spat = b.buf16(BT, ntap * C), samp = b.buf16(rows, ntap * C);
         {
           void* sp = tapbuf.p; void* dp = spat.p; const int ldx = ntap * C;
-          add_op(lb + ".unwindow", [sp, dp, ldx, BT, GH, GW, dt](cudaStream_t st) { return unwindow_launch(dt, sp, ldx, dp, ldx, BT, ldx, GH, GW, st); },
-                 spat.p, BT, ldx, ldx, 0, 4.0 * BT * ldx);
+          b.op(lb + ".unwindow", [sp, dp, ldx, BT, GH, GW, dt](cudaStream_t st) { return unwindow_launch(dt, sp, ldx, dp, ldx, BT, ldx, GH, GW, st); },
+               {spat.p, BT, ldx, ldx, 0}, 4.0 * BT * ldx);
         }
-        for (int t = 0; t < ntap; ++t) {
-          GemmOpt o; o.act = ACT_RELU; o.conv = 2; o.cB = B; o.cOH = H; o.cOW = W;
-          Mat src = col(spat, t * C), dst = col(samp, t * C);
-          add_gemm(lb + ".down" + std::to_string(t), src, rows, 9 * C, k + "samp" + std::to_string(t) + ".down", C, dst.p, dst.ld, o);
-        }
-        GemmOpt o; o.act = ACT_SILU;
-        add_gemm(lb + ".cv1", samp, rows, ntap * C, k + "cv1", 2 * c2, c2f.p, c2f.ld, o);
+        for (int t = 0; t < ntap; ++t)
+          b.gemm(lb + ".down" + std::to_string(t), conv3(AMODE_CONV3_S2, ACT_RELU), col(spat, t * C), rows, 9 * C,
+                 k + "samp" + std::to_string(t) + ".down", C, col(samp, t * C));
+        b.gemm(lb + ".cv1", act(ACT_SILU), samp, rows, ntap * C, k + "cv1", 2 * c2, c2f);
       }
       for (int j = 0; j < 3; ++j) {
-        GemmOpt o; o.act = ACT_SILU; o.conv = 1; o.cB = B; o.cOH = H; o.cOW = W;
-        Mat src = col(c2f, (1 + j) * c2), dst = col(c2f, (2 + j) * c2);
-        add_gemm(lb + ".m" + std::to_string(j) + "a", src, rows, 9 * c2, k + "m" + std::to_string(j) + "a", c2, tmp.p, tmp.ld, o);
-        add_gemm(lb + ".m" + std::to_string(j) + "b", tmp, rows, 9 * c2, k + "m" + std::to_string(j) + "b", c2, dst.p, dst.ld, o);
+        const std::string m = "m" + std::to_string(j);
+        b.gemm(lb + "." + m + "a", conv3(AMODE_CONV3_S1, ACT_SILU), col(c2f, (1 + j) * c2), rows, 9 * c2, k + m + "a", c2, tmp);
+        b.gemm(lb + "." + m + "b", conv3(AMODE_CONV3_S1, ACT_SILU), tmp, rows, 9 * c2, k + m + "b", c2, col(c2f, (2 + j) * c2));
       }
-      { GemmOpt o; o.act = ACT_SILU; add_gemm(lb + ".cv2", c2f, rows, 5 * c2, k + "cv2", d, pout.p, pout.ld, o); }
-      add_ln(lb, pout, memory, k + "ln", 1e-6f, rows, d, nullptr, 0, nullptr, Mat{nullptr, 0}, Mat{nullptr, 0}, 1LL * H * W, S, lvl_start[l], BS);
+      b.gemm(lb + ".cv2", act(ACT_SILU), c2f, rows, 5 * c2, k + "cv2", d, pout);
+      LayerNormArgs a{}; a.y_group = 1LL * H * W; a.y_group_stride = S; a.y_row_off = lvl_start[l];   // rows of the memory of each image
+      b.layernorm(lb, pout, memory, k + "ln", 1e-6f, rows, d, a);
     }
 
     // ================================================================ two-stage query selection
     // value_proj of all decoder layers, HEAD-MAJOR [B][layer][head][S][16] (msda.cu stages whole (image, head) slabs)
-    Mat value = buf16(BS, NL * d), om = buf16(BS, d), omn = buf16(BS, d);
-    float* cls_all = buf32(BS * ldc);
-    float* score = buf32(BS);
-    int* topk_idx = static_cast<int*>(salloc(static_cast<size_t>(BQ) * 4));
-    Mat sel = buf16(BQ, d), h1 = buf16(BQ, d), h2 = buf16(BQ, d);
-    float* delta_ts = buf32(BQ * 4);
-    float* enc_logits = buf32(BQ * ncls);
-    float* enc_boxes = buf32(BQ * 4);
-    float* refpoint = buf32(BQ * 4);
-    Mat sine = buf16(BQ, 2 * d), qpos = buf16(BQ, d);
-    { GemmOpt o; o.hm_S = S; o.hm_heads = M; o.hm_slices = NL; o.row_zero = pad_b; add_gemm("value_proj", memory, BS, d, "value", NL * d, value.p, 16, o, BS * NL * M); }
-    add_gemm("enc_output", memory, BS, d, "enc_out", d, om.p, om.ld, GemmOpt{});
-    add_ln("enc_output_norm", om, omn, "enc_ln", 1e-5f, BS, d, invalid_b, static_cast<int>(BS), pass ? w32("enc_out.b") : nullptr);
-    { GemmOpt o; o.out_fp32 = 1; add_gemm("enc_class", omn, BS, d, "enc_cls", ncls, cls_all, ldc, o); }
-    add_op("enc_score", [cls_all, ncls, ldc, score, BS](cudaStream_t st) { return rowmax_launch(cls_all, ldc, ncls, score, BS, st); }, score, BS, 1, 1, 1, 4.0 * BS * ncls);
-    add_op("topk", [this, score, B, S, nq, topk_idx](cudaStream_t st) {
+    Mat value = b.buf16(BS, NL * d), om = b.buf16(BS, d), omn = b.buf16(BS, d);
+    float* cls_all = b.buf32(BS * ldc);
+    float* score = b.buf32(BS);
+    int* topk_idx = static_cast<int*>(b.alloc(static_cast<size_t>(BQ) * 4));
+    Mat sel = b.buf16(BQ, d), h1 = b.buf16(BQ, d), h2 = b.buf16(BQ, d);
+    float* delta_ts = b.buf32(BQ * 4);
+    float* enc_logits = b.buf32(BQ * ncls);
+    float* enc_boxes = b.buf32(BQ * 4);
+    float* refpoint = b.buf32(BQ * 4);
+    Mat sine = b.buf16(BQ, 2 * d), qpos = b.buf16(BQ, d);
+    { GemmDesc g; g.hm_S = S; g.hm_heads = M; g.hm_slices = NL; g.row_zero = pad_b; b.gemm("value_proj", g, memory, BS, d, "value", NL * d, Mat{value.p, 16}); }
+    b.gemm("enc_output", GemmDesc{}, memory, BS, d, "enc_out", d, om);
+    { LayerNormArgs a{}; a.row_flag = invalid_b; a.flag_mod = static_cast<int>(BS); a.override_vec = b.w32("enc_out.b");
+      b.layernorm("enc_output_norm", om, omn, "enc_ln", 1e-5f, BS, d, a); }
+    b.gemm("enc_class", f32, omn, BS, d, "enc_cls", ncls, Mat{cls_all, ldc});
+    b.op("enc_score", [cls_all, ncls, ldc, score, BS](cudaStream_t st) { return rowmax_launch(cls_all, ldc, ncls, score, BS, st); },
+         {score, BS, 1, 1, 1}, 4.0 * BS * ncls);
+    b.op("topk", [this, score, B, S, nq, topk_idx](cudaStream_t st) {
       if (in_topk_override_ != nullptr)
         return static_cast<int>(cudaMemcpyAsync(topk_idx, in_topk_override_, static_cast<size_t>(B) * nq * 4, cudaMemcpyDeviceToDevice, st));
       return topk_launch(score, B, S, nq, topk_idx, st);
-    }, nullptr, 0, 0, 0, 0, 4.0 * BS);
+    }, {nullptr, 0, 0, 0, 0}, 4.0 * BS);
     {
       void* omp = omn.p; void* selp = sel.p;
-      add_op("gather_topk", [omp, d, cls_all, ncls, ldc, topk_idx, B, S, nq, selp, enc_logits, dt](cudaStream_t st) {
+      b.op("gather_topk", [omp, d, cls_all, ncls, ldc, topk_idx, B, S, nq, selp, enc_logits, dt](cudaStream_t st) {
         return gather_topk_launch(dt, omp, d, cls_all, ldc, ncls, topk_idx, B, S, nq, d, selp, enc_logits, st);
-      }, sel.p, BQ, d, d, 0, 4.0 * BQ * d);
+      }, {sel.p, BQ, d, d, 0}, 4.0 * BQ * d);
     }
-    { GemmOpt o; o.act = ACT_RELU; add_gemm("enc_box0", sel, BQ, d, "enc_box0", d, h1.p, h1.ld, o); }
-    { GemmOpt o; o.act = ACT_RELU; add_gemm("enc_box1", h1, BQ, d, "enc_box1", d, h2.p, h2.ld, o); }
-    { GemmOpt o; o.out_fp32 = 1; add_gemm("enc_box2", h2, BQ, d, "enc_box2", 4, delta_ts, 4, o); }
+    b.gemm("enc_box0", act(ACT_RELU), sel, BQ, d, "enc_box0", d, h1);
+    b.gemm("enc_box1", act(ACT_RELU), h1, BQ, d, "enc_box1", d, h2);
+    b.gemm("enc_box2", f32, h2, BQ, d, "enc_box2", 4, Mat{delta_ts, 4});
     {
-      const float* rpe = pass ? w32("refpoint_embed") : nullptr;
+      const float* rpe = b.w32("refpoint_embed");
       void* sp = sine.p;
-      add_op("query_init", [delta_ts, prop_b, topk_idx, rpe, B, nq, d, enc_boxes, refpoint, sp, dt, S, L, vr_b](cudaStream_t st) {
+      b.op("query_init", [delta_ts, prop_b, topk_idx, rpe, B, nq, d, enc_boxes, refpoint, sp, dt, S, L, vr_b](cudaStream_t st) {
         return query_init_launch(dt, delta_ts, prop_b, topk_idx, rpe, B, nq, d, enc_boxes, refpoint, sp, S, L, vr_b, st);
-      }, refpoint, BQ, 4, 4, 1, 4.0 * BQ * d);
+      }, {refpoint, BQ, 4, 4, 1}, 4.0 * BQ * d);
     }
-    { GemmOpt o; o.act = ACT_RELU; add_gemm("ref_point_head0", sine, BQ, 2 * d, "rph0", d, h1.p, h1.ld, o); }
-    add_gemm("query_pos", h1, BQ, d, "rph1", d, qpos.p, qpos.ld, GemmOpt{});
+    b.gemm("ref_point_head0", act(ACT_RELU), sine, BQ, 2 * d, "rph0", d, h1);
+    b.gemm("query_pos", GemmDesc{}, h1, BQ, d, "rph1", d, qpos);
 
     // ================================================================ decoder
-    Mat tgt = buf16(BQ, d), tq = buf16(BQ, d), t1 = buf16(BQ, d), ta = buf16(BQ, d), tb = buf16(BQ, d);
-    Mat qk = buf16(BQ, 2 * d), vb = buf16(BQ, d), sa = buf16(BQ, d), oa = buf16(BQ, 3 * M * L * P), ms = buf16(BQ, d), ffh = buf16(BQ, ff);
-    Mat hs = buf16(NL * BQ, d);
+    Mat tgt = b.buf16(BQ, d), tq = b.buf16(BQ, d), t1 = b.buf16(BQ, d), ta = b.buf16(BQ, d), tb = b.buf16(BQ, d);
+    Mat qk = b.buf16(BQ, 2 * d), vb = b.buf16(BQ, d), sa = b.buf16(BQ, d), oa = b.buf16(BQ, 3 * M * L * P), ms = b.buf16(BQ, d), ffh = b.buf16(BQ, ff);
+    Mat hs = b.buf16(NL * BQ, d);
     {
-      void* qf = pass ? w16("query_feat") : nullptr; void* tp = tgt.p; void* tqp = tq.p; void* qp = qpos.p;
-      add_op("tgt_init", [qf, d, nq, tp, BQ, dt](cudaStream_t st) { return add_rows_launch(dt, qf, d, nq, nullptr, 0, tp, d, BQ, d, st); }, tgt.p, BQ, d, d, 0, 4.0 * BQ * d);
-      add_op("tgt_plus_pos", [qf, d, nq, qp, tqp, BQ, dt](cudaStream_t st) { return add_rows_launch(dt, qf, d, nq, qp, d, tqp, d, BQ, d, st); }, tq.p, BQ, d, d, 0, 6.0 * BQ * d);
+      void* qf = b.w16("query_feat"); void* tp = tgt.p; void* tqp = tq.p; void* qp = qpos.p;
+      b.op("tgt_init", [qf, d, nq, tp, BQ, dt](cudaStream_t st) { return add_rows_launch(dt, qf, d, nq, nullptr, 0, tp, d, BQ, d, st); },
+           {tgt.p, BQ, d, d, 0}, 4.0 * BQ * d);
+      b.op("tgt_plus_pos", [qf, d, nq, qp, tqp, BQ, dt](cudaStream_t st) { return add_rows_launch(dt, qf, d, nq, qp, d, tqp, d, BQ, d, st); },
+           {tq.p, BQ, d, d, 0}, 6.0 * BQ * d);
     }
     MsdaArgs mbase;
     std::memset(&mbase, 0, sizeof mbase);
@@ -874,61 +833,57 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
     mbase.batch = B; mbase.nq = nq; mbase.heads = M; mbase.levels = L; mbase.points = P; mbase.S = S;
     for (int l = 0; l < L; ++l) { mbase.lvl_h[l] = lvl_h[l]; mbase.lvl_w[l] = lvl_w[l]; mbase.lvl_start[l] = lvl_start[l]; }
     if (msda_plan(&mbase)) { *err = "deformable attention: invalid level table"; return -1; }   // nbands = 0: direct-gather kernel
+    LayerNormArgs plus_pos{}; plus_pos.add_src = qpos.p; plus_pos.ld_add = qpos.ld; plus_pos.y2 = tq.p; plus_pos.ldy2 = tq.ld;   // tq = y + qpos
     Mat cur = tgt;
     for (int i = 0; i < NL; ++i) {
       const std::string k = "dec" + std::to_string(i) + ".", lb = "dec" + std::to_string(i);
-      add_gemm(lb + ".qk", tq, BQ, d, k + "qk", 2 * d, qk.p, qk.ld, GemmOpt{});
-      add_gemm(lb + ".v", cur, BQ, d, k + "v", d, vb.p, vb.ld, GemmOpt{});
-      add_attn(lb + ".self_attn", col(qk, 0), col(qk, d), vb, sa, B, nq, cfg_.sa_heads, d / cfg_.sa_heads);
-      { GemmOpt o; o.resid = cur; add_gemm(lb + ".sa_out", sa, BQ, d, k + "so", d, t1.p, t1.ld, o); }
-      add_ln(lb + ".norm1", t1, ta, k + "n1", 1e-5f, BQ, d, nullptr, 0, nullptr, qpos, tq);
-      add_gemm(lb + ".offs_attn", tq, BQ, d, k + "oa", 3 * M * L * P, oa.p, oa.ld, GemmOpt{});
+      b.gemm(lb + ".qk", GemmDesc{}, tq, BQ, d, k + "qk", 2 * d, qk);
+      b.gemm(lb + ".v", GemmDesc{}, cur, BQ, d, k + "v", d, vb);
+      b.attention(lb + ".self_attn", col(qk, 0), col(qk, d), vb, sa, B, nq, cfg_.sa_heads, d / cfg_.sa_heads);
+      b.gemm(lb + ".sa_out", resid(cur), sa, BQ, d, k + "so", d, t1);
+      b.layernorm(lb + ".norm1", t1, ta, k + "n1", 1e-5f, BQ, d, plus_pos);
+      b.gemm(lb + ".offs_attn", GemmDesc{}, tq, BQ, d, k + "oa", 3 * M * L * P, oa);
       {
         MsdaArgs ma = mbase;
         ma.value = cptr(value.p) + static_cast<size_t>(i) * M * S * MSDA_D * 2;
-        add_op(lb + ".msda", [ma, dt](cudaStream_t st) { return msda_launch(dt, ma, st); }, ms.p, BQ, d, d, 0,
-               2.0 * std::min<double>(1.0 * BS * d, 1.0 * BQ * M * L * P * 4 * 16) + 2.0 * BQ * M * L * P * 3 + 2.0 * BQ * d);
+        b.op(lb + ".msda", [ma, dt](cudaStream_t st) { return msda_launch(dt, ma, st); }, {ms.p, BQ, d, d, 0},
+             2.0 * std::min<double>(1.0 * BS * d, 1.0 * BQ * M * L * P * 4 * 16) + 2.0 * BQ * M * L * P * 3 + 2.0 * BQ * d);
       }
-      { GemmOpt o; o.resid = ta; add_gemm(lb + ".ca_out", ms, BQ, d, k + "co", d, t1.p, t1.ld, o); }
-      add_ln(lb + ".norm2", t1, tb, k + "n2", 1e-5f, BQ, d);
-      { GemmOpt o; o.act = ACT_RELU; add_gemm(lb + ".linear1", tb, BQ, d, k + "l1", ff, ffh.p, ffh.ld, o); }
-      { GemmOpt o; o.resid = tb; add_gemm(lb + ".linear2", ffh, BQ, ff, k + "l2", d, t1.p, t1.ld, o); }
+      b.gemm(lb + ".ca_out", resid(ta), ms, BQ, d, k + "co", d, t1);
+      b.layernorm(lb + ".norm2", t1, tb, k + "n2", 1e-5f, BQ, d);
+      b.gemm(lb + ".linear1", act(ACT_RELU), tb, BQ, d, k + "l1", ff, ffh);
+      b.gemm(lb + ".linear2", resid(tb), ffh, BQ, ff, k + "l2", d, t1);
       // norm3 and the decoder's output norm of this layer's hidden state (transformer.py:279-285) in one launch
-      Mat hsl{cptr(hs.p) + static_cast<size_t>(i) * BQ * d * 2, d};
-      add_ln(lb, t1, tgt, k + "n3", 1e-5f, BQ, d, nullptr, 0, nullptr, qpos, tq, 0, 0, 0, -1, "dec_norm", hsl, 1e-5f);
+      LayerNormArgs a = plus_pos; a.y3 = cptr(hs.p) + static_cast<size_t>(i) * BQ * d * 2; a.ldy3 = d; a.eps3 = 1e-5f;
+      b.layernorm(lb, t1, tgt, k + "n3", 1e-5f, BQ, d, a, "dec_norm");
       cur = tgt;
     }
     // ================================================================ heads
-    float* logits = buf32(NL * BQ * ldc);
-    float* delta = buf32(NL * BQ * 4);
-    float* boxes = buf32(NL * BQ * 4);
-    Mat bh1 = buf16(NL * BQ, d), bh2 = buf16(NL * BQ, d);
-    { GemmOpt o; o.out_fp32 = 1; add_gemm("class_embed", hs, NL * BQ, d, "cls", ncls, logits, ldc, o); }
-    { GemmOpt o; o.act = ACT_RELU; add_gemm("bbox0", hs, NL * BQ, d, "box0", d, bh1.p, bh1.ld, o); }
-    { GemmOpt o; o.act = ACT_RELU; add_gemm("bbox1", bh1, NL * BQ, d, "box1", d, bh2.p, bh2.ld, o); }
-    { GemmOpt o; o.out_fp32 = 1; add_gemm("bbox2", bh2, NL * BQ, d, "box2", 4, delta, 4, o); }
-    add_op("final_boxes", [delta, refpoint, BQ, NL, boxes](cudaStream_t st) { return final_boxes_launch(delta, refpoint, BQ, NL, boxes, st); },
-           boxes, NL * BQ, 4, 4, 1, 32.0 * NL * BQ);
-    out_logits_ = logits; out_boxes_ = boxes; out_enc_logits_ = enc_logits; out_enc_boxes_ = enc_boxes; topk_idx_ = topk_idx;
+    float* logits = b.buf32(NL * BQ * ldc);
+    float* delta = b.buf32(NL * BQ * 4);
+    float* boxes = b.buf32(NL * BQ * 4);
+    Mat bh1 = b.buf16(NL * BQ, d), bh2 = b.buf16(NL * BQ, d);
+    b.gemm("class_embed", f32, hs, NL * BQ, d, "cls", ncls, Mat{logits, ldc});
+    b.gemm("bbox0", act(ACT_RELU), hs, NL * BQ, d, "box0", d, bh1);
+    b.gemm("bbox1", act(ACT_RELU), bh1, NL * BQ, d, "box1", d, bh2);
+    b.gemm("bbox2", f32, bh2, NL * BQ, d, "box2", 4, Mat{delta, 4});
+    b.op("final_boxes", [delta, refpoint, BQ, NL, boxes](cudaStream_t st) { return final_boxes_launch(delta, refpoint, BQ, NL, boxes, st); },
+         {boxes, NL * BQ, 4, 4, 1}, 32.0 * NL * BQ);
+    p->logits = logits; p->boxes = boxes; p->enc_logits = enc_logits; p->enc_boxes = enc_boxes; p->topk_idx = topk_idx;
 
+    if (b.failed()) return -1;
     if (pass == 0) {
-      if (fail) return -1;
-      const size_t need = soff_ + 4096;
+      const size_t need = b.bytes() + 4096;
       if (need > sarena_.bytes) {
         if (sarena_.p) cudaFree(sarena_.p);
         sarena_.p = nullptr;
         if (cudaMalloc(&sarena_.p, need) != cudaSuccess) { *err = "cudaMalloc(workspace, " + std::to_string(need >> 20) + " MiB) failed"; sarena_.bytes = 0; return -1; }
         sarena_.bytes = need;
       }
-    } else if (fail) {
-      return -1;
     }
   }
-  drop_graphs();
-  eager_runs_ = 0;
-  planned_B_ = B;
-  planned_H_ = IH;
-  planned_W_ = IW;
+  p->B = B; p->H = IH; p->W = IW; p->ldc = ldc;
+  plan_ = std::move(p);
   return 0;
 }
 
@@ -959,11 +914,8 @@ int Engine::forward(const ForwardIn& in, int B, int H, int W, float* pred_logits
            std::to_string(kMinSide) + ", " + std::to_string(kMaxSide) + "] (4x4 windows of 16-pixel patches)";
     return -1;
   }
-  if ((B != planned_B_ || H != planned_H_ || W != planned_W_) && plan(B, H, W, err)) {
-    planned_B_ = planned_H_ = planned_W_ = 0;   // a failed plan leaves no schedule behind
-    ops_.clear();
-    return -1;
-  }
+  if ((!plan_ || B != plan_->B || H != plan_->H || W != plan_->W) && plan(B, H, W, err)) return -1;
+  Plan& p = *plan_;
   if (in.kind == IN_FRAMES ? !in.frames : in.kind == IN_FRAMES_NV12 ? !in.frames_nv12 : !in.images) { *err = "lwdetr_forward: null images"; return -1; }
   in_ = in; in_topk_override_ = topk_override;
   // the schedule (and profile_ops, later) reads the engine's copy: the caller's array is free on return.  Neither the source
@@ -978,30 +930,29 @@ int Engine::forward(const ForwardIn& in, int B, int H, int W, float* pred_logits
     frames_padded_ = frames_padded(in.frames_nv12, B, H, W);
   }
   // The first forward of a plan always runs eagerly (it also performs the one-time cudaFuncSetAttribute calls).
-  const bool graph_ok = use_graph_ && captures_.empty() && eager_runs_ > 0;
+  const bool graph_ok = use_graph_ && captures_.empty() && p.eager_runs > 0;
   if (graph_ok) {
     if (!gstream_) {
       if (cudaStreamCreateWithFlags(&gstream_, cudaStreamNonBlocking) != cudaSuccess ||
           cudaEventCreateWithFlags(&ev_in_, cudaEventDisableTiming) != cudaSuccess ||
           cudaEventCreateWithFlags(&ev_out_, cudaEventDisableTiming) != cudaSuccess) { *err = "graph stream setup failed"; return -1; }
     }
-    const GraphKey key{topk_override};
-    auto it = graphs_.find(key);
-    if (it == graphs_.end()) {
-      if (graphs_.size() >= 8) drop_graphs();
+    auto it = p.graphs.find(topk_override);
+    if (it == p.graphs.end()) {
+      if (p.graphs.size() >= 8) p.clear_graphs();
       cudaGraph_t g = nullptr;
       if (cudaStreamBeginCapture(gstream_, cudaStreamCaptureModeThreadLocal) != cudaSuccess) { *err = std::string("graph capture begin failed: ") + cudaGetErrorString(cudaGetLastError()); return -1; }
       int rc = 0;
-      for (auto& op : ops_) { if (op.reads_input) continue; rc = op.run(gstream_); if (rc) break; }
+      for (auto& op : p.ops) { if (op.reads_input) continue; rc = op.run(gstream_); if (rc) break; }
       cudaError_t ce = cudaStreamEndCapture(gstream_, &g);
       if (rc || ce != cudaSuccess) { if (g) cudaGraphDestroy(g); *err = "graph capture failed"; return -1; }
       cudaGraphExec_t ex = nullptr;
       if (cudaGraphInstantiate(&ex, g, 0) != cudaSuccess) { cudaGraphDestroy(g); *err = "graph instantiate failed"; return -1; }
       cudaGraphDestroy(g);
-      it = graphs_.emplace(key, ex).first;
+      it = p.graphs.emplace(topk_override, ex).first;
     }
     // the input-reading ops on the caller's stream, then the graph ordered after them, then the caller's stream after the graph
-    for (auto& op : ops_) {
+    for (auto& op : p.ops) {
       if (!op.reads_input) continue;
       const int rc = op.run(st);
       if (rc) { *err = "op " + op.label + " failed to launch"; return -1; }
@@ -1010,30 +961,30 @@ int Engine::forward(const ForwardIn& in, int B, int H, int W, float* pred_logits
         cudaGraphLaunch(it->second, gstream_) != cudaSuccess || cudaEventRecord(ev_out_, gstream_) != cudaSuccess ||
         cudaStreamWaitEvent(st, ev_out_, 0) != cudaSuccess) { *err = std::string("graph launch failed: ") + cudaGetErrorString(cudaGetLastError()); return -1; }
   } else {
-    for (auto& op : ops_) {
+    for (auto& op : p.ops) {
       const int rc = op.run(st);
       if (rc) { *err = "op " + op.label + " failed to launch: " + (rc > 0 ? cudaGetErrorString(static_cast<cudaError_t>(rc)) : "bad arguments"); return -1; }
       if (!captures_.empty() && do_capture(op, st)) { *err = "capture after " + op.label + " failed: " + cudaGetErrorString(cudaGetLastError()); return -1; }
     }
-    ++eager_runs_;
+    ++p.eager_runs;
   }
   // results -> caller buffers (dense)
   const int nq = cfg_.num_queries, ncls = cfg_.num_classes, NL = cfg_.dec_layers;
   const long long BQ = 1LL * B * nq;
   auto copy_logits = [&](float* dst, int layer) {
-    return cudaMemcpy2DAsync(dst, ncls * 4, out_logits_ + static_cast<size_t>(layer) * BQ * ldc_, static_cast<size_t>(ldc_) * 4, ncls * 4, static_cast<size_t>(BQ), cudaMemcpyDeviceToDevice, st);
+    return cudaMemcpy2DAsync(dst, ncls * 4, p.logits + static_cast<size_t>(layer) * BQ * p.ldc, static_cast<size_t>(p.ldc) * 4, ncls * 4, static_cast<size_t>(BQ), cudaMemcpyDeviceToDevice, st);
   };
   cudaError_t e = cudaSuccess;
   if (pred_logits) e = copy_logits(pred_logits, NL - 1);
-  if (e == cudaSuccess && pred_boxes) e = cudaMemcpyAsync(pred_boxes, out_boxes_ + static_cast<size_t>(NL - 1) * BQ * 4, BQ * 16, cudaMemcpyDeviceToDevice, st);
+  if (e == cudaSuccess && pred_boxes) e = cudaMemcpyAsync(pred_boxes, p.boxes + static_cast<size_t>(NL - 1) * BQ * 4, BQ * 16, cudaMemcpyDeviceToDevice, st);
   if (aux) {
     for (int l = 0; l + 1 < NL && e == cudaSuccess; ++l) {
       if (aux->aux_logits) e = copy_logits(aux->aux_logits + static_cast<size_t>(l) * BQ * ncls, l);
-      if (e == cudaSuccess && aux->aux_boxes) e = cudaMemcpyAsync(aux->aux_boxes + static_cast<size_t>(l) * BQ * 4, out_boxes_ + static_cast<size_t>(l) * BQ * 4, BQ * 16, cudaMemcpyDeviceToDevice, st);
+      if (e == cudaSuccess && aux->aux_boxes) e = cudaMemcpyAsync(aux->aux_boxes + static_cast<size_t>(l) * BQ * 4, p.boxes + static_cast<size_t>(l) * BQ * 4, BQ * 16, cudaMemcpyDeviceToDevice, st);
     }
-    if (e == cudaSuccess && aux->enc_logits) e = cudaMemcpyAsync(aux->enc_logits, out_enc_logits_, BQ * ncls * 4, cudaMemcpyDeviceToDevice, st);
-    if (e == cudaSuccess && aux->enc_boxes) e = cudaMemcpyAsync(aux->enc_boxes, out_enc_boxes_, BQ * 16, cudaMemcpyDeviceToDevice, st);
-    if (e == cudaSuccess && aux->topk_index) e = cudaMemcpyAsync(aux->topk_index, topk_idx_, BQ * 4, cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess && aux->enc_logits) e = cudaMemcpyAsync(aux->enc_logits, p.enc_logits, BQ * ncls * 4, cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess && aux->enc_boxes) e = cudaMemcpyAsync(aux->enc_boxes, p.enc_boxes, BQ * 16, cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess && aux->topk_index) e = cudaMemcpyAsync(aux->topk_index, p.topk_idx, BQ * 4, cudaMemcpyDeviceToDevice, st);
   }
   if (e != cudaSuccess) { *err = std::string("result copy failed: ") + cudaGetErrorString(e); return -1; }
   return 0;
@@ -1041,16 +992,17 @@ int Engine::forward(const ForwardIn& in, int B, int H, int W, float* pred_logits
 
 int Engine::profile_ops(int iters, std::vector<float>* ms, cudaStream_t st, std::string* err) {
   DeviceGuard guard(device_);
-  if (planned_B_ <= 0) { *err = "profile_ops: run a forward first"; return -1; }
-  ms->assign(ops_.size(), 0.f);
+  if (!plan_) { *err = "profile_ops: run a forward first"; return -1; }
+  const std::vector<Op>& ops = plan_->ops;
+  ms->assign(ops.size(), 0.f);
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0); cudaEventCreate(&e1);
-  for (size_t i = 0; i < ops_.size(); ++i) {
-    ops_[i].run(st);   // warm
+  for (size_t i = 0; i < ops.size(); ++i) {
+    ops[i].run(st);   // warm
     cudaEventRecord(e0, st);
-    for (int k = 0; k < iters; ++k) ops_[i].run(st);
+    for (int k = 0; k < iters; ++k) ops[i].run(st);
     cudaEventRecord(e1, st);
-    if (cudaEventSynchronize(e1) != cudaSuccess) { *err = "profile_ops: op " + ops_[i].label + " failed"; return -1; }
+    if (cudaEventSynchronize(e1) != cudaSuccess) { *err = "profile_ops: op " + ops[i].label + " failed"; return -1; }
     float t = 0.f;
     cudaEventElapsedTime(&t, e0, e1);
     (*ms)[i] = t / iters;

@@ -6,6 +6,7 @@
 
 #include <functional>
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -47,6 +48,46 @@ struct ForwardIn {
   float mean[3] = {0.f, 0.f, 0.f}, stdv[3] = {1.f, 1.f, 1.f};   // IN_U8_NHWC: (x/255 - mean) / std
 };
 
+// Switches to a device for the duration of a call (the caller's current device is restored afterwards).
+struct DeviceGuard {
+  int prev = -1;
+  explicit DeviceGuard(int dev) {
+    if (cudaGetDevice(&prev) != cudaSuccess) prev = -1;
+    if (prev != dev) cudaSetDevice(dev); else prev = -1;
+  }
+  ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
+};
+
+// The kernel schedule of one (batch size, height, width): its ops, their CUDA graphs and the result buffers the ops write
+// (in the engine's workspace arena).  Destroying a plan destroys its graphs.
+struct Plan {
+  int B = 0, H = 0, W = 0;
+  std::vector<Op> ops;
+  // CUDA graphs: the two ops that read caller-owned memory (mask tables, patch gather) are launched eagerly on the caller's
+  // stream; everything behind them only touches engine-owned buffers and is ONE executable graph per plan - whatever
+  // tensor, input encoding or mask the caller passes.  (The test-only top-k override pointer is the one caller pointer left
+  // inside, hence the key.)  Captured on an internal stream: the caller's stream may be the legacy default stream, which
+  // cannot be captured.
+  std::map<const int32_t*, cudaGraphExec_t> graphs;
+  int eager_runs = 0;
+  // result buffers
+  float* logits = nullptr;       // [layers, B, nq, ldc]
+  int ldc = 96;                  // row pitch of the class-logit buffers: num_classes rounded up to 32
+  float* boxes = nullptr;        // [layers, B, nq, 4]
+  float* enc_logits = nullptr;   // [B, nq, ncls]
+  float* enc_boxes = nullptr;    // [B, nq, 4]
+  int* topk_idx = nullptr;       // [B, nq]
+
+  Plan() = default;
+  Plan(const Plan&) = delete;
+  Plan& operator=(const Plan&) = delete;
+  ~Plan() { clear_graphs(); }
+  void clear_graphs() {
+    for (auto& kv : graphs) cudaGraphExecDestroy(kv.second);
+    graphs.clear();
+  }
+};
+
 class Engine {
  public:
   // supported input sides (pixels, multiples of 64: 4x4 windows of 16-pixel patches)
@@ -66,8 +107,8 @@ class Engine {
   size_t arena_used() const { return woff_; }
   bool weights_loaded() const { return weights_loaded_; }
   int device() const { return device_; }
-  int num_ops() const { return static_cast<int>(ops_.size()); }
-  const Op& op(int i) const { return ops_[i]; }
+  int num_ops() const { return plan_ ? static_cast<int>(plan_->ops.size()) : 0; }
+  const Op& op(int i) const { return plan_->ops[i]; }
   const lwdetr_config& config() const { return cfg_; }
   // per-op timing of the last planned batch (CUDA events, `iters` runs per op); returns ms per op
   int profile_ops(int iters, std::vector<float>* ms, cudaStream_t st, std::string* err);
@@ -76,7 +117,6 @@ class Engine {
   struct DevBuf { void* p = nullptr; size_t bytes = 0; };
   int plan(int B, int H, int W, std::string* err);
   void* walloc(size_t bytes);      // weight arena (bump)
-  void* salloc(size_t bytes);      // workspace arena (bump)
   std::vector<uint16_t> to16(const std::vector<float>& v) const;   // round to the compute dtype
   void* upload16(const std::vector<float>& v);
   float* upload32(const std::vector<float>& v);
@@ -87,44 +127,26 @@ class Engine {
   int dtype_;
   bool e4m3_ = false;   // LWDETR_F16_E4M3: dtype_ is DT_F16; the encoder's LN->qkv and LN->fc1 run in e4m3
   int device_ = 0;    // CUDA device the engine was created on; every entry point switches to it (one handle per device)
-  int planned_B_ = 0, planned_H_ = 0, planned_W_ = 0;   // shape of the current schedule (0: none)
   bool weights_loaded_ = false;
   int use_graph_ = 0;
   int fuse_ln_ = 1;   // ViT LayerNorms folded into the consuming GEMM's epilogue (option "fuse_layernorm"; no effect on the
                       // encoder in the e4m3 mode)
-  // CUDA graphs: the two ops that read caller-owned memory (mask tables, patch gather) are launched eagerly on the
-  // caller's stream; everything behind them only touches engine-owned buffers and is ONE executable graph per planned
-  // (batch size, height, width) - whatever tensor, input encoding or mask the caller passes.  (The test-only top-k override pointer is
-  // the one caller pointer left inside, hence the key.)  Captured on an internal stream: the caller's stream may be the
-  // legacy default stream, which cannot be captured.
-  struct GraphKey { const void* topk; bool operator<(const GraphKey& o) const { return topk < o.topk; } };
-  std::map<GraphKey, cudaGraphExec_t> graphs_;
-  cudaStream_t gstream_ = nullptr;
+  std::unique_ptr<Plan> plan_;   // the current schedule, or none (dropped whenever what it was built from changes)
+  cudaStream_t gstream_ = nullptr;   // graph capture and launch
   cudaEvent_t ev_in_ = nullptr, ev_out_ = nullptr;
-  int eager_runs_ = 0;
-  void drop_graphs();
-  std::vector<Op> ops_;
   std::vector<Capture> captures_;
-  // arenas
+  // arenas: packed weights (bump), and the workspace every plan lays out from its base (grow-only)
   DevBuf warena_, sarena_;
-  size_t woff_ = 0, soff_ = 0;
+  size_t woff_ = 0;
   // packed weights (device pointers), keyed by short names
   std::map<std::string, void*> W_;
   std::map<std::string, float*> F_;
-  std::vector<uint8_t> invalid_rows_;   // per memory token
   // live I/O pointers patched into the schedule at forward() time
   ForwardIn in_;
   std::vector<lwdetr_frame> frames_;   // the engine's copy of an IN_FRAMES batch's descriptors (in_.frames points here)
   std::vector<lwdetr_frame_nv12> frames_nv12_;   // the same for IN_FRAMES_NV12 (in_.frames_nv12 points here)
   bool frames_padded_ = false;         // some frame leaves part of the canvas unfilled: mask_setup takes the device-made mask
   const int32_t* in_topk_override_ = nullptr;
-  // result buffers (engine owned)
-  float* out_logits_ = nullptr;   // [layers, B, nq, ldc_]
-  int ldc_ = 96;                  // row pitch of the class-logit buffers: num_classes rounded up to 32
-  float* out_boxes_ = nullptr;    // [layers, B, nq, 4]
-  float* out_enc_logits_ = nullptr;  // [B, nq, ncls]
-  float* out_enc_boxes_ = nullptr;   // [B, nq, 4]
-  int* topk_idx_ = nullptr;          // [B, nq]
 };
 
 // host helpers exposed for CPU tests
