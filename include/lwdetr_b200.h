@@ -353,6 +353,94 @@ LWDETR_API int lwdetr_tracker_export(lwdetr_tracker* t, int stream_id, lwdetr_tr
 LWDETR_API int lwdetr_query_best(const float* pred_logits, const float* pred_boxes, const float* target_sizes, int B, int nq, int num_classes,
                                  float* scores, int32_t* labels, float* boxes, void* stream);
 
+/* lwdetr_track_ex: lwdetr_track with the camera motion of each frame (lwdetr_gmc_estimate's output), for moving cameras.
+ * motion: DEVICE float64 [B, 4] (a, b, tx, ty), 8-byte aligned, the similarity x' = a x - b y + tx, y' = b x + a y + ty from
+ * the stream's previous frame to this one in frame pixels; NULL is lwdetr_track, bit for bit.  With a motion, step 1 of the
+ * contract above gains a warp (BoT-SORT's multi_gmc): after the pool is predicted, every record of the stream (confirmed,
+ * lost and unconfirmed) is warped, each operation rounded on its own, with s2 = a * a + b * b and s = sqrt(s2):
+ *   cx' = (a * cx - b * cy) + tx;  cy' = (b * cx + a * cy) + ty;  vx' = a * vx - b * vy;  vy' = b * vx + a * vy;
+ *   h' = s * h;  vh' = s * vh;  a (aspect) and va unchanged;
+ *   P, C and V of x, y and h multiplied by s2; those of the aspect unchanged.
+ * This is exact, not an approximation: ByteTrack's x and y noise are both std(., h), so the x and y blocks of the covariance
+ * are always equal (P_x = P_y, C_x = C_y, V_x = V_y) and a rotation by R = s Q maps sigma^2 I to s^2 sigma^2 I; the block
+ * structure of the state survives.  (BoT-SORT's kron(I4, R) would also rotate the (aspect, h) pair, which has no meaning
+ * in the xyah state; the aspect is left alone and h scales with the frame.) */
+LWDETR_API int lwdetr_track_ex(lwdetr_tracker* t, const float* scores, const int32_t* labels, const float* boxes, const double* motion,
+                               int B, int k, const int32_t* stream_ids, int max_out, int32_t* out_ids, float* out_scores,
+                               int32_t* out_labels, float* out_boxes, int32_t* out_index, int32_t* counts, void* stream);
+
+/* Camera-motion estimation (global motion compensation, BoT-SORT's sparseOptFlow with the deviations stated here) per video
+ * stream on the device, for lwdetr_track_ex.  The C composition per batch of frames, one frame per stream:
+ * lwdetr_forward_frames (or _nv12) -> lwdetr_query_best -> lwdetr_gmc_estimate (or _nv12) on the same frame descriptors ->
+ * lwdetr_track_ex with its motion.  Calls on one estimator must be ordered on one CUDA stream.
+ * The contract (tools/gmc_spec.py restates it in numpy), d = downscale:
+ *   1. grey and downscale: RGB grey g = (9798 R + 19235 G + 3735 B + 16384) >> 15 (cv2.COLOR_RGB2GRAY, bit for bit); NV12: the
+ *      luma byte.  Level 0 is (floor(h / d), floor(w / d)); pixel (y, x) = (S + d*d / 2) / (d*d) in integers, S the sum of
+ *      the d x d block of grey at (d y, d x) (for d = 2 that is cv2.resize's INTER_LINEAR / INTER_AREA halving).
+ *   2. pyramid: level l from level l - 1 as cv2.pyrDown, bit for bit: ((w + 1) / 2, (h + 1) / 2), the 5-tap [1 4 6 4 1]
+ *      kernel in both axes, BORDER_REFLECT_101, (sum + 128) >> 8.  Levels used: the largest L <= levels with both sides of
+ *      level L > window (cv2.buildOpticalFlowPyramid's rule).
+ *   3. corners on level 0: Sobel 3x3 derivatives dx, dy (BORDER_REFLECT_101), their products summed over the 3x3 block
+ *      (BORDER_REFLECT_101 on the products), exact in integers: Sxx, Sxy, Syy.  Response R = (Sxx + Syy) - sqrt((Sxx - Syy)^2
+ *      + 4 Sxy^2) in float64, the integer under the root exact, the root and the subtraction rounded once each: that is
+ *      cv2.cornerMinEigenVal(blockSize 3, ksize 3) times 2 * 3060^2.  The frame is cut into c x c cells, c the smallest side
+ *      with ceil(w0 / c) * ceil(h0 / c) <= max_points (row-major cells); each cell keeps its best pixel (largest R, lowest
+ *      pixel index y * w0 + x on ties) when R > 0 and R >= (double)quality * max R over the frame.  The corners, in cell
+ *      order, are kept for the stream's next frame.  (goodFeaturesToTrack's global top list is replaced on purpose: no sort,
+ *      deterministic, points spread over the frame for the robust fit.)
+ *   4. pyramidal Lucas-Kanade of the previous frame's corners into this frame: cv2.calcOpticalFlowPyrLK's iteration
+ *      (window x window, the levels of 2., iterations, eps, min_eig; Scharr derivatives of the previous level with
+ *      BORDER_REFLECT_101, 0 outside the image; images BORDER_REFLECT_101; 14-bit bilinear weights), except that the window
+ *      sums are exact int64 before their scaling to float.  A corner is matched when level 0 ends with status 1.
+ *   5. fit: each matched pair maps to frame pixels, x_f = d * (x + 0.5) - 0.5 (both axes, both frames), in float64.  With n
+ *      pairs (n >= min_inliers, else status LWDETR_GMC_FEW_POINTS), hypothesis h in [0, hypotheses) takes pairs
+ *      i = H(2h) mod n and j = H(2h + 1) mod (n - 1), plus 1 when >= i, with H(k) = mix(k * 0x9e3779b9 + 0x7f4a7c15) (uint32
+ *      arithmetic) and mix(x): x ^= x >> 16; x *= 0x7feb352d; x ^= x >> 15; x *= 0x846ca68b; x ^= x >> 16.  Its similarity
+ *      (dp = p_j - p_i, dq = q_j - q_i, n2 = dpx dpx + dpy dpy, skipped unless n2 > 0): a = (dqx dpx + dqy dpy) / n2,
+ *      b = (dqy dpx - dqx dpy) / n2, tx = qx_i - (a px_i - b py_i), ty = qy_i - (b px_i + a py_i).  Its inliers: pairs with
+ *      ex^2 + ey^2 <= (ransac_thresh * d)^2, ex = ((a px - b py) + tx) - qx, ey = ((b px + a py) + ty) - qy; every operation
+ *      of this step is float64 rounded on its own.  The most inliers wins, the lowest h on ties; fewer than min_inliers:
+ *      LWDETR_GMC_FEW_INLIERS.  Then 3 rounds: the inliers of the current model refit it by least squares (centred sums,
+ *      a = sum(px' qx' + py' qy') / sum(px'^2 + py'^2), b = sum(px' qy' - py' qx') / sum(px'^2 + py'^2), t from the means),
+ *      summed in a fixed order, so a call is bit-reproducible; the final model's inlier count is returned (fewer than
+ *      min_inliers: LWDETR_GMC_FEW_INLIERS).
+ *   6. outputs per frame: motion float64 [B, 4] (a, b, tx, ty) from the stream's previous frame to this one, frame pixels;
+ *      status int32 [B]; inliers int32 [B].  Every status but LWDETR_GMC_OK gives the identity (1, 0, 0, 0).  A stream's first
+ *      frame (after create or reset) and a frame whose size differs from the stream's previous one (re)start the stream.
+ * lwdetr_gmc_params_default: downscale 2, max_points 1024, quality 0.01, levels 3, window 21, iterations 30, eps 0.01,
+ *   min_eig 1e-4, ransac_thresh 3 (level-0 pixels), hypotheses 1024, min_inliers 10, max_height 2160, max_width 3840.
+ * lwdetr_gmc_create: params validated (downscale in [1, 8], max_points in [16, 4096], quality in (0, 1], levels in [0, 5],
+ *   window odd in [5, 31], iterations in [1, 100], eps > 0, min_eig >= 0, ransac_thresh > 0, hypotheses in [1, 4096],
+ *   min_inliers in [2, max_points], max sides in [16 d, 8192]); allocates the device table (two pyramids and corner lists
+ *   per stream, sized by the largest frame) on the current device.  Synchronous.
+ * lwdetr_gmc_reset: the n streams listed (HOST; ids distinct and in [0, num_streams), else an error and nothing happens)
+ *   start again at their next frame.
+ * lwdetr_gmc_estimate / _nv12: one frame for each of B streams (stream_ids HOST; ids distinct and in [0, num_streams), else
+ *   an error and nothing happens); frames as lwdetr_forward_frames takes them (dst_h, dst_w and colorspace are not read;
+ *   NV12: the luma plane only), sides at least 16 d and at most the table's largest frame.  motion 8-byte aligned; all
+ *   DEVICE; asynchronous, nothing allocated or copied per call, safe to capture in a CUDA graph. */
+enum { LWDETR_GMC_OK = 0, LWDETR_GMC_FIRST_FRAME = 1, LWDETR_GMC_SIZE_CHANGED = 2, LWDETR_GMC_FEW_POINTS = 3, LWDETR_GMC_FEW_INLIERS = 4 };
+typedef struct {
+  int32_t downscale, max_points;
+  float quality;
+  int32_t levels, window, iterations;
+  float eps, min_eig, ransac_thresh;
+  int32_t hypotheses, min_inliers, max_height, max_width;
+} lwdetr_gmc_params;
+typedef struct lwdetr_gmc lwdetr_gmc;
+LWDETR_API void lwdetr_gmc_params_default(lwdetr_gmc_params* p);
+LWDETR_API int lwdetr_gmc_create(int num_streams, const lwdetr_gmc_params* params, lwdetr_gmc** out);
+LWDETR_API void lwdetr_gmc_destroy(lwdetr_gmc* g);
+LWDETR_API int lwdetr_gmc_reset(lwdetr_gmc* g, const int32_t* streams, int n, void* stream);
+/* Inspection (tests), synchronous (waits for the device): one stream's state after its last frame.  levels: that frame's
+ * pyramid, levels 0..info[3] one after another, each dense at its size (levels_bytes must hold them); corners float [max_points,
+ * 2]: its corners (info[4] of them); flow float [max_points, 4] (from x, y, to x, y, level-0 pixels) and found int8
+ * [max_points]: the last call's Lucas-Kanade results for the previous frame's info[5] corners (meaningful when that call had
+ * a previous frame of the same size).  info = (has a last frame, its height, its width, levels used or -1, corners, corners
+ * of the previous frame). */
+LWDETR_API int lwdetr_gmc_export(lwdetr_gmc* g, int stream_id, uint8_t* levels, int64_t levels_bytes, float* corners, float* flow,
+                                 int8_t* found, int32_t info[6]);
+
 /* The LWDETR_F16_E4M3 mode's two kernels.
  * lwdetr_layernorm_e4m3: fp16 rows x [rows, ldx] -> e4m3 codes q [rows, ldq] (uint8) and fp32 row_scale [rows], as the mode's
  *   activation contract above (x^ without the LayerNorm affine, eps as given).  C % 8 == 0, C <= 1024, ldx and ldq
@@ -523,6 +611,12 @@ LWDETR_API int lwdetr_forward_frames_nv12(lwdetr_handle* h, const lwdetr_frame_n
 /* lwdetr_resize_patches on NV12 frames. */
 LWDETR_API int lwdetr_resize_patches_nv12(int dtype, const lwdetr_frame_nv12* frames, int B, int height, int width,
                                           const float mean[3], const float std[3], void* A, uint8_t* mask, void* stream);
+
+/* Camera motion of B frames (lwdetr_gmc_create above; declared here, after the frame descriptors). */
+LWDETR_API int lwdetr_gmc_estimate(lwdetr_gmc* g, const lwdetr_frame* frames, int B, const int32_t* stream_ids, double* motion,
+                                   int32_t* status, int32_t* inliers, void* stream);
+LWDETR_API int lwdetr_gmc_estimate_nv12(lwdetr_gmc* g, const lwdetr_frame_nv12* frames, int B, const int32_t* stream_ids,
+                                        double* motion, int32_t* status, int32_t* inliers, void* stream);
 
 /* Multi-GPU init (SURVEY.md 8e): ONE ncclBroadcast of the packed weight arena from rank `root`, stream-ordered on
  * `stream`; the only collective of the path (images shard across ranks as independent replicas, nothing on the hot path).

@@ -39,6 +39,14 @@ _SIGNATURES = {
     "lwdetr_tracker_reset": (_i, [_vp, _vp, _i, _vp]),
     "lwdetr_track": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_tracker_export": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
+    "lwdetr_track_ex": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "lwdetr_gmc_params_default": (None, [_vp]),
+    "lwdetr_gmc_create": (_i, [_i, _vp, _vp]),
+    "lwdetr_gmc_destroy": (None, [_vp]),
+    "lwdetr_gmc_reset": (_i, [_vp, _vp, _i, _vp]),
+    "lwdetr_gmc_export": (_i, [_vp, _i, _vp, _i64, _vp, _vp, _vp, _vp]),
+    "lwdetr_gmc_estimate": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
+    "lwdetr_gmc_estimate_nv12": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_query_best": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "lwdetr_layernorm_e4m3": (_i, [_vp, _i, _i64, _i, _f, _vp, _i, _vp, _vp]),
     "lwdetr_gemm_e4m3": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _i, _vp]),
@@ -473,11 +481,13 @@ class Tracker:
         arr, n = self._ids(streams)
         check(lib().lwdetr_tracker_reset(self._t, ctypes.cast(arr, _vp), n, stream_ptr(self.device)), "lwdetr_tracker_reset")
 
-    def update(self, scores, labels, boxes, stream_ids=None, max_out=None):
+    def update(self, scores, labels, boxes, stream_ids=None, max_out=None, motion=None):
         """One frame for each of B distinct streams: scores fp32 [B, k], labels int [B, k], xyxy boxes fp32 [B, k, 4] (CUDA;
         stream_ids default range(B)) -> (ids int32 [B, max_out], scores fp32, labels int32, boxes fp32 [B, max_out, 4], index
         int32 (the entry of each track), counts int32 [B]); unused slots id 0, score 0, label -1, zero box, index -1.
-        max_out defaults to k.  Stream-ordered, no synchronisation."""
+        max_out defaults to k.  motion: float64 [B, 4] camera motion of each frame (MotionEstimator.estimate), which warps
+        every track of the stream after the predict (lwdetr_track_ex); None tracks as for a still camera.  Stream-ordered,
+        no synchronisation."""
         import torch
         B, k = scores.shape
         if tuple(labels.shape) != (B, k) or tuple(boxes.shape) != (B, k, 4):
@@ -497,8 +507,15 @@ class Tracker:
         o_b = torch.empty(B, m, 4, device=dev, dtype=torch.float32)
         o_i = torch.empty(B, m, device=dev, dtype=torch.int32)
         counts = torch.empty(B, device=dev, dtype=torch.int32)
-        check(lib().lwdetr_track(self._t, ptr(scores), ptr(labels), ptr(boxes), B, k, ctypes.cast(ids, _vp), m, ptr(o_id), ptr(o_s),
-                                 ptr(o_l), ptr(o_b), ptr(o_i), ptr(counts), stream_ptr(dev)), "lwdetr_track")
+        if motion is None:
+            check(lib().lwdetr_track(self._t, ptr(scores), ptr(labels), ptr(boxes), B, k, ctypes.cast(ids, _vp), m, ptr(o_id), ptr(o_s),
+                                     ptr(o_l), ptr(o_b), ptr(o_i), ptr(counts), stream_ptr(dev)), "lwdetr_track")
+        else:
+            if tuple(motion.shape) != (B, 4):
+                raise RuntimeError("Tracker.update: motion must be [%d, 4], got %s" % (B, tuple(motion.shape)))
+            motion = motion.to(device=dev, dtype=torch.float64).contiguous()
+            check(lib().lwdetr_track_ex(self._t, ptr(scores), ptr(labels), ptr(boxes), ptr(motion), B, k, ctypes.cast(ids, _vp), m,
+                                        ptr(o_id), ptr(o_s), ptr(o_l), ptr(o_b), ptr(o_i), ptr(counts), stream_ptr(dev)), "lwdetr_track_ex")
         return o_id, o_s, o_l, o_b, o_i, counts
 
     def export(self, stream_id):
@@ -516,6 +533,103 @@ class Tracker:
                      label=r.label, index=r.index, mean=np.array(r.mean[:], np.float64), cov=np.array(r.cov[:], np.float64))
                 for r in arr[:min(cnt.value, cap)]]
         return recs, tuple(fno)
+
+
+class GmcParams(ctypes.Structure):
+    """lwdetr_gmc_params (include/lwdetr_b200.h)."""
+    _fields_ = [("downscale", ctypes.c_int32), ("max_points", ctypes.c_int32), ("quality", _f), ("levels", ctypes.c_int32),
+                ("window", ctypes.c_int32), ("iterations", ctypes.c_int32), ("eps", _f), ("min_eig", _f), ("ransac_thresh", _f),
+                ("hypotheses", ctypes.c_int32), ("min_inliers", ctypes.c_int32), ("max_height", ctypes.c_int32),
+                ("max_width", ctypes.c_int32)]
+
+
+GMC_OK, GMC_FIRST_FRAME, GMC_SIZE_CHANGED, GMC_FEW_POINTS, GMC_FEW_INLIERS = 0, 1, 2, 3, 4
+
+
+class MotionEstimator:
+    """Camera motion per video stream on the device (lwdetr_gmc_*, the contract in include/lwdetr_b200.h): the similarity
+    from each stream's previous frame to its current one, for Tracker.update(motion=...).  Parameters are
+    lwdetr_gmc_params' fields (defaults: lwdetr_gmc_params_default; max_height / max_width bound the frames and size the
+    device table).  All calls of one estimator must run on one CUDA stream (the current one at each call)."""
+
+    def __init__(self, num_streams, device=None, **params):
+        import torch
+        p = GmcParams()
+        lib().lwdetr_gmc_params_default(ctypes.byref(p))
+        bad = set(params) - {n for n, _ in GmcParams._fields_}
+        if bad:
+            raise RuntimeError("MotionEstimator: unknown parameters %s" % ", ".join(sorted(bad)))
+        for n, v in params.items():
+            setattr(p, n, v)
+        self.params = p
+        self.num_streams = int(num_streams)
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self._g = _vp()
+        with torch.cuda.device(self.device):
+            check(lib().lwdetr_gmc_create(self.num_streams, ctypes.byref(p), ctypes.byref(self._g)), "lwdetr_gmc_create")
+
+    def close(self):
+        if self._g:
+            lib().lwdetr_gmc_destroy(self._g)
+            self._g = _vp()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def reset(self, streams):
+        """The streams start again at their next frame (stream-ordered)."""
+        arr, n = Tracker._ids(streams)
+        check(lib().lwdetr_gmc_reset(self._g, ctypes.cast(arr, _vp), n, stream_ptr(self.device)), "lwdetr_gmc_reset")
+
+    def estimate(self, frames, streams=None):
+        """One frame for each of B distinct streams (capi.Frames, or frames as Frames takes them; an NV12 frame is read
+        through its luma plane only, so its colorspace does not matter) -> (motion float64 [B, 4] (a, b, tx, ty): x' = a x -
+        b y + tx, y' = b x + a y + ty from the stream's previous frame to this one in frame pixels; status int32 [B]
+        (GMC_*); inliers int32 [B]).  streams defaults to range(B).  Stream-ordered, no synchronisation."""
+        import torch
+        if not isinstance(frames, Frames):
+            nv12 = isinstance(frames, torch.Tensor) and frames.dim() == 3 and frames.shape[2] != 3
+            nv12 = nv12 or (not isinstance(frames, torch.Tensor) and len(frames) > 0 and _is_nv12(frames[0]))
+            frames = Frames(frames, self.device, "bt601" if nv12 else None)
+        B = len(frames.items)
+        ids, n = Tracker._ids(range(B) if streams is None else streams)
+        if n != B:
+            raise RuntimeError("MotionEstimator.estimate: %d stream ids for %d frames" % (n, B))
+        dev = self.device
+        motion = torch.empty(B, 4, device=dev, dtype=torch.float64)
+        status = torch.empty(B, device=dev, dtype=torch.int32)
+        inliers = torch.empty(B, device=dev, dtype=torch.int32)
+        descs = frames.descs(frames.sizes)
+        name = "lwdetr_gmc_estimate_nv12" if frames.nv12 else "lwdetr_gmc_estimate"
+        check(getattr(lib(), name)(self._g, descs, B, ctypes.cast(ids, _vp), ptr(motion), ptr(status), ptr(inliers), stream_ptr(dev)), name)
+        return motion, status, inliers
+
+    def export(self, stream_id):
+        """Synchronous (waits for the device): one stream's state after its last frame (lwdetr_gmc_export) as a dict: levels
+        (list of uint8 [h_l, w_l] arrays), corners float32 [n, 2] (level-0 x, y), flow float32 [m, 4] and found bool [m]
+        (the last call's Lucas-Kanade of the previous frame's m corners), valid, size."""
+        import numpy as np
+        p = self.params
+        cap = (p.max_height // p.downscale + 1) * (p.max_width // p.downscale + 1) * 2
+        lv = np.zeros(cap, np.uint8)
+        corners = np.zeros((p.max_points, 2), np.float32)
+        flow = np.zeros((p.max_points, 4), np.float32)
+        found = np.zeros(p.max_points, np.int8)
+        info = (ctypes.c_int32 * 6)()
+        check(lib().lwdetr_gmc_export(self._g, int(stream_id), lv.ctypes.data_as(_vp), cap, corners.ctypes.data_as(_vp),
+                                      flow.ctypes.data_as(_vp), found.ctypes.data_as(_vp), ctypes.cast(info, _vp)), "lwdetr_gmc_export")
+        valid, h, w, nlev, nc, nf = list(info)
+        levels, o = [], 0
+        lh, lw = h // p.downscale, w // p.downscale
+        for _ in range(nlev + 1):
+            levels.append(lv[o:o + lh * lw].reshape(lh, lw).copy())
+            o += lh * lw
+            lh, lw = (lh + 1) // 2, (lw + 1) // 2
+        return dict(valid=bool(valid), size=(h, w), levels=levels, corners=corners[:nc].copy(), flow=flow[:nf].copy(),
+                    found=found[:nf].astype(bool))
 
 
 def layernorm_e4m3(x, eps=1e-6):
@@ -741,6 +855,16 @@ class Frames:
             self.items = frame_list(frames, device)
             self.sizes = [(f.shape[0], f.shape[1]) for f in self.items]
         self.device = self.items[0][0].device if self.nv12 else self.items[0].device
+
+    def select(self, rows):
+        """The frames at positions `rows`, as one Frames (nothing copied)."""
+        out = Frames.__new__(Frames)
+        out.__dict__.update(self.__dict__)
+        out.items = [self.items[i] for i in rows]
+        out.sizes = [self.sizes[i] for i in rows]
+        if self.nv12:
+            out.codes = [self.codes[i] for i in rows]
+        return out
 
     def descs(self, dsts):
         """ctypes pointer to the HOST array of lwdetr_frame / lwdetr_frame_nv12 for these frames and their (dst_h, dst_w)."""

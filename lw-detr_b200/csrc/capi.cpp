@@ -15,6 +15,7 @@
 #include "attn.h"
 #include "engine.h"
 #include "gemm_tc.h"
+#include "gmc.h"
 #include "msda.h"
 #include "resize.h"
 #include "rowops.h"
@@ -389,23 +390,39 @@ int lwdetr_tracker_reset(lwdetr_tracker* t, const int32_t* streams, int n, void*
   return 0;
 }
 
+static int track_common(const char* name, lwdetr_tracker* t, const float* scores, const int32_t* labels, const float* boxes,
+                        const double* motion, int B, int k, const int32_t* stream_ids, int max_out, int32_t* out_ids, float* out_scores,
+                        int32_t* out_labels, float* out_boxes, int32_t* out_index, int32_t* counts, void* stream) {
+  const std::string fn(name);
+  if (!t || !scores || !labels || !boxes || !stream_ids || !out_ids || !out_scores || !out_labels || !out_boxes || !out_index || !counts)
+    return fail(fn + ": null pointer");
+  if (B < 1 || k < 1 || k > lwb::TRACK_MAX || max_out < 1) return fail(fn + ": need B >= 1, k in [1, 1024] and max_out >= 1");
+  if (reinterpret_cast<uintptr_t>(boxes) % 16 || reinterpret_cast<uintptr_t>(out_boxes) % 16)
+    return fail(fn + ": boxes and out_boxes must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(motion) % 8) return fail(fn + ": motion must be 8-byte aligned");
+  const std::string err = check_streams(t, stream_ids, B);
+  if (!err.empty()) return fail(fn + ": " + err);
+  lwb::DeviceGuard g(t->device);
+  int e = lwb::track_launch(t->table, t->params, scores, labels, boxes, motion, B, k, stream_ids, max_out, out_ids, out_scores, out_labels,
+                            out_boxes, out_index, counts, static_cast<cudaStream_t>(stream));
+  if (e == -2) return fail(fn + ": a limit is exceeded");
+  if (!e) e = tracker_mark(t, stream);
+  if (e) return cuda_fail(e, (fn + " launch").c_str());
+  return 0;
+}
+
 int lwdetr_track(lwdetr_tracker* t, const float* scores, const int32_t* labels, const float* boxes, int B, int k, const int32_t* stream_ids,
                  int max_out, int32_t* out_ids, float* out_scores, int32_t* out_labels, float* out_boxes, int32_t* out_index,
                  int32_t* counts, void* stream) {
-  if (!t || !scores || !labels || !boxes || !stream_ids || !out_ids || !out_scores || !out_labels || !out_boxes || !out_index || !counts)
-    return fail("lwdetr_track: null pointer");
-  if (B < 1 || k < 1 || k > lwb::TRACK_MAX || max_out < 1) return fail("lwdetr_track: need B >= 1, k in [1, 1024] and max_out >= 1");
-  if (reinterpret_cast<uintptr_t>(boxes) % 16 || reinterpret_cast<uintptr_t>(out_boxes) % 16)
-    return fail("lwdetr_track: boxes and out_boxes must be 16-byte aligned");
-  const std::string err = check_streams(t, stream_ids, B);
-  if (!err.empty()) return fail("lwdetr_track: " + err);
-  lwb::DeviceGuard g(t->device);
-  int e = lwb::track_launch(t->table, t->params, scores, labels, boxes, B, k, stream_ids, max_out, out_ids, out_scores, out_labels,
-                            out_boxes, out_index, counts, static_cast<cudaStream_t>(stream));
-  if (e == -2) return fail("lwdetr_track: a limit is exceeded");
-  if (!e) e = tracker_mark(t, stream);
-  if (e) return cuda_fail(e, "lwdetr_track launch");
-  return 0;
+  return track_common("lwdetr_track", t, scores, labels, boxes, nullptr, B, k, stream_ids, max_out, out_ids, out_scores, out_labels,
+                      out_boxes, out_index, counts, stream);
+}
+
+int lwdetr_track_ex(lwdetr_tracker* t, const float* scores, const int32_t* labels, const float* boxes, const double* motion, int B, int k,
+                    const int32_t* stream_ids, int max_out, int32_t* out_ids, float* out_scores, int32_t* out_labels, float* out_boxes,
+                    int32_t* out_index, int32_t* counts, void* stream) {
+  return track_common("lwdetr_track_ex", t, scores, labels, boxes, motion, B, k, stream_ids, max_out, out_ids, out_scores, out_labels,
+                      out_boxes, out_index, counts, stream);
 }
 
 int lwdetr_tracker_export(lwdetr_tracker* t, int stream_id, lwdetr_track_record* host, int cap, int32_t* count, int32_t frame_next_overflow[3]) {
@@ -430,6 +447,191 @@ int lwdetr_tracker_export(lwdetr_tracker* t, int stream_id, lwdetr_track_record*
   frame_next_overflow[1] = h.next_id;
   frame_next_overflow[2] = h.overflow;
   return 0;
+}
+
+struct lwdetr_gmc {
+  lwb::GmcTable table;
+  int device;
+};
+
+void lwdetr_gmc_params_default(lwdetr_gmc_params* p) {
+  if (!p) return;
+  p->downscale = 2;
+  p->max_points = 1024;
+  p->quality = 0.01f;
+  p->levels = 3;
+  p->window = 21;
+  p->iterations = 30;
+  p->eps = 0.01f;
+  p->min_eig = 1e-4f;
+  p->ransac_thresh = 3.0f;
+  p->hypotheses = 1024;
+  p->min_inliers = 10;
+  p->max_height = 2160;
+  p->max_width = 3840;
+}
+
+int lwdetr_gmc_create(int num_streams, const lwdetr_gmc_params* params, lwdetr_gmc** out) {
+  if (!params || !out) return fail("lwdetr_gmc_create: null pointer");
+  const lwdetr_gmc_params& p = *params;
+  if (num_streams < 1) return fail("lwdetr_gmc_create: num_streams must be >= 1");
+  if (p.downscale < 1 || p.downscale > 8) return fail("lwdetr_gmc_create: downscale must be in [1, 8]");
+  if (p.max_points < 16 || p.max_points > lwb::GMC_MAX_POINTS) return fail("lwdetr_gmc_create: max_points must be in [16, 4096]");
+  if (!(p.quality > 0.f && p.quality <= 1.f)) return fail("lwdetr_gmc_create: quality must be in (0, 1]");
+  if (p.levels < 0 || p.levels > lwb::GMC_MAX_LEVELS) return fail("lwdetr_gmc_create: levels must be in [0, 5]");
+  if (p.window < 5 || p.window > lwb::GMC_MAX_WINDOW || p.window % 2 == 0) return fail("lwdetr_gmc_create: window must be odd in [5, 31]");
+  if (p.iterations < 1 || p.iterations > 100) return fail("lwdetr_gmc_create: iterations must be in [1, 100]");
+  if (!(p.eps > 0.f && p.eps < 1e30f) || !(p.min_eig >= 0.f && p.min_eig < 1e30f) || !(p.ransac_thresh > 0.f && p.ransac_thresh < 1e30f))
+    return fail("lwdetr_gmc_create: need eps > 0, min_eig >= 0 and ransac_thresh > 0, all finite");
+  if (p.hypotheses < 1 || p.hypotheses > lwb::GMC_MAX_HYPOTHESES) return fail("lwdetr_gmc_create: hypotheses must be in [1, 4096]");
+  if (p.min_inliers < 2 || p.min_inliers > p.max_points) return fail("lwdetr_gmc_create: min_inliers must be in [2, max_points]");
+  const int lo = lwb::GMC_MIN_SIDE * p.downscale;
+  if (p.max_height < lo || p.max_width < lo || p.max_height > 8192 || p.max_width > 8192)
+    return fail("lwdetr_gmc_create: max_height and max_width must be in [16 * downscale, 8192]");
+  lwdetr_gmc* g = new (std::nothrow) lwdetr_gmc;
+  if (!g) return fail("lwdetr_gmc_create: out of memory");
+  lwb::GmcTable& t = g->table;
+  t = lwb::GmcTable{};
+  t.num_streams = num_streams;
+  t.p = p;
+  if (cudaGetDevice(&g->device) != cudaSuccess) { delete g; return fail("lwdetr_gmc_create: no CUDA device (there is no CPU fallback)"); }
+  lwb::GmcGeo geo;
+  lwb::gmc_geometry(p.max_height, p.max_width, p, &geo);
+  long long off = 0;
+  for (int l = 0; l <= lwb::GMC_MAX_LEVELS; ++l) {
+    t.off[l] = off;
+    if (l <= p.levels) off += (static_cast<long long>(geo.lw[l]) * geo.lh[l] + 15) / 16 * 16;
+  }
+  t.slot_bytes = off;
+  const size_t ns = static_cast<size_t>(num_streams), mp = static_cast<size_t>(p.max_points);
+  cudaError_t e = cudaMalloc(&t.head, ns * sizeof(lwb::GmcHead));
+  if (e == cudaSuccess) e = cudaMalloc(&t.pyr, ns * 2 * static_cast<size_t>(t.slot_bytes));
+  if (e == cudaSuccess) e = cudaMalloc(&t.pts, ns * 2 * mp * sizeof(float2));
+  if (e == cudaSuccess) e = cudaMalloc(&t.cell_r, ns * mp * sizeof(double));
+  if (e == cudaSuccess) e = cudaMalloc(&t.cell_i, ns * mp * sizeof(int32_t));
+  if (e == cudaSuccess) e = cudaMalloc(&t.flow, ns * mp * sizeof(float4));
+  if (e == cudaSuccess) e = cudaMalloc(&t.found, ns * mp);
+  if (e == cudaSuccess) e = cudaMemset(t.head, 0, ns * sizeof(lwb::GmcHead));
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) {
+    lwdetr_gmc_destroy(g);
+    return cuda_fail(e, "lwdetr_gmc_create");
+  }
+  *out = g;
+  return 0;
+}
+
+void lwdetr_gmc_destroy(lwdetr_gmc* g) {
+  if (!g) return;
+  lwb::DeviceGuard dg(g->device);
+  lwb::GmcTable& t = g->table;
+  cudaFree(t.head);
+  cudaFree(t.pyr);
+  cudaFree(t.pts);
+  cudaFree(t.cell_r);
+  cudaFree(t.cell_i);
+  cudaFree(t.flow);
+  cudaFree(t.found);
+  delete g;
+}
+
+static std::string check_ids(int num_streams, const int32_t* ids, int n) {
+  std::vector<char> seen(static_cast<size_t>(num_streams), 0);
+  for (int i = 0; i < n; ++i) {
+    if (ids[i] < 0 || ids[i] >= num_streams)
+      return "stream id " + std::to_string(ids[i]) + " outside [0, " + std::to_string(num_streams) + ")";
+    if (seen[ids[i]]++) return "stream id " + std::to_string(ids[i]) + " appears twice in one call";
+  }
+  return "";
+}
+
+int lwdetr_gmc_reset(lwdetr_gmc* g, const int32_t* streams, int n, void* stream) {
+  if (!g || (n > 0 && !streams)) return fail("lwdetr_gmc_reset: null pointer");
+  if (n < 0) return fail("lwdetr_gmc_reset: n must be >= 0");
+  const std::string err = check_ids(g->table.num_streams, streams, n);
+  if (!err.empty()) return fail("lwdetr_gmc_reset: " + err);
+  if (n == 0) return 0;
+  lwb::DeviceGuard dg(g->device);
+  if (int e = lwb::gmc_reset_launch(g->table, streams, n, static_cast<cudaStream_t>(stream))) return cuda_fail(e, "lwdetr_gmc_reset launch");
+  return 0;
+}
+
+int lwdetr_gmc_export(lwdetr_gmc* g, int stream_id, uint8_t* levels, int64_t levels_bytes, float* corners, float* flow, int8_t* found,
+                      int32_t info[6]) {
+  if (!g || !info || (levels_bytes > 0 && !levels) || !corners || !flow || !found) return fail("lwdetr_gmc_export: null pointer");
+  const lwb::GmcTable& t = g->table;
+  if (stream_id < 0 || stream_id >= t.num_streams) return fail("lwdetr_gmc_export: stream id outside [0, num_streams)");
+  lwb::DeviceGuard dg(g->device);
+  lwb::GmcHead h;
+  cudaError_t e = cudaDeviceSynchronize();
+  if (e == cudaSuccess) e = cudaMemcpy(&h, t.head + stream_id, sizeof(h), cudaMemcpyDeviceToHost);
+  if (e != cudaSuccess) return cuda_fail(e, "lwdetr_gmc_export");
+  lwb::GmcGeo geo;
+  lwb::gmc_geometry(h.valid ? h.h : lwb::GMC_MIN_SIDE * t.p.downscale, h.valid ? h.w : lwb::GMC_MIN_SIDE * t.p.downscale, t.p, &geo);
+  const int nlev = h.valid ? geo.nlev : -1;
+  long long need = 0;
+  for (int l = 0; l <= nlev; ++l) need += static_cast<long long>(geo.lw[l]) * geo.lh[l];
+  if (need > levels_bytes) return fail("lwdetr_gmc_export: levels buffer too small");
+  const size_t mp = static_cast<size_t>(t.p.max_points), sid = static_cast<size_t>(stream_id);
+  const uint8_t* slot = t.pyr + (sid * 2 + h.cur) * static_cast<size_t>(t.slot_bytes);
+  long long o = 0;
+  for (int l = 0; l <= nlev && e == cudaSuccess; ++l) {
+    const size_t n = static_cast<size_t>(geo.lw[l]) * geo.lh[l];
+    e = cudaMemcpy(levels + o, slot + t.off[l], n, cudaMemcpyDeviceToHost);
+    o += static_cast<long long>(n);
+  }
+  if (e == cudaSuccess) e = cudaMemcpy(corners, t.pts + (sid * 2 + h.cur) * mp, mp * sizeof(float2), cudaMemcpyDeviceToHost);
+  if (e == cudaSuccess) e = cudaMemcpy(flow, t.flow + sid * mp, mp * sizeof(float4), cudaMemcpyDeviceToHost);
+  if (e == cudaSuccess) e = cudaMemcpy(found, t.found + sid * mp, mp, cudaMemcpyDeviceToHost);
+  if (e != cudaSuccess) return cuda_fail(e, "lwdetr_gmc_export");
+  info[0] = h.valid;
+  info[1] = h.h;
+  info[2] = h.w;
+  info[3] = nlev;
+  info[4] = h.npts[h.cur];
+  info[5] = h.npts[h.cur ^ 1];
+  return 0;
+}
+
+static int gmc_estimate_common(const char* name, lwdetr_gmc* g, const std::vector<lwb::GmcFrameHost>& fr, int B, const int32_t* stream_ids,
+                               double* motion, int32_t* status, int32_t* inliers, void* stream) {
+  const std::string fn(name);
+  if (!motion || !status || !inliers) return fail(fn + ": null pointer");
+  if (reinterpret_cast<uintptr_t>(motion) % 8) return fail(fn + ": motion must be 8-byte aligned");
+  const std::string err = check_ids(g->table.num_streams, stream_ids, B);
+  if (!err.empty()) return fail(fn + ": " + err);
+  const lwdetr_gmc_params& p = g->table.p;
+  const int lo = lwb::GMC_MIN_SIDE * p.downscale;
+  for (int i = 0; i < B; ++i) {
+    const lwb::GmcFrameHost& f = fr[i];
+    if (!f.data) return fail(fn + ": null frame pointer");
+    if (f.h < lo || f.w < lo || f.h > p.max_height || f.w > p.max_width)
+      return fail(fn + ": frame " + std::to_string(i) + " is " + std::to_string(f.h) + " x " + std::to_string(f.w) + "; sides must be in [" +
+                  std::to_string(lo) + ", max_height / max_width = " + std::to_string(p.max_height) + " x " + std::to_string(p.max_width) + "]");
+    if (f.pitch < static_cast<long long>(f.w) * (f.nv12 ? 1 : 3)) return fail(fn + ": frame " + std::to_string(i) + ": pitch too small");
+  }
+  lwb::DeviceGuard dg(g->device);
+  if (int e = lwb::gmc_estimate_launch(g->table, fr.data(), B, stream_ids, motion, status, inliers, static_cast<cudaStream_t>(stream)))
+    return cuda_fail(e, (fn + " launch").c_str());
+  return 0;
+}
+
+int lwdetr_gmc_estimate(lwdetr_gmc* g, const lwdetr_frame* frames, int B, const int32_t* stream_ids, double* motion, int32_t* status,
+                        int32_t* inliers, void* stream) {
+  if (!g || !frames || !stream_ids) return fail("lwdetr_gmc_estimate: null pointer");
+  if (B < 1) return fail("lwdetr_gmc_estimate: B must be >= 1");
+  std::vector<lwb::GmcFrameHost> fr(static_cast<size_t>(B));
+  for (int i = 0; i < B; ++i) fr[i] = lwb::GmcFrameHost{frames[i].data, frames[i].pitch_bytes, frames[i].height, frames[i].width, 0};
+  return gmc_estimate_common("lwdetr_gmc_estimate", g, fr, B, stream_ids, motion, status, inliers, stream);
+}
+
+int lwdetr_gmc_estimate_nv12(lwdetr_gmc* g, const lwdetr_frame_nv12* frames, int B, const int32_t* stream_ids, double* motion,
+                             int32_t* status, int32_t* inliers, void* stream) {
+  if (!g || !frames || !stream_ids) return fail("lwdetr_gmc_estimate_nv12: null pointer");
+  if (B < 1) return fail("lwdetr_gmc_estimate_nv12: B must be >= 1");
+  std::vector<lwb::GmcFrameHost> fr(static_cast<size_t>(B));
+  for (int i = 0; i < B; ++i) fr[i] = lwb::GmcFrameHost{frames[i].luma, frames[i].luma_pitch, frames[i].height, frames[i].width, 1};
+  return gmc_estimate_common("lwdetr_gmc_estimate_nv12", g, fr, B, stream_ids, motion, status, inliers, stream);
 }
 
 int lwdetr_query_best(const float* pred_logits, const float* pred_boxes, const float* target_sizes, int B, int nq, int num_classes,

@@ -4,6 +4,7 @@
 // copies nothing and replays correctly from a CUDA graph.  Per frame:
 //   1. the frame's entries and the stream's records are loaded; the pool (confirmed tracks, then lost ones) is predicted,
 //      one thread per track, in float64 with every operation rounded on its own (__dadd_rn / __dmul_rn / __ddiv_rn);
+//      with a camera motion (lwdetr_track_ex) every record is then warped by the frame's similarity;
 //   2. each association lists its admissible (track, detection) pairs, finds the connected components by label
 //      propagation in shared memory, sorts the nodes by (component, index) and gives each component to one warp, which
 //      runs the shortest-augmenting-path Hungarian method on it: lanes scan the component's columns (costs recomputed on
@@ -43,6 +44,7 @@ struct TrackArgs {
   int32_t* counts;
   TrackHead* head;
   lwdetr_track_record* rec;
+  const double* motion;                  // [rows][4] (a, b, tx, ty) or null
   float track_thresh, low_thresh, new_thresh, match_thresh, second_thresh, unconf_thresh, dup_thresh;
   int k, max_out, capacity, max_time_lost, fuse, class_aware, row0;
   int stream[LAUNCH_STREAMS];            // stream of CTA i: batch row row0 + i
@@ -69,6 +71,7 @@ __device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a,
 __device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
 __device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
 __device__ __forceinline__ double ddiv(double a, double b) { return __ddiv_rn(a, b); }
+__device__ __forceinline__ double dsqrt(double a) { return __dsqrt_rn(a); }
 
 struct KState {
   double p[4], v[4], P[4], C[4], V[4];
@@ -133,6 +136,26 @@ __device__ void predict(KState& s, bool tracked) {
     s.P[q] = dadd(dadd(dadd(s.P[q], dadd(s.C[q], s.C[q])), s.V[q]), dmul(sp, sp));
     s.C[q] = dadd(s.C[q], s.V[q]);
     s.V[q] = dadd(s.V[q], dmul(sv, sv));
+  }
+}
+
+// camera motion x' = a x - b y + tx, y' = b x + a y + ty applied to the state.  s = sqrt(a^2 + b^2); x, y and h scale by s,
+// so their (P, C, V) scale by s^2 (the x and y blocks are equal, so the rotation leaves them diagonal); the aspect keeps its own.
+__device__ void warp_state(KState& s, const double* m) {
+  const double a = m[0], b = m[1];
+  const double s2 = dadd(dmul(a, a), dmul(b, b)), sc = dsqrt(s2);
+  const double cx = s.p[0], cy = s.p[1], vx = s.v[0], vy = s.v[1];
+  s.p[0] = dadd(dsub(dmul(a, cx), dmul(b, cy)), m[2]);
+  s.p[1] = dadd(dadd(dmul(b, cx), dmul(a, cy)), m[3]);
+  s.v[0] = dsub(dmul(a, vx), dmul(b, vy));
+  s.v[1] = dadd(dmul(b, vx), dmul(a, vy));
+  s.p[3] = dmul(sc, s.p[3]);
+  s.v[3] = dmul(sc, s.v[3]);
+  const int scaled[3] = {0, 1, 3};
+  for (int q : scaled) {
+    s.P[q] = dmul(s2, s.P[q]);
+    s.C[q] = dmul(s2, s.C[q]);
+    s.V[q] = dmul(s2, s.V[q]);
   }
 }
 
@@ -418,10 +441,9 @@ __global__ void __launch_bounds__(NT, 1) track_kernel(const __grid_constant__ Tr
     const bool lost = sl >= nT, act = r.activated != 0;
     KState ks;
     load_state(r, ks);
-    if (lost || act) {
-      predict(ks, !lost);
-      store_state(r, ks);
-    }
+    if (lost || act) predict(ks, !lost);
+    if (a.motion) warp_state(ks, a.motion + row * 4);
+    if (lost || act || a.motion) store_state(r, ks);
     S.tbox[sl] = state_box(ks.p);
     S.tlab[sl] = r.label;
     S.tdiff[sl] = r.end_frame - r.start_frame;
@@ -651,7 +673,7 @@ __global__ void query_best_kernel(const float* __restrict__ logits, const float*
 }  // namespace
 
 int track_launch(const TrackTable& t, const lwdetr_track_params& p, const float* scores, const int32_t* labels, const float* boxes,
-                 int B, int k, const int32_t* streams, int max_out, int32_t* out_ids, float* out_scores, int32_t* out_labels,
+                 const double* motion, int B, int k, const int32_t* streams, int max_out, int32_t* out_ids, float* out_scores, int32_t* out_labels,
                  float* out_boxes, int32_t* out_index, int32_t* counts, cudaStream_t st) {
   if (B < 1 || k < 1 || k > TRACK_MAX || max_out < 1) return -2;
   const int smem = static_cast<int>(sizeof(Smem));
@@ -669,6 +691,7 @@ int track_launch(const TrackTable& t, const lwdetr_track_params& p, const float*
   a.counts = counts;
   a.head = t.head;
   a.rec = t.rec;
+  a.motion = motion;
   a.track_thresh = p.track_thresh;
   a.low_thresh = p.low_thresh;
   a.new_thresh = p.new_track_thresh;

@@ -21,8 +21,9 @@ struct TrackTable {
 };
 
 // -2: a limit is exceeded (k, streams); otherwise a cudaError_t.  streams: HOST, B distinct ids in [0, num_streams).
+// motion: DEVICE [B][4] camera motion of each frame (lwdetr_track_ex), or null.
 int track_launch(const TrackTable& t, const lwdetr_track_params& p, const float* scores, const int32_t* labels, const float* boxes,
-                 int B, int k, const int32_t* streams, int max_out, int32_t* out_ids, float* out_scores, int32_t* out_labels,
+                 const double* motion, int B, int k, const int32_t* streams, int max_out, int32_t* out_ids, float* out_scores, int32_t* out_labels,
                  float* out_boxes, int32_t* out_index, int32_t* counts, cudaStream_t st);
 // frame and next id back to 1, lists emptied, overflow count 0, for n HOST stream ids
 int track_reset_launch(const TrackTable& t, const int32_t* streams, int n, cudaStream_t st);

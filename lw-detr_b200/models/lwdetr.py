@@ -206,7 +206,7 @@ class LWDETR(nn.Module):
 
     @torch.no_grad()
     def track(self, frames, tracker, streams=None, size=None, fit="stretch", short_side=None, max_side=None, colorspace=None,
-              max_out=None):
+              max_out=None, motion=None):
         """Multi-object tracking of video streams: frames (RGB or NV12, taken exactly as detect() takes them) run as one
         forward; each query gives one detection, its best class (capi.query_best, boxes in the frame's original pixels);
         then capi.Tracker `tracker` (ByteTrack on the device, include/lwdetr_b200.h) updates each frame's stream.
@@ -214,8 +214,11 @@ class LWDETR(nn.Module):
         batched offline) are tracked in list order: tracker launch r takes the r-th frame of every stream.
         Returns per frame {"ids", "scores", "labels", "boxes", "queries"}: the activated tracks in ByteTrack's list order,
         cut to the frame's count (one read-back for the call), "queries" the query each track took its detection from.
-        max_out (default num_queries) bounds the tracks returned per frame.  How ByteTrack's thresholds (tuned on YOLOX
-        scores) suit LW-DETR's score distribution, in MOTA / IDF1 / HOTA, is not measured here."""
+        max_out (default num_queries) bounds the tracks returned per frame.  motion: a capi.MotionEstimator for moving
+        cameras; each frame round then estimates every frame's camera motion from the same frame descriptors (nothing
+        copied) and warps the stream's tracks by it before the association (Tracker.update(motion=...)).  How ByteTrack's
+        thresholds (tuned on YOLOX scores) suit LW-DETR's score distribution, in MOTA / IDF1 / HOTA, with or without
+        motion, is not measured here."""
         if self.training:
             raise RuntimeError("lwdetr_b200 implements the inference forward only; call model.eval()")
         dev = next(self.parameters()).device
@@ -239,8 +242,9 @@ class LWDETR(nn.Module):
         res, counts = [None] * n, []
         for rows in rounds:
             idx = torch.tensor(rows, device=dev)
-            got = tracker.update(scores[idx], labels[idx], boxes[idx], [streams[i] for i in rows],
-                                 self.num_queries if max_out is None else max_out)
+            ids = [streams[i] for i in rows]
+            mo = None if motion is None else motion.estimate(fb.select(rows), ids)[0]
+            got = tracker.update(scores[idx], labels[idx], boxes[idx], ids, self.num_queries if max_out is None else max_out, motion=mo)
             counts.append(got[5])
             for j, i in enumerate(rows):
                 res[i] = (got, j)

@@ -7,7 +7,10 @@ Everything is float64 with each operation rounded on its own (numpy does not fus
   assignment by the shortest-augmenting-path Hungarian method on the n x (m + n) matrix whose column m + i is row i's own
   "unmatched" column of cost L (solve()), which is what lap.lapjv(cost, extend_cost=True, cost_limit=L) returns up to ties.
 
-scene() is a seeded generator of synthetic detection sequences for the tests and the benchmark.
+With a camera motion (lwdetr_track_ex), warp() moves every track after the predict, in the header's operation order.
+
+scene() is a seeded generator of synthetic detection sequences for the tests and the benchmark, optionally seen through a
+moving camera (camera_path()).
 """
 import numpy as np
 
@@ -100,6 +103,28 @@ def kalman_update(t, z):
     t.P = t.P - (Kp * Kp) * S
     t.C = t.C - (Kp * Kv) * S
     t.V = t.V - (Kv * Kv) * S
+
+
+def warp(t, m):
+    """Camera motion (a, b, tx, ty) applied to a track: centre by the similarity, velocity by its linear part, h and v_h by
+    s = sqrt(a^2 + b^2), (P, C, V) of x, y and h by s^2; the aspect keeps its state."""
+    a, b, tx, ty = (np.float64(x) for x in m)
+    s2 = a * a + b * b
+    s = np.sqrt(s2)
+    p, v = t.p.copy(), t.v.copy()
+    cx, cy, vx, vy = p[0], p[1], v[0], v[1]
+    p[0] = (a * cx - b * cy) + tx
+    p[1] = (b * cx + a * cy) + ty
+    v[0] = a * vx - b * vy
+    v[1] = b * vx + a * vy
+    p[3] = s * p[3]
+    v[3] = s * v[3]
+    t.p, t.v = p, v
+    t.P, t.C, t.V = t.P.copy(), t.C.copy(), t.V.copy()
+    for q in (0, 1, 3):
+        t.P[q] = s2 * t.P[q]
+        t.C[q] = s2 * t.C[q]
+        t.V[q] = s2 * t.V[q]
 
 
 # ---------------------------------------------------------------------------------------------- costs and assignment
@@ -255,9 +280,9 @@ class Stream:
         t.state, t.activated, t.end = TRACKED, True, self.frame
         t.score, t.label, t.index = scores[d], labels[d], int(d)
 
-    def update(self, scores, labels, boxes):
+    def update(self, scores, labels, boxes, motion=None):
         """One frame: scores fp32 [k], labels int32 [k], boxes fp32 [k, 4] (xyxy) -> the output tracks, a list of
-        (id, score fp32, label, box fp32 [4], index)."""
+        (id, score fp32, label, box fp32 [4], index).  motion: the frame's camera motion (a, b, tx, ty) or None."""
         p, frame = self.p, self.frame
         scores = np.asarray(scores, np.float32).reshape(-1)
         labels = np.asarray(labels).astype(np.int32).reshape(-1)
@@ -273,6 +298,9 @@ class Stream:
         pool = [t for t in self.tracked if t.activated] + self.lost
         for t in pool:
             predict(t)
+        if motion is not None:
+            for t in self.tracked + self.lost:
+                warp(t, motion)
         # 1. pool x high detections
         m1, _, _ = solve(self._cost(pool, high, p["match_thresh"], p["fuse_score"], e), p["match_thresh"])
         refound = []
@@ -370,8 +398,50 @@ def outputs_array(outs, max_out):
 
 
 # ---------------------------------------------------------------------------------------------- synthetic scenes
+CAMERA = dict(seed=0, pan=10.0, shake=4.0, zoom=0.004, rotate=0.15)
+
+
+def camera_path(frames, size, seed=0, pan=10.0, shake=4.0, zoom=0.004, rotate=0.15):
+    """A seeded moving camera: per frame the similarity (a, b, tx, ty) from the previous frame's pixels to this one's
+    (frame 0: the identity).  Pans of +-pan px per frame (one third of it vertically) that start and stop abruptly every 10
+    to 40 frames and turn back before the view drifts far, hand shake of `shake` px (std of the camera's offset), a slow
+    zoom with per-frame log-scale std `zoom` and a slow roll with per-frame std `rotate` degrees, both about the frame
+    centre.  Returns float64 [frames, 4]."""
+    rng = np.random.default_rng(seed)
+    H, W = size
+    cx, cy = W / 2.0, H / 2.0
+    out = np.zeros((frames, 4))
+    out[0] = (1.0, 0.0, 0.0, 0.0)
+    off = np.zeros(2)
+    vel = np.zeros(2)
+    left = 0
+    jit = np.zeros(2)
+    ls = th = 0.0
+    for f in range(1, frames):
+        if left == 0:
+            left = int(rng.integers(10, 41))
+            choice = int(rng.integers(-1, 2))
+            if abs(off[0]) > 0.15 * W:
+                choice = -int(np.sign(off[0]))
+            vel = np.array([choice * pan, rng.choice([-1, 0, 1]) * pan / 3])
+            if abs(off[1]) > 0.15 * H:
+                vel[1] = -np.sign(off[1]) * pan / 3
+        left -= 1
+        off = off + vel
+        j = rng.normal(0, shake, 2)
+        dls = 0.9 * ls + rng.normal(0, zoom) - ls
+        dth = 0.9 * th + rng.normal(0, rotate) - th
+        ls, th = ls + dls, th + dth
+        s, t = np.exp(dls), np.deg2rad(dth)
+        a, b = s * np.cos(t), s * np.sin(t)
+        d = vel + j - jit
+        jit = j
+        out[f] = (a, b, cx - (a * cx - b * cy) + d[0], cy - (b * cx + a * cy) + d[1])
+    return out
+
+
 def scene(seed, frames, objects=20, k=None, ncls=3, size=(1080, 1920), clutter=3, miss=0.05, low_dip=0.1, occlusion=0.02,
-          crossing=True, echo=0.0):
+          crossing=True, echo=0.0, camera=None, truth=False):
     """Seeded synthetic detections: `objects` ground-truth boxes alive at a time on average, moving at constant velocity with
     small accelerations, born and dying over the sequence; per frame each visible object gives a detection with jitter
     (score mostly high, dipping into the low band with probability low_dip), is missed with probability `miss`, and starts
@@ -381,16 +451,25 @@ def scene(seed, frames, objects=20, k=None, ncls=3, size=(1080, 1920), clutter=3
     pixels to the side (IoU about 0.9 with the first): such echoes start tracks on top of tracks, which the duplicate removal
     between the tracked and the lost list then resolves.  Returns a
     list of (scores fp32 [k_f], labels int32 [k_f], boxes fp32 [k_f, 4]) in shuffled order, or with k given, padded to k
-    entries (score 0, zero box) or cut to its first k."""
+    entries (score 0, zero box) or cut to its first k.
+    camera (a dict of camera_path's options, CAMERA the defaults): the same objects and detections seen through a moving
+    camera; every box is mapped by the camera's accumulated similarity (centre by the similarity, sides by its scale).  The
+    camera draws from its own generator, so the scene's draws are those of the still scene.  truth: also give the object of
+    each entry (int32 per entry, -1 for clutter and echoes).  With camera or truth the result is (frames, motion float64
+    [frames, 4] or None, truth or None)."""
     rng = np.random.default_rng(seed)
     H, W = size
     objs = []
+    gid = [0]
+    motion = None if camera is None else camera_path(frames, size, **camera)
+    cam = np.array([1.0, 0.0, 0.0, 0.0])
 
     def spawn(t0):
         h = rng.uniform(30, 300)
         w = h * rng.uniform(0.3, 1.2)
         o = dict(cx=rng.uniform(w, W - w), cy=rng.uniform(h, H - h), w=w, h=h, vx=rng.normal(0, 4), vy=rng.normal(0, 2),
-                 label=int(rng.integers(ncls)), die=t0 + int(rng.integers(40, 4 * frames + 40)), hidden=0)
+                 label=int(rng.integers(ncls)), die=t0 + int(rng.integers(40, 4 * frames + 40)), hidden=0, gid=gid[0])
+        gid[0] += 1
         objs.append(o)
     for _ in range(objects):
         spawn(0)
@@ -398,8 +477,12 @@ def scene(seed, frames, objects=20, k=None, ncls=3, size=(1080, 1920), clutter=3
         a, b = objs[0], objs[1]
         a.update(cx=W * 0.3, cy=H * 0.5, vx=6.0, vy=0.0)
         b.update(cx=W * 0.7, cy=H * 0.5 + 10, vx=-6.0, vy=0.0, h=a["h"] * 1.1, w=a["w"] * 0.9)
-    out = []
+    out, gts = [], []
     for f in range(frames):
+        if motion is not None:                 # accumulated camera: the previous one followed by this frame's motion
+            a, b, tx, ty = motion[f]
+            ca, cb, ctx, cty = cam
+            cam = np.array([a * ca - b * cb, b * ca + a * cb, (a * ctx - b * cty) + tx, (b * ctx + a * cty) + ty])
         objs = [o for o in objs if o["die"] > f and -o["w"] < o["cx"] < W + o["w"] and -o["h"] < o["cy"] < H + o["h"]]
         while len(objs) < objects and rng.random() < 0.3:
             spawn(f)
@@ -421,7 +504,7 @@ def scene(seed, frames, objects=20, k=None, ncls=3, size=(1080, 1920), clutter=3
             cx, cy = o["cx"] + rng.normal(0, j), o["cy"] + rng.normal(0, j)
             w, h = o["w"] * (1 + rng.normal(0, 0.03)), o["h"] * (1 + rng.normal(0, 0.03))
             s = rng.uniform(0.15, 0.5) if rng.random() < low_dip else rng.uniform(0.55, 0.98)
-            det.append((s, o["label"], cx - w / 2, cy - h / 2, cx + w / 2, cy + h / 2))
+            det.append((s, o["label"], cx - w / 2, cy - h / 2, cx + w / 2, cy + h / 2, o["gid"]))
             if echo > 0:
                 if o.get("echo", 0) == 0 and rng.random() < echo:
                     o["echo"] = int(rng.integers(2, 12))
@@ -429,16 +512,43 @@ def scene(seed, frames, objects=20, k=None, ncls=3, size=(1080, 1920), clutter=3
                     o["echo"] -= 1
                     dx = 0.025 * w * (1 + rng.normal(0, 0.1))
                     ew, eh = w * (1 + rng.normal(0, 0.01)), h * (1 + rng.normal(0, 0.01))     # its own size: no exact IoU ties
-                    det.append((rng.uniform(0.65, 0.98), o["label"], cx + dx - ew / 2, cy - eh / 2, cx + dx + ew / 2, cy + eh / 2))
+                    det.append((rng.uniform(0.65, 0.98), o["label"], cx + dx - ew / 2, cy - eh / 2, cx + dx + ew / 2, cy + eh / 2, -1))
         for _ in range(rng.poisson(clutter)):
             h = rng.uniform(20, 200)
             w = h * rng.uniform(0.3, 1.5)
             x, y = rng.uniform(0, W - w), rng.uniform(0, H - h)
-            det.append((rng.uniform(0.05, 0.65), int(rng.integers(ncls)), x, y, x + w, y + h))
+            det.append((rng.uniform(0.05, 0.65), int(rng.integers(ncls)), x, y, x + w, y + h, -1))
         rng.shuffle(det)
-        a = np.array(det, np.float64).reshape(-1, 6)
-        out.append(pad(a[:, 0].astype(np.float32), a[:, 1].astype(np.int32), a[:, 2:].astype(np.float32), k))
-    return out
+        a = np.array(det, np.float64).reshape(-1, 7)
+        bx = a[:, 2:6]
+        if motion is not None:
+            ca, cb, ctx, cty = cam
+            s = np.sqrt(ca * ca + cb * cb)
+            mx, my = (bx[:, 0] + bx[:, 2]) / 2, (bx[:, 1] + bx[:, 3]) / 2
+            hw, hh = s * (bx[:, 2] - bx[:, 0]) / 2, s * (bx[:, 3] - bx[:, 1]) / 2
+            nx, ny = (ca * mx - cb * my) + ctx, (cb * mx + ca * my) + cty
+            bx = np.stack([nx - hw, ny - hh, nx + hw, ny + hh], 1)
+        out.append(pad(a[:, 0].astype(np.float32), a[:, 1].astype(np.int32), bx.astype(np.float32), k))
+        g = a[:, 6].astype(np.int32)
+        gts.append(g if k is None else np.r_[g, np.full(max(0, k - len(g)), -1, np.int32)][:k])
+    if camera is None and not truth:
+        return out
+    return out, motion, (gts if truth else None)
+
+
+def id_switches(stream_outputs, truth):
+    """Identity switches over a sequence: outputs of Stream.update per frame and the true object of each entry; a switch is
+    an object whose matched track id differs from the id it last had."""
+    last, n = {}, 0
+    for outs, g in zip(stream_outputs, truth):
+        for tid, _, _, _, idx in outs:
+            o = int(g[idx])
+            if o < 0:
+                continue
+            if o in last and last[o] != tid:
+                n += 1
+            last[o] = tid
+    return n
 
 
 def pad(scores, labels, boxes, k):
