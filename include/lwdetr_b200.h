@@ -369,6 +369,56 @@ LWDETR_API int lwdetr_track_ex(lwdetr_tracker* t, const float* scores, const int
                                int B, int k, const int32_t* stream_ids, int max_out, int32_t* out_ids, float* out_scores,
                                int32_t* out_labels, float* out_boxes, int32_t* out_index, int32_t* counts, void* stream);
 
+/* Tracking by appearance: BoT-SORT's re-identification cost (the with_reid path of BoTSORT.update, its defaults) on top of
+ * the contract above, with an embedding per entry - the decoder's last hidden state of each query (lwdetr_last_hidden; the
+ * C composition is lwdetr_forward_frames -> lwdetr_last_hidden -> lwdetr_query_best -> lwdetr_track_reid) or any ReID
+ * model's.  The restatement in numpy is tools/track_spec.py (Stream with reid_params()).
+ * Parameters (lwdetr_reid_params_default: D = 256 and BoT-SORT's 0.5 / 0.25 / 0.9): embedding_dim D in [1, 2048],
+ * proximity_thresh in [0, 1), appearance_thresh in [0, 1], ema_alpha in [0, 1]; all fp32, widened.
+ * Fixed order: the sum of D float64 terms is taken as 32 partial sums from 0, partial j adding terms j, j + 32, ... in
+ * ascending order, combined by the xor butterfly 16, 8, 4, 2, 1 (partial j + partial j ^ o); norm |x| = sqrt(sum x_i * x_i),
+ * dot(x, y) = sum x_i * y_i, every operation rounded on its own.
+ * Entry embedding e (D values widened exactly to float64): ne = |e|; an entry whose ne is not finite or not > 0 has no
+ * appearance.  Only high entries are looked at.
+ * Track embedding t, fp32: a birth from an entry with appearance sets t = e / ne (each element rounded to fp32); an update
+ * by a high entry with appearance (steps 2 and 4) sets t = e / ne when the track has none, else s = alpha * t + (1 - alpha)
+ * * (e / ne) per element and t = s / |s| rounded to fp32 (BoT-SORT's update_features; t unchanged when |s| is not finite
+ * or not > 0).  A low entry (step 3) leaves t as it is; a track born from an entry without appearance has none until an
+ * update gives it one.
+ * Cost in steps 2 (pool x high) and 4 (unconfirmed x high left) only; step 3 stays IoU only.  With the track's box as in
+ * the contract: emb = max(0, 1 - dot(t, e) / ne) / 2; emb' = emb when (1 - iou) <= proximity_thresh and
+ * emb <= appearance_thresh, else 1 (also 1 when either side has no appearance); cost = min(the IoU cost above, fused with
+ * the score if fuse_score, emb'); admissible iff cost < L and the class gate passes.  emb' < 1 needs iou >= 1 -
+ * proximity_thresh > 0, so an admissible pair still overlaps.
+ * Deviations from BoT-SORT: the track embedding is stored in fp32; the distance does not normalise t and e again (BoT-SORT's
+ * cdist(..., "cosine") divides by both norms); a non-finite or zero embedding means no appearance (BoT-SORT gives NaN);
+ * lwdetr_tile_merge's entries carry no embeddings.
+ *
+ * lwdetr_tracker_create_reid: lwdetr_tracker_create plus the appearance state: the embedding table (num_streams *
+ *   capacity * D * 4 bytes: one slot per track a stream can hold; a track keeps its slot for life, so nothing moves per
+ *   frame), a slot per record and a per-stream scratch of 8192 proximity pairs (12 bytes each) per frame.  Synchronous.
+ * lwdetr_track_reid: lwdetr_track_ex with embeddings DEVICE [B, k, D], row stride ld_emb >= D elements, of type emb_dtype
+ *   (LWDETR_ET_F32, _F16 or _BF16: the engine's 16-bit rows need no conversion), aligned to their element size.  NULL
+ *   embeddings, or a tracker made by lwdetr_tracker_create, give lwdetr_track_ex's bits.  Asynchronous, nothing allocated
+ *   per call, safe to capture in a CUDA graph.  lwdetr_track and lwdetr_track_ex on a tracker made by
+ *   lwdetr_tracker_create_reid are lwdetr_track_reid with NULL embeddings: the same bits, and the tracks keep their
+ *   embeddings, so the calls can be mixed on one tracker.
+ * lwdetr_tracker_export_embeddings: synchronous like lwdetr_tracker_export; the D floats of each record in that function's
+ *   order into host [cap][D], has[i] = 1 when record i has an embedding (its row is then valid), *count = the record count.
+ * lwdetr_tracker_reset also forgets the streams' embeddings. */
+typedef struct {
+  int32_t embedding_dim;
+  float proximity_thresh, appearance_thresh, ema_alpha;
+} lwdetr_reid_params;
+LWDETR_API void lwdetr_reid_params_default(lwdetr_reid_params* p);
+LWDETR_API int lwdetr_tracker_create_reid(int num_streams, const lwdetr_track_params* params, const lwdetr_reid_params* reid,
+                                          lwdetr_tracker** out);
+LWDETR_API int lwdetr_track_reid(lwdetr_tracker* t, const float* scores, const int32_t* labels, const float* boxes, const double* motion,
+                                 const void* embeddings, int emb_dtype, int ld_emb, int B, int k, const int32_t* stream_ids, int max_out,
+                                 int32_t* out_ids, float* out_scores, int32_t* out_labels, float* out_boxes, int32_t* out_index,
+                                 int32_t* counts, void* stream);
+LWDETR_API int lwdetr_tracker_export_embeddings(lwdetr_tracker* t, int stream_id, float* host, int cap, int32_t* count, int8_t* has);
+
 /* Camera-motion estimation (global motion compensation, BoT-SORT's sparseOptFlow with the deviations stated here) per video
  * stream on the device, for lwdetr_track_ex.  The C composition per batch of frames, one frame per stream:
  * lwdetr_forward_frames (or _nv12) -> lwdetr_query_best -> lwdetr_gmc_estimate (or _nv12) on the same frame descriptors ->
@@ -637,6 +687,14 @@ LWDETR_API int lwdetr_set_option(lwdetr_handle* h, const char* name, int value);
 LWDETR_API int lwdetr_add_capture(lwdetr_handle* h, const char* label, float* dst, int64_t capacity);
 LWDETR_API int64_t lwdetr_capture_result(lwdetr_handle* h, int index);
 LWDETR_API void lwdetr_clear_captures(lwdetr_handle* h);
+
+/* lwdetr_last_hidden: the last forward's final-layer decoder hidden state (after the decoder's output norm: the rows
+ * class_embed and bbox_embed read), [B, num_queries, hidden_dim] in the compute dtype (fp16 in the e4m3 mode), into DEVICE
+ * dst with a row stride of ld_dst >= hidden_dim elements.  Ordered on `stream` like the forward's own result copies, so
+ * call it on the forward's stream; the source is valid until the next forward.  It adds nothing to the forward's schedule
+ * or its CUDA graphs.  Row q of frame b is the feature of query q, i.e. of lwdetr_query_best's entry q: the built-in
+ * appearance embedding for lwdetr_track_reid (emb_dtype LWDETR_ET_F16 or _BF16). */
+LWDETR_API int lwdetr_last_hidden(lwdetr_handle* h, void* dst, int ld_dst, void* stream);
 
 /* Schedule introspection / per-op timing of the last planned batch size. */
 LWDETR_API int lwdetr_num_ops(lwdetr_handle* h);

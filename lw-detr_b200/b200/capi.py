@@ -40,6 +40,11 @@ _SIGNATURES = {
     "lwdetr_track": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_tracker_export": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
     "lwdetr_track_ex": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "lwdetr_reid_params_default": (None, [_vp]),
+    "lwdetr_tracker_create_reid": (_i, [_i, _vp, _vp, _vp]),
+    "lwdetr_track_reid": (_i, [_vp] * 6 + [_i] * 4 + [_vp, _i] + [_vp] * 7),
+    "lwdetr_tracker_export_embeddings": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
+    "lwdetr_last_hidden": (_i, [_vp, _vp, _i, _vp]),
     "lwdetr_gmc_params_default": (None, [_vp]),
     "lwdetr_gmc_create": (_i, [_i, _vp, _vp]),
     "lwdetr_gmc_destroy": (None, [_vp]),
@@ -436,15 +441,38 @@ class TrackRecord(ctypes.Structure):
                [("score", _f), ("index", ctypes.c_int32), ("mean", ctypes.c_double * 8), ("cov", ctypes.c_double * 12)]
 
 
+class ReidParams(ctypes.Structure):
+    """lwdetr_reid_params (include/lwdetr_b200.h)."""
+    _fields_ = [("embedding_dim", ctypes.c_int32), ("proximity_thresh", _f), ("appearance_thresh", _f), ("ema_alpha", _f)]
+
+
+def _emb_dtype(dtype):
+    import torch
+    codes = {torch.float32: ET_F32, torch.float16: ET_F16, torch.bfloat16: ET_BF16}
+    if dtype not in codes:
+        raise RuntimeError("Tracker.update: embeddings must be float32, float16 or bfloat16, got %s" % dtype)
+    return codes[dtype]
+
+
 class Tracker:
     """ByteTrack on the device for num_streams camera streams (lwdetr_tracker_*, the contract in include/lwdetr_b200.h).
     Parameters are lwdetr_track_params' fields, ByteTrack's defaults unless given; new_track_thresh defaults to
-    track_thresh + 0.1.  All calls of one tracker must run on one CUDA stream (the current one at each call)."""
+    track_thresh + 0.1.  With embedding_dim (lwdetr_reid_params: embedding_dim, proximity_thresh, appearance_thresh,
+    ema_alpha; BoT-SORT's defaults unless given) the tracker also associates by appearance (BoT-SORT's re-identification
+    cost, lwdetr_track_reid); update() then takes embeddings.  All calls of one tracker must run on one CUDA stream (the
+    current one at each call)."""
+
+    REID = ("embedding_dim", "proximity_thresh", "appearance_thresh", "ema_alpha")
 
     def __init__(self, num_streams, device=None, **params):
         import torch
         p = TrackParams()
         lib().lwdetr_track_params_default(ctypes.byref(p))
+        reid = {n: params.pop(n) for n in self.REID if n in params and params[n] is not None}
+        for n in self.REID:
+            params.pop(n, None)
+        if reid and "embedding_dim" not in reid:
+            raise RuntimeError("Tracker: %s given without embedding_dim" % ", ".join(sorted(reid)))
         names = {n for n, _ in TrackParams._fields_}
         bad = set(params) - names
         if bad:
@@ -457,8 +485,20 @@ class Tracker:
         self.num_streams = int(num_streams)
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         self._t = _vp()
+        self.reid = None
+        if reid:
+            r = ReidParams()
+            lib().lwdetr_reid_params_default(ctypes.byref(r))
+            for n, v in reid.items():
+                setattr(r, n, v)
+            self.reid = r
+        self.embedding_dim = int(self.reid.embedding_dim) if self.reid is not None else None
         with torch.cuda.device(self.device):
-            check(lib().lwdetr_tracker_create(self.num_streams, ctypes.byref(p), ctypes.byref(self._t)), "lwdetr_tracker_create")
+            if self.reid is None:
+                check(lib().lwdetr_tracker_create(self.num_streams, ctypes.byref(p), ctypes.byref(self._t)), "lwdetr_tracker_create")
+            else:
+                check(lib().lwdetr_tracker_create_reid(self.num_streams, ctypes.byref(p), ctypes.byref(self.reid), ctypes.byref(self._t)),
+                      "lwdetr_tracker_create_reid")
 
     def close(self):
         if self._t:
@@ -481,13 +521,15 @@ class Tracker:
         arr, n = self._ids(streams)
         check(lib().lwdetr_tracker_reset(self._t, ctypes.cast(arr, _vp), n, stream_ptr(self.device)), "lwdetr_tracker_reset")
 
-    def update(self, scores, labels, boxes, stream_ids=None, max_out=None, motion=None):
+    def update(self, scores, labels, boxes, stream_ids=None, max_out=None, motion=None, embeddings=None):
         """One frame for each of B distinct streams: scores fp32 [B, k], labels int [B, k], xyxy boxes fp32 [B, k, 4] (CUDA;
         stream_ids default range(B)) -> (ids int32 [B, max_out], scores fp32, labels int32, boxes fp32 [B, max_out, 4], index
         int32 (the entry of each track), counts int32 [B]); unused slots id 0, score 0, label -1, zero box, index -1.
         max_out defaults to k.  motion: float64 [B, 4] camera motion of each frame (MotionEstimator.estimate), which warps
-        every track of the stream after the predict (lwdetr_track_ex); None tracks as for a still camera.  Stream-ordered,
-        no synchronisation."""
+        every track of the stream after the predict (lwdetr_track_ex); None tracks as for a still camera.
+        embeddings (a tracker with embedding_dim D only): CUDA [B, k, D] float32, float16 or bfloat16, any row stride (the
+        last dimension contiguous), the appearance of each entry (lwdetr_track_reid); None: no entry has appearance, which
+        gives ByteTrack's result.  Stream-ordered, no synchronisation."""
         import torch
         B, k = scores.shape
         if tuple(labels.shape) != (B, k) or tuple(boxes.shape) != (B, k, 4):
@@ -507,13 +549,32 @@ class Tracker:
         o_b = torch.empty(B, m, 4, device=dev, dtype=torch.float32)
         o_i = torch.empty(B, m, device=dev, dtype=torch.int32)
         counts = torch.empty(B, device=dev, dtype=torch.int32)
-        if motion is None:
-            check(lib().lwdetr_track(self._t, ptr(scores), ptr(labels), ptr(boxes), B, k, ctypes.cast(ids, _vp), m, ptr(o_id), ptr(o_s),
-                                     ptr(o_l), ptr(o_b), ptr(o_i), ptr(counts), stream_ptr(dev)), "lwdetr_track")
-        else:
+        if motion is not None:
             if tuple(motion.shape) != (B, 4):
                 raise RuntimeError("Tracker.update: motion must be [%d, 4], got %s" % (B, tuple(motion.shape)))
             motion = motion.to(device=dev, dtype=torch.float64).contiguous()
+        if self.reid is not None:
+            code, ld = ET_F32, 0
+            if embeddings is not None:
+                D = self.embedding_dim
+                if tuple(embeddings.shape) != (B, k, D):
+                    raise RuntimeError("Tracker.update: embeddings must be [%d, %d, %d], got %s" % (B, k, D, tuple(embeddings.shape)))
+                if embeddings.device != dev:
+                    raise RuntimeError("Tracker.update: embeddings are on %s but the tracker lives on %s" % (embeddings.device, dev))
+                code = _emb_dtype(embeddings.dtype)
+                if embeddings.stride(2) != 1 or embeddings.stride(0) != k * embeddings.stride(1):
+                    embeddings = embeddings.contiguous()
+                ld = embeddings.stride(1)
+            check(lib().lwdetr_track_reid(self._t, ptr(scores), ptr(labels), ptr(boxes), ptr(motion), ptr(embeddings), code, ld, B, k,
+                                          ctypes.cast(ids, _vp), m, ptr(o_id), ptr(o_s), ptr(o_l), ptr(o_b), ptr(o_i), ptr(counts),
+                                          stream_ptr(dev)), "lwdetr_track_reid")
+            self._last_embeddings = embeddings      # keep alive until the stream has consumed it
+        elif embeddings is not None:
+            raise RuntimeError("Tracker.update: embeddings need a tracker made with embedding_dim")
+        elif motion is None:
+            check(lib().lwdetr_track(self._t, ptr(scores), ptr(labels), ptr(boxes), B, k, ctypes.cast(ids, _vp), m, ptr(o_id), ptr(o_s),
+                                     ptr(o_l), ptr(o_b), ptr(o_i), ptr(counts), stream_ptr(dev)), "lwdetr_track")
+        else:
             check(lib().lwdetr_track_ex(self._t, ptr(scores), ptr(labels), ptr(boxes), ptr(motion), B, k, ctypes.cast(ids, _vp), m,
                                         ptr(o_id), ptr(o_s), ptr(o_l), ptr(o_b), ptr(o_i), ptr(counts), stream_ptr(dev)), "lwdetr_track_ex")
         return o_id, o_s, o_l, o_b, o_i, counts
@@ -533,6 +594,21 @@ class Tracker:
                      label=r.label, index=r.index, mean=np.array(r.mean[:], np.float64), cov=np.array(r.cov[:], np.float64))
                 for r in arr[:min(cnt.value, cap)]]
         return recs, tuple(fno)
+
+    def export_embeddings(self, stream_id):
+        """Synchronous, a tracker with embedding_dim D only: (embeddings float32 [n, D], has bool [n]) of one stream's
+        records in export()'s order; a row is valid where has is True (the track has an embedding)."""
+        import numpy as np
+        if self.reid is None:
+            raise RuntimeError("Tracker.export_embeddings: the tracker was made without embedding_dim")
+        cap, D = int(self.params.capacity), self.embedding_dim
+        emb = np.zeros((cap, D), np.float32)
+        has = np.zeros(cap, np.int8)
+        cnt = ctypes.c_int32()
+        check(lib().lwdetr_tracker_export_embeddings(self._t, int(stream_id), emb.ctypes.data_as(_vp), cap, ctypes.byref(cnt),
+                                                     has.ctypes.data_as(_vp)), "lwdetr_tracker_export_embeddings")
+        n = min(cnt.value, cap)
+        return emb[:n], has[:n].astype(bool)
 
 
 class GmcParams(ctypes.Structure):
@@ -1041,7 +1117,7 @@ class Engine:
         return res, logits, boxes, aux
 
     def forward_frames(self, frames, size=None, fit="stretch", short_side=None, max_side=None, want_aux=True, topk_override=None,
-                       mean=IMAGENET_MEAN, std=IMAGENET_STD, colorspace=None, dsts=None):
+                       mean=IMAGENET_MEAN, std=IMAGENET_STD, colorspace=None, dsts=None, want_hidden=False):
         """Raw camera / decoder frames of any size, RGB or NV12 (told apart by their form):
           RGB: a list of CUDA uint8 [h, w, 3] tensors (each its own size; views with packed RGB pixels are fine) or one
             [B, h, w, 3] tensor;
@@ -1056,7 +1132,9 @@ class Engine:
         are not part of the plan: only a new (B, H, W) re-plans.  dsts: explicit (dst_h, dst_w) per frame, each placed
         top-left on the run size `size` (default img_size x img_size) with the padding mask (the crop views of tiled
         detection, b200.config.tile_views); fit / short_side / max_side do not apply then.  Returns the dict of forward(),
-        plus "frame_sizes": the (dst_h, dst_w) of each frame."""
+        plus "frame_sizes": the (dst_h, dst_w) of each frame, and with want_hidden "hidden": the final decoder layer's
+        hidden state [B, num_queries, hidden_dim] in the activation dtype (lwdetr_last_hidden), the rows class_embed reads;
+        row q is the feature of query q (the appearance embedding Tracker.update takes)."""
         import torch
         from .config import explicit_frame_sizes, frame_sizes
         fb = Frames(frames, self.device, colorspace)
@@ -1077,6 +1155,10 @@ class Engine:
                                    stream_ptr(self.device)), name)
         self._last_inputs = (fb.items, ov, None)    # keep alive until the stream has consumed them
         res["frame_sizes"] = dsts
+        if want_hidden:
+            hidden = torch.empty(B, self.cfg.num_queries, self.cfg.hidden_dim, device=self.device, dtype=io_dtype(self.dtype))
+            check(lib().lwdetr_last_hidden(self._h, ptr(hidden), self.cfg.hidden_dim, stream_ptr(self.device)), "lwdetr_last_hidden")
+            res["hidden"] = hidden
         return res
 
     # ---- debug captures -------------------------------------------------------------------------

@@ -279,6 +279,7 @@ static_assert(sizeof(lwdetr_track_record) == 192, "track record layout");
 
 struct lwdetr_tracker {
   lwb::TrackTable table;
+  lwb::ReidTable reid;   // embedding_dim 0 and null pointers without appearance
   lwdetr_track_params params;
   int device;
   cudaEvent_t done;      // recorded after every launch on the table (an external event node inside a CUDA graph capture)
@@ -333,6 +334,7 @@ int lwdetr_tracker_create(int num_streams, const lwdetr_track_params* params, lw
   t->table.capacity = p.capacity;
   t->table.head = nullptr;
   t->table.rec = nullptr;
+  t->reid = lwb::ReidTable{};
   t->done = nullptr;
   t->copy = nullptr;
   if (cudaGetDevice(&t->device) != cudaSuccess) { delete t; return fail("lwdetr_tracker_create: no CUDA device (there is no CPU fallback)"); }
@@ -356,10 +358,20 @@ int lwdetr_tracker_create(int num_streams, const lwdetr_track_params* params, lw
   return 0;
 }
 
+static void free_reid(lwb::ReidTable& r) {
+  cudaFree(r.slot);
+  cudaFree(r.has);
+  cudaFree(r.emb);
+  cudaFree(r.pkey);
+  cudaFree(r.pval);
+  r = lwb::ReidTable{};
+}
+
 void lwdetr_tracker_destroy(lwdetr_tracker* t) {
   if (!t) return;
   lwb::DeviceGuard g(t->device);
   cudaStreamSynchronize(t->copy);
+  free_reid(t->reid);
   cudaFree(t->table.head);
   cudaFree(t->table.rec);
   cudaEventDestroy(t->done);
@@ -392,7 +404,8 @@ int lwdetr_tracker_reset(lwdetr_tracker* t, const int32_t* streams, int n, void*
 
 static int track_common(const char* name, lwdetr_tracker* t, const float* scores, const int32_t* labels, const float* boxes,
                         const double* motion, int B, int k, const int32_t* stream_ids, int max_out, int32_t* out_ids, float* out_scores,
-                        int32_t* out_labels, float* out_boxes, int32_t* out_index, int32_t* counts, void* stream) {
+                        int32_t* out_labels, float* out_boxes, int32_t* out_index, int32_t* counts, void* stream,
+                        const lwb::ReidInput* reid = nullptr) {
   const std::string fn(name);
   if (!t || !scores || !labels || !boxes || !stream_ids || !out_ids || !out_scores || !out_labels || !out_boxes || !out_index || !counts)
     return fail(fn + ": null pointer");
@@ -402,9 +415,13 @@ static int track_common(const char* name, lwdetr_tracker* t, const float* scores
   if (reinterpret_cast<uintptr_t>(motion) % 8) return fail(fn + ": motion must be 8-byte aligned");
   const std::string err = check_streams(t, stream_ids, B);
   if (!err.empty()) return fail(fn + ": " + err);
+  // a tracker with appearance always runs the appearance instantiation (without embeddings when none are given: ByteTrack's
+  // bits), which keeps each record's embedding slot; the ByteTrack one would leave the slot array stale
+  const lwb::ReidInput none{&t->reid, nullptr, LWDETR_ET_F32, 0};
+  if (!reid && t->reid.emb) reid = &none;
   lwb::DeviceGuard g(t->device);
   int e = lwb::track_launch(t->table, t->params, scores, labels, boxes, motion, B, k, stream_ids, max_out, out_ids, out_scores, out_labels,
-                            out_boxes, out_index, counts, static_cast<cudaStream_t>(stream));
+                            out_boxes, out_index, counts, static_cast<cudaStream_t>(stream), reid);
   if (e == -2) return fail(fn + ": a limit is exceeded");
   if (!e) e = tracker_mark(t, stream);
   if (e) return cuda_fail(e, (fn + " launch").c_str());
@@ -423,6 +440,88 @@ int lwdetr_track_ex(lwdetr_tracker* t, const float* scores, const int32_t* label
                     int32_t* out_index, int32_t* counts, void* stream) {
   return track_common("lwdetr_track_ex", t, scores, labels, boxes, motion, B, k, stream_ids, max_out, out_ids, out_scores, out_labels,
                       out_boxes, out_index, counts, stream);
+}
+
+void lwdetr_reid_params_default(lwdetr_reid_params* p) {
+  if (!p) return;
+  p->embedding_dim = 256;
+  p->proximity_thresh = 0.5f;
+  p->appearance_thresh = 0.25f;
+  p->ema_alpha = 0.9f;
+}
+
+int lwdetr_tracker_create_reid(int num_streams, const lwdetr_track_params* params, const lwdetr_reid_params* reid, lwdetr_tracker** out) {
+  if (!params || !reid || !out) return fail("lwdetr_tracker_create_reid: null pointer");
+  const lwdetr_reid_params& r = *reid;
+  if (r.embedding_dim < 1 || r.embedding_dim > 2048) return fail("lwdetr_tracker_create_reid: embedding_dim must be in [1, 2048]");
+  if (!(r.proximity_thresh >= 0.f && r.proximity_thresh < 1.f)) return fail("lwdetr_tracker_create_reid: proximity_thresh must be in [0, 1)");
+  if (!(r.appearance_thresh >= 0.f && r.appearance_thresh <= 1.f) || !(r.ema_alpha >= 0.f && r.ema_alpha <= 1.f))
+    return fail("lwdetr_tracker_create_reid: appearance_thresh and ema_alpha must be in [0, 1]");
+  lwdetr_tracker* t = nullptr;
+  if (int rc = lwdetr_tracker_create(num_streams, params, &t)) return rc;
+  lwb::ReidTable& rt = t->reid;
+  const size_t ns = static_cast<size_t>(num_streams), cap = static_cast<size_t>(params->capacity), pairs = ns * lwb::TRACK_PAIRS;
+  cudaError_t e = cudaMalloc(&rt.slot, ns * 2 * cap * sizeof(int16_t));
+  if (e == cudaSuccess) e = cudaMalloc(&rt.has, ns * cap);
+  if (e == cudaSuccess) e = cudaMalloc(&rt.emb, ns * cap * r.embedding_dim * sizeof(float));
+  if (e == cudaSuccess) e = cudaMalloc(&rt.pkey, pairs * sizeof(uint32_t));
+  if (e == cudaSuccess) e = cudaMalloc(&rt.pval, pairs * sizeof(double));
+  if (e != cudaSuccess) {
+    lwdetr_tracker_destroy(t);
+    return cuda_fail(e, "lwdetr_tracker_create_reid");
+  }
+  rt.params = r;
+  *out = t;
+  return 0;
+}
+
+int lwdetr_track_reid(lwdetr_tracker* t, const float* scores, const int32_t* labels, const float* boxes, const double* motion,
+                      const void* embeddings, int emb_dtype, int ld_emb, int B, int k, const int32_t* stream_ids, int max_out,
+                      int32_t* out_ids, float* out_scores, int32_t* out_labels, float* out_boxes, int32_t* out_index, int32_t* counts,
+                      void* stream) {
+  if (t && t->reid.emb && embeddings) {
+    if (emb_dtype != LWDETR_ET_F32 && emb_dtype != LWDETR_ET_F16 && emb_dtype != LWDETR_ET_BF16)
+      return fail("lwdetr_track_reid: emb_dtype must be LWDETR_ET_F32, _F16 or _BF16");
+    if (ld_emb < t->reid.params.embedding_dim) return fail("lwdetr_track_reid: ld_emb is smaller than embedding_dim");
+    if (reinterpret_cast<uintptr_t>(embeddings) % (emb_dtype == LWDETR_ET_F32 ? 4 : 2))
+      return fail("lwdetr_track_reid: embeddings must be aligned to their element size");
+  }
+  const lwb::ReidInput in{t ? &t->reid : nullptr, embeddings, emb_dtype, ld_emb};
+  return track_common("lwdetr_track_reid", t, scores, labels, boxes, motion, B, k, stream_ids, max_out, out_ids, out_scores, out_labels,
+                      out_boxes, out_index, counts, stream, t && t->reid.emb && embeddings ? &in : nullptr);
+}
+
+int lwdetr_tracker_export_embeddings(lwdetr_tracker* t, int stream_id, float* host, int cap, int32_t* count, int8_t* has) {
+  if (!t || !count || (cap > 0 && (!host || !has))) return fail("lwdetr_tracker_export_embeddings: null pointer");
+  if (!t->reid.emb) return fail("lwdetr_tracker_export_embeddings: the tracker was made without appearance (lwdetr_tracker_create_reid)");
+  if (stream_id < 0 || stream_id >= t->table.num_streams) return fail("lwdetr_tracker_export_embeddings: stream id outside [0, num_streams)");
+  lwb::DeviceGuard g(t->device);
+  const int capacity = t->table.capacity, D = t->reid.params.embedding_dim;
+  lwb::TrackHead h;
+  std::vector<int16_t> slot(static_cast<size_t>(capacity));
+  std::vector<uint8_t> full(static_cast<size_t>(capacity));
+  cudaError_t e = cudaStreamWaitEvent(t->copy, t->done, 0);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&h, t->table.head + stream_id, sizeof(h), cudaMemcpyDeviceToHost, t->copy);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(t->copy);
+  if (e != cudaSuccess) return cuda_fail(e, "lwdetr_tracker_export_embeddings");
+  const int n = h.n_tracked + h.n_lost;
+  const int m = n < cap ? n : (cap > 0 ? cap : 0);
+  if (m > 0) {
+    const size_t s0 = static_cast<size_t>(stream_id);
+    e = cudaMemcpyAsync(slot.data(), t->reid.slot + (s0 * 2 + h.parity) * capacity, static_cast<size_t>(m) * sizeof(int16_t),
+                        cudaMemcpyDeviceToHost, t->copy);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(full.data(), t->reid.has + s0 * capacity, static_cast<size_t>(capacity), cudaMemcpyDeviceToHost, t->copy);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(t->copy);
+    for (int i = 0; i < m && e == cudaSuccess; ++i) {
+      has[i] = static_cast<int8_t>(full[slot[i]]);
+      e = cudaMemcpyAsync(host + static_cast<size_t>(i) * D, t->reid.emb + (s0 * capacity + slot[i]) * D, static_cast<size_t>(D) * sizeof(float),
+                          cudaMemcpyDeviceToHost, t->copy);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(t->copy);
+    if (e != cudaSuccess) return cuda_fail(e, "lwdetr_tracker_export_embeddings");
+  }
+  *count = n;
+  return 0;
 }
 
 int lwdetr_tracker_export(lwdetr_tracker* t, int stream_id, lwdetr_track_record* host, int cap, int32_t* count, int32_t frame_next_overflow[3]) {
@@ -906,6 +1005,13 @@ int lwdetr_op_cost(lwdetr_handle* h, int i, double* flops, double* bytes) {
   if (bytes) *bytes = h->eng->op(i).bytes;
   return 0;
 }
+int lwdetr_last_hidden(lwdetr_handle* h, void* dst, int ld_dst, void* stream) {
+  if (!h || !dst) return fail("lwdetr_last_hidden: null pointer");
+  std::string err;
+  if (h->eng->last_hidden(dst, ld_dst, static_cast<cudaStream_t>(stream), &err)) return fail(err);
+  return 0;
+}
+
 int lwdetr_profile_ops(lwdetr_handle* h, int iters, float* ms_per_op, void* stream) {
   if (!h || !ms_per_op || iters < 1) return fail("lwdetr_profile_ops: bad arguments");
   std::vector<float> ms;

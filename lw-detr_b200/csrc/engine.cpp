@@ -870,6 +870,7 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
     b.op("final_boxes", [delta, refpoint, BQ, NL, boxes](cudaStream_t st) { return final_boxes_launch(delta, refpoint, BQ, NL, boxes, st); },
          {boxes, NL * BQ, 4, 4, 1}, 32.0 * NL * BQ);
     p->logits = logits; p->boxes = boxes; p->enc_logits = enc_logits; p->enc_boxes = enc_boxes; p->topk_idx = topk_idx;
+    p->hidden = hs.p;
 
     if (b.failed()) return -1;
     if (pass == 0) {
@@ -987,6 +988,19 @@ int Engine::forward(const ForwardIn& in, int B, int H, int W, float* pred_logits
     if (e == cudaSuccess && aux->topk_index) e = cudaMemcpyAsync(aux->topk_index, p.topk_idx, BQ * 4, cudaMemcpyDeviceToDevice, st);
   }
   if (e != cudaSuccess) { *err = std::string("result copy failed: ") + cudaGetErrorString(e); return -1; }
+  return 0;
+}
+
+int Engine::last_hidden(void* dst, int ld, cudaStream_t st, std::string* err) {
+  DeviceGuard guard(device_);
+  if (!plan_ || plan_->eager_runs == 0) { *err = "lwdetr_last_hidden: run a forward first"; return -1; }
+  const int d = cfg_.hidden_dim;
+  if (ld < d) { *err = "lwdetr_last_hidden: ld_dst is smaller than hidden_dim"; return -1; }
+  const size_t BQ = static_cast<size_t>(plan_->B) * cfg_.num_queries;
+  const char* src = static_cast<const char*>(plan_->hidden) + (cfg_.dec_layers - 1) * BQ * d * 2;
+  const cudaError_t e = cudaMemcpy2DAsync(dst, static_cast<size_t>(ld) * 2, src, static_cast<size_t>(d) * 2, static_cast<size_t>(d) * 2, BQ,
+                                          cudaMemcpyDeviceToDevice, st);
+  if (e != cudaSuccess) { *err = std::string("lwdetr_last_hidden: ") + cudaGetErrorString(e); return -1; }
   return 0;
 }
 

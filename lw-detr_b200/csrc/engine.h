@@ -77,6 +77,7 @@ struct Plan {
   float* enc_logits = nullptr;   // [B, nq, ncls]
   float* enc_boxes = nullptr;    // [B, nq, 4]
   int* topk_idx = nullptr;       // [B, nq]
+  const void* hidden = nullptr;  // [layers, B, nq, hidden_dim] decoder output (after its norm), compute dtype
 
   Plan() = default;
   Plan(const Plan&) = delete;
@@ -112,6 +113,8 @@ class Engine {
   const lwdetr_config& config() const { return cfg_; }
   // per-op timing of the last planned batch (CUDA events, `iters` runs per op); returns ms per op
   int profile_ops(int iters, std::vector<float>* ms, cudaStream_t st, std::string* err);
+  // the last forward's final-layer decoder hidden state [B * nq, hidden_dim] into dst (row stride ld elements), on st
+  int last_hidden(void* dst, int ld, cudaStream_t st, std::string* err);
 
  private:
   struct DevBuf { void* p = nullptr; size_t bytes = 0; };

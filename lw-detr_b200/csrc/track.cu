@@ -12,9 +12,21 @@
 //      search never leaves its component, so this gives the bits of the whole-matrix solve;
 //   3. the lifecycle (updates, lost, removed, births under the capacity, ageing, duplicates) and a compaction into the
 //      other buffer in ByteTrack's list order; the activated tracked tracks are the output.
+// lwdetr_track_reid is a second instantiation of the same kernel (ReidArgs / SmemReid; the ByteTrack one compiles as
+// before).  After the entry lists it computes each high entry's norm (one warp each), lists the (track, high entry) pairs
+// that pass the proximity test, both with appearance, sorted by (track, entry) into a per-stream global table of
+// TRACK_PAIRS, and gives each its emb' (one warp per pair).  The Hungarian lanes look a pair up by binary search within its
+// track's row (row offsets in shared memory).  Beyond TRACK_PAIRS pairs a lane computes emb' itself, in the same summation
+// order, so the bits do not depend on the table.  Track embeddings live in stable per-stream slots: a record carries its
+// slot through the compaction (a parallel slot array, double-buffered like the records) and a birth takes the lowest free
+// slot, so a frame moves no embedding; only updates and births write D floats.
 #include "track.h"
 
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
 #include <climits>
+#include <type_traits>
 #include <vector>
 
 #include "launch.h"
@@ -50,6 +62,18 @@ struct TrackArgs {
   int stream[LAUNCH_STREAMS];            // stream of CTA i: batch row row0 + i
 };
 
+struct ReidArgs : TrackArgs {
+  const void* emb;                       // entry embeddings [rows][k] rows of ld_emb elements, or null (no appearance)
+  long long ld_emb;
+  int dtype, dim;                        // LWDETR_ET_*, D
+  float prox, app, alpha;
+  int16_t* slot;                         // [streams][2][capacity], parallel to rec
+  uint8_t* has;                          // [streams][capacity] by slot
+  float* temb;                           // [streams][capacity][dim] by slot
+  uint32_t* pkey;                        // [streams][TRACK_PAIRS]: (record << 16) | entry, ascending
+  double* pval;                          // [streams][TRACK_PAIRS]: emb' of the pair
+};
+
 struct Smem {
   double4 tbox[MAXN];                    // track slot boxes (after predict / update)
   double u[2 * MAXN], v[2 * MAXN], minv[2 * MAXN];
@@ -66,6 +90,22 @@ struct Smem {
   int wsum[NW];
   int n_edges, changed, n_removed;
 };
+
+struct SmemReid : Smem {
+  double enorm[MAXN];                    // entry norm ne, 0 without appearance (high entries only)
+  int16_t tslot[MAXN], bslot[MAXN], poff[MAXN + 1];
+  uint8_t thas[MAXN], sused[MAXN];
+  const uint32_t* pkey;                  // this stream's pair table
+  const double* pval;
+  const float* temb;                     // this stream's track embeddings
+  const char* erow;                      // entry 0 of this frame's embeddings, or null
+  long long ld_bytes;
+  double prox, app;
+  int dtype, dim, overflow, app_on;
+};
+
+template <class SM>
+constexpr bool kReid = std::is_same<SM, SmemReid>::value;
 
 __device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
 __device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
@@ -192,12 +232,70 @@ struct Assoc {
   bool fuse, class_aware;
 };
 
-// cost of (track box tb with label tl, entry e), +inf when not admissible.  L <= 1 (checked by the C ABI), so a pair
-// without overlap (cost 1) is never admissible.
-__device__ __forceinline__ double pair_cost(const Smem& S, double4 tb, int tl, int e, const Assoc& A) {
+__device__ __forceinline__ double emb_at(const char* row, int dtype, int i) {
+  if (dtype == LWDETR_ET_F32) return reinterpret_cast<const float*>(row)[i];
+  if (dtype == LWDETR_ET_F16) return __half2float(reinterpret_cast<const __half*>(row)[i]);
+  return __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(row)[i]);
+}
+
+// the header's fixed order, one lane: partial J of dot(t, e) (terms J, J + 32, ... from 0), combined as the xor butterfly
+// 16, 8, 4, 2, 1 combines them for lane 0
+template <int J, int O>
+__device__ double tree_dot(const float* t, const char* e, int dtype, int D) {
+  if constexpr (O == 32) {
+    double p = 0.0;
+    for (int i = J; i < D; i += 32) p = dadd(p, dmul(t[i], emb_at(e, dtype, i)));
+    return p;
+  } else {
+    return dadd(tree_dot<J, 2 * O>(t, e, dtype, D), tree_dot<J + O, 2 * O>(t, e, dtype, D));
+  }
+}
+
+// the same order over a warp: every lane holds its partial, every lane ends with the sum
+__device__ __forceinline__ double warp_tree(double p) {
+  for (int o = 16; o > 0; o >>= 1) p = dadd(p, __shfl_xor_sync(0xffffffffu, p, o));
+  return p;
+}
+
+// emb' = max(0, 1 - dot / ne) / 2, or 1 above appearance_thresh
+__device__ __forceinline__ double emb_cost(double dot, double ne, double app) {
+  const double m = ddiv(fmax(0.0, dsub(1.0, ddiv(dot, ne))), 2.0);
+  return m <= app ? m : 1.0;
+}
+
+// emb' of (record sl, entry e) whose IoU is io: from the pair table, or computed here when the table overflowed
+__device__ double appearance(const SmemReid& S, int sl, int e, double io) {
+  if (!(dsub(1.0, io) <= S.prox)) return 1.0;
+  if (S.overflow) {
+    if (!S.thas[sl] || !(S.enorm[e] > 0.0)) return 1.0;
+    const char* er = S.erow + e * S.ld_bytes;
+    return emb_cost(tree_dot<0, 1>(S.temb + static_cast<long long>(S.tslot[sl]) * S.dim, er, S.dtype, S.dim), S.enorm[e], S.app);
+  }
+  const uint32_t key = (static_cast<uint32_t>(sl) << 16) | static_cast<uint32_t>(e);
+  int lo = S.poff[sl];
+  const int end = S.poff[sl + 1];
+  for (int hi = end; lo < hi;) {
+    const int mid = (lo + hi) >> 1;
+    if (S.pkey[mid] < key) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo < end && S.pkey[lo] == key ? S.pval[lo] : 1.0;
+}
+
+// cost of (record sl: track box tb with label tl, entry e), +inf when not admissible.  L <= 1 (checked by the C ABI), so
+// a pair without overlap (cost 1) is never admissible; with appearance the cost is min(cost, emb'), and emb' < 1 needs
+// 1 - iou <= proximity_thresh < 1, so that still holds.
+template <class SM>
+__device__ __forceinline__ double pair_cost(const SM& S, double4 tb, int tl, int e, const Assoc& A, int sl) {
   if (A.class_aware && tl != S.elab[e]) return INF;
   const double io = iou_d(tb, widen(S.ebox[e]));
-  const double c = A.fuse ? dsub(1.0, dmul(io, static_cast<double>(S.escore[e]))) : dsub(1.0, io);
+  double c = A.fuse ? dsub(1.0, dmul(io, static_cast<double>(S.escore[e]))) : dsub(1.0, io);
+  if constexpr (kReid<SM>) {
+    if (S.app_on) {
+      const double m = appearance(S, sl, e, io);
+      if (m < c) c = m;
+    }
+  }
   return c < A.L ? c : INF;
 }
 
@@ -245,7 +343,8 @@ __device__ void bitonic_sort_asc(uint32_t* key, int np2) {
 
 // One warp: the Hungarian method on one component, nodes key[q0, q1) sorted rows first (R of them), then C columns.
 // Local column t < C is the t-th real column, t = C + i the own "unmatched" column of local row i (cost L).
-__device__ void solve_component(Smem& S, int q0, int R, int C, int nr, const int16_t* rows, const int16_t* cols, const Assoc& A) {
+template <class SM>
+__device__ void solve_component(SM& S, int q0, int R, int C, int nr, const int16_t* rows, const int16_t* cols, const Assoc& A) {
   const int lane = threadIdx.x & 31;
   const int T = R + C;
   double* u = S.u + q0;
@@ -283,7 +382,7 @@ __device__ void solve_component(Smem& S, int q0, int R, int C, int nr, const int
       int bt = INT_MAX;
       for (int t = lane; t < T; t += 32) {
         if (used[t]) continue;
-        const double c = t < C ? pair_cost(S, tb, tl, cols[(key[R + t] & 2047) - nr], A) : (t - C == i0 ? A.L : INF);
+        const double c = t < C ? pair_cost(S, tb, tl, cols[(key[R + t] & 2047) - nr], A, slot) : (t - C == i0 ? A.L : INF);
         const double cur = dsub(dsub(c, ui0), v[t]);
         double mv = minv[t];
         if (cur < mv) {
@@ -333,7 +432,8 @@ __device__ void solve_component(Smem& S, int q0, int R, int C, int nr, const int
 }
 
 // rows: nr track slots, cols: nc entry indices -> S.match[r]: the column position matched to row r, or -1.
-__device__ void associate(Smem& S, const int16_t* rows, int nr, const int16_t* cols, int nc, const Assoc& A) {
+template <class SM>
+__device__ void associate(SM& S, const int16_t* rows, int nr, const int16_t* cols, int nc, const Assoc& A) {
   const int tid = threadIdx.x;
   for (int r = tid; r < nr; r += NT) S.match[r] = -1;
   if (tid == 0) S.n_edges = 0;
@@ -343,7 +443,7 @@ __device__ void associate(Smem& S, const int16_t* rows, int nr, const int16_t* c
   for (int idx = tid; idx < nr * nc; idx += NT) {
     const int r = idx / nc, c = idx - r * nc;
     const int slot = rows[r];
-    if (pair_cost(S, S.tbox[slot], S.tlab[slot], cols[c], A) < INF) {
+    if (pair_cost(S, S.tbox[slot], S.tlab[slot], cols[c], A, slot) < INF) {
       const int e = atomicAdd(&S.n_edges, 1);
       if (e < EMAX) S.edge[e] = (static_cast<uint32_t>(r) << 16) | static_cast<uint32_t>(c);
     }
@@ -413,10 +513,38 @@ __device__ __forceinline__ float4 narrow(double4 b) {
   return make_float4(__double2float_rn(b.x), __double2float_rn(b.y), __double2float_rn(b.z), __double2float_rn(b.w));
 }
 
-__global__ void __launch_bounds__(NT, 1) track_kernel(const __grid_constant__ TrackArgs a) {
+// An update of a track's embedding t (slot es) by an entry with appearance (row er, norm ne), one warp: t = e / ne for a
+// track without one, else s = alpha t + (1 - alpha) e / ne and t = s / |s| (t unchanged when |s| is not finite or not > 0).
+// Each lane recomputes its s_i in the second pass, so nothing of length D is kept.
+__device__ void ema_update(const ReidArgs& a, float* t, uint8_t* has, const char* er, double ne) {
+  const int lane = threadIdx.x & 31, D = a.dim;
+  if (!*has) {
+    for (int i = lane; i < D; i += 32) t[i] = __double2float_rn(ddiv(emb_at(er, a.dtype, i), ne));
+    __syncwarp();
+    if (lane == 0) *has = 1;
+    return;
+  }
+  const double al = a.alpha, om = dsub(1.0, al);
+  double p = 0.0;
+  for (int i = lane; i < D; i += 32) {
+    const double si = dadd(dmul(al, static_cast<double>(t[i])), dmul(om, ddiv(emb_at(er, a.dtype, i), ne)));
+    p = dadd(p, dmul(si, si));
+  }
+  const double n = dsqrt(warp_tree(p));
+  if (!(isfinite(n) && n > 0.0)) return;
+  for (int i = lane; i < D; i += 32) {
+    const double si = dadd(dmul(al, static_cast<double>(t[i])), dmul(om, ddiv(emb_at(er, a.dtype, i), ne)));
+    t[i] = __double2float_rn(ddiv(si, n));
+  }
+}
+
+template <class Args>
+__global__ void __launch_bounds__(NT, 1) track_kernel(const __grid_constant__ Args a) {
+  constexpr bool REID = std::is_same<Args, ReidArgs>::value;
+  using SM = std::conditional_t<REID, SmemReid, Smem>;
   pdl_sync();   // programmatic dependent launch: release the successor, wait for the predecessor (launch.h)
   extern __shared__ __align__(16) uint8_t sm_track[];
-  Smem& S = *reinterpret_cast<Smem*>(sm_track);
+  SM& S = *reinterpret_cast<SM*>(sm_track);
   const int tid = threadIdx.x;
   const int sid = a.stream[blockIdx.x];
   const long long row = a.row0 + blockIdx.x;
@@ -430,6 +558,29 @@ __global__ void __launch_bounds__(NT, 1) track_kernel(const __grid_constant__ Tr
   const float4* bx = a.boxes + row * k;
 
   if (tid == 0) S.n_removed = 0;
+  [[maybe_unused]] const int lane = tid & 31, warp = tid >> 5;
+  [[maybe_unused]] int16_t *slot_cur = nullptr, *slot_nxt = nullptr;
+  [[maybe_unused]] uint8_t* has = nullptr;
+  [[maybe_unused]] float* temb = nullptr;
+  if constexpr (REID) {
+    slot_cur = a.slot + (static_cast<long long>(sid) * 2 + parity) * cap;
+    slot_nxt = a.slot + (static_cast<long long>(sid) * 2 + (parity ^ 1)) * cap;
+    has = a.has + static_cast<long long>(sid) * cap;
+    temb = a.temb + static_cast<long long>(sid) * cap * a.dim;
+    if (tid == 0) {
+      const int esz = a.dtype == LWDETR_ET_F32 ? 4 : 2;
+      S.pkey = a.pkey + static_cast<long long>(sid) * TRACK_PAIRS;
+      S.pval = a.pval + static_cast<long long>(sid) * TRACK_PAIRS;
+      S.temb = temb;
+      S.ld_bytes = a.ld_emb * esz;
+      S.erow = a.emb ? static_cast<const char*>(a.emb) + row * k * S.ld_bytes : nullptr;
+      S.prox = a.prox;
+      S.app = a.app;
+      S.dtype = a.dtype;
+      S.dim = a.dim;
+      S.app_on = 0;
+    }
+  }
   for (int i = tid; i < k; i += NT) {
     S.ebox[i] = bx[i];
     S.escore[i] = sc[i];
@@ -449,6 +600,10 @@ __global__ void __launch_bounds__(NT, 1) track_kernel(const __grid_constant__ Tr
     S.tdiff[sl] = r.end_frame - r.start_frame;
     S.tdet[sl] = -1;
     S.tf[sl] = static_cast<uint8_t>((act ? TF_ACT : 0) | (lost ? TF_LOSTLIST : 0));
+    if constexpr (REID) {
+      S.tslot[sl] = slot_cur[sl];
+      S.thas[sl] = has[slot_cur[sl]];
+    }
   }
   __syncthreads();
   const auto valid = [&](int i) {
@@ -463,6 +618,68 @@ __global__ void __launch_bounds__(NT, 1) track_kernel(const __grid_constant__ Tr
                               [&](int sl, int r) { S.pool[r] = static_cast<int16_t>(sl); });
   const int nu = ordered_scan(S, nT, [&](int sl) { return !(S.tf[sl] & TF_ACT); },
                               [&](int sl, int r) { S.unconf[r] = static_cast<int16_t>(sl); });
+  [[maybe_unused]] const auto update_embedding = [&](int sl, int e) {
+    if constexpr (REID) {
+      if (S.enorm[e] > 0.0) {
+        const int es = S.tslot[sl];
+        ema_update(a, temb + static_cast<long long>(es) * a.dim, has + es, S.erow + e * S.ld_bytes, S.enorm[e]);
+      }
+    }
+  };
+  if constexpr (REID) {
+    // entry norms of the high entries, one warp each, in the fixed order
+    for (int c = warp; c < nh; c += NW) {
+      const int e = S.high[c];
+      double p = 0.0;
+      if (S.erow) {
+        const char* er = S.erow + e * S.ld_bytes;
+        for (int i = lane; i < a.dim; i += 32) {
+          const double x = emb_at(er, a.dtype, i);
+          p = dadd(p, dmul(x, x));
+        }
+      }
+      const double ne = dsqrt(warp_tree(p));
+      if (lane == 0) S.enorm[e] = isfinite(ne) && ne > 0.0 ? ne : 0.0;
+    }
+    __syncthreads();
+    // the (record, high entry) pairs within proximity, both with appearance, in (record, entry) order
+    uint32_t* pkey = a.pkey + static_cast<long long>(sid) * TRACK_PAIRS;
+    double* pval = a.pval + static_cast<long long>(sid) * TRACK_PAIRS;
+    const int npairs = ordered_scan(S, nS * nh, [&](int idx) {
+      const int sl = idx / nh, e = S.high[idx - sl * nh];
+      return S.thas[sl] && S.enorm[e] > 0.0 && dsub(1.0, iou_d(S.tbox[sl], widen(S.ebox[e]))) <= S.prox;
+    }, [&](int idx, int r) {
+      const int sl = idx / nh, e = S.high[idx - sl * nh];
+      if (r < TRACK_PAIRS) pkey[r] = (static_cast<uint32_t>(sl) << 16) | static_cast<uint32_t>(e);
+    });
+    const bool overflow = npairs > TRACK_PAIRS;
+    if (tid == 0) S.overflow = overflow;
+    if (!overflow) {
+      __syncthreads();                   // the keys written by other threads
+      for (int i = warp; i < npairs; i += NW) {
+        const uint32_t key = pkey[i];
+        const int sl = key >> 16, e = key & 0xffff;
+        const float* t = temb + static_cast<long long>(S.tslot[sl]) * a.dim;
+        const char* er = S.erow + e * S.ld_bytes;
+        double p = 0.0;
+        for (int j = lane; j < a.dim; j += 32) p = dadd(p, dmul(static_cast<double>(t[j]), emb_at(er, a.dtype, j)));
+        const double dot = warp_tree(p);
+        if (lane == 0) pval[i] = emb_cost(dot, S.enorm[e], S.app);
+      }
+      for (int sl = tid; sl <= nS; sl += NT) {
+        const uint32_t key = static_cast<uint32_t>(sl) << 16;
+        int lo = 0;
+        for (int hi = npairs; lo < hi;) {
+          const int mid = (lo + hi) >> 1;
+          if (pkey[mid] < key) lo = mid + 1;
+          else hi = mid;
+        }
+        S.poff[sl] = static_cast<int16_t>(lo);
+      }
+    }
+    if (tid == 0) S.app_on = 1;
+    __syncthreads();
+  }
 
   // a matched track takes the entry's measurement, score, label and this frame
   const auto take = [&](int sl, int e) {
@@ -496,6 +713,11 @@ __global__ void __launch_bounds__(NT, 1) track_kernel(const __grid_constant__ Tr
     }
   }
   __syncthreads();
+  if constexpr (REID) {
+    for (int r = warp; r < np; r += NW)
+      if (S.match[r] >= 0) update_embedding(S.pool[r], S.high[S.match[r]]);
+    if (tid == 0) S.app_on = 0;          // association 2 (low entries) is IoU only
+  }
   const int nrest = ordered_scan(S, nh, [&](int c) { return !S.eused[S.high[c]]; },
                                  [&](int c, int r) { S.rest[r] = S.high[c]; });
   const int nrt = ordered_scan(S, np, [&](int r) { return S.match[r] < 0 && !(S.tf[S.pool[r]] & TF_LOSTLIST); },
@@ -514,6 +736,9 @@ __global__ void __launch_bounds__(NT, 1) track_kernel(const __grid_constant__ Tr
   }
   __syncthreads();
   // 3. unconfirmed tracks x the high detections left
+  if constexpr (REID) {
+    if (tid == 0) S.app_on = 1;
+  }
   associate(S, S.unconf, nu, S.rest, nrest, Assoc{static_cast<double>(a.unconf_thresh), a.fuse != 0, a.class_aware != 0});
   for (int r = tid; r < nu; r += NT) {
     const int sl = S.unconf[r], c = S.match[r];
@@ -539,6 +764,27 @@ __global__ void __launch_bounds__(NT, 1) track_kernel(const __grid_constant__ Tr
                                  [&](int c, int r) { S.births[r] = S.rest[c]; });
   const int nb = min(ncand, cap - live);
   for (int b = tid; b < nb; b += NT) S.bdrop[b] = 0;
+  if constexpr (REID) {
+    for (int r = warp; r < nu; r += NW)
+      if (S.match[r] >= 0) update_embedding(S.unconf[r], S.rest[S.match[r]]);
+    // births take the lowest slots no live record holds (there are cap - live >= nb of them)
+    for (int es = tid; es < cap; es += NT) S.sused[es] = 0;
+    __syncthreads();
+    for (int sl = tid; sl < nS; sl += NT)
+      if (!(S.tf[sl] & TF_REMOVED)) S.sused[S.tslot[sl]] = 1;
+    __syncthreads();
+    ordered_scan(S, cap, [&](int es) { return !S.sused[es]; },
+                 [&](int es, int r) { if (r < nb) S.bslot[r] = static_cast<int16_t>(es); });
+    for (int b = warp; b < nb; b += NW) {
+      const int e = S.births[b], es = S.bslot[b];
+      if (S.enorm[e] > 0.0) {
+        float* t = temb + static_cast<long long>(es) * a.dim;
+        const char* er = S.erow + e * S.ld_bytes;
+        for (int i = lane; i < a.dim; i += 32) t[i] = __double2float_rn(ddiv(emb_at(er, a.dtype, i), S.enorm[e]));
+      }
+      if (lane == 0) has[es] = S.enorm[e] > 0.0;
+    }
+  }
   // new lists: tracked = still-tracked previous tracked, births, refound; lost = remaining previous lost, new lost
   const int nA = ordered_scan(S, nT, [&](int sl) { return (S.tf[sl] & TF_MATCHED) != 0; },
                               [&](int sl, int r) { S.tlist[r] = static_cast<int16_t>(sl); });
@@ -583,6 +829,7 @@ __global__ void __launch_bounds__(NT, 1) track_kernel(const __grid_constant__ Tr
   const int newT = ordered_scan(S, ntr, [&](int i) { return !dropped(S.tlist[i]); }, [&](int i, int r) {
     const int x = S.tlist[i];
     lwdetr_track_record& o = nxt[r];
+    if constexpr (REID) slot_nxt[r] = x < MAXN ? S.tslot[x] : S.bslot[x - MAXN];
     if (x < MAXN) {
       o = cur[x];
     } else {
@@ -600,8 +847,10 @@ __global__ void __launch_bounds__(NT, 1) track_kernel(const __grid_constant__ Tr
       o.index = e;
     }
   });
-  const int newL = ordered_scan(S, nlo, [&](int j) { return !dropped(S.llist[j]); },
-                                [&](int j, int r) { nxt[newT + r] = cur[S.llist[j]]; });
+  const int newL = ordered_scan(S, nlo, [&](int j) { return !dropped(S.llist[j]); }, [&](int j, int r) {
+    nxt[newT + r] = cur[S.llist[j]];
+    if constexpr (REID) slot_nxt[newT + r] = S.tslot[S.llist[j]];
+  });
   const long long ob = row * a.max_out;
   const int nout = ordered_scan(S, ntr, [&](int i) {
     const int x = S.tlist[i];
@@ -674,11 +923,12 @@ __global__ void query_best_kernel(const float* __restrict__ logits, const float*
 
 int track_launch(const TrackTable& t, const lwdetr_track_params& p, const float* scores, const int32_t* labels, const float* boxes,
                  const double* motion, int B, int k, const int32_t* streams, int max_out, int32_t* out_ids, float* out_scores, int32_t* out_labels,
-                 float* out_boxes, int32_t* out_index, int32_t* counts, cudaStream_t st) {
+                 float* out_boxes, int32_t* out_index, int32_t* counts, cudaStream_t st, const ReidInput* reid) {
   if (B < 1 || k < 1 || k > TRACK_MAX || max_out < 1) return -2;
-  const int smem = static_cast<int>(sizeof(Smem));
-  if (int e = ensure_max_dyn_smem(reinterpret_cast<const void*>(track_kernel), smem)) return e;
-  std::vector<TrackArgs> hold(1);        // ~4 KB of parameters: kept off the stack
+  const int smem = static_cast<int>(reid ? sizeof(SmemReid) : sizeof(Smem));
+  const void* kern = reid ? reinterpret_cast<const void*>(track_kernel<ReidArgs>) : reinterpret_cast<const void*>(track_kernel<TrackArgs>);
+  if (int e = ensure_max_dyn_smem(kern, smem)) return e;
+  std::vector<ReidArgs> hold(1);         // ~4 KB of parameters: kept off the stack
   TrackArgs& a = hold[0];
   a.scores = scores;
   a.labels = labels;
@@ -705,11 +955,28 @@ int track_launch(const TrackTable& t, const lwdetr_track_params& p, const float*
   a.max_time_lost = static_cast<int>(p.frame_rate / 30.0 * p.track_buffer);
   a.fuse = p.fuse_score;
   a.class_aware = p.class_aware;
+  ReidArgs& r = hold[0];
+  if (reid) {
+    const ReidTable& rt = *reid->table;
+    r.emb = reid->emb;
+    r.ld_emb = reid->ld;
+    r.dtype = reid->dtype;
+    r.dim = rt.params.embedding_dim;
+    r.prox = rt.params.proximity_thresh;
+    r.app = rt.params.appearance_thresh;
+    r.alpha = rt.params.ema_alpha;
+    r.slot = rt.slot;
+    r.has = rt.has;
+    r.temb = rt.emb;
+    r.pkey = rt.pkey;
+    r.pval = rt.pval;
+  }
   for (int b0 = 0; b0 < B; b0 += LAUNCH_STREAMS) {
     const int nb = B - b0 < LAUNCH_STREAMS ? B - b0 : LAUNCH_STREAMS;
     a.row0 = b0;
     for (int i = 0; i < nb; ++i) a.stream[i] = streams[b0 + i];
-    launch_k(track_kernel, dim3(nb), dim3(NT), static_cast<size_t>(smem), st, a);
+    if (reid) launch_k(track_kernel<ReidArgs>, dim3(nb), dim3(NT), static_cast<size_t>(smem), st, r);
+    else launch_k(track_kernel<TrackArgs>, dim3(nb), dim3(NT), static_cast<size_t>(smem), st, a);
     if (cudaError_t e = cudaGetLastError()) return static_cast<int>(e);
   }
   return 0;

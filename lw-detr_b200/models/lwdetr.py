@@ -206,7 +206,7 @@ class LWDETR(nn.Module):
 
     @torch.no_grad()
     def track(self, frames, tracker, streams=None, size=None, fit="stretch", short_side=None, max_side=None, colorspace=None,
-              max_out=None, motion=None):
+              max_out=None, motion=None, appearance=False):
         """Multi-object tracking of video streams: frames (RGB or NV12, taken exactly as detect() takes them) run as one
         forward; each query gives one detection, its best class (capi.query_best, boxes in the frame's original pixels);
         then capi.Tracker `tracker` (ByteTrack on the device, include/lwdetr_b200.h) updates each frame's stream.
@@ -216,9 +216,14 @@ class LWDETR(nn.Module):
         cut to the frame's count (one read-back for the call), "queries" the query each track took its detection from.
         max_out (default num_queries) bounds the tracks returned per frame.  motion: a capi.MotionEstimator for moving
         cameras; each frame round then estimates every frame's camera motion from the same frame descriptors (nothing
-        copied) and warps the stream's tracks by it before the association (Tracker.update(motion=...)).  How ByteTrack's
-        thresholds (tuned on YOLOX scores) suit LW-DETR's score distribution, in MOTA / IDF1 / HOTA, with or without
-        motion, is not measured here."""
+        copied) and warps the stream's tracks by it before the association (Tracker.update(motion=...)).
+        appearance (a tracker made with embedding_dim): True feeds each frame's final decoder hidden state (one row per
+        query, Engine.forward_frames(want_hidden=True)) to Tracker.update(embeddings=...), BoT-SORT's appearance cost with
+        the detector's own features; the tracker's embedding_dim must be hidden_dim.  A CUDA tensor [len(frames),
+        num_queries, D] passes the caller's own embeddings instead (any ReID model's).  With motion= as well this is
+        BoT-SORT with both compensations.  How ByteTrack's thresholds (tuned on YOLOX scores) suit LW-DETR's score
+        distribution, and whether the decoder's features tell identities apart on real footage, in MOTA / IDF1 / HOTA, is
+        not measured here."""
         if self.training:
             raise RuntimeError("lwdetr_b200 implements the inference forward only; call model.eval()")
         dev = next(self.parameters()).device
@@ -229,7 +234,20 @@ class LWDETR(nn.Module):
         streams = list(range(n)) if streams is None else [int(s) for s in streams]
         if len(streams) != n:
             raise RuntimeError("lwdetr_b200: %d streams for %d frames" % (len(streams), n))
-        out = self.engine().forward_frames(fb, size=size, fit=fit, short_side=short_side, max_side=max_side, want_aux=False)
+        emb = None
+        if isinstance(appearance, torch.Tensor):
+            if tuple(appearance.shape[:2]) != (n, self.num_queries) or appearance.dim() != 3:
+                raise RuntimeError("lwdetr_b200: appearance must be [%d, %d, D], got %s" % (n, self.num_queries, tuple(appearance.shape)))
+            emb = appearance
+        else:
+            appearance = bool(appearance)
+        if appearance is True and tracker.embedding_dim != self.cfg.hidden_dim:
+            raise RuntimeError("lwdetr_b200: appearance=True feeds the decoder's %d-wide features, but the tracker's embedding_dim is %s"
+                               % (self.cfg.hidden_dim, tracker.embedding_dim))
+        out = self.engine().forward_frames(fb, size=size, fit=fit, short_side=short_side, max_side=max_side, want_aux=False,
+                                           want_hidden=appearance is True)
+        if appearance is True:
+            emb = out["hidden"]
         sizes = torch.tensor(fb.sizes, dtype=torch.float32, device=dev)
         scores, labels, boxes = capi.query_best(out["pred_logits"], out["pred_boxes"], sizes)
         rounds, seen = [], {}
@@ -244,7 +262,11 @@ class LWDETR(nn.Module):
             idx = torch.tensor(rows, device=dev)
             ids = [streams[i] for i in rows]
             mo = None if motion is None else motion.estimate(fb.select(rows), ids)[0]
-            got = tracker.update(scores[idx], labels[idx], boxes[idx], ids, self.num_queries if max_out is None else max_out, motion=mo)
+            em = None
+            if emb is not None:     # consecutive frames (one round, the usual case) as a view: no copy
+                em = emb[rows[0]:rows[-1] + 1] if rows == list(range(rows[0], rows[-1] + 1)) else emb[idx]
+            got = tracker.update(scores[idx], labels[idx], boxes[idx], ids, self.num_queries if max_out is None else max_out, motion=mo,
+                                 embeddings=em)
             counts.append(got[5])
             for j, i in enumerate(rows):
                 res[i] = (got, j)

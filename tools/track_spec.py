@@ -9,6 +9,10 @@ Everything is float64 with each operation rounded on its own (numpy does not fus
 
 With a camera motion (lwdetr_track_ex), warp() moves every track after the predict, in the header's operation order.
 
+With appearance (lwdetr_track_reid, BoT-SORT's with_reid path), Stream takes reid parameters (reid_params()) and each
+frame's entry embeddings: each track keeps an fp32 unit embedding, and the pool x high and unconfirmed x rest associations
+take min(IoU cost, appearance cost) (appearance_cost()); fixed_sum() is the header's fixed summation order.
+
 scene() is a seeded generator of synthetic detection sequences for the tests and the benchmark, optionally seen through a
 moving camera (camera_path()).
 """
@@ -43,7 +47,7 @@ def params(**kw):
 
 # ---------------------------------------------------------------------------------------------- Kalman filter (xyah)
 class Track:
-    __slots__ = ("id", "state", "activated", "start", "end", "score", "label", "index", "p", "v", "P", "C", "V")
+    __slots__ = ("id", "state", "activated", "start", "end", "score", "label", "index", "p", "v", "P", "C", "V", "emb")
 
     def box(self):
         """xyxy float64 from the state: w = a * h, x1 = cx - w / 2, y1 = cy - h / 2, x2 = x1 + w, y2 = y1 + h."""
@@ -143,14 +147,17 @@ def iou(a, b):
         return np.where(ok, inter / np.where(ok, union, 1.0), 0.0)
 
 
-def cost_matrix(tboxes, tlabels, dboxes, dscores, dlabels, L, fuse, class_aware):
+def cost_matrix(tboxes, tlabels, dboxes, dscores, dlabels, L, fuse, class_aware, emb=None):
     """[n, m] float64: 1 - iou (fuse: 1 - iou * score), +inf where the pair is not admissible (cost >= L, or labels
-    differ under class_aware)."""
+    differ under class_aware).  emb: the [n, m] appearance cost emb' (appearance_cost()); the cost is then
+    min(that cost, emb')."""
     n, m = len(tboxes), len(dboxes)
     if n == 0 or m == 0:
         return np.full((n, m), INF)
     io = iou(tboxes, np.asarray(dboxes, np.float64))
     c = 1.0 - io * np.asarray(dscores, np.float32).astype(np.float64)[None, :] if fuse else 1.0 - io
+    if emb is not None:
+        c = np.minimum(c, emb)
     ok = c < np.float64(L)
     if class_aware:
         ok &= np.asarray(tlabels)[:, None] == np.asarray(dlabels)[None, :]
@@ -255,12 +262,94 @@ def solve_by_components(cost, L):
     return match, u, v
 
 
+# ---------------------------------------------------------------------------------------------- appearance
+REID_DEFAULTS = dict(embedding_dim=256, proximity_thresh=0.5, appearance_thresh=0.25, ema_alpha=0.9)
+
+
+def reid_params(**kw):
+    """lwdetr_reid_params with BoT-SORT's defaults; thresholds and alpha are float32, as the struct holds them."""
+    bad = set(kw) - set(REID_DEFAULTS)
+    if bad:
+        raise TypeError("unknown appearance parameters: %s" % ", ".join(sorted(bad)))
+    r = dict(REID_DEFAULTS)
+    r.update(kw)
+    for k in ("proximity_thresh", "appearance_thresh", "ema_alpha"):
+        r[k] = np.float32(r[k])
+    r["embedding_dim"] = int(r["embedding_dim"])
+    return r
+
+
+def fixed_sum(x):
+    """The header's summation order of D float64 terms: 32 partial sums from 0, partial j adding terms j, j + 32, ... in
+    ascending order, then the xor butterfly 16, 8, 4, 2, 1 (lane j adds lane j ^ o; addition commutes, so every lane
+    ends with the same bits); the value of lane 0."""
+    x = np.asarray(x, np.float64)
+    p = np.zeros(32)
+    for j0 in range(0, len(x), 32):
+        c = x[j0:j0 + 32]
+        p[:len(c)] = p[:len(c)] + c
+    lane = np.arange(32)
+    for o in (16, 8, 4, 2, 1):
+        p = p + p[lane ^ o]
+    return p[0]
+
+
+def fixed_norm(x):
+    x = np.asarray(x, np.float64)
+    return np.sqrt(fixed_sum(x * x))
+
+
+def fixed_dot(a, b):
+    return fixed_sum(np.asarray(a, np.float64) * np.asarray(b, np.float64))
+
+
+def entry_norms(emb):
+    """ne of every entry [k, D] (widened exactly to float64); 0 where the entry has no appearance (ne not finite or not
+    > 0)."""
+    ne = np.array([fixed_norm(e) for e in np.asarray(emb, np.float64)]) if len(emb) else np.zeros(0)
+    return np.where(np.isfinite(ne) & (ne > 0), ne, 0.0)
+
+
+def appearance_cost(tracks, tboxes, dets, dboxes, emb, ne, r):
+    """[n, m] emb': max(0, 1 - dot(t, e) / ne) / 2 where the track and the entry have appearance, (1 - iou) <=
+    proximity_thresh and that value <= appearance_thresh; 1 elsewhere."""
+    out = np.ones((len(tracks), len(dets)))
+    if len(tracks) == 0 or len(dets) == 0:
+        return out
+    io = iou(tboxes, dboxes)
+    prox, app = np.float64(r["proximity_thresh"]), np.float64(r["appearance_thresh"])
+    for i, t in enumerate(tracks):
+        if t.emb is None:
+            continue
+        for j, d in enumerate(dets):
+            if ne[d] > 0 and 1.0 - io[i, j] <= prox:
+                e = np.float64(max(0.0, 1.0 - fixed_dot(t.emb, emb[d]) / ne[d])) / 2.0
+                out[i, j] = e if e <= app else 1.0
+    return out
+
+
+def ema(t, e, ne, r):
+    """A track's embedding after an update by an entry with appearance: e / ne at first, else s = alpha t + (1 - alpha)
+    e / ne normalised in the fixed order (unchanged when |s| is not finite or not > 0); fp32."""
+    f = np.asarray(e, np.float64) / ne
+    if t.emb is None:
+        t.emb = f.astype(np.float32)
+        return
+    a = np.float64(r["ema_alpha"])
+    s = a * t.emb.astype(np.float64) + (1.0 - a) * f
+    n = fixed_norm(s)
+    if np.isfinite(n) and n > 0:
+        t.emb = (s / n).astype(np.float32)
+
+
 # ---------------------------------------------------------------------------------------------- one stream
 class Stream:
-    """The tracker state of one camera stream: tracked and lost lists in ByteTrack's list order."""
+    """The tracker state of one camera stream: tracked and lost lists in ByteTrack's list order.  r: reid_params() for
+    the appearance mode (lwdetr_track_reid), None for ByteTrack."""
 
-    def __init__(self, p):
+    def __init__(self, p, r=None):
         self.p = p
+        self.r = r
         self.reset()
 
     def reset(self):
@@ -268,26 +357,40 @@ class Stream:
         self.tracked, self.lost = [], []
         self.dropped = dict(tracked=0, birth=0, lost=0)       # duplicate removals so far (step 8), for the tests
 
-    def _cost(self, tracks, dets, L, fuse, e):
+    def _cost(self, tracks, dets, L, fuse, e, app=None):
         scores, labels, boxes = e
         tb = np.array([t.box() for t in tracks]).reshape(-1, 4)
-        return cost_matrix(tb, [t.label for t in tracks], boxes[dets].reshape(-1, 4), scores[dets], labels[dets], L, fuse,
-                           self.p["class_aware"])
+        db = boxes[dets].reshape(-1, 4)
+        emb = None if app is None else appearance_cost(tracks, tb, dets, db.astype(np.float64), app[0], app[1], self.r)
+        return cost_matrix(tb, [t.label for t in tracks], db, scores[dets], labels[dets], L, fuse, self.p["class_aware"], emb)
 
-    def _update(self, t, d, e):
+    def _update(self, t, d, e, app=None):
+        """app: (embeddings, norms) for an update by a high entry in the appearance mode; a low entry leaves the
+        track's embedding as it is."""
         scores, labels, boxes = e
         kalman_update(t, measurement(boxes[d]))
         t.state, t.activated, t.end = TRACKED, True, self.frame
         t.score, t.label, t.index = scores[d], labels[d], int(d)
+        if app is not None and app[1][d] > 0:
+            ema(t, app[0][d], app[1][d], self.r)
 
-    def update(self, scores, labels, boxes, motion=None):
+    def update(self, scores, labels, boxes, motion=None, embeddings=None):
         """One frame: scores fp32 [k], labels int32 [k], boxes fp32 [k, 4] (xyxy) -> the output tracks, a list of
-        (id, score fp32, label, box fp32 [4], index).  motion: the frame's camera motion (a, b, tx, ty) or None."""
+        (id, score fp32, label, box fp32 [4], index).  motion: the frame's camera motion (a, b, tx, ty) or None.
+        embeddings: [k, D] entry embeddings (values exactly widened to float64) in the appearance mode, None for
+        none (then no entry has appearance)."""
         p, frame = self.p, self.frame
         scores = np.asarray(scores, np.float32).reshape(-1)
         labels = np.asarray(labels).astype(np.int32).reshape(-1)
         boxes = np.asarray(boxes, np.float32).reshape(-1, 4)
         e = (scores, labels, boxes)
+        app = None
+        if self.r is not None:
+            emb = np.zeros((len(scores), self.r["embedding_dim"])) if embeddings is None else np.asarray(embeddings, np.float64)
+            ne = np.zeros(len(scores)) if embeddings is None else entry_norms(emb)
+            app = (emb, ne)
+        elif embeddings is not None:
+            raise ValueError("embeddings given to a stream without appearance parameters")
         bd = boxes.astype(np.float64)
         with np.errstate(invalid="ignore"):
             valid = np.isfinite(bd).all(1) & (bd[:, 2] - bd[:, 0] > 0) & (bd[:, 3] - bd[:, 1] > 0)
@@ -302,13 +405,13 @@ class Stream:
             for t in self.tracked + self.lost:
                 warp(t, motion)
         # 1. pool x high detections
-        m1, _, _ = solve(self._cost(pool, high, p["match_thresh"], p["fuse_score"], e), p["match_thresh"])
+        m1, _, _ = solve(self._cost(pool, high, p["match_thresh"], p["fuse_score"], e, app), p["match_thresh"])
         refound = []
         for t, c in zip(pool, m1):
             if c >= 0:
                 if t.state == LOST:
                     refound.append(t)
-                self._update(t, high[c], e)
+                self._update(t, high[c], e, app)
         used = np.zeros(len(high), bool)
         used[m1[m1 >= 0]] = True
         rest = high[~used]
@@ -323,11 +426,11 @@ class Stream:
                 t.state = LOST
                 new_lost.append(t)
         # 3. unconfirmed tracks x the high detections left
-        m3, _, _ = solve(self._cost(unconf, rest, p["unconfirmed_thresh"], p["fuse_score"], e), p["unconfirmed_thresh"])
+        m3, _, _ = solve(self._cost(unconf, rest, p["unconfirmed_thresh"], p["fuse_score"], e, app), p["unconfirmed_thresh"])
         removed = set()
         for t, c in zip(unconf, m3):
             if c >= 0:
-                self._update(t, rest[c], e)
+                self._update(t, rest[c], e, app)
             else:
                 removed.add(id(t))
         used = np.zeros(len(rest), bool)
@@ -349,6 +452,9 @@ class Stream:
                 t.state, t.activated, t.start, t.end = TRACKED, frame == 1, frame, frame
                 t.score, t.label, t.index = scores[d], labels[d], int(d)
                 initiate(t, measurement(boxes[d]))
+                t.emb = None
+                if app is not None and app[1][d] > 0:
+                    ema(t, app[0][d], app[1][d], self.r)
                 births.append(t)
         # 7. new lists
         tracked = [t for t in self.tracked if t.state == TRACKED and id(t) not in removed] + births + refound
@@ -381,6 +487,10 @@ class Stream:
         return [dict(id=t.id, state=t.state, activated=int(t.activated), start=t.start, end=t.end, score=np.float32(t.score),
                      label=int(t.label), index=t.index, mean=np.concatenate([t.p, t.v]), cov=np.concatenate([t.P, t.C, t.V]))
                 for t in self.tracked + self.lost]
+
+    def export_embeddings(self):
+        """The fp32 embedding of every record in list order (tracked, then lost), None for a track without one."""
+        return [t.emb for t in self.tracked + self.lost]
 
 
 def outputs_array(outs, max_out):
@@ -441,7 +551,7 @@ def camera_path(frames, size, seed=0, pan=10.0, shake=4.0, zoom=0.004, rotate=0.
 
 
 def scene(seed, frames, objects=20, k=None, ncls=3, size=(1080, 1920), clutter=3, miss=0.05, low_dip=0.1, occlusion=0.02,
-          crossing=True, echo=0.0, camera=None, truth=False):
+          crossing=True, echo=0.0, camera=None, truth=False, crossings=1, appearance=None):
     """Seeded synthetic detections: `objects` ground-truth boxes alive at a time on average, moving at constant velocity with
     small accelerations, born and dying over the sequence; per frame each visible object gives a detection with jitter
     (score mostly high, dipping into the low band with probability low_dip), is missed with probability `miss`, and starts
@@ -456,7 +566,11 @@ def scene(seed, frames, objects=20, k=None, ncls=3, size=(1080, 1920), clutter=3
     camera; every box is mapped by the camera's accumulated similarity (centre by the similarity, sides by its scale).  The
     camera draws from its own generator, so the scene's draws are those of the still scene.  truth: also give the object of
     each entry (int32 per entry, -1 for clutter and echoes).  With camera or truth the result is (frames, motion float64
-    [frames, 4] or None, truth or None)."""
+    [frames, 4] or None, truth or None).
+    crossings: the number of object pairs aimed at each other (with crossing), at heights spread over the frame.
+    appearance (a dict of appearance_embeddings' options, APPEARANCE the defaults): also an embedding per entry, float32
+    [k_f, dim] per frame; the result is then (frames, motion, truth, embeddings).  The embeddings
+    draw from their own generator, so the scene's draws are those of the scene without them."""
     rng = np.random.default_rng(seed)
     H, W = size
     objs = []
@@ -473,10 +587,13 @@ def scene(seed, frames, objects=20, k=None, ncls=3, size=(1080, 1920), clutter=3
         objs.append(o)
     for _ in range(objects):
         spawn(0)
-    if crossing and objects >= 2:              # two objects aimed at each other
-        a, b = objs[0], objs[1]
-        a.update(cx=W * 0.3, cy=H * 0.5, vx=6.0, vy=0.0)
-        b.update(cx=W * 0.7, cy=H * 0.5 + 10, vx=-6.0, vy=0.0, h=a["h"] * 1.1, w=a["w"] * 0.9)
+    for i in range(min(crossings, objects // 2) if crossing else 0):     # pairs of objects aimed at each other
+        a, b = objs[2 * i], objs[2 * i + 1]
+        cy = H * 0.5 if crossings == 1 else H * (0.15 + 0.7 * i / (crossings - 1))
+        a.update(cx=W * 0.3, cy=cy, vx=6.0, vy=0.0)
+        b.update(cx=W * 0.7, cy=cy + 10, vx=-6.0, vy=0.0, h=a["h"] * 1.1, w=a["w"] * 0.9)
+        if crossings > 1:                      # one class per pair, so that class-aware gating cannot tell them apart
+            b["label"] = a["label"]
     out, gts = [], []
     for f in range(frames):
         if motion is not None:                 # accumulated camera: the previous one followed by this frame's motion
@@ -531,9 +648,46 @@ def scene(seed, frames, objects=20, k=None, ncls=3, size=(1080, 1920), clutter=3
         out.append(pad(a[:, 0].astype(np.float32), a[:, 1].astype(np.int32), bx.astype(np.float32), k))
         g = a[:, 6].astype(np.int32)
         gts.append(g if k is None else np.r_[g, np.full(max(0, k - len(g)), -1, np.int32)][:k])
+    if appearance is not None:
+        return out, motion, (gts if truth else None), appearance_embeddings(gts, **appearance)
     if camera is None and not truth:
         return out
     return out, motion, (gts if truth else None)
+
+
+APPEARANCE = dict(seed=0, dim=64, cosine=0.9, same=False)
+
+
+def appearance_embeddings(truth, seed=0, dim=64, cosine=0.9, same=False):
+    """Seeded embeddings for scene(): a random unit vector per object (one shared by all objects with `same`, the
+    control); per entry of an object that vector turned by exactly arccos(cosine) towards a random direction; a random
+    unit vector for clutter, echoes and padding (object -1).  Each row is then scaled by a factor in [0.5, 2), so that the
+    normalisation matters.  truth: the object of each entry per frame.  Returns float32 [k_f, dim] per frame."""
+    rng = np.random.default_rng(seed)
+    base = {}
+
+    def unit(n):
+        v = rng.normal(size=(n, dim))
+        return v / np.linalg.norm(v, axis=1, keepdims=True)
+    shared = unit(1)[0]
+    out = []
+    for g in truth:
+        e = np.zeros((len(g), dim))
+        for i, o in enumerate(g):
+            o = int(o)
+            if o < 0:
+                e[i] = unit(1)[0]
+                continue
+            if o not in base:
+                base[o] = shared if same else unit(1)[0]
+            u = base[o]
+            n = rng.normal(size=dim)
+            n -= (n @ u) * u
+            n /= np.linalg.norm(n)
+            e[i] = cosine * u + np.sqrt(1.0 - cosine * cosine) * n
+        e *= rng.uniform(0.5, 2.0, (len(g), 1))
+        out.append(e.astype(np.float32))
+    return out
 
 
 def id_switches(stream_outputs, truth):
