@@ -131,10 +131,41 @@ LWDETR_API int lwdetr_layernorm_ex(int dtype, lwdetr_layernorm_args* args, void*
 /* softmax(Q K^T * scale) V for `nseq` independent sequences of `seqlen` tokens and `heads` heads of
  * width dh in {16, 32, 64}; token (s, t) is matrix row s*seqlen + t, head h occupies columns
  * [h*dh, (h+1)*dh).  Window attention: nseq = 16*B, seqlen = 100; global: nseq = B, seqlen = 1600
- * (vit.py:120-140, 195-222); decoder self-attention: nseq = B, seqlen = nq (attention.py:563-606). */
+ * (vit.py:120-140, 195-222); decoder self-attention: nseq = B, seqlen = nq (attention.py:563-606).
+ * dtype LWDETR_F16 or LWDETR_BF16.  Refused before anything is launched, with an error naming the limit: q, k, v or out
+ * not 16-byte aligned; a leading dimension that is not a multiple of 8 or is below heads * dh; dh outside {16, 32, 64};
+ * nseq, seqlen or heads not positive; nseq or heads above 65535 (the grid of the chosen kernel); and on the packed path
+ * nseq * seqlen of 2^31 or more.
+ * Kernels: a PACKED q / k / v (k = q + heads*dh, v = q + 2*heads*dh elements, one leading dimension, the ViT's qkv matrix)
+ * runs on the wgmma / TMA kernel (LWDETR_ATTN_WG) at every length.  Anything else (the decoder's q / k column slices of
+ * one matrix and a separate v) runs on mma.sync kernels: LWDETR_ATTN_MMA_SHORT (persistent CTAs over (sequence, head)
+ * items) up to 112 tokens, LWDETR_ATTN_MMA with 4 warps per CTA below 1024 tokens and with 8 from there.  The environment
+ * variable LWDETR_B200_ATTN_POLY (read once per process) moves part of the exponentials of the mma.sync kernels at head
+ * dims 16 and 32 to a polynomial on the FMA pipe: 1 = n-tiles 2 and 5 of every 8 (mask 0x24), 2 = n-tiles 0, 3 and 6
+ * (0x49); LWDETR_ATTN_MMA takes it with 8 warps only. */
 LWDETR_API int lwdetr_attention(int dtype, const void* q, int ldq, const void* k, int ldk, const void* v, int ldv,
                                 void* out, int ldo, int nseq, int seqlen, int heads, int dh, float scale,
                                 void* stream);
+
+/* lwdetr_attention with the arguments in a struct, reporting the kernel instance it chose (the same choice a launch
+ * makes, under the same checks).  dry_run != 0: check and choose only, with no CUDA call at all (no launch, no device
+ * query), so the pointers are never dereferenced and it runs without a device.
+ *   kernel     LWDETR_ATTN_WG, LWDETR_ATTN_MMA or LWDETR_ATTN_MMA_SHORT;
+ *   warps      4 or 8 for LWDETR_ATTN_MMA, 0 otherwise;
+ *   poly_mask  0, 0x24 or 0x49: bit i set = n-tile i of each 64-key chunk takes the polynomial exp2. */
+enum { LWDETR_ATTN_WG = 0, LWDETR_ATTN_MMA = 1, LWDETR_ATTN_MMA_SHORT = 2 };
+typedef struct {
+  int32_t dtype;
+  const void* q; int32_t ldq;
+  const void* k; int32_t ldk;
+  const void* v; int32_t ldv;
+  void* out; int32_t ldo;
+  int32_t nseq, seqlen, heads, dh;
+  float scale;
+  int32_t dry_run;
+  int32_t kernel, warps, poly_mask;   /* out */
+} lwdetr_attention_args;
+LWDETR_API int lwdetr_attention_ex(lwdetr_attention_args* args, void* stream);
 
 /* Multi-scale deformable attention forward with the REFERENCE OPERATOR'S OWN INTERFACE:
  *   MultiScaleDeformableAttention.ms_deform_attn_forward(value, spatial_shapes, level_start_index, sampling_loc,

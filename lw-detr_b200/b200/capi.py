@@ -25,6 +25,7 @@ _SIGNATURES = {
     "lwdetr_layernorm": (_i, [_i, _vp, _i, _vp, _i, _vp, _vp, _f, _i64, _i, _vp]),
     "lwdetr_layernorm_ex": (_i, [_i, _vp, _vp]),
     "lwdetr_attention": (_i, [_i, _vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _i, _f, _vp]),
+    "lwdetr_attention_ex": (_i, [_vp, _vp]),
     "lwdetr_ms_deform_attn_forward": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "lwdetr_ms_deform_attn_backward": (_i, [_vp] * 9 + [_i] * 8 + [_vp]),
     "lwdetr_msda_forward": (_i, [_i, _vp, _i64, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
@@ -252,6 +253,31 @@ def attention(q, k, v, out, nseq, seqlen, heads, dh, scale):
                                  ptr(out), out.stride(0), nseq, seqlen, heads, dh, scale, stream_ptr()),
           "lwdetr_attention")
     return out
+
+
+ATTN_KERNELS = {0: "wg", 1: "mma", 2: "mma_short"}
+
+
+class AttentionArgs(ctypes.Structure):
+    """lwdetr_attention_args (include/lwdetr_b200.h)."""
+    _fields_ = [("dtype", _i), ("q", _vp), ("ldq", _i), ("k", _vp), ("ldk", _i), ("v", _vp), ("ldv", _i), ("out", _vp), ("ldo", _i),
+                ("nseq", _i), ("seqlen", _i), ("heads", _i), ("dh", _i), ("scale", _f), ("dry_run", _i),
+                ("kernel", _i), ("warps", _i), ("poly_mask", _i)]
+
+
+def attention_ex(q, k, v, out, nseq, seqlen, heads, dh, scale, dry_run=False, dtype=None):
+    """lwdetr_attention_ex.  q / k / v / out: 2-D views [nseq*seqlen, heads*dh] (any row stride), or (address, leading
+    dimension) pairs of integers, which a dry run never dereferences (dtype then names the torch dtype).  Returns
+    {"kernel": "wg" | "mma" | "mma_short", "warps": 4 | 8 | 0, "poly_mask": 0 | 0x24 | 0x49} of the kernel that ran (dry_run:
+    would run; nothing is launched and no CUDA call is made)."""
+    def mat(t):
+        return t if isinstance(t, tuple) else (t.data_ptr(), t.stride(0))
+    a = AttentionArgs()
+    a.dtype = kernel_dtype_code(q.dtype if dtype is None else dtype)
+    (a.q, a.ldq), (a.k, a.ldk), (a.v, a.ldv), (a.out, a.ldo) = mat(q), mat(k), mat(v), mat(out)
+    a.nseq, a.seqlen, a.heads, a.dh, a.scale, a.dry_run = nseq, seqlen, heads, dh, float(scale), 1 if dry_run else 0
+    check(lib().lwdetr_attention_ex(ctypes.byref(a), None if dry_run else stream_ptr()), "lwdetr_attention_ex")
+    return {"kernel": ATTN_KERNELS[a.kernel], "warps": a.warps, "poly_mask": a.poly_mask}
 
 
 def value_to_head_major(value, B, S, M):

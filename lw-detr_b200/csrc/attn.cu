@@ -12,13 +12,14 @@
 //   attn_kernel       - sequences longer than 112 tokens (decoder self-attention)
 //   attn_short_kernel - sequences of up to 112 tokens, persistent CTAs walking (sequence, head) items
 // The packed qkv matrix of the ViT blocks is dispatched to the wgmma / TMA kernel in attn_wg.cu instead
-// (attention_launch below); these kernels serve q / k / v given as separate matrices.
+// (attention_plan below); these kernels serve q / k / v given as separate matrices.
 #include "attn.h"
 #include "launch.h"
 #include "ptx.cuh"
 
 #include <algorithm>
 #include <cstdlib>
+#include <string>
 
 namespace lwb {
 
@@ -135,9 +136,8 @@ __device__ __forceinline__ void attn_chunk(const uint32_t (&qf)[DH / 16][4], con
       }
       float p0, p1, p2, p3;
       if ((PM >> nt) & 1u) {
-        constexpr float kMagic = 12582912.f;
-        exp2_poly2(s[nt][0], s[nt][1], m_run[0] - 125.f * inv_scale_log2, c2, f2_pack(kMagic - msc[0], kMagic - msc[0]), f2_pack(-msc[0], -msc[0]), p0, p1);
-        exp2_poly2(s[nt][2], s[nt][3], m_run[1] - 125.f * inv_scale_log2, c2, f2_pack(kMagic - msc[1], kMagic - msc[1]), f2_pack(-msc[1], -msc[1]), p2, p3);
+        exp2_poly2(s[nt][0], s[nt][1], m_run[0] - 125.f * inv_scale_log2, c2, f2_pack(-msc[0], -msc[0]), p0, p1);
+        exp2_poly2(s[nt][2], s[nt][3], m_run[1] - 125.f * inv_scale_log2, c2, f2_pack(-msc[1], -msc[1]), p2, p3);
       } else {
         p0 = fast_exp2(fmaf(s[nt][0], scale_log2, -msc[0]));
         p1 = fast_exp2(fmaf(s[nt][1], scale_log2, -msc[0]));
@@ -396,40 +396,92 @@ static int poly_policy() {
   return v;
 }
 
+template <typename T, int DH>
+static int run_short(uint32_t pm, const AttnArgs& a, cudaStream_t st) {
+  if constexpr (DH != 64) {
+    if (pm == 0x24u) return launch_short<T, DH, 0x24u>(a, st);
+    if (pm == 0x49u) return launch_short<T, DH, 0x49u>(a, st);
+  }
+  return pm == 0 ? launch_short<T, DH>(a, st) : -2;
+}
+
+template <typename T, int DH>
+static int run_long(int warps, uint32_t pm, const AttnArgs& a, cudaStream_t st) {
+  if (warps == 4) return pm == 0 ? launch<T, DH, 4>(a, st) : -2;
+  if constexpr (DH != 64) {
+    if (pm == 0x24u) return launch<T, DH, 8, 0x24u>(a, st);
+    if (pm == 0x49u) return launch<T, DH, 8, 0x49u>(a, st);
+  }
+  return pm == 0 ? launch<T, DH, 8>(a, st) : -2;
+}
+
 template <typename T>
-static int dispatch(const AttnArgs& a, int dh, cudaStream_t st) {
-  const int pol = poly_policy();
-  if (a.seqlen <= 112) {
-    if (dh == 16) return pol == 1 ? launch_short<T, 16, 0x24u>(a, st) : pol == 2 ? launch_short<T, 16, 0x49u>(a, st) : launch_short<T, 16>(a, st);
-    if (dh == 32) return pol == 1 ? launch_short<T, 32, 0x24u>(a, st) : pol == 2 ? launch_short<T, 32, 0x49u>(a, st) : launch_short<T, 32>(a, st);
-    if (dh == 64) return launch_short<T, 64>(a, st);
-    return -2;
-  }
-  const int warps = a.seqlen >= 1024 ? 8 : 4;
-  if (warps == 8 && pol > 0) {
-    if (dh == 16) return pol == 1 ? launch<T, 16, 8, 0x24u>(a, st) : launch<T, 16, 8, 0x49u>(a, st);
-    if (dh == 32) return pol == 1 ? launch<T, 32, 8, 0x24u>(a, st) : launch<T, 32, 8, 0x49u>(a, st);
-  }
-#define LWB_ATTN_CASE(D, W) if (dh == D && warps == W) return launch<T, D, W>(a, st);
-  LWB_ATTN_CASE(16, 8) LWB_ATTN_CASE(16, 4)
-  LWB_ATTN_CASE(32, 8) LWB_ATTN_CASE(32, 4)
-  LWB_ATTN_CASE(64, 8) LWB_ATTN_CASE(64, 4)
-#undef LWB_ATTN_CASE
-  return -2;
+static int run_mma(const AttnPlan& pl, const AttnArgs& a, int dh, cudaStream_t st) {
+  if (pl.kernel == ATTN_MMA_SHORT)
+    return dh == 16 ? run_short<T, 16>(pl.poly_mask, a, st) : dh == 32 ? run_short<T, 32>(pl.poly_mask, a, st) : run_short<T, 64>(pl.poly_mask, a, st);
+  return dh == 16 ? run_long<T, 16>(pl.warps, pl.poly_mask, a, st) : dh == 32 ? run_long<T, 32>(pl.warps, pl.poly_mask, a, st)
+                                                                              : run_long<T, 64>(pl.warps, pl.poly_mask, a, st);
 }
 
 int attention_wg_launch(int dtype, const AttnArgs& a, int dh, int C, cudaStream_t st);      // attn_wg.cu
 
 // Packed qkv (the ViT blocks) runs on the wgmma / TMA kernel of attn_wg.cu at every sequence length; separate q / k / v
-// matrices (decoder self-attention) take the mma.sync kernels above.
-int attention_launch(int dtype, const AttnArgs& a, int dh, cudaStream_t st) {
+// matrices (decoder self-attention) take the mma.sync kernels above: attn_short_kernel up to 112 tokens, attn_kernel with 4
+// warps below 1024 tokens and with 8 from there.  Every kernel moves q / k / v / out rows in 16-byte pieces (cp.async, TMA,
+// U4 stores), so the matrices must start on 16-byte boundaries and their rows must be multiples of 8 elements.
+int attention_plan(int dtype, const AttnArgs& a, int dh, AttnPlan* plan, std::string* err) {
+  auto refuse = [err](const std::string& m) { *err = m; return -2; };
+  if (dtype != DT_F16 && dtype != DT_BF16) return refuse("dtype must be LWDETR_F16 or LWDETR_BF16");
+  if (dh != 16 && dh != 32 && dh != 64) return refuse("head dim must be 16, 32 or 64, got " + std::to_string(dh));
+  if (a.nseq < 1 || a.seqlen < 1 || a.heads < 1)
+    return refuse("nseq, seqlen and heads must be positive, got " + std::to_string(a.nseq) + ", " + std::to_string(a.seqlen) + ", " +
+                  std::to_string(a.heads));
+  const long long width = static_cast<long long>(a.heads) * dh;
+  if ((a.ldq | a.ldk | a.ldv | a.ldo) % 8) return refuse("leading dimensions must be multiples of 8");
+  if (a.ldq < width || a.ldk < width || a.ldv < width || a.ldo < width) return refuse("leading dimensions must be at least heads * dh");
+  const char* names[4] = {"q", "k", "v", "out"};
+  const void* ptrs[4] = {a.q, a.k, a.v, a.o};
+  for (int i = 0; i < 4; ++i)
+    if (reinterpret_cast<uintptr_t>(ptrs[i]) & 15) return refuse(std::string(names[i]) + " must be 16-byte aligned");
   const long long dk = (static_cast<const char*>(a.k) - static_cast<const char*>(a.q)) / 2;
   const long long dv = (static_cast<const char*>(a.v) - static_cast<const char*>(a.q)) / 2;
-  const bool packed = dk > 0 && dv == 2 * dk && a.ldq == a.ldk && a.ldq == a.ldv && dk == static_cast<long long>(a.heads) * dh &&
-                      a.ldq >= 3 * dk && (a.ldq % 8) == 0 && (reinterpret_cast<uintptr_t>(a.q) & 15) == 0 &&
-                      (a.ldo % 8) == 0 && (reinterpret_cast<uintptr_t>(a.o) & 15) == 0;   // TMA rows and the 16-byte output stores
-  if (packed && (dh == 16 || dh == 32 || dh == 64)) return attention_wg_launch(dtype, a, dh, static_cast<int>(dk), st);
-  return dtype == DT_BF16 ? dispatch<__nv_bfloat16>(a, dh, st) : dispatch<__half>(a, dh, st);
+  const bool packed = dk > 0 && dv == 2 * dk && a.ldq == a.ldk && a.ldq == a.ldv && dk == width && a.ldq >= 3 * dk;
+  AttnPlan p;
+  if (packed) {
+    // grid (query tiles, heads, nseq); the first row of a sequence is an int TMA coordinate
+    if (a.heads > 65535) return refuse("heads must be at most 65535 (grid y of attn_wg_kernel)");
+    if (a.nseq > 65535) return refuse("nseq must be at most 65535 (grid z of attn_wg_kernel)");
+    if (static_cast<long long>(a.nseq) * a.seqlen > 2147483647LL) return refuse("nseq * seqlen must be below 2^31 (attn_wg_kernel rows)");
+    p.kernel = ATTN_WG;
+    p.C = static_cast<int>(dk);
+  } else {
+    const int pol = poly_policy();
+    if (a.seqlen <= 112) {
+      p.kernel = ATTN_MMA_SHORT;
+      if (dh != 64) p.poly_mask = pol == 1 ? 0x24u : pol == 2 ? 0x49u : 0u;
+    } else {
+      // grid (query tiles, heads, nseq)
+      if (a.heads > 65535) return refuse("heads must be at most 65535 (grid y of attn_kernel)");
+      if (a.nseq > 65535) return refuse("nseq must be at most 65535 (grid z of attn_kernel)");
+      p.kernel = ATTN_MMA;
+      p.warps = a.seqlen >= 1024 ? 8 : 4;
+      if (p.warps == 8 && pol > 0 && dh != 64) p.poly_mask = pol == 1 ? 0x24u : 0x49u;
+    }
+  }
+  *plan = p;
+  return 0;
+}
+
+int attention_run(int dtype, const AttnArgs& a, int dh, const AttnPlan& plan, cudaStream_t st) {
+  if (plan.kernel == ATTN_WG) return attention_wg_launch(dtype, a, dh, plan.C, st);
+  return dtype == DT_BF16 ? run_mma<__nv_bfloat16>(plan, a, dh, st) : run_mma<__half>(plan, a, dh, st);
+}
+
+int attention_launch(int dtype, const AttnArgs& a, int dh, cudaStream_t st) {
+  AttnPlan plan;
+  std::string err;
+  if (attention_plan(dtype, a, dh, &plan, &err)) return -2;
+  return attention_run(dtype, a, dh, plan, st);
 }
 
 }  // namespace lwb

@@ -45,7 +45,27 @@ lwb::GemmDesc gemm_desc(const lwdetr_gemm_args& a) {
   d.hm_S = a.hm_S; d.hm_heads = a.hm_heads; d.hm_slices = a.hm_slices; d.row_zero = a.row_zero;
   return d;
 }
+// lwdetr_attention and lwdetr_attention_ex: check and plan (no CUDA call), report the plan, launch unless a dry run
+int attention_call(lwdetr_attention_args* p, void* stream, const char* fn) {
+  const std::string name(fn);
+  if (!p->q || !p->k || !p->v || !p->out) return fail(name + ": null pointer");
+  lwb::AttnArgs a{};
+  a.q = p->q; a.k = p->k; a.v = p->v; a.ldq = p->ldq; a.ldk = p->ldk; a.ldv = p->ldv; a.o = p->out; a.ldo = p->ldo;
+  a.seqlen = p->seqlen; a.nseq = p->nseq; a.heads = p->heads; a.scale_log2 = p->scale * 1.4426950408889634f;
+  lwb::AttnPlan plan;
+  std::string err;
+  if (lwb::attention_plan(p->dtype, a, p->dh, &plan, &err)) return fail(name + ": " + err);
+  p->kernel = plan.kernel;
+  p->warps = plan.warps;
+  p->poly_mask = static_cast<int32_t>(plan.poly_mask);
+  if (p->dry_run) return 0;
+  int e = lwb::attention_run(p->dtype, a, p->dh, plan, static_cast<cudaStream_t>(stream));
+  if (e) return cuda_fail(e, (name + " launch").c_str());
+  return 0;
+}
 }  // namespace
+
+static_assert(LWDETR_ATTN_WG == lwb::ATTN_WG && LWDETR_ATTN_MMA == lwb::ATTN_MMA && LWDETR_ATTN_MMA_SHORT == lwb::ATTN_MMA_SHORT, "attention kernel codes");
 
 extern "C" {
 
@@ -144,15 +164,13 @@ int lwdetr_layernorm_ex(int dtype, lwdetr_layernorm_args* p, void* stream) {
 
 int lwdetr_attention(int dtype, const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, void* out, int ldo,
                      int nseq, int seqlen, int heads, int dh, float scale, void* stream) {
-  if (!q || !k || !v || !out) return fail("lwdetr_attention: null pointer");
-  if ((ldq | ldk | ldv | ldo) % 8) return fail("lwdetr_attention: leading dimensions must be multiples of 8");
-  lwb::AttnArgs a{};
-  a.q = q; a.k = k; a.v = v; a.ldq = ldq; a.ldk = ldk; a.ldv = ldv; a.o = out; a.ldo = ldo; a.seqlen = seqlen; a.nseq = nseq;
-  a.heads = heads; a.scale_log2 = scale * 1.4426950408889634f;
-  int e = lwb::attention_launch(dtype, a, dh, static_cast<cudaStream_t>(stream));
-  if (e == -2) return fail("lwdetr_attention: head dim must be 16, 32 or 64");
-  if (e) return cuda_fail(e, "lwdetr_attention launch");
-  return 0;
+  lwdetr_attention_args a = {dtype, q, ldq, k, ldk, v, ldv, out, ldo, nseq, seqlen, heads, dh, scale};
+  return attention_call(&a, stream, "lwdetr_attention");
+}
+
+int lwdetr_attention_ex(lwdetr_attention_args* a, void* stream) {
+  if (!a) return fail("lwdetr_attention_ex: null pointer");
+  return attention_call(a, stream, "lwdetr_attention_ex");
 }
 
 int lwdetr_ms_deform_attn_forward(int etype, const void* value, const int64_t* spatial_shapes, const int64_t* level_start_index,

@@ -155,17 +155,19 @@ __device__ __forceinline__ uint64_t f2_mul(uint64_t a, uint64_t b) {
 
 
 // 2^(s*c - m) for a PAIR of scores without the MUFU (the exp-bound attention kernels can move a fraction of their exponentials
-// to the FMA pipe): t = round(s*c - m) + 1.5*2^23 by one FMA per score, the fraction f = s*c - m - round(..) in [-0.5, 0.5] by
-// two more, a degree-3 polynomial for 2^f (max relative error 7.5e-5, an order of magnitude below the 16-bit rounding
-// of P) and the integer part added into the exponent field.  The raw scores are clamped at smin = (m - 125)/c first:
-// below that 2^x is 0 for every purpose here, and an unclamped argument would wrap the exponent field.
-__device__ __forceinline__ void exp2_poly2(float s0, float s1, float smin, uint64_t c2, uint64_t magic_minus_m2, uint64_t negm2, float& e0, float& e1) {
+// to the FMA pipe): y = s*c - m by one FMA per score (the argument the MUFU path feeds ex2), t = round(y) + 1.5*2^23 by one
+// add, the fraction f = y - round(y) in [-0.5, 0.5] by two more, a degree-3 polynomial for 2^f (max relative error 7.5e-5 on
+// [-0.5, 0.5], an order of magnitude below the 16-bit rounding of P) and the integer part added into the exponent field.
+// y is formed before the magic add: 1.5*2^23 - m rounded to fp32 (ulp 1 there) would drop the fraction of m and leave f in
+// [-1, 1], where the polynomial is off by up to 1.2e-2.  The raw scores are clamped at smin = (m - 125)/c first: below
+// that 2^x is 0 for every purpose here, and an unclamped argument would wrap the exponent field.
+__device__ __forceinline__ void exp2_poly2(float s0, float s1, float smin, uint64_t c2, uint64_t negm2, float& e0, float& e1) {
   constexpr float kMagic = 12582912.f;   // 1.5 * 2^23
   const uint64_t s2 = f2_pack(fmaxf(s0, smin), fmaxf(s1, smin));
-  const uint64_t t2 = f2_fma(s2, c2, magic_minus_m2);
+  const uint64_t y2 = f2_fma(s2, c2, negm2);
+  const uint64_t t2 = f2_add(y2, f2_pack(kMagic, kMagic));
   const uint64_t r2 = f2_add(t2, f2_pack(-kMagic, -kMagic));
-  const uint64_t u2 = f2_fma(r2, f2_pack(-1.f, -1.f), negm2);
-  const uint64_t f2 = f2_fma(s2, c2, u2);
+  const uint64_t f2 = f2_fma(r2, f2_pack(-1.f, -1.f), y2);
   uint64_t p2 = f2_fma(f2, f2_pack(0.05517164617776871f, 0.05517164617776871f), f2_pack(0.2426111251115799f, 0.2426111251115799f));
   p2 = f2_fma(p2, f2, f2_pack(0.6932609677314758f, 0.6932609677314758f));
   p2 = f2_fma(p2, f2, f2_pack(0.9999280571937561f, 0.9999280571937561f));

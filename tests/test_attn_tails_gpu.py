@@ -1,6 +1,7 @@
 """The packed-qkv attention kernel (attn_wg.cu) against fp32 softmax attention at the last chunk of a sequence: keys
 beyond the sequence's end are masked, and a tail of at most 40 keys (the second chunk of a 100-token window) computes
-5 n-tiles of 8 keys instead of 8."""
+5 n-tiles of 8 keys instead of 8.  Every case passes one packed qkv matrix, so only the wgmma kernel runs here; the
+tails of the mma.sync kernels (decoder self-attention) are tested in test_attn_mma_gpu.py."""
 import pytest
 import torch
 

@@ -29,8 +29,9 @@ REL_L2 = {torch.float16: 1e-3, torch.bfloat16: 8e-3}
                                                   (2, 300, 12, 32), (5, 37, 4, 16),
                                                   # wgmma path (packed qkv): ragged tails, single-tile last CTA
                                                   (2, 700, 6, 32), (3, 640, 4, 64), (2, 520, 4, 32), (1, 1153, 4, 64),
-                                                  # head dim 16 at any length, head dim 32 windows: one to ten query tiles, ragged key
-                                                  # tails, a second warpgroup with no rows, many (window, head) items, single-item launches
+                                                  # wgmma path as well (every case here passes one packed qkv matrix; the decoder's
+                                                  # mma.sync kernels are tested in test_attn_mma_gpu.py): one to ten query tiles,
+                                                  # ragged key tails, a second warpgroup with no rows, many (window, head) CTAs
                                                   (3, 300, 4, 16), (2, 129, 4, 16), (1, 1153, 4, 16), (2, 513, 12, 16), (1, 64, 4, 16), (7, 128, 4, 16),
                                                   (640, 100, 12, 16), (70, 100, 12, 32), (3, 1, 4, 16), (2, 65, 4, 32)])
 def test_attention_matches_softmax_reference(dt, nseq, seqlen, heads, dh):
