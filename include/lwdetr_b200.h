@@ -699,6 +699,59 @@ LWDETR_API int lwdetr_gmc_estimate(lwdetr_gmc* g, const lwdetr_frame* frames, in
 LWDETR_API int lwdetr_gmc_estimate_nv12(lwdetr_gmc* g, const lwdetr_frame_nv12* frames, int B, const int32_t* stream_ids,
                                         double* motion, int32_t* status, int32_t* inliers, void* stream);
 
+/* Detection crops for second-stage networks (ReID, attribute, vehicle-type or plate models, a second detector pass): each
+ * box cut out of its frame on the device and resized to one out_h x out_w size, so no frame leaves the device and no host
+ * resize runs.  The C composition of tracking by a crop-based ReID network (BoT-SORT's FastReID configuration), with no
+ * synchronisation, so that it can be captured in one CUDA graph:
+ *   lwdetr_forward_frames (or _nv12) -> lwdetr_query_best -> lwdetr_crop_select (threshold = track_thresh: the high entries,
+ *   the only ones lwdetr_track_reid looks at) -> lwdetr_crops with N = B * k and the selection's device count -> the host's
+ *   own fixed-batch ReID engine on the N crops (rows past the count are left as they were) -> lwdetr_scatter_rows with the
+ *   same count -> lwdetr_track_reid.  tools/crop_spec.py restates this contract in numpy.
+ * Crop rectangle of a box (x1, y1, x2, y2), fp32 xyxy in the pixels of an h x w frame: cx0 = clamp(floor(x1), 0, w),
+ *   cx1 = clamp(floor(x2), 0, w), cy0 / cy1 likewise with h; the crop is rows [cy0, cy1) and columns [cx0, cx1).  It is
+ *   valid when cx1 > cx0, cy1 > cy0 and all four coordinates are finite.  This is the truncation of BoT-SORT's
+ *   tlbr.astype(int) slicing for boxes inside the frame; deviations: BoT-SORT clamps the end to w - 1 (here w: the last
+ *   column and row stay reachable), and an empty slice makes it fail (here: an invalid crop).
+ * Filters, per axis n_in (crop side) -> n_out, scale = n_in / n_out in fp32; horizontal pass, then vertical, both in fp32;
+ *   the result is rounded half up (floor(v + 0.5)) to a level and clamped to [0, 255]:
+ *   LWDETR_CROP_BILINEAR, cv2.resize(INTER_LINEAR) as BoT-SORT / FastReID use it: f = (o + 0.5) * scale - 0.5 (fp32, each
+ *     operation rounded), s = floor(f), t = f - s; s < 0 gives s = 0, t = 0; s >= n_in - 1 gives the one tap n_in - 1;
+ *     otherwise taps s, s + 1 with weights 1 - t, t.  No antialiasing.  Within one level of cv2, not equal to it: cv2 uses
+ *     11-bit fixed-point weights (on random crops some 12 % of values differ by one level).
+ *   LWDETR_CROP_ANTIALIAS: the triangle filter of lwdetr_frame (PIL / F.interpolate(antialias=True), the torchreid-style
+ *     pipelines), at ANY downscale: boxes are device data, so nothing can be refused per crop, and a whole 8192-pixel frame
+ *     to an 8-pixel side is computed exactly.  (The frame path's limit of 16x per axis does not apply here.)
+ * Values: normalize != 0: (v / 255 - mean[c]) / std[c] as for lwdetr_frame; normalize = 0: the level v itself (FastReID
+ *   normalises inside the model and takes 0..255).  RGB channel order.  NV12 frames: every source pixel converted as
+ *   lwdetr_frame_nv12 states, chroma at (y >> 1, x >> 1) of the WHOLE frame, so crops at odd offsets are exact: the result
+ *   is the RGB result of the converted frame.
+ * lwdetr_crops / _nv12: frames a HOST array of B descriptors (B in [1, 1024]; dst_h / dst_w are not read; the caller may
+ *   reuse it as soon as the call returns), sources as lwdetr_frame allows (sides in [8, 8192], any pitch and alignment);
+ *   boxes fp32 [N, 4] and frame_index int32 [N] (the frame of each box; one outside [0, B) makes an invalid crop), N in
+ *   [1, 65536]; count int32 [1] or NULL: crops at or past *count are not written (nor their flags); out [N, 3, out_h, out_w]
+ *   NCHW of out_dtype (LWDETR_ET_F32, _F16 or _BF16), out sides in [8, 1024]; valid int8 [N]: 1 for a valid crop, 0 for an
+ *   invalid one, whose output is zeros.  All DEVICE.  Asynchronous, nothing allocated or copied per call, safe to capture in
+ *   a CUDA graph; stream-ordered like lwdetr_forward_frames.
+ * lwdetr_crop_select: entries scores fp32 [B, k] and xyxy boxes fp32 [B, k, 4] (lwdetr_query_best's or lwdetr_tile_merge's
+ *   output), frame_hw a HOST int32 [B][2] array of each frame's (height, width).  Keeps every entry with score > threshold
+ *   whose crop is valid, in (frame, entry) order (an ordered compaction: deterministic): frame_of int32, entry int32 (the
+ *   flat index b * k + j) and sel_boxes fp32 [., 4] of each, and *count, all DEVICE with room for B * k rows; rows past the
+ *   count are not written.  B in [1, 1024], k >= 1.  Asynchronous, graph-safe.
+ * lwdetr_scatter_rows: rows [N, D] of etype (LWDETR_ET_F32, _F16 or _BF16; row stride ld_rows >= D elements) -> out
+ *   [num_out, D] dense of the same type: row i < *count (count NULL: i < N) goes to row entry[i], every other row is zeros
+ *   (a zero embedding is "no appearance" for lwdetr_track_reid).  All DEVICE.  Asynchronous, graph-safe. */
+enum { LWDETR_CROP_BILINEAR = 0, LWDETR_CROP_ANTIALIAS = 1 };
+LWDETR_API int lwdetr_crops(const lwdetr_frame* frames, int B, const float* boxes, const int32_t* frame_index, int N, const int32_t* count,
+                            int out_h, int out_w, int filter, int normalize, const float mean[3], const float std[3], int out_dtype,
+                            void* out, int8_t* valid, void* stream);
+LWDETR_API int lwdetr_crops_nv12(const lwdetr_frame_nv12* frames, int B, const float* boxes, const int32_t* frame_index, int N,
+                                 const int32_t* count, int out_h, int out_w, int filter, int normalize, const float mean[3],
+                                 const float std[3], int out_dtype, void* out, int8_t* valid, void* stream);
+LWDETR_API int lwdetr_crop_select(const float* scores, const float* boxes, int B, int k, const int32_t* frame_hw, float threshold,
+                                  int32_t* frame_of, int32_t* entry, float* sel_boxes, int32_t* count, void* stream);
+LWDETR_API int lwdetr_scatter_rows(int etype, const void* rows, int ld_rows, int D, const int32_t* entry, const int32_t* count, int N,
+                                   void* out, int num_out, void* stream);
+
 /* Multi-GPU init (SURVEY.md 8e): ONE ncclBroadcast of the packed weight arena from rank `root`, stream-ordered on
  * `stream`; the only collective of the path (images shard across ranks as independent replicas, nothing on the hot path).
  * Every rank first calls lwdetr_load_weights with tensors of the right shapes (any values on the non-root ranks): that

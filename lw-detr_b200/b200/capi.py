@@ -54,6 +54,10 @@ _SIGNATURES = {
     "lwdetr_gmc_estimate": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_gmc_estimate_nv12": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_query_best": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "lwdetr_crops": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
+    "lwdetr_crops_nv12": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
+    "lwdetr_crop_select": (_i, [_vp, _vp, _i, _i, _vp, _f, _vp, _vp, _vp, _vp, _vp]),
+    "lwdetr_scatter_rows": (_i, [_i, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp]),
     "lwdetr_layernorm_e4m3": (_i, [_vp, _i, _i64, _i, _f, _vp, _i, _vp, _vp]),
     "lwdetr_gemm_e4m3": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _i, _vp]),
     "lwdetr_vit_mlp": (_i, [_i, _vp, _i, _i, _vp, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp]),
@@ -998,6 +1002,99 @@ def resize_patches(frames, dsts, size, dtype, mean=None, std=None, want_mask=Fal
     check(getattr(lib(), name)(kernel_dtype_code(dtype), fb.descs(dsts), B, H, W, ctypes.cast(_norm3(mean), _vp),
                                ctypes.cast(_norm3(std), _vp), ptr(A), ptr(mask), stream_ptr(dev)), name)
     return A, mask
+
+
+CROP_FILTERS = {"bilinear": 0, "antialias": 1}     # LWDETR_CROP_BILINEAR (cv2 INTER_LINEAR) / LWDETR_CROP_ANTIALIAS (PIL triangle)
+_ET_OF = {"float32": ET_F32, "float16": ET_F16, "bfloat16": ET_BF16}
+
+
+def _et_code(dtype, what):
+    code = _ET_OF.get(str(dtype).replace("torch.", ""))
+    if code is None:
+        raise RuntimeError("%s: dtype must be float32, float16 or bfloat16, got %s" % (what, dtype))
+    return code
+
+
+def crops(frames, boxes, frame_index, size=(256, 128), filter="bilinear", mean=None, std=None, normalize=True, dtype=None,
+          count=None, colorspace=None, out=None, valid=None):
+    """lwdetr_crops(_nv12): each box cut out of its frame on the device and resized to size = (h, w) (include/lwdetr_b200.h).
+    frames: RGB or NV12 (capi.Frames, or frames as Frames takes them with colorspace); boxes fp32 [N, 4] xyxy in frame pixels
+    and frame_index int [N] (CUDA).  filter "bilinear" (cv2.resize INTER_LINEAR, BoT-SORT / FastReID) or "antialias" (the PIL
+    triangle filter of the frame path, any downscale).  normalize: (v / 255 - mean) / std (default ImageNet's), else the
+    level 0..255 itself.  dtype float32 (default), float16 or bfloat16.  count: CUDA int32 [1]; crops at or past it are not
+    written (out / valid may be passed to keep their earlier contents there).  Returns (crops [N, 3, h, w], valid bool [N]):
+    an invalid crop (empty or non-finite box) is zeros.  Stream-ordered, no synchronisation."""
+    import torch
+    if filter not in CROP_FILTERS:
+        raise RuntimeError("crops: filter must be one of %s, got %r" % (", ".join(CROP_FILTERS), filter))
+    fb = frames if isinstance(frames, Frames) else Frames(frames, colorspace=colorspace)
+    dev, B = fb.device, len(fb.items)
+    dtype = torch.float32 if dtype is None else dtype
+    code = _et_code(dtype, "crops")
+    if boxes.dim() != 2 or boxes.shape[1] != 4 or tuple(frame_index.shape) != (boxes.shape[0],):
+        raise RuntimeError("crops: boxes must be [N, 4] and frame_index [N], got %s and %s" % (tuple(boxes.shape), tuple(frame_index.shape)))
+    N = boxes.shape[0]
+    h, w = int(size[0]), int(size[1])
+    boxes = boxes.to(device=dev, dtype=torch.float32).contiguous()
+    fidx = frame_index.to(device=dev, dtype=torch.int32).contiguous()
+    if out is None:
+        out = torch.empty(N, 3, h, w, device=dev, dtype=dtype)
+    if valid is None:
+        valid = torch.empty(N, device=dev, dtype=torch.int8)
+    if tuple(out.shape) != (N, 3, h, w) or out.dtype != dtype or not out.is_contiguous() or valid.dtype != torch.int8 or valid.numel() != N:
+        raise RuntimeError("crops: out must be a contiguous [%d, 3, %d, %d] %s tensor and valid int8 [%d]" % (N, h, w, dtype, N))
+    if count is not None:
+        count = count.to(device=dev, dtype=torch.int32).contiguous()
+    mean, std = IMAGENET_MEAN if mean is None else mean, IMAGENET_STD if std is None else std
+    if N:
+        name = "lwdetr_crops_nv12" if fb.nv12 else "lwdetr_crops"
+        check(getattr(lib(), name)(fb.descs(fb.sizes), B, ptr(boxes), ptr(fidx), N, ptr(count), h, w, CROP_FILTERS[filter],
+                                   1 if normalize else 0, ctypes.cast(_norm3(mean), _vp), ctypes.cast(_norm3(std), _vp), code, ptr(out),
+                                   ptr(valid), stream_ptr(dev)), name)
+    return out, valid.view(torch.bool)
+
+
+def crop_select(scores, boxes, sizes, threshold):
+    """lwdetr_crop_select: the entries (scores fp32 [B, k], xyxy boxes fp32 [B, k, 4], CUDA; sizes: each frame's (h, w)) with
+    score > threshold and a valid crop, in (frame, entry) order -> (frame int32 [B*k], entry int32 [B*k] (flat b * k + j),
+    boxes fp32 [B*k, 4], count int32 [1]), all CUDA; rows at or past the count are not written.  No synchronisation."""
+    import torch
+    B, k = scores.shape
+    if tuple(boxes.shape) != (B, k, 4) or len(sizes) != B:
+        raise RuntimeError("crop_select: scores %s, boxes %s and %d frame sizes do not describe one [B, k] set"
+                           % (tuple(scores.shape), tuple(boxes.shape), len(sizes)))
+    dev = scores.device
+    scores = scores.to(dtype=torch.float32).contiguous()
+    boxes = boxes.to(device=dev, dtype=torch.float32).contiguous()
+    hw = (ctypes.c_int32 * (2 * B))(*[int(v) for s in sizes for v in s])
+    frame = torch.empty(B * k, device=dev, dtype=torch.int32)
+    entry = torch.empty(B * k, device=dev, dtype=torch.int32)
+    sel = torch.empty(B * k, 4, device=dev, dtype=torch.float32)
+    count = torch.empty(1, device=dev, dtype=torch.int32)
+    check(lib().lwdetr_crop_select(ptr(scores), ptr(boxes), B, k, ctypes.cast(hw, _vp), float(threshold), ptr(frame), ptr(entry), ptr(sel),
+                                   ptr(count), stream_ptr(dev)), "lwdetr_crop_select")
+    return frame, entry, sel, count
+
+
+def scatter_rows(rows, entry, num_out, count=None):
+    """lwdetr_scatter_rows: rows [N, D] (CUDA float32 / float16 / bfloat16, last dimension contiguous) -> [num_out, D] of
+    the same dtype with row i (i < count, default N) at entry[i] and zeros elsewhere.  No synchronisation."""
+    import torch
+    N, D = rows.shape
+    if rows.stride(1) != 1:
+        rows = rows.contiguous()
+    code = _et_code(rows.dtype, "scatter_rows")
+    entry = entry.to(device=rows.device, dtype=torch.int32).contiguous()
+    if entry.numel() < N:
+        raise RuntimeError("scatter_rows: %d entries for %d rows" % (entry.numel(), N))
+    out = torch.empty(int(num_out), D, device=rows.device, dtype=rows.dtype)
+    if count is not None:
+        count = count.to(device=rows.device, dtype=torch.int32).contiguous()
+    if N == 0:
+        return out.zero_()
+    check(lib().lwdetr_scatter_rows(code, ptr(rows), rows.stride(0), D, ptr(entry), ptr(count), N, ptr(out), int(num_out),
+                                    stream_ptr(rows.device)), "lwdetr_scatter_rows")
+    return out
 
 
 class AuxOut(ctypes.Structure):

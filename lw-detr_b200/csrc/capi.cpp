@@ -13,6 +13,7 @@
 #include <vector>
 
 #include "attn.h"
+#include "crops.h"
 #include "engine.h"
 #include "gemm_tc.h"
 #include "gmc.h"
@@ -932,7 +933,78 @@ static int resize_patches(const char* fn, int dtype, const F* frames, int B, int
   return 0;
 }
 
+// lwdetr_crops and lwdetr_crops_nv12
+template <typename F>
+static int crops_call(const char* fn, const F* frames, int B, const float* boxes, const int32_t* frame_index, int N, const int32_t* count,
+                      int out_h, int out_w, int filter, int normalize, const float mean[3], const float std[3], int out_dtype, void* out,
+                      int8_t* valid, void* stream) {
+  const std::string f(fn);
+  if (!frames || !boxes || !frame_index || !out || !valid || (normalize && (!mean || !std))) return fail(f + ": null pointer");
+  if (B < 1 || B > lwb::kCropMaxFrames) return fail(f + ": B must be in [1, " + std::to_string(lwb::kCropMaxFrames) + "]");
+  if (N < 1 || N > lwb::kCropMaxCount) return fail(f + ": N must be in [1, " + std::to_string(lwb::kCropMaxCount) + "]");
+  if (out_h < lwb::kCropMinSide || out_w < lwb::kCropMinSide || out_h > lwb::kCropMaxSide || out_w > lwb::kCropMaxSide)
+    return fail(f + ": output sides must be in [" + std::to_string(lwb::kCropMinSide) + ", " + std::to_string(lwb::kCropMaxSide) + "]");
+  if (filter != LWDETR_CROP_BILINEAR && filter != LWDETR_CROP_ANTIALIAS) return fail(f + ": filter must be LWDETR_CROP_BILINEAR or LWDETR_CROP_ANTIALIAS");
+  if (out_dtype != LWDETR_ET_F32 && out_dtype != LWDETR_ET_F16 && out_dtype != LWDETR_ET_BF16)
+    return fail(f + ": out_dtype must be LWDETR_ET_F32, _F16 or _BF16");
+  if (reinterpret_cast<uintptr_t>(out) % (out_dtype == LWDETR_ET_F32 ? 4 : 2) || reinterpret_cast<uintptr_t>(boxes) % 4 ||
+      reinterpret_cast<uintptr_t>(frame_index) % 4 || reinterpret_cast<uintptr_t>(count) % 4)
+    return fail(f + ": out, boxes, frame_index and count must be aligned to their element size");
+  lwb::CropDesc d = {};
+  d.out_h = out_h; d.out_w = out_w; d.filter = filter; d.normalize = normalize ? 1 : 0; d.etype = out_dtype;
+  for (int c = 0; c < 3; ++c) {
+    d.mean[c] = normalize ? mean[c] : 0.f;
+    d.stdv[c] = normalize ? std[c] : 1.f;
+    if (!(d.stdv[c] > 0.f)) return fail(f + ": std must be positive");
+  }
+  std::string err;
+  if (lwb::crop_frames_check(frames, B, &err)) return fail(f + ": " + err);
+  const int e = lwb::crops_launch(frames, B, boxes, frame_index, N, count, d, out, valid, static_cast<cudaStream_t>(stream));
+  if (e == -2) return fail(f + ": the tap tables of these frame and output sizes exceed a CTA's shared memory");
+  if (e) return cuda_fail(e, (f + " launch").c_str());
+  return 0;
+}
+
 extern "C" {
+
+int lwdetr_crops(const lwdetr_frame* frames, int B, const float* boxes, const int32_t* frame_index, int N, const int32_t* count, int out_h,
+                 int out_w, int filter, int normalize, const float mean[3], const float std[3], int out_dtype, void* out, int8_t* valid,
+                 void* stream) {
+  return crops_call("lwdetr_crops", frames, B, boxes, frame_index, N, count, out_h, out_w, filter, normalize, mean, std, out_dtype, out,
+                    valid, stream);
+}
+
+int lwdetr_crops_nv12(const lwdetr_frame_nv12* frames, int B, const float* boxes, const int32_t* frame_index, int N, const int32_t* count,
+                      int out_h, int out_w, int filter, int normalize, const float mean[3], const float std[3], int out_dtype, void* out,
+                      int8_t* valid, void* stream) {
+  return crops_call("lwdetr_crops_nv12", frames, B, boxes, frame_index, N, count, out_h, out_w, filter, normalize, mean, std, out_dtype,
+                    out, valid, stream);
+}
+
+int lwdetr_crop_select(const float* scores, const float* boxes, int B, int k, const int32_t* frame_hw, float threshold, int32_t* frame_of,
+                       int32_t* entry, float* sel_boxes, int32_t* count, void* stream) {
+  if (!scores || !boxes || !frame_hw || !frame_of || !entry || !sel_boxes || !count) return fail("lwdetr_crop_select: null pointer");
+  if (B < 1 || B > lwb::kCropMaxFrames || k < 1) return fail("lwdetr_crop_select: need B in [1, 1024] and k >= 1");
+  if (threshold != threshold) return fail("lwdetr_crop_select: threshold is NaN");
+  for (int b = 0; b < B; ++b)
+    if (frame_hw[2 * b] < 1 || frame_hw[2 * b + 1] < 1) return fail("lwdetr_crop_select: frame " + std::to_string(b) + " has a side below 1");
+  const int e = lwb::crop_select_launch(scores, boxes, B, k, frame_hw, threshold, frame_of, entry, sel_boxes, count,
+                                        static_cast<cudaStream_t>(stream));
+  if (e) return cuda_fail(e, "lwdetr_crop_select launch");
+  return 0;
+}
+
+int lwdetr_scatter_rows(int etype, const void* rows, int ld_rows, int D, const int32_t* entry, const int32_t* count, int N, void* out,
+                        int num_out, void* stream) {
+  if (!rows || !entry || !out) return fail("lwdetr_scatter_rows: null pointer");
+  if (etype != LWDETR_ET_F32 && etype != LWDETR_ET_F16 && etype != LWDETR_ET_BF16) return fail("lwdetr_scatter_rows: etype must be LWDETR_ET_F32, _F16 or _BF16");
+  if (D < 1 || N < 1 || num_out < 1 || ld_rows < D) return fail("lwdetr_scatter_rows: need D, N and num_out >= 1 and ld_rows >= D");
+  const int es = etype == LWDETR_ET_F32 ? 4 : 2;
+  if (reinterpret_cast<uintptr_t>(rows) % es || reinterpret_cast<uintptr_t>(out) % es) return fail("lwdetr_scatter_rows: rows and out must be aligned to their element size");
+  const int e = lwb::scatter_rows_launch(etype, rows, ld_rows, D, entry, count, N, out, num_out, static_cast<cudaStream_t>(stream));
+  if (e) return cuda_fail(e, "lwdetr_scatter_rows launch");
+  return 0;
+}
 
 int lwdetr_forward_frames(lwdetr_handle* h, const lwdetr_frame* frames, const float mean[3], const float std[3], int B, int height,
                           int width, float* pred_logits, float* pred_boxes, const lwdetr_aux_out* aux, const int32_t* topk_override,

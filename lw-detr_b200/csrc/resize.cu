@@ -24,6 +24,7 @@
 // same way and converted once per CTA into the interleaved RGB rows the horizontal pass reads, so the NV12 result is the RGB
 // result of the converted frame by construction.  tools/yuv_spec.py restates the conversion.
 #include "resize.h"
+#include "frame.cuh"
 #include "gemm_tc.h"
 #include "launch.h"
 #include "ptx.cuh"
@@ -51,12 +52,6 @@ struct ResizeNorm {
   float mean[3], stdv[3];
 };
 static_assert(sizeof(FrameGroup<lwdetr_frame_nv12>) + sizeof(ResizeNorm) + 64 <= 4096, "NV12 group exceeds 4 KB of kernel parameters");
-
-// NV12 -> RGB rows of include/lwdetr_b200.h: cY, cRv, cGu, cGv, cBu per colorspace; codes 0 and 1 are limited range
-__constant__ int kCsc[4][5] = {{1220542, 1673527, -409993, -852492, 2116026},
-                               {1220945, 1879825, -223607, -558796, 2215014},
-                               {1048576, 1470104, -360853, -748826, 1858077},
-                               {1048576, 1651297, -196424, -490864, 1945738}};
 
 // bytes of one staged source row: the 16-byte aligned global span covering `nbytes` from any start address
 __host__ __device__ inline int staged_row_bytes(int nbytes) { return ((nbytes + 15) & ~15) + 16; }
@@ -105,7 +100,6 @@ __device__ __forceinline__ const uint8_t* src_col(const lwdetr_frame& f, int x) 
 __device__ __forceinline__ const uint8_t* src_col(const lwdetr_frame_nv12& f, int x) { return f.luma + x; }
 __device__ __forceinline__ long long src_pitch(const lwdetr_frame& f) { return f.pitch_bytes; }
 __device__ __forceinline__ long long src_pitch(const lwdetr_frame_nv12& f) { return f.luma_pitch; }
-__device__ __forceinline__ int shift20(int v) { return min(max((v + (1 << 19)) >> 20, 0), 255); }
 }  // namespace
 
 // F: the source format, lwdetr_frame (packed RGB) or lwdetr_frame_nv12.  Only the staging of a chunk's source rows differs:
@@ -259,22 +253,6 @@ __global__ void __launch_bounds__(256) frame_mask_kernel(const __grid_constant__
 }
 
 namespace {
-// what is wrong with a frame's plane pointers, and (checked after its sides) with its pitches and colour space: "" when nothing
-std::string pointers_error(const lwdetr_frame& f) { return f.data ? "" : "null data pointer"; }
-std::string pointers_error(const lwdetr_frame_nv12& f) { return !f.luma ? "null luma pointer" : !f.chroma ? "null chroma pointer" : ""; }
-std::string layout_error(const lwdetr_frame& f) {
-  if (f.pitch_bytes < 3LL * f.width) return "pitch_bytes " + std::to_string(f.pitch_bytes) + " is smaller than 3 * width";
-  return "";
-}
-std::string layout_error(const lwdetr_frame_nv12& f) {
-  if (f.luma_pitch < f.width) return "luma_pitch " + std::to_string(f.luma_pitch) + " is smaller than width";
-  const long long cw = 2LL * ((f.width + 1) / 2);
-  if (f.chroma_pitch < cw) return "chroma_pitch " + std::to_string(f.chroma_pitch) + " is smaller than 2 * ceil(width / 2) = " + std::to_string(cw);
-  if (f.colorspace < LWDETR_CSC_BT601_LIMITED || f.colorspace > LWDETR_CSC_BT709_FULL)
-    return "unknown colorspace " + std::to_string(f.colorspace) + " (LWDETR_CSC_BT601_LIMITED .. LWDETR_CSC_BT709_FULL)";
-  return "";
-}
-
 template <typename F>
 int frames_check_impl(const F* frames, int B, int H, int W, std::string* err) {
   for (int b = 0; b < B; ++b) {

@@ -206,7 +206,8 @@ class LWDETR(nn.Module):
 
     @torch.no_grad()
     def track(self, frames, tracker, streams=None, size=None, fit="stretch", short_side=None, max_side=None, colorspace=None,
-              max_out=None, motion=None, appearance=False):
+              max_out=None, motion=None, appearance=False, reid=None, reid_size=(256, 128), reid_filter="bilinear", reid_mean=None,
+              reid_std=None, reid_normalize=True):
         """Multi-object tracking of video streams: frames (RGB or NV12, taken exactly as detect() takes them) run as one
         forward; each query gives one detection, its best class (capi.query_best, boxes in the frame's original pixels);
         then capi.Tracker `tracker` (ByteTrack on the device, include/lwdetr_b200.h) updates each frame's stream.
@@ -221,8 +222,16 @@ class LWDETR(nn.Module):
         query, Engine.forward_frames(want_hidden=True)) to Tracker.update(embeddings=...), BoT-SORT's appearance cost with
         the detector's own features; the tracker's embedding_dim must be hidden_dim.  A CUDA tensor [len(frames),
         num_queries, D] passes the caller's own embeddings instead (any ReID model's).  With motion= as well this is
-        BoT-SORT with both compensations.  How ByteTrack's thresholds (tuned on YOLOX scores) suit LW-DETR's score
-        distribution, and whether the decoder's features tell identities apart on real footage, in MOTA / IDF1 / HOTA, is
+        BoT-SORT with both compensations.
+        reid (a tracker made with embedding_dim D): a crop-based ReID network, any callable taking crops [N, 3, h, w] and
+        returning [N, D] (BoT-SORT's FastReID configuration); not combined with appearance=.  The entries the appearance cost
+        looks at (score > the tracker's track_thresh) with a valid crop are selected on the device (capi.crop_select), cut out
+        of the frames and resized to reid_size = (h, w) by reid_filter ("bilinear": cv2 INTER_LINEAR, as FastReID; or
+        "antialias"), with (v / 255 - reid_mean) / reid_std (default ImageNet's), or the levels 0..255 with
+        reid_normalize=False (capi.crops, float32); reid runs once on all of them under no_grad, and its rows are scattered
+        back to their entries (zeros elsewhere: no appearance).  Zero crops: reid is not called.  This costs one extra
+        synchronisation per call, the read-back of the crop count that sizes reid's batch.
+        How ByteTrack's thresholds (tuned on YOLOX scores) suit LW-DETR's score distribution, and whether the decoder's features tell identities apart on real footage, in MOTA / IDF1 / HOTA, is
         not measured here."""
         if self.training:
             raise RuntimeError("lwdetr_b200 implements the inference forward only; call model.eval()")
@@ -235,6 +244,11 @@ class LWDETR(nn.Module):
         if len(streams) != n:
             raise RuntimeError("lwdetr_b200: %d streams for %d frames" % (len(streams), n))
         emb = None
+        if reid is not None:
+            if not (appearance is False or appearance is None):
+                raise RuntimeError("lwdetr_b200: pass reid= or appearance=, not both")
+            if tracker.embedding_dim is None:
+                raise RuntimeError("lwdetr_b200: reid= needs a tracker made with embedding_dim")
         if isinstance(appearance, torch.Tensor):
             if tuple(appearance.shape[:2]) != (n, self.num_queries) or appearance.dim() != 3:
                 raise RuntimeError("lwdetr_b200: appearance must be [%d, %d, D], got %s" % (n, self.num_queries, tuple(appearance.shape)))
@@ -250,6 +264,8 @@ class LWDETR(nn.Module):
             emb = out["hidden"]
         sizes = torch.tensor(fb.sizes, dtype=torch.float32, device=dev)
         scores, labels, boxes = capi.query_best(out["pred_logits"], out["pred_boxes"], sizes)
+        if reid is not None:
+            emb = self._reid_embeddings(fb, scores, boxes, tracker, reid, reid_size, reid_filter, reid_mean, reid_std, reid_normalize)
         rounds, seen = [], {}
         for i, s in enumerate(streams):
             r = seen.get(s, 0)
@@ -280,6 +296,37 @@ class LWDETR(nn.Module):
             dets.append({"ids": ids[j, :c], "scores": sc[j, :c], "labels": lab[j, :c].long(), "boxes": bx[j, :c],
                          "queries": q[j, :c].long()})
         return dets
+
+    def _reid_embeddings(self, fb, scores, boxes, tracker, reid, size, filter, mean, std, normalize):
+        """[frames, num_queries, D] embeddings of the high entries by the crop-based network `reid`, zeros elsewhere; None when
+        no entry has a crop."""
+        frame, entry, sel, count = capi.crop_select(scores, boxes, fb.sizes, float(tracker.params.track_thresh))
+        c = int(count.item())                     # sizes reid's batch: the call's one extra synchronisation
+        if c == 0:
+            return None
+        crops, _ = capi.crops(fb, sel[:c], frame[:c], size, filter, mean, std, normalize)
+        with torch.no_grad():
+            rows = reid(crops)
+        D = tracker.embedding_dim
+        if not isinstance(rows, torch.Tensor) or tuple(rows.shape) != (c, D):
+            raise RuntimeError("lwdetr_b200: reid must return [%d, %d] (crops, the tracker's embedding_dim), got %s"
+                               % (c, D, tuple(rows.shape) if isinstance(rows, torch.Tensor) else type(rows)))
+        return capi.scatter_rows(rows, entry[:c], scores.numel()).view(scores.shape[0], scores.shape[1], D)
+
+    @torch.no_grad()
+    def crops(self, frames, dets, size=(256, 128), filter="bilinear", mean=None, std=None, normalize=True, dtype=None, colorspace=None):
+        """The input of a second-stage network (ReID, attributes, vehicle type, plates) from detect()'s per-frame result
+        list: every box of every frame cut out of its frame on the device and resized to size = (h, w) (capi.crops: filter,
+        mean / std / normalize and dtype as there).  Returns (crops [N, 3, h, w], frame_of_each int64 [N]), boxes in frame
+        order, then the order of each frame's list; a box with an empty or non-finite crop gives zeros."""
+        fb = capi.Frames(frames, next(self.parameters()).device, colorspace)
+        if len(dets) != len(fb.items):
+            raise RuntimeError("lwdetr_b200: %d detection lists for %d frames" % (len(dets), len(fb.items)))
+        dev = fb.device
+        boxes = [d["boxes"].to(device=dev, dtype=torch.float32).reshape(-1, 4) for d in dets]
+        frame = torch.cat([torch.full((b.shape[0],), f, dtype=torch.int64, device=dev) for f, b in enumerate(boxes)])
+        out, _ = capi.crops(fb, torch.cat(boxes), frame, size, filter, mean, std, normalize, dtype)
+        return out, frame
 
     def _pack_outputs(self, out):
         if self._export:
