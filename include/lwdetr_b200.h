@@ -346,7 +346,8 @@ LWDETR_API int lwdetr_tile_merge(const float* scores, const int32_t* labels, con
  *
  * lwdetr_tracker_create: num_streams >= 1 independent streams, params validated (thresholds in [0, 1], the three
  *   association thresholds in (0, 1], capacity in [1, 1024], track_buffer >= 0, frame_rate >= 1); allocates the device
- *   table (num_streams * capacity * 2 records) on the current device, every stream at frame 1.  Synchronous.
+ *   table (num_streams * capacity * 2 records) on the current device, every stream at frame 1.  Synchronous, on a
+ *   stream of the tracker's own.
  * lwdetr_tracker_reset: the n streams listed (HOST array; ids distinct and in [0, num_streams), else an error and nothing
  *   happens) back to frame 1, next id 1, empty lists, overflow 0.
  * lwdetr_track: one frame for each of B streams (stream_ids, HOST; ids distinct and in [0, num_streams), else an error and
@@ -427,7 +428,8 @@ LWDETR_API int lwdetr_track_ex(lwdetr_tracker* t, const float* scores, const int
  *
  * lwdetr_tracker_create_reid: lwdetr_tracker_create plus the appearance state: the embedding table (num_streams *
  *   capacity * D * 4 bytes: one slot per track a stream can hold; a track keeps its slot for life, so nothing moves per
- *   frame), a slot per record and a per-stream scratch of 8192 proximity pairs (12 bytes each) per frame.  Synchronous.
+ *   frame), a slot per record and a per-stream scratch of 8192 proximity pairs (12 bytes each) per frame, in one
+ *   allocation with the table.  Synchronous, on a stream of the tracker's own.
  * lwdetr_track_reid: lwdetr_track_ex with embeddings DEVICE [B, k, D], row stride ld_emb >= D elements, of type emb_dtype
  *   (LWDETR_ET_F32, _F16 or _BF16: the engine's 16-bit rows need no conversion), aligned to their element size.  NULL
  *   embeddings, or a tracker made by lwdetr_tracker_create, give lwdetr_track_ex's bits.  Asynchronous, nothing allocated
@@ -493,7 +495,7 @@ LWDETR_API int lwdetr_tracker_export_embeddings(lwdetr_tracker* t, int stream_id
  * lwdetr_gmc_create: params validated (downscale in [1, 8], max_points in [16, 4096], quality in (0, 1], levels in [0, 5],
  *   window odd in [5, 31], iterations in [1, 100], eps > 0, min_eig >= 0, ransac_thresh > 0, hypotheses in [1, 4096],
  *   min_inliers in [2, max_points], max sides in [16 d, 8192]); allocates the device table (two pyramids and corner lists
- *   per stream, sized by the largest frame) on the current device.  Synchronous.
+ *   per stream, sized by the largest frame) on the current device.  Synchronous, on a stream of the estimator's own.
  * lwdetr_gmc_reset: the n streams listed (HOST; ids distinct and in [0, num_streams), else an error and nothing happens)
  *   start again at their next frame.
  * lwdetr_gmc_estimate / _nv12: one frame for each of B streams (stream_ids HOST; ids distinct and in [0, num_streams), else
@@ -513,12 +515,13 @@ LWDETR_API void lwdetr_gmc_params_default(lwdetr_gmc_params* p);
 LWDETR_API int lwdetr_gmc_create(int num_streams, const lwdetr_gmc_params* params, lwdetr_gmc** out);
 LWDETR_API void lwdetr_gmc_destroy(lwdetr_gmc* g);
 LWDETR_API int lwdetr_gmc_reset(lwdetr_gmc* g, const int32_t* streams, int n, void* stream);
-/* Inspection (tests), synchronous (waits for the device): one stream's state after its last frame.  levels: that frame's
- * pyramid, levels 0..info[3] one after another, each dense at its size (levels_bytes must hold them); corners float [max_points,
- * 2]: its corners (info[4] of them); flow float [max_points, 4] (from x, y, to x, y, level-0 pixels) and found int8
- * [max_points]: the last call's Lucas-Kanade results for the previous frame's info[5] corners (meaningful when that call had
- * a previous frame of the same size).  info = (has a last frame, its height, its width, levels used or -1, corners, corners
- * of the previous frame). */
+/* Inspection (tests), synchronous: it waits for the estimator's last lwdetr_gmc_estimate / _nv12 / lwdetr_gmc_reset launch
+ * (also when that launch was replayed from a CUDA graph) and for nothing else on the device, then copies one stream's state
+ * after its last frame.  levels: that frame's pyramid, levels 0..info[3] one after another, each dense at its size
+ * (levels_bytes must hold them); corners float [max_points, 2]: its corners (info[4] of them); flow float [max_points, 4]
+ * (from x, y, to x, y, level-0 pixels) and found int8 [max_points]: the last call's Lucas-Kanade results for the previous
+ * frame's info[5] corners (meaningful when that call had a previous frame of the same size).  info = (has a last frame, its
+ * height, its width, levels used or -1, corners, corners of the previous frame). */
 LWDETR_API int lwdetr_gmc_export(lwdetr_gmc* g, int stream_id, uint8_t* levels, int64_t levels_bytes, float* corners, float* flow,
                                  int8_t* found, int32_t info[6]);
 

@@ -484,55 +484,34 @@ def _emb_dtype(dtype):
     return codes[dtype]
 
 
-class Tracker:
-    """ByteTrack on the device for num_streams camera streams (lwdetr_tracker_*, the contract in include/lwdetr_b200.h).
-    Parameters are lwdetr_track_params' fields, ByteTrack's defaults unless given; new_track_thresh defaults to
-    track_thresh + 0.1.  With embedding_dim (lwdetr_reid_params: embedding_dim, proximity_thresh, appearance_thresh,
-    ema_alpha; BoT-SORT's defaults unless given) the tracker also associates by appearance (BoT-SORT's re-identification
-    cost, lwdetr_track_reid); update() then takes embeddings.  All calls of one tracker must run on one CUDA stream (the
-    current one at each call)."""
+class _DeviceObject:
+    """What Tracker and MotionEstimator share: a C object made on one device from a parameter struct (its handle in _t),
+    reset per stream and destroyed by close()."""
 
-    REID = ("embedding_dim", "proximity_thresh", "appearance_thresh", "ema_alpha")
+    RESET = DESTROY = None                               # the subclass's C calls
 
-    def __init__(self, num_streams, device=None, **params):
+    def __init__(self, num_streams, device, create, *params):
         import torch
-        p = TrackParams()
-        lib().lwdetr_track_params_default(ctypes.byref(p))
-        reid = {n: params.pop(n) for n in self.REID if n in params and params[n] is not None}
-        for n in self.REID:
-            params.pop(n, None)
-        if reid and "embedding_dim" not in reid:
-            raise RuntimeError("Tracker: %s given without embedding_dim" % ", ".join(sorted(reid)))
-        names = {n for n, _ in TrackParams._fields_}
-        bad = set(params) - names
-        if bad:
-            raise RuntimeError("Tracker: unknown parameters %s" % ", ".join(sorted(bad)))
-        if params.get("new_track_thresh") is None:
-            params["new_track_thresh"] = params.get("track_thresh", 0.5) + 0.1
-        for n, v in params.items():
-            setattr(p, n, v)
-        self.params = p
         self.num_streams = int(num_streams)
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         self._t = _vp()
-        self.reid = None
-        if reid:
-            r = ReidParams()
-            lib().lwdetr_reid_params_default(ctypes.byref(r))
-            for n, v in reid.items():
-                setattr(r, n, v)
-            self.reid = r
-        self.embedding_dim = int(self.reid.embedding_dim) if self.reid is not None else None
         with torch.cuda.device(self.device):
-            if self.reid is None:
-                check(lib().lwdetr_tracker_create(self.num_streams, ctypes.byref(p), ctypes.byref(self._t)), "lwdetr_tracker_create")
-            else:
-                check(lib().lwdetr_tracker_create_reid(self.num_streams, ctypes.byref(p), ctypes.byref(self.reid), ctypes.byref(self._t)),
-                      "lwdetr_tracker_create_reid")
+            check(getattr(lib(), create)(self.num_streams, *[ctypes.byref(p) for p in params], ctypes.byref(self._t)), create)
+
+    def _params(self, struct, default, params):
+        """struct from the C call `default`, then the keyword arguments; a name struct lacks is an error."""
+        p = struct()
+        getattr(lib(), default)(ctypes.byref(p))
+        bad = set(params) - {n for n, _ in struct._fields_}
+        if bad:
+            raise RuntimeError("%s: unknown parameters %s" % (type(self).__name__, ", ".join(sorted(bad))))
+        for n, v in params.items():
+            setattr(p, n, v)
+        return p
 
     def close(self):
         if self._t:
-            lib().lwdetr_tracker_destroy(self._t)
+            getattr(lib(), self.DESTROY)(self._t)
             self._t = _vp()
 
     def __del__(self):
@@ -547,9 +526,38 @@ class Tracker:
         return (ctypes.c_int32 * max(len(ids), 1))(*ids), len(ids)
 
     def reset(self, streams):
-        """Streams back to frame 1 and id 1 with empty lists (stream-ordered)."""
+        """The streams start again (stream-ordered): a tracker's at frame 1 and id 1 with empty lists, an estimator's at
+        their next frame."""
         arr, n = self._ids(streams)
-        check(lib().lwdetr_tracker_reset(self._t, ctypes.cast(arr, _vp), n, stream_ptr(self.device)), "lwdetr_tracker_reset")
+        check(getattr(lib(), self.RESET)(self._t, ctypes.cast(arr, _vp), n, stream_ptr(self.device)), self.RESET)
+
+
+class Tracker(_DeviceObject):
+    """ByteTrack on the device for num_streams camera streams (lwdetr_tracker_*, the contract in include/lwdetr_b200.h).
+    Parameters are lwdetr_track_params' fields, ByteTrack's defaults unless given; new_track_thresh defaults to
+    track_thresh + 0.1.  With embedding_dim (lwdetr_reid_params: embedding_dim, proximity_thresh, appearance_thresh,
+    ema_alpha; BoT-SORT's defaults unless given) the tracker also associates by appearance (BoT-SORT's re-identification
+    cost, lwdetr_track_reid); update() then takes embeddings.  All calls of one tracker must run on one CUDA stream (the
+    current one at each call)."""
+
+    REID = ("embedding_dim", "proximity_thresh", "appearance_thresh", "ema_alpha")
+    RESET, DESTROY = "lwdetr_tracker_reset", "lwdetr_tracker_destroy"
+
+    def __init__(self, num_streams, device=None, **params):
+        reid = {n: params.pop(n) for n in self.REID if n in params and params[n] is not None}
+        for n in self.REID:
+            params.pop(n, None)
+        if reid and "embedding_dim" not in reid:
+            raise RuntimeError("Tracker: %s given without embedding_dim" % ", ".join(sorted(reid)))
+        if params.get("new_track_thresh") is None:
+            params["new_track_thresh"] = params.get("track_thresh", 0.5) + 0.1
+        self.params = self._params(TrackParams, "lwdetr_track_params_default", params)
+        self.reid = self._params(ReidParams, "lwdetr_reid_params_default", reid) if reid else None
+        self.embedding_dim = int(self.reid.embedding_dim) if reid else None
+        if reid:
+            super().__init__(num_streams, device, "lwdetr_tracker_create_reid", self.params, self.reid)
+        else:
+            super().__init__(num_streams, device, "lwdetr_tracker_create", self.params)
 
     def update(self, scores, labels, boxes, stream_ids=None, max_out=None, motion=None, embeddings=None):
         """One frame for each of B distinct streams: scores fp32 [B, k], labels int [B, k], xyxy boxes fp32 [B, k, 4] (CUDA;
@@ -652,43 +660,17 @@ class GmcParams(ctypes.Structure):
 GMC_OK, GMC_FIRST_FRAME, GMC_SIZE_CHANGED, GMC_FEW_POINTS, GMC_FEW_INLIERS = 0, 1, 2, 3, 4
 
 
-class MotionEstimator:
+class MotionEstimator(_DeviceObject):
     """Camera motion per video stream on the device (lwdetr_gmc_*, the contract in include/lwdetr_b200.h): the similarity
     from each stream's previous frame to its current one, for Tracker.update(motion=...).  Parameters are
     lwdetr_gmc_params' fields (defaults: lwdetr_gmc_params_default; max_height / max_width bound the frames and size the
     device table).  All calls of one estimator must run on one CUDA stream (the current one at each call)."""
 
+    RESET, DESTROY = "lwdetr_gmc_reset", "lwdetr_gmc_destroy"
+
     def __init__(self, num_streams, device=None, **params):
-        import torch
-        p = GmcParams()
-        lib().lwdetr_gmc_params_default(ctypes.byref(p))
-        bad = set(params) - {n for n, _ in GmcParams._fields_}
-        if bad:
-            raise RuntimeError("MotionEstimator: unknown parameters %s" % ", ".join(sorted(bad)))
-        for n, v in params.items():
-            setattr(p, n, v)
-        self.params = p
-        self.num_streams = int(num_streams)
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        self._g = _vp()
-        with torch.cuda.device(self.device):
-            check(lib().lwdetr_gmc_create(self.num_streams, ctypes.byref(p), ctypes.byref(self._g)), "lwdetr_gmc_create")
-
-    def close(self):
-        if self._g:
-            lib().lwdetr_gmc_destroy(self._g)
-            self._g = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def reset(self, streams):
-        """The streams start again at their next frame (stream-ordered)."""
-        arr, n = Tracker._ids(streams)
-        check(lib().lwdetr_gmc_reset(self._g, ctypes.cast(arr, _vp), n, stream_ptr(self.device)), "lwdetr_gmc_reset")
+        self.params = self._params(GmcParams, "lwdetr_gmc_params_default", params)
+        super().__init__(num_streams, device, "lwdetr_gmc_create", self.params)
 
     def estimate(self, frames, streams=None):
         """One frame for each of B distinct streams (capi.Frames, or frames as Frames takes them; an NV12 frame is read
@@ -701,7 +683,7 @@ class MotionEstimator:
             nv12 = nv12 or (not isinstance(frames, torch.Tensor) and len(frames) > 0 and _is_nv12(frames[0]))
             frames = Frames(frames, self.device, "bt601" if nv12 else None)
         B = len(frames.items)
-        ids, n = Tracker._ids(range(B) if streams is None else streams)
+        ids, n = self._ids(range(B) if streams is None else streams)
         if n != B:
             raise RuntimeError("MotionEstimator.estimate: %d stream ids for %d frames" % (n, B))
         dev = self.device
@@ -710,13 +692,14 @@ class MotionEstimator:
         inliers = torch.empty(B, device=dev, dtype=torch.int32)
         descs = frames.descs(frames.sizes)
         name = "lwdetr_gmc_estimate_nv12" if frames.nv12 else "lwdetr_gmc_estimate"
-        check(getattr(lib(), name)(self._g, descs, B, ctypes.cast(ids, _vp), ptr(motion), ptr(status), ptr(inliers), stream_ptr(dev)), name)
+        check(getattr(lib(), name)(self._t, descs, B, ctypes.cast(ids, _vp), ptr(motion), ptr(status), ptr(inliers), stream_ptr(dev)), name)
         return motion, status, inliers
 
     def export(self, stream_id):
-        """Synchronous (waits for the device): one stream's state after its last frame (lwdetr_gmc_export) as a dict: levels
-        (list of uint8 [h_l, w_l] arrays), corners float32 [n, 2] (level-0 x, y), flow float32 [m, 4] and found bool [m]
-        (the last call's Lucas-Kanade of the previous frame's m corners), valid, size."""
+        """Synchronous, waiting for this estimator's last estimate() or reset() and for nothing else on the device: one
+        stream's state after its last frame (lwdetr_gmc_export) as a dict: levels (list of uint8 [h_l, w_l] arrays), corners
+        float32 [n, 2] (level-0 x, y), flow float32 [m, 4] and found bool [m] (the last call's Lucas-Kanade of the previous
+        frame's m corners), valid, size."""
         import numpy as np
         p = self.params
         cap = (p.max_height // p.downscale + 1) * (p.max_width // p.downscale + 1) * 2
@@ -725,7 +708,7 @@ class MotionEstimator:
         flow = np.zeros((p.max_points, 4), np.float32)
         found = np.zeros(p.max_points, np.int8)
         info = (ctypes.c_int32 * 6)()
-        check(lib().lwdetr_gmc_export(self._g, int(stream_id), lv.ctypes.data_as(_vp), cap, corners.ctypes.data_as(_vp),
+        check(lib().lwdetr_gmc_export(self._t, int(stream_id), lv.ctypes.data_as(_vp), cap, corners.ctypes.data_as(_vp),
                                       flow.ctypes.data_as(_vp), found.ctypes.data_as(_vp), ctypes.cast(info, _vp)), "lwdetr_gmc_export")
         valid, h, w, nlev, nc, nf = list(info)
         levels, o = [], 0

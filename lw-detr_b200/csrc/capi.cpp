@@ -7,7 +7,9 @@
 
 #include <string>
 
+#include <algorithm>
 #include <map>
+#include <memory>
 #include <new>
 #include <type_traits>
 #include <vector>
@@ -64,6 +66,99 @@ int attention_call(lwdetr_attention_args* p, void* stream, const char* fn) {
   if (e) return cuda_fail(e, (name + " launch").c_str());
   return 0;
 }
+
+// HOST stream ids of one call of a tracker or an estimator: distinct and in [0, num_streams); "" when they are
+std::string check_ids(int num_streams, const int32_t* ids, int n) {
+  std::vector<char> seen(static_cast<size_t>(num_streams), 0);
+  for (int i = 0; i < n; ++i) {
+    if (ids[i] < 0 || ids[i] >= num_streams)
+      return "stream id " + std::to_string(ids[i]) + " outside [0, " + std::to_string(num_streams) + ")";
+    if (seen[ids[i]]++) return "stream id " + std::to_string(ids[i]) + " appears twice in one call";
+  }
+  return "";
+}
+
+// Buffers one after another at 256-byte aligned offsets, cudaMalloc's alignment, on which the kernels' float4, double and
+// 16-byte pyramid accesses rely.  With a null base it only counts the bytes, so one layout function both sizes and assigns.
+struct Carver {
+  char* base = nullptr;
+  size_t bytes = 0;
+  template <class T> void take(T*& p, size_t n) {
+    bytes = (bytes + 255) / 256 * 256;
+    p = base ? reinterpret_cast<T*>(base + bytes) : nullptr;
+    bytes += n * sizeof(T);
+  }
+};
+
+// The device side of a tracker or an estimator: its buffers in one allocation, an event marking its last launch, and a
+// non-blocking stream for its set-up and its reads, so that a read waits for the object's own work and nothing else.
+struct DeviceState {
+  int device = 0;
+  void* arena = nullptr;
+  cudaEvent_t done = nullptr;   // recorded after every launch on the state (an external event node inside a CUDA graph capture)
+  cudaStream_t copy = nullptr;
+
+  DeviceState() = default;
+  DeviceState(const DeviceState&) = delete;
+  DeviceState& operator=(const DeviceState&) = delete;
+
+  // On the current device: lays the buffers out with layout(Carver&), allocates them in one piece, assigns them, then runs
+  // init() (the set-up copies, enqueued on `copy`) and waits for it.  0, or -1 with the error set.
+  template <class Layout, class Init> int create(const char* fn, Layout layout, Init init) {
+    if (cudaGetDevice(&device) != cudaSuccess) return fail(std::string(fn) + ": no CUDA device (there is no CPU fallback)");
+    Carver size;
+    layout(size);
+    cudaError_t e = cudaEventCreateWithFlags(&done, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&copy, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaMalloc(&arena, size.bytes);
+    if (e == cudaSuccess) {
+      Carver at{static_cast<char*>(arena)};
+      layout(at);
+      e = init();
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(copy);
+    return e == cudaSuccess ? 0 : cuda_fail(e, fn);
+  }
+
+  // marks the object's last launch on `stream`, so that read() waits for exactly that work.  Inside a stream capture the
+  // record becomes an external event node, so every replay of the graph records it (the flag is accepted only while capturing)
+  int mark(void* stream) const {
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    if (cudaError_t e = cudaStreamIsCapturing(st, &cs)) return static_cast<int>(e);
+    return static_cast<int>(cs == cudaStreamCaptureStatusActive ? cudaEventRecordWithFlags(done, st, cudaEventRecordExternal)
+                                                                : cudaEventRecord(done, st));
+  }
+
+  struct Copy { void* dst; const void* src; size_t bytes; };
+  // device-to-host copies once the last marked launch is done, all on `copy`, waited for once
+  cudaError_t read(const std::vector<Copy>& parts) const {
+    lwb::DeviceGuard g(device);
+    cudaError_t e = cudaStreamWaitEvent(copy, done, 0);
+    for (size_t i = 0; i < parts.size() && e == cudaSuccess; ++i)
+      if (parts[i].bytes) e = cudaMemcpyAsync(parts[i].dst, parts[i].src, parts[i].bytes, cudaMemcpyDeviceToHost, copy);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(copy);
+    return e;
+  }
+
+  // the first step of an export: heads[stream_id] of a table of num_streams, once the last marked launch is done
+  template <class Head> int read_head(const char* fn, const Head* heads, int num_streams, int stream_id, Head* h) const {
+    if (stream_id < 0 || stream_id >= num_streams) return fail(std::string(fn) + ": stream id outside [0, num_streams)");
+    if (cudaError_t e = read({{h, heads + stream_id, sizeof(Head)}})) return cuda_fail(e, fn);
+    return 0;
+  }
+
+  ~DeviceState() {
+    if (!done) return;          // create() failed before it made anything
+    lwb::DeviceGuard g(device);
+    if (copy) {
+      cudaStreamSynchronize(copy);
+      cudaStreamDestroy(copy);
+    }
+    cudaFree(arena);
+    cudaEventDestroy(done);
+  }
+};
 }  // namespace
 
 static_assert(LWDETR_ATTN_WG == lwb::ATTN_WG && LWDETR_ATTN_MMA == lwb::ATTN_MMA && LWDETR_ATTN_MMA_SHORT == lwb::ATTN_MMA_SHORT, "attention kernel codes");
@@ -300,21 +395,8 @@ struct lwdetr_tracker {
   lwb::TrackTable table;
   lwb::ReidTable reid;   // embedding_dim 0 and null pointers without appearance
   lwdetr_track_params params;
-  int device;
-  cudaEvent_t done;      // recorded after every launch on the table (an external event node inside a CUDA graph capture)
-  cudaStream_t copy;     // non-blocking: lwdetr_tracker_export waits for `done` only, not for the rest of the device
+  DeviceState state;
 };
-
-// marks the tracker's last launch on `stream`, so that lwdetr_tracker_export waits for exactly that work.  Inside a stream
-// capture the record becomes an external event node, so every replay of the graph records it (the flag is accepted only
-// while capturing)
-static int tracker_mark(lwdetr_tracker* t, void* stream) {
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-  if (cudaError_t e = cudaStreamIsCapturing(st, &cs)) return static_cast<int>(e);
-  return static_cast<int>(cs == cudaStreamCaptureStatusActive ? cudaEventRecordWithFlags(t->done, st, cudaEventRecordExternal)
-                                                              : cudaEventRecord(t->done, st));
-}
 
 void lwdetr_track_params_default(lwdetr_track_params* p) {
   if (!p) return;
@@ -332,9 +414,10 @@ void lwdetr_track_params_default(lwdetr_track_params* p) {
   p->capacity = 512;
 }
 
-int lwdetr_tracker_create(int num_streams, const lwdetr_track_params* params, lwdetr_tracker** out) {
-  if (!params || !out) return fail("lwdetr_tracker_create: null pointer");
-  const lwdetr_track_params& p = *params;
+// lwdetr_tracker_create and, with reid (already checked), lwdetr_tracker_create_reid: the tracker's checks (their messages
+// name lwdetr_tracker_create for both calls), then the table and any appearance state in one arena
+static int tracker_create(const char* fn, int num_streams, const lwdetr_track_params& p, const lwdetr_reid_params* reid,
+                          lwdetr_tracker** out) {
   if (num_streams < 1) return fail("lwdetr_tracker_create: num_streams must be >= 1");
   const float th[] = {p.track_thresh, p.low_thresh, p.new_track_thresh, p.duplicate_thresh};
   for (float v : th)
@@ -346,77 +429,48 @@ int lwdetr_tracker_create(int num_streams, const lwdetr_track_params* params, lw
   if (p.track_buffer < 0 || p.frame_rate < 1) return fail("lwdetr_tracker_create: need track_buffer >= 0 and frame_rate >= 1");
   if ((p.fuse_score != 0 && p.fuse_score != 1) || (p.class_aware != 0 && p.class_aware != 1))
     return fail("lwdetr_tracker_create: fuse_score and class_aware must be 0 or 1");
-  lwdetr_tracker* t = new (std::nothrow) lwdetr_tracker;
-  if (!t) return fail("lwdetr_tracker_create: out of memory");
+  std::unique_ptr<lwdetr_tracker> t(new (std::nothrow) lwdetr_tracker{});
+  if (!t) return fail(std::string(fn) + ": out of memory");
   t->params = p;
   t->table.num_streams = num_streams;
   t->table.capacity = p.capacity;
-  t->table.head = nullptr;
-  t->table.rec = nullptr;
-  t->reid = lwb::ReidTable{};
-  t->done = nullptr;
-  t->copy = nullptr;
-  if (cudaGetDevice(&t->device) != cudaSuccess) { delete t; return fail("lwdetr_tracker_create: no CUDA device (there is no CPU fallback)"); }
-  std::vector<lwb::TrackHead> h(static_cast<size_t>(num_streams));
-  for (auto& x : h) { x = lwb::TrackHead{}; x.frame = 1; x.next_id = 1; }
-  const size_t rec_bytes = static_cast<size_t>(num_streams) * 2 * p.capacity * sizeof(lwdetr_track_record);
-  cudaError_t e = cudaMalloc(&t->table.head, h.size() * sizeof(lwb::TrackHead));
-  if (e == cudaSuccess) e = cudaMalloc(&t->table.rec, rec_bytes);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&t->done, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&t->copy, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaMemcpy(t->table.head, h.data(), h.size() * sizeof(lwb::TrackHead), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) {
-    cudaFree(t->table.head);
-    cudaFree(t->table.rec);
-    if (t->done) cudaEventDestroy(t->done);
-    if (t->copy) cudaStreamDestroy(t->copy);
-    delete t;
-    return cuda_fail(e, "lwdetr_tracker_create");
-  }
-  *out = t;
+  if (reid) t->reid.params = *reid;
+  const size_t ns = static_cast<size_t>(num_streams), cap = static_cast<size_t>(p.capacity), pairs = ns * lwb::TRACK_PAIRS;
+  const std::vector<lwb::TrackHead> h(ns, lwb::TrackHead{1, 1});     // every stream at frame 1, next id 1
+  const auto layout = [&](Carver& c) {
+    c.take(t->table.head, ns);
+    c.take(t->table.rec, ns * 2 * cap);
+    if (!reid) return;
+    c.take(t->reid.slot, ns * 2 * cap);
+    c.take(t->reid.has, ns * cap);
+    c.take(t->reid.emb, ns * cap * reid->embedding_dim);
+    c.take(t->reid.pkey, pairs);
+    c.take(t->reid.pval, pairs);
+  };
+  const auto init = [&] {
+    return cudaMemcpyAsync(t->table.head, h.data(), ns * sizeof(lwb::TrackHead), cudaMemcpyHostToDevice, t->state.copy);
+  };
+  if (int rc = t->state.create(fn, layout, init)) return rc;
+  *out = t.release();
   return 0;
 }
 
-static void free_reid(lwb::ReidTable& r) {
-  cudaFree(r.slot);
-  cudaFree(r.has);
-  cudaFree(r.emb);
-  cudaFree(r.pkey);
-  cudaFree(r.pval);
-  r = lwb::ReidTable{};
+int lwdetr_tracker_create(int num_streams, const lwdetr_track_params* params, lwdetr_tracker** out) {
+  if (!params || !out) return fail("lwdetr_tracker_create: null pointer");
+  return tracker_create("lwdetr_tracker_create", num_streams, *params, nullptr, out);
 }
 
-void lwdetr_tracker_destroy(lwdetr_tracker* t) {
-  if (!t) return;
-  lwb::DeviceGuard g(t->device);
-  cudaStreamSynchronize(t->copy);
-  free_reid(t->reid);
-  cudaFree(t->table.head);
-  cudaFree(t->table.rec);
-  cudaEventDestroy(t->done);
-  cudaStreamDestroy(t->copy);
-  delete t;
-}
-
-static std::string check_streams(const lwdetr_tracker* t, const int32_t* ids, int n) {
-  std::vector<char> seen(static_cast<size_t>(t->table.num_streams), 0);
-  for (int i = 0; i < n; ++i) {
-    if (ids[i] < 0 || ids[i] >= t->table.num_streams)
-      return "stream id " + std::to_string(ids[i]) + " outside [0, " + std::to_string(t->table.num_streams) + ")";
-    if (seen[ids[i]]++) return "stream id " + std::to_string(ids[i]) + " appears twice in one call";
-  }
-  return "";
-}
+void lwdetr_tracker_destroy(lwdetr_tracker* t) { delete t; }
 
 int lwdetr_tracker_reset(lwdetr_tracker* t, const int32_t* streams, int n, void* stream) {
   if (!t || (n > 0 && !streams)) return fail("lwdetr_tracker_reset: null pointer");
   if (n < 0) return fail("lwdetr_tracker_reset: n must be >= 0");
-  const std::string err = check_streams(t, streams, n);
+  const std::string err = check_ids(t->table.num_streams, streams, n);
   if (!err.empty()) return fail("lwdetr_tracker_reset: " + err);
   if (n == 0) return 0;
-  lwb::DeviceGuard g(t->device);
+  lwb::DeviceGuard g(t->state.device);
   int e = lwb::track_reset_launch(t->table, streams, n, static_cast<cudaStream_t>(stream));
-  if (!e) e = tracker_mark(t, stream);
+  if (!e) e = t->state.mark(stream);
   if (e) return cuda_fail(e, "lwdetr_tracker_reset launch");
   return 0;
 }
@@ -432,17 +486,17 @@ static int track_common(const char* name, lwdetr_tracker* t, const float* scores
   if (reinterpret_cast<uintptr_t>(boxes) % 16 || reinterpret_cast<uintptr_t>(out_boxes) % 16)
     return fail(fn + ": boxes and out_boxes must be 16-byte aligned");
   if (reinterpret_cast<uintptr_t>(motion) % 8) return fail(fn + ": motion must be 8-byte aligned");
-  const std::string err = check_streams(t, stream_ids, B);
+  const std::string err = check_ids(t->table.num_streams, stream_ids, B);
   if (!err.empty()) return fail(fn + ": " + err);
   // a tracker with appearance always runs the appearance instantiation (without embeddings when none are given: ByteTrack's
   // bits), which keeps each record's embedding slot; the ByteTrack one would leave the slot array stale
   const lwb::ReidInput none{&t->reid, nullptr, LWDETR_ET_F32, 0};
   if (!reid && t->reid.emb) reid = &none;
-  lwb::DeviceGuard g(t->device);
+  lwb::DeviceGuard g(t->state.device);
   int e = lwb::track_launch(t->table, t->params, scores, labels, boxes, motion, B, k, stream_ids, max_out, out_ids, out_scores, out_labels,
                             out_boxes, out_index, counts, static_cast<cudaStream_t>(stream), reid);
   if (e == -2) return fail(fn + ": a limit is exceeded");
-  if (!e) e = tracker_mark(t, stream);
+  if (!e) e = t->state.mark(stream);
   if (e) return cuda_fail(e, (fn + " launch").c_str());
   return 0;
 }
@@ -476,22 +530,7 @@ int lwdetr_tracker_create_reid(int num_streams, const lwdetr_track_params* param
   if (!(r.proximity_thresh >= 0.f && r.proximity_thresh < 1.f)) return fail("lwdetr_tracker_create_reid: proximity_thresh must be in [0, 1)");
   if (!(r.appearance_thresh >= 0.f && r.appearance_thresh <= 1.f) || !(r.ema_alpha >= 0.f && r.ema_alpha <= 1.f))
     return fail("lwdetr_tracker_create_reid: appearance_thresh and ema_alpha must be in [0, 1]");
-  lwdetr_tracker* t = nullptr;
-  if (int rc = lwdetr_tracker_create(num_streams, params, &t)) return rc;
-  lwb::ReidTable& rt = t->reid;
-  const size_t ns = static_cast<size_t>(num_streams), cap = static_cast<size_t>(params->capacity), pairs = ns * lwb::TRACK_PAIRS;
-  cudaError_t e = cudaMalloc(&rt.slot, ns * 2 * cap * sizeof(int16_t));
-  if (e == cudaSuccess) e = cudaMalloc(&rt.has, ns * cap);
-  if (e == cudaSuccess) e = cudaMalloc(&rt.emb, ns * cap * r.embedding_dim * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&rt.pkey, pairs * sizeof(uint32_t));
-  if (e == cudaSuccess) e = cudaMalloc(&rt.pval, pairs * sizeof(double));
-  if (e != cudaSuccess) {
-    lwdetr_tracker_destroy(t);
-    return cuda_fail(e, "lwdetr_tracker_create_reid");
-  }
-  rt.params = r;
-  *out = t;
-  return 0;
+  return tracker_create("lwdetr_tracker_create_reid", num_streams, *params, reid, out);
 }
 
 int lwdetr_track_reid(lwdetr_tracker* t, const float* scores, const int32_t* labels, const float* boxes, const double* motion,
@@ -513,31 +552,24 @@ int lwdetr_track_reid(lwdetr_tracker* t, const float* scores, const int32_t* lab
 int lwdetr_tracker_export_embeddings(lwdetr_tracker* t, int stream_id, float* host, int cap, int32_t* count, int8_t* has) {
   if (!t || !count || (cap > 0 && (!host || !has))) return fail("lwdetr_tracker_export_embeddings: null pointer");
   if (!t->reid.emb) return fail("lwdetr_tracker_export_embeddings: the tracker was made without appearance (lwdetr_tracker_create_reid)");
-  if (stream_id < 0 || stream_id >= t->table.num_streams) return fail("lwdetr_tracker_export_embeddings: stream id outside [0, num_streams)");
-  lwb::DeviceGuard g(t->device);
-  const int capacity = t->table.capacity, D = t->reid.params.embedding_dim;
   lwb::TrackHead h;
-  std::vector<int16_t> slot(static_cast<size_t>(capacity));
-  std::vector<uint8_t> full(static_cast<size_t>(capacity));
-  cudaError_t e = cudaStreamWaitEvent(t->copy, t->done, 0);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(&h, t->table.head + stream_id, sizeof(h), cudaMemcpyDeviceToHost, t->copy);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(t->copy);
-  if (e != cudaSuccess) return cuda_fail(e, "lwdetr_tracker_export_embeddings");
+  if (int rc = t->state.read_head("lwdetr_tracker_export_embeddings", t->table.head, t->table.num_streams, stream_id, &h)) return rc;
   const int n = h.n_tracked + h.n_lost;
   const int m = n < cap ? n : (cap > 0 ? cap : 0);
   if (m > 0) {
-    const size_t s0 = static_cast<size_t>(stream_id);
-    e = cudaMemcpyAsync(slot.data(), t->reid.slot + (s0 * 2 + h.parity) * capacity, static_cast<size_t>(m) * sizeof(int16_t),
-                        cudaMemcpyDeviceToHost, t->copy);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(full.data(), t->reid.has + s0 * capacity, static_cast<size_t>(capacity), cudaMemcpyDeviceToHost, t->copy);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(t->copy);
-    for (int i = 0; i < m && e == cudaSuccess; ++i) {
-      has[i] = static_cast<int8_t>(full[slot[i]]);
-      e = cudaMemcpyAsync(host + static_cast<size_t>(i) * D, t->reid.emb + (s0 * capacity + slot[i]) * D, static_cast<size_t>(D) * sizeof(float),
-                          cudaMemcpyDeviceToHost, t->copy);
-    }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(t->copy);
+    // the stream's whole embedding block in one copy, the rows gathered into record order here
+    const size_t s0 = static_cast<size_t>(stream_id), C = static_cast<size_t>(t->table.capacity), D = t->reid.params.embedding_dim;
+    std::vector<int16_t> slot(static_cast<size_t>(m));
+    std::vector<uint8_t> full(C);
+    std::vector<float> emb(C * D);
+    const cudaError_t e = t->state.read({{slot.data(), t->reid.slot + (s0 * 2 + h.parity) * C, slot.size() * sizeof(int16_t)},
+                                         {full.data(), t->reid.has + s0 * C, C},
+                                         {emb.data(), t->reid.emb + s0 * C * D, emb.size() * sizeof(float)}});
     if (e != cudaSuccess) return cuda_fail(e, "lwdetr_tracker_export_embeddings");
+    for (int i = 0; i < m; ++i) {
+      has[i] = static_cast<int8_t>(full[slot[i]]);
+      std::copy_n(emb.data() + slot[i] * D, D, host + i * D);
+    }
   }
   *count = n;
   return 0;
@@ -545,21 +577,13 @@ int lwdetr_tracker_export_embeddings(lwdetr_tracker* t, int stream_id, float* ho
 
 int lwdetr_tracker_export(lwdetr_tracker* t, int stream_id, lwdetr_track_record* host, int cap, int32_t* count, int32_t frame_next_overflow[3]) {
   if (!t || !count || !frame_next_overflow || (cap > 0 && !host)) return fail("lwdetr_tracker_export: null pointer");
-  if (stream_id < 0 || stream_id >= t->table.num_streams) return fail("lwdetr_tracker_export: stream id outside [0, num_streams)");
-  lwb::DeviceGuard g(t->device);
   lwb::TrackHead h;
-  cudaError_t e = cudaStreamWaitEvent(t->copy, t->done, 0);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(&h, t->table.head + stream_id, sizeof(h), cudaMemcpyDeviceToHost, t->copy);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(t->copy);
-  if (e != cudaSuccess) return cuda_fail(e, "lwdetr_tracker_export");
+  if (int rc = t->state.read_head("lwdetr_tracker_export", t->table.head, t->table.num_streams, stream_id, &h)) return rc;
   const int n = h.n_tracked + h.n_lost;
   const int m = n < cap ? n : (cap > 0 ? cap : 0);
   const lwdetr_track_record* src = t->table.rec + (static_cast<size_t>(stream_id) * 2 + h.parity) * t->table.capacity;
-  if (m > 0) {
-    e = cudaMemcpyAsync(host, src, static_cast<size_t>(m) * sizeof(lwdetr_track_record), cudaMemcpyDeviceToHost, t->copy);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(t->copy);
-    if (e != cudaSuccess) return cuda_fail(e, "lwdetr_tracker_export");
-  }
+  if (cudaError_t e = t->state.read({{host, src, static_cast<size_t>(m) * sizeof(lwdetr_track_record)}}))
+    return cuda_fail(e, "lwdetr_tracker_export");
   *count = n;
   frame_next_overflow[0] = h.frame;
   frame_next_overflow[1] = h.next_id;
@@ -569,7 +593,7 @@ int lwdetr_tracker_export(lwdetr_tracker* t, int stream_id, lwdetr_track_record*
 
 struct lwdetr_gmc {
   lwb::GmcTable table;
-  int device;
+  DeviceState state;
 };
 
 void lwdetr_gmc_params_default(lwdetr_gmc_params* p) {
@@ -606,13 +630,11 @@ int lwdetr_gmc_create(int num_streams, const lwdetr_gmc_params* params, lwdetr_g
   const int lo = lwb::GMC_MIN_SIDE * p.downscale;
   if (p.max_height < lo || p.max_width < lo || p.max_height > 8192 || p.max_width > 8192)
     return fail("lwdetr_gmc_create: max_height and max_width must be in [16 * downscale, 8192]");
-  lwdetr_gmc* g = new (std::nothrow) lwdetr_gmc;
+  std::unique_ptr<lwdetr_gmc> g(new (std::nothrow) lwdetr_gmc{});
   if (!g) return fail("lwdetr_gmc_create: out of memory");
   lwb::GmcTable& t = g->table;
-  t = lwb::GmcTable{};
   t.num_streams = num_streams;
   t.p = p;
-  if (cudaGetDevice(&g->device) != cudaSuccess) { delete g; return fail("lwdetr_gmc_create: no CUDA device (there is no CPU fallback)"); }
   lwb::GmcGeo geo;
   lwb::gmc_geometry(p.max_height, p.max_width, p, &geo);
   long long off = 0;
@@ -622,46 +644,22 @@ int lwdetr_gmc_create(int num_streams, const lwdetr_gmc_params* params, lwdetr_g
   }
   t.slot_bytes = off;
   const size_t ns = static_cast<size_t>(num_streams), mp = static_cast<size_t>(p.max_points);
-  cudaError_t e = cudaMalloc(&t.head, ns * sizeof(lwb::GmcHead));
-  if (e == cudaSuccess) e = cudaMalloc(&t.pyr, ns * 2 * static_cast<size_t>(t.slot_bytes));
-  if (e == cudaSuccess) e = cudaMalloc(&t.pts, ns * 2 * mp * sizeof(float2));
-  if (e == cudaSuccess) e = cudaMalloc(&t.cell_r, ns * mp * sizeof(double));
-  if (e == cudaSuccess) e = cudaMalloc(&t.cell_i, ns * mp * sizeof(int32_t));
-  if (e == cudaSuccess) e = cudaMalloc(&t.flow, ns * mp * sizeof(float4));
-  if (e == cudaSuccess) e = cudaMalloc(&t.found, ns * mp);
-  if (e == cudaSuccess) e = cudaMemset(t.head, 0, ns * sizeof(lwb::GmcHead));
-  if (e == cudaSuccess) e = cudaDeviceSynchronize();
-  if (e != cudaSuccess) {
-    lwdetr_gmc_destroy(g);
-    return cuda_fail(e, "lwdetr_gmc_create");
-  }
-  *out = g;
+  const auto layout = [&](Carver& c) {
+    c.take(t.head, ns);
+    c.take(t.pyr, ns * 2 * static_cast<size_t>(t.slot_bytes));
+    c.take(t.pts, ns * 2 * mp);
+    c.take(t.cell_r, ns * mp);
+    c.take(t.cell_i, ns * mp);
+    c.take(t.flow, ns * mp);
+    c.take(t.found, ns * mp);
+  };
+  const auto init = [&] { return cudaMemsetAsync(t.head, 0, ns * sizeof(lwb::GmcHead), g->state.copy); };
+  if (int rc = g->state.create("lwdetr_gmc_create", layout, init)) return rc;
+  *out = g.release();
   return 0;
 }
 
-void lwdetr_gmc_destroy(lwdetr_gmc* g) {
-  if (!g) return;
-  lwb::DeviceGuard dg(g->device);
-  lwb::GmcTable& t = g->table;
-  cudaFree(t.head);
-  cudaFree(t.pyr);
-  cudaFree(t.pts);
-  cudaFree(t.cell_r);
-  cudaFree(t.cell_i);
-  cudaFree(t.flow);
-  cudaFree(t.found);
-  delete g;
-}
-
-static std::string check_ids(int num_streams, const int32_t* ids, int n) {
-  std::vector<char> seen(static_cast<size_t>(num_streams), 0);
-  for (int i = 0; i < n; ++i) {
-    if (ids[i] < 0 || ids[i] >= num_streams)
-      return "stream id " + std::to_string(ids[i]) + " outside [0, " + std::to_string(num_streams) + ")";
-    if (seen[ids[i]]++) return "stream id " + std::to_string(ids[i]) + " appears twice in one call";
-  }
-  return "";
-}
+void lwdetr_gmc_destroy(lwdetr_gmc* g) { delete g; }
 
 int lwdetr_gmc_reset(lwdetr_gmc* g, const int32_t* streams, int n, void* stream) {
   if (!g || (n > 0 && !streams)) return fail("lwdetr_gmc_reset: null pointer");
@@ -669,8 +667,10 @@ int lwdetr_gmc_reset(lwdetr_gmc* g, const int32_t* streams, int n, void* stream)
   const std::string err = check_ids(g->table.num_streams, streams, n);
   if (!err.empty()) return fail("lwdetr_gmc_reset: " + err);
   if (n == 0) return 0;
-  lwb::DeviceGuard dg(g->device);
-  if (int e = lwb::gmc_reset_launch(g->table, streams, n, static_cast<cudaStream_t>(stream))) return cuda_fail(e, "lwdetr_gmc_reset launch");
+  lwb::DeviceGuard dg(g->state.device);
+  int e = lwb::gmc_reset_launch(g->table, streams, n, static_cast<cudaStream_t>(stream));
+  if (!e) e = g->state.mark(stream);
+  if (e) return cuda_fail(e, "lwdetr_gmc_reset launch");
   return 0;
 }
 
@@ -678,12 +678,8 @@ int lwdetr_gmc_export(lwdetr_gmc* g, int stream_id, uint8_t* levels, int64_t lev
                       int32_t info[6]) {
   if (!g || !info || (levels_bytes > 0 && !levels) || !corners || !flow || !found) return fail("lwdetr_gmc_export: null pointer");
   const lwb::GmcTable& t = g->table;
-  if (stream_id < 0 || stream_id >= t.num_streams) return fail("lwdetr_gmc_export: stream id outside [0, num_streams)");
-  lwb::DeviceGuard dg(g->device);
   lwb::GmcHead h;
-  cudaError_t e = cudaDeviceSynchronize();
-  if (e == cudaSuccess) e = cudaMemcpy(&h, t.head + stream_id, sizeof(h), cudaMemcpyDeviceToHost);
-  if (e != cudaSuccess) return cuda_fail(e, "lwdetr_gmc_export");
+  if (int rc = g->state.read_head("lwdetr_gmc_export", t.head, t.num_streams, stream_id, &h)) return rc;
   lwb::GmcGeo geo;
   lwb::gmc_geometry(h.valid ? h.h : lwb::GMC_MIN_SIDE * t.p.downscale, h.valid ? h.w : lwb::GMC_MIN_SIDE * t.p.downscale, t.p, &geo);
   const int nlev = h.valid ? geo.nlev : -1;
@@ -692,16 +688,17 @@ int lwdetr_gmc_export(lwdetr_gmc* g, int stream_id, uint8_t* levels, int64_t lev
   if (need > levels_bytes) return fail("lwdetr_gmc_export: levels buffer too small");
   const size_t mp = static_cast<size_t>(t.p.max_points), sid = static_cast<size_t>(stream_id);
   const uint8_t* slot = t.pyr + (sid * 2 + h.cur) * static_cast<size_t>(t.slot_bytes);
+  std::vector<DeviceState::Copy> parts;
   long long o = 0;
-  for (int l = 0; l <= nlev && e == cudaSuccess; ++l) {
+  for (int l = 0; l <= nlev; ++l) {
     const size_t n = static_cast<size_t>(geo.lw[l]) * geo.lh[l];
-    e = cudaMemcpy(levels + o, slot + t.off[l], n, cudaMemcpyDeviceToHost);
+    parts.push_back({levels + o, slot + t.off[l], n});
     o += static_cast<long long>(n);
   }
-  if (e == cudaSuccess) e = cudaMemcpy(corners, t.pts + (sid * 2 + h.cur) * mp, mp * sizeof(float2), cudaMemcpyDeviceToHost);
-  if (e == cudaSuccess) e = cudaMemcpy(flow, t.flow + sid * mp, mp * sizeof(float4), cudaMemcpyDeviceToHost);
-  if (e == cudaSuccess) e = cudaMemcpy(found, t.found + sid * mp, mp, cudaMemcpyDeviceToHost);
-  if (e != cudaSuccess) return cuda_fail(e, "lwdetr_gmc_export");
+  parts.push_back({corners, t.pts + (sid * 2 + h.cur) * mp, mp * sizeof(float2)});
+  parts.push_back({flow, t.flow + sid * mp, mp * sizeof(float4)});
+  parts.push_back({found, t.found + sid * mp, mp});
+  if (cudaError_t e = g->state.read(parts)) return cuda_fail(e, "lwdetr_gmc_export");
   info[0] = h.valid;
   info[1] = h.h;
   info[2] = h.w;
@@ -728,9 +725,10 @@ static int gmc_estimate_common(const char* name, lwdetr_gmc* g, const std::vecto
                   std::to_string(lo) + ", max_height / max_width = " + std::to_string(p.max_height) + " x " + std::to_string(p.max_width) + "]");
     if (f.pitch < static_cast<long long>(f.w) * (f.nv12 ? 1 : 3)) return fail(fn + ": frame " + std::to_string(i) + ": pitch too small");
   }
-  lwb::DeviceGuard dg(g->device);
-  if (int e = lwb::gmc_estimate_launch(g->table, fr.data(), B, stream_ids, motion, status, inliers, static_cast<cudaStream_t>(stream)))
-    return cuda_fail(e, (fn + " launch").c_str());
+  lwb::DeviceGuard dg(g->state.device);
+  int e = lwb::gmc_estimate_launch(g->table, fr.data(), B, stream_ids, motion, status, inliers, static_cast<cudaStream_t>(stream));
+  if (!e) e = g->state.mark(stream);
+  if (e) return cuda_fail(e, (fn + " launch").c_str());
   return 0;
 }
 
