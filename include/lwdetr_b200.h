@@ -525,6 +525,89 @@ LWDETR_API int lwdetr_gmc_reset(lwdetr_gmc* g, const int32_t* streams, int n, vo
 LWDETR_API int lwdetr_gmc_export(lwdetr_gmc* g, int stream_id, uint8_t* levels, int64_t levels_bytes, float* corners, float* flow,
                                  int8_t* found, int32_t info[6]);
 
+/* Line crossings and zone occupancy per camera stream, on the tracker's outputs (what DeepStream's nvdsanalytics and
+ * supervision's LineZone / PolygonZone compute after a tracker).  The C composition per batch of frames: ... ->
+ * lwdetr_track (or _ex / _reid) -> lwdetr_zones_update on its out_ids, out_labels, out_boxes and counts with the same
+ * stream_ids, on the same CUDA stream; nothing is read back in between, so the pair can be captured in one CUDA graph.
+ * Calls on one zones object must be ordered on one CUDA stream.  tools/zone_spec.py restates this contract in numpy.
+ * Geometry per stream, float64 frame pixels: up to 32 lines (ax, ay, bx, by) of non-zero length and up to 32 polygons of 3
+ *   to 256 vertices, at most 2048 vertices in all; any polygon (concave, self-intersecting).  Zones are fixed in frame
+ *   pixels: with a moving camera (lwdetr_track_ex) they stay image regions, not world regions.
+ * Parameters (lwdetr_zones_params_default): num_classes in [1, 1024] (default 91, LW-DETR's COCO head); capacity, the
+ *   records per stream, in [1, 4096] (default 1024); forget_after >= 0 (default 30, ByteTrack's max_time_lost at its
+ *   defaults); zone_anchor in [0, 9) (default LWDETR_ANCHOR_BOTTOM_CENTER, as PolygonZone); line_anchors a non-zero mask
+ *   of anchor bits below 1 << 9 (default the four corners, as LineZone).
+ * Anchors of an fp32 xyxy box widened to float64: anchor 3 * row + column, rows y1, (y1 + y2) * 0.5, y2 and columns x1,
+ *   (x1 + x2) * 0.5, x2.  Everything is float64 with each operation rounded on its own (no FMA), in the order written.
+ * Line side: dx = bx - ax, dy = by - ay, L2 = dx * dx + dy * dy; per anchor t = (px - ax) * dx + (py - ay) * dy and
+ *   c = dx * (py - ay) - dy * (px - ax).  The frame's decision is +1 when every selected anchor has 0 <= t <= L2 and c > 0,
+ *   -1 when every one has 0 <= t <= L2 and c < 0, else 0.  Each (track, line) keeps its last non-zero side s; a decision
+ *   d != 0 with s != 0 and d != s is a crossing, LWDETR_ZONE_LINE_IN for d = +1 and _LINE_OUT for d = -1, counted in
+ *   line_counts[line][label][in = 0 | out = 1]; then s = d.  A track's first decision only records its side.  In image
+ *   coordinates (y down), for a line drawn left to right "in" is downward; swapping the endpoints swaps in and out.
+ * Zone membership of the zone anchor: the crossing-number (even-odd) rule, for i = 0..n-1 and j = (i + n - 1) % n:
+ *   if ((yi > py) != (yj > py)) && (px < (xj - xi) * (py - yi) / (yj - yi) + xi) inside = !inside.
+ *   Points on edges and vertices get what this half-open rule gives (a horizontal edge never flips).
+ * A frame of a stream (frames count its update calls from 1; a stream absent from a call does not advance):
+ *   - entries at index >= min(counts[b], max_out), with id <= 0 or a non-finite box are absent; a repeated id's later
+ *     entries are ignored too (the tracker never repeats one).  An absent track keeps its record as it is;
+ *   - present tracks in input order: inside = the mask of the zones holding its anchor; occupancy[zone] counts them.  A
+ *     track without a record takes one if the stream holds fewer than capacity records (else it is not recorded, makes no
+ *     event and adds 1 to the stream's overflow); then lines ascending (crossings as above), then zones ascending: turning
+ *     inside is LWDETR_ZONE_ENTER (entry frame = frame, entries[zone][label] += 1), turning outside is LWDETR_ZONE_EXIT with
+ *     dwell = frame - entry frame (entry frame back to 0).  The record takes the frame as last_seen and the entry's label;
+ *   - then every record with frame - last_seen > forget_after, in ascending id, is dropped, and for each zone it was
+ *     inside (ascending) makes LWDETR_ZONE_FORGET with its last label and dwell = last_seen - entry frame.  So every enter
+ *     is matched by exactly one exit or forget.
+ *   A label outside [0, num_classes) counts in the extra column num_classes.  Events are (id, kind, index (line or zone),
+ *   label (as given), dwell (0 for line and enter events)).
+ * lwdetr_zones_create: num_streams >= 1, params validated; one device allocation (geometry, records, counters) on the
+ *   current device, every stream at frame 1 without geometry.  Synchronous, on a stream of the object's own.
+ * lwdetr_zones_set: one stream's geometry from HOST arrays, lines [n_lines][4], polygons' vertex counts [n_polygons] and
+ *   vertices [sum of counts][2]; replaces the geometry and clears the stream's records, counters and overflow (the frame
+ *   count goes on).  A limit overrun, a non-finite coordinate or a zero-length line is an error and nothing changes.
+ *   Synchronous: it waits for the object's last launch and nothing else on the device; not callable during a stream capture.
+ * lwdetr_zones_reset: the n streams listed (HOST; ids distinct and in [0, num_streams), else an error and nothing happens)
+ *   back to frame 1 with no records, zero counters and overflow; their geometry is kept.  Stream-ordered.
+ * lwdetr_zones_update: one frame for each of B streams (stream_ids HOST, distinct and in [0, num_streams)); ids, labels int32
+ *   [B, max_out], boxes fp32 [B, max_out, 4] (16-byte aligned), counts int32 [B]: exactly lwdetr_track's outputs;
+ *   max_out in [1, 1024].  Outputs: inside uint32 [B, max_out] (0 for absent entries), occupancy int32 [B, 32] (0 past the
+ *   stream's polygons), events int32 [B, max_events, 5] (the first max_events of the frame's events in order, unused rows
+ *   zero; may be NULL when max_events = 0) and event_counts int32 [B], the true number.  The counters count every event.
+ *   All DEVICE; asynchronous, nothing allocated or copied per call, safe to capture in a CUDA graph.
+ * lwdetr_zones_export: one stream, synchronous: it waits for the object's last launch and nothing else on the device.
+ *   frame_overflow = (frame, overflow); line_counts int32 [n_lines][num_classes + 1][2] and entries int32
+ *   [n_polygons][num_classes + 1] (n_* of the stream's geometry: info = (n_lines, n_polygons, records)); then up to cap
+ *   records in ascending id: lwdetr_zone_record with sides[l] in {-1, 0, +1} and entry[z] the entry frame (0 when
+ *   outside). */
+enum {
+  LWDETR_ANCHOR_TOP_LEFT = 0, LWDETR_ANCHOR_TOP_CENTER = 1, LWDETR_ANCHOR_TOP_RIGHT = 2, LWDETR_ANCHOR_CENTER_LEFT = 3,
+  LWDETR_ANCHOR_CENTER = 4, LWDETR_ANCHOR_CENTER_RIGHT = 5, LWDETR_ANCHOR_BOTTOM_LEFT = 6, LWDETR_ANCHOR_BOTTOM_CENTER = 7,
+  LWDETR_ANCHOR_BOTTOM_RIGHT = 8
+};
+enum { LWDETR_ZONE_LINE_IN = 1, LWDETR_ZONE_LINE_OUT = 2, LWDETR_ZONE_ENTER = 3, LWDETR_ZONE_EXIT = 4, LWDETR_ZONE_FORGET = 5 };
+typedef struct {
+  int32_t num_classes, capacity, forget_after, zone_anchor, line_anchors;
+} lwdetr_zones_params;
+typedef struct {
+  int32_t id, last_seen, label;
+  uint32_t inside;
+  int8_t sides[32];
+  int32_t entry[32];
+} lwdetr_zone_record;
+typedef struct lwdetr_zones lwdetr_zones;
+LWDETR_API void lwdetr_zones_params_default(lwdetr_zones_params* p);
+LWDETR_API int lwdetr_zones_create(int num_streams, const lwdetr_zones_params* params, lwdetr_zones** out);
+LWDETR_API void lwdetr_zones_destroy(lwdetr_zones* z);
+LWDETR_API int lwdetr_zones_set(lwdetr_zones* z, int stream_id, const double* lines, int n_lines, const int32_t* polygon_sizes,
+                                int n_polygons, const double* vertices);
+LWDETR_API int lwdetr_zones_reset(lwdetr_zones* z, const int32_t* streams, int n, void* stream);
+LWDETR_API int lwdetr_zones_update(lwdetr_zones* z, const int32_t* ids, const int32_t* labels, const float* boxes, const int32_t* counts,
+                                   int B, int max_out, const int32_t* stream_ids, uint32_t* inside, int32_t* occupancy, int32_t* events,
+                                   int max_events, int32_t* event_counts, void* stream);
+LWDETR_API int lwdetr_zones_export(lwdetr_zones* z, int stream_id, int32_t frame_overflow[2], int32_t info[3], int32_t* line_counts,
+                                   int32_t* entries, lwdetr_zone_record* records, int cap);
+
 /* The LWDETR_F16_E4M3 mode's two kernels.
  * lwdetr_layernorm_e4m3: fp16 rows x [rows, ldx] -> e4m3 codes q [rows, ldq] (uint8) and fp32 row_scale [rows], as the mode's
  *   activation contract above (x^ without the LayerNorm affine, eps as given).  C % 8 == 0, C <= 1024, ldx and ldq

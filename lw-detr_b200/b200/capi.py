@@ -53,6 +53,13 @@ _SIGNATURES = {
     "lwdetr_gmc_export": (_i, [_vp, _i, _vp, _i64, _vp, _vp, _vp, _vp]),
     "lwdetr_gmc_estimate": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_gmc_estimate_nv12": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
+    "lwdetr_zones_params_default": (None, [_vp]),
+    "lwdetr_zones_create": (_i, [_i, _vp, _vp]),
+    "lwdetr_zones_destroy": (None, [_vp]),
+    "lwdetr_zones_set": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp]),
+    "lwdetr_zones_reset": (_i, [_vp, _vp, _i, _vp]),
+    "lwdetr_zones_update": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp]),
+    "lwdetr_zones_export": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _i]),
     "lwdetr_query_best": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "lwdetr_crops": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     "lwdetr_crops_nv12": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
@@ -485,7 +492,7 @@ def _emb_dtype(dtype):
 
 
 class _DeviceObject:
-    """What Tracker and MotionEstimator share: a C object made on one device from a parameter struct (its handle in _t),
+    """What Tracker, MotionEstimator and Zones share: a C object made on one device from a parameter struct (its handle in _t),
     reset per stream and destroyed by close()."""
 
     RESET = DESTROY = None                               # the subclass's C calls
@@ -527,7 +534,7 @@ class _DeviceObject:
 
     def reset(self, streams):
         """The streams start again (stream-ordered): a tracker's at frame 1 and id 1 with empty lists, an estimator's at
-        their next frame."""
+        their next frame, a zones object's at frame 1 with no records and zero counters (geometry kept)."""
         arr, n = self._ids(streams)
         check(getattr(lib(), self.RESET)(self._t, ctypes.cast(arr, _vp), n, stream_ptr(self.device)), self.RESET)
 
@@ -719,6 +726,134 @@ class MotionEstimator(_DeviceObject):
             lh, lw = (lh + 1) // 2, (lw + 1) // 2
         return dict(valid=bool(valid), size=(h, w), levels=levels, corners=corners[:nc].copy(), flow=flow[:nf].copy(),
                     found=found[:nf].astype(bool))
+
+
+class ZonesParams(ctypes.Structure):
+    """lwdetr_zones_params (include/lwdetr_b200.h)."""
+    _fields_ = [(n, ctypes.c_int32) for n in ("num_classes", "capacity", "forget_after", "zone_anchor", "line_anchors")]
+
+
+class ZoneRecord(ctypes.Structure):
+    """lwdetr_zone_record (include/lwdetr_b200.h)."""
+    _fields_ = [("id", ctypes.c_int32), ("last_seen", ctypes.c_int32), ("label", ctypes.c_int32), ("inside", ctypes.c_uint32),
+                ("sides", ctypes.c_int8 * 32), ("entry", ctypes.c_int32 * 32)]
+
+
+ANCHORS = ("top_left", "top_center", "top_right", "center_left", "center", "center_right", "bottom_left", "bottom_center",
+           "bottom_right")
+ZONE_LINE_IN, ZONE_LINE_OUT, ZONE_ENTER, ZONE_EXIT, ZONE_FORGET = 1, 2, 3, 4, 5
+
+
+def zone_geometry(lines=(), polygons=()):
+    """One stream's geometry checked against lwdetr_zones_set's rules without any device call: (lines float64 [L, 4],
+    polygon sizes int32 [Z], vertices float64 [V, 2]).  Up to 32 lines (ax, ay, bx, by) of non-zero length, up to 32
+    polygons of 3 to 256 (x, y) vertices and 2048 vertices in all, every coordinate finite; else ValueError."""
+    import numpy as np
+    lines = [tuple(float(v) for v in l) for l in lines]
+    if len(lines) > 32:
+        raise ValueError("Zones.set: at most 32 lines, got %d" % len(lines))
+    for i, l in enumerate(lines):
+        if len(l) != 4:
+            raise ValueError("Zones.set: line %d must be (ax, ay, bx, by), got %d numbers" % (i, len(l)))
+        if not all(np.isfinite(l)):
+            raise ValueError("Zones.set: line %d has a non-finite coordinate" % i)
+        if l[0] == l[2] and l[1] == l[3]:
+            raise ValueError("Zones.set: line %d has zero length" % i)
+    polys = [np.asarray(p, np.float64) for p in polygons]
+    if len(polys) > 32:
+        raise ValueError("Zones.set: at most 32 polygons, got %d" % len(polys))
+    for i, p in enumerate(polys):
+        if p.ndim != 2 or p.shape[1] != 2 or not 3 <= len(p) <= 256:
+            raise ValueError("Zones.set: polygon %d must be 3 to 256 (x, y) vertices, got shape %s" % (i, p.shape))
+        if not np.isfinite(p).all():
+            raise ValueError("Zones.set: polygon %d has a non-finite coordinate" % i)
+    sizes = np.array([len(p) for p in polys], np.int32)
+    if sizes.sum() > 2048:
+        raise ValueError("Zones.set: at most 2048 vertices per stream, got %d" % sizes.sum())
+    verts = np.ascontiguousarray(np.concatenate(polys) if polys else np.zeros((0, 2)), np.float64)
+    return np.array(lines, np.float64).reshape(-1, 4), sizes, verts
+
+
+class Zones(_DeviceObject):
+    """Line crossings and zone occupancy per camera stream on the device (lwdetr_zones_*, the contract in
+    include/lwdetr_b200.h, restated in tools/zone_spec.py): supervision's LineZone / PolygonZone, fed by Tracker.update.
+    Parameters are lwdetr_zones_params' fields: num_classes (default 91), capacity (records per stream, default 1024),
+    forget_after (frames, default 30), zone_anchor (an anchor index or a name of ANCHORS, default "bottom_center") and
+    line_anchors (a bit mask or a list of anchors, default the four corners).  Zones are fixed in frame pixels, also when the
+    tracker follows a moving camera.  All calls of one object must run on one CUDA stream (the current one at each call)."""
+
+    RESET, DESTROY = "lwdetr_zones_reset", "lwdetr_zones_destroy"
+
+    def __init__(self, num_streams, device=None, **params):
+        if isinstance(params.get("zone_anchor"), str):
+            params["zone_anchor"] = ANCHORS.index(params["zone_anchor"])
+        la = params.get("line_anchors")
+        if la is not None and not isinstance(la, int):
+            params["line_anchors"] = sum(1 << (ANCHORS.index(a) if isinstance(a, str) else int(a)) for a in set(la))
+        self.params = self._params(ZonesParams, "lwdetr_zones_params_default", params)
+        super().__init__(num_streams, device, "lwdetr_zones_create", self.params)
+
+    def set(self, stream, lines=(), polygons=()):
+        """Replaces one stream's geometry (frame pixels; zone_geometry's rules, checked before any device call) and clears
+        its records and counters.  Synchronous: waits for this object's last launch only.  Not during a stream capture."""
+        stream = int(stream)
+        if not 0 <= stream < self.num_streams:
+            raise ValueError("Zones.set: stream %d outside [0, %d)" % (stream, self.num_streams))
+        ln, sizes, verts = zone_geometry(lines, polygons)
+        check(lib().lwdetr_zones_set(self._t, stream, ln.ctypes.data_as(_vp), len(ln), sizes.ctypes.data_as(_vp), len(sizes),
+                                     verts.ctypes.data_as(_vp)), "lwdetr_zones_set")
+
+    def update(self, ids, labels, boxes, counts, stream_ids=None, max_events=1024):
+        """One frame for each of B distinct streams, on Tracker.update's outputs as they are: ids int32 [B, max_out], labels
+        [B, max_out], xyxy boxes fp32 [B, max_out, 4], counts [B] (CUDA; stream_ids default range(B)) -> (inside int32 [B,
+        max_out]: the bits of each track's uint32 zone mask; occupancy int32 [B, 32]; events int32 [B, max_events, 5] rows
+        (id, kind, index, label, dwell), kind ZONE_*, the frame's first max_events in order, unused rows zero; event_counts
+        int32 [B], the true number).  Stream-ordered, no synchronisation; graph-safe."""
+        import torch
+        B, m = ids.shape
+        if tuple(labels.shape) != (B, m) or tuple(boxes.shape) != (B, m, 4) or tuple(counts.shape) != (B,):
+            raise RuntimeError("Zones.update: ids %s, labels %s, boxes %s and counts %s do not describe one [B, max_out] set"
+                               % (tuple(ids.shape), tuple(labels.shape), tuple(boxes.shape), tuple(counts.shape)))
+        dev = self.device
+        ids = ids.to(device=dev, dtype=torch.int32).contiguous()
+        labels = labels.to(device=dev, dtype=torch.int32).contiguous()
+        boxes = boxes.to(device=dev, dtype=torch.float32).contiguous()
+        counts = counts.to(device=dev, dtype=torch.int32).contiguous()
+        sids, n = self._ids(range(B) if stream_ids is None else stream_ids)
+        if n != B:
+            raise RuntimeError("Zones.update: %d stream ids for %d frames" % (n, B))
+        E = int(max_events)
+        inside = torch.empty(B, m, device=dev, dtype=torch.int32)
+        occupancy = torch.empty(B, 32, device=dev, dtype=torch.int32)
+        events = torch.empty(B, E, 5, device=dev, dtype=torch.int32)
+        event_counts = torch.empty(B, device=dev, dtype=torch.int32)
+        check(lib().lwdetr_zones_update(self._t, ptr(ids), ptr(labels), ptr(boxes), ptr(counts), B, m, ctypes.cast(sids, _vp), ptr(inside),
+                                        ptr(occupancy), ptr(events) if E else None, E, ptr(event_counts), stream_ptr(dev)),
+              "lwdetr_zones_update")
+        return inside, occupancy, events, event_counts
+
+    def export(self, stream):
+        """Synchronous, waiting for this object's last update() or reset() and for nothing else on the device: one stream's
+        state as a dict of numpy arrays: frame, overflow, line_counts int32 [L, num_classes + 1, 2] (in, out), entries int32
+        [Z, num_classes + 1] (the last column: labels outside [0, num_classes)), and the records in ascending id: ids,
+        last_seen, labels int32 [n], sides int8 [n, L], inside uint32 [n], entry int32 [n, Z] (entry frames, 0 outside)."""
+        import numpy as np
+        nc = int(self.params.num_classes) + 1
+        cap = int(self.params.capacity)
+        lc = np.zeros((32, nc, 2), np.int32)
+        en = np.zeros((32, nc), np.int32)
+        recs = (ZoneRecord * cap)()
+        fo = (ctypes.c_int32 * 2)()
+        info = (ctypes.c_int32 * 3)()
+        check(lib().lwdetr_zones_export(self._t, int(stream), ctypes.cast(fo, _vp), ctypes.cast(info, _vp), lc.ctypes.data_as(_vp),
+                                        en.ctypes.data_as(_vp), ctypes.cast(recs, _vp), cap), "lwdetr_zones_export")
+        L, Z, n = list(info)
+        raw = np.frombuffer(recs, np.dtype([("id", "<i4"), ("last_seen", "<i4"), ("label", "<i4"), ("inside", "<u4"), ("sides", "i1", 32),
+                                            ("entry", "<i4", 32)]))[:n]
+        return dict(frame=fo[0], overflow=fo[1], line_counts=lc.reshape(-1)[:L * nc * 2].reshape(L, nc, 2).copy(),
+                    entries=en.reshape(-1)[:Z * nc].reshape(Z, nc).copy(), ids=raw["id"].copy(), last_seen=raw["last_seen"].copy(),
+                    labels=raw["label"].copy(), sides=raw["sides"][:, :L].copy(), inside=raw["inside"].copy(),
+                    entry=raw["entry"][:, :Z].copy())
 
 
 def layernorm_e4m3(x, eps=1e-6):

@@ -8,6 +8,7 @@
 #include <string>
 
 #include <algorithm>
+#include <cmath>
 #include <map>
 #include <memory>
 #include <new>
@@ -24,6 +25,7 @@
 #include "rowops.h"
 #include "tiles.h"
 #include "track.h"
+#include "zones.h"
 
 
 namespace {
@@ -67,7 +69,7 @@ int attention_call(lwdetr_attention_args* p, void* stream, const char* fn) {
   return 0;
 }
 
-// HOST stream ids of one call of a tracker or an estimator: distinct and in [0, num_streams); "" when they are
+// HOST stream ids of one call of a tracker, an estimator or a zones object: distinct and in [0, num_streams); "" when they are
 std::string check_ids(int num_streams, const int32_t* ids, int n) {
   std::vector<char> seen(static_cast<size_t>(num_streams), 0);
   for (int i = 0; i < n; ++i) {
@@ -90,7 +92,7 @@ struct Carver {
   }
 };
 
-// The device side of a tracker or an estimator: its buffers in one allocation, an event marking its last launch, and a
+// The device side of a tracker, an estimator or a zones object: its buffers in one allocation, an event marking its last launch, and a
 // non-blocking stream for its set-up and its reads, so that a read waits for the object's own work and nothing else.
 struct DeviceState {
   int device = 0;
@@ -588,6 +590,182 @@ int lwdetr_tracker_export(lwdetr_tracker* t, int stream_id, lwdetr_track_record*
   frame_next_overflow[0] = h.frame;
   frame_next_overflow[1] = h.next_id;
   frame_next_overflow[2] = h.overflow;
+  return 0;
+}
+
+static_assert(sizeof(lwdetr_zone_record) == 176, "zone record layout");
+
+struct lwdetr_zones {
+  lwb::ZoneTable table;
+  lwdetr_zones_params params;
+  std::vector<int32_t> n_lines, n_polys;   // each stream's geometry, as the last lwdetr_zones_set gave it
+  DeviceState state;
+};
+
+void lwdetr_zones_params_default(lwdetr_zones_params* p) {
+  if (!p) return;
+  p->num_classes = 91;
+  p->capacity = 1024;
+  p->forget_after = 30;
+  p->zone_anchor = LWDETR_ANCHOR_BOTTOM_CENTER;
+  p->line_anchors = (1 << LWDETR_ANCHOR_TOP_LEFT) | (1 << LWDETR_ANCHOR_TOP_RIGHT) | (1 << LWDETR_ANCHOR_BOTTOM_LEFT) |
+                    (1 << LWDETR_ANCHOR_BOTTOM_RIGHT);
+}
+
+int lwdetr_zones_create(int num_streams, const lwdetr_zones_params* params, lwdetr_zones** out) {
+  if (!params || !out) return fail("lwdetr_zones_create: null pointer");
+  const lwdetr_zones_params& p = *params;
+  if (num_streams < 1) return fail("lwdetr_zones_create: num_streams must be >= 1");
+  if (p.num_classes < 1 || p.num_classes > lwb::ZONE_CLASSES) return fail("lwdetr_zones_create: num_classes must be in [1, 1024]");
+  if (p.capacity < 1 || p.capacity > lwb::ZONE_CAPACITY) return fail("lwdetr_zones_create: capacity must be in [1, 4096]");
+  if (p.forget_after < 0) return fail("lwdetr_zones_create: forget_after must be >= 0");
+  if (p.zone_anchor < 0 || p.zone_anchor > 8) return fail("lwdetr_zones_create: zone_anchor must be in [0, 9)");
+  if (p.line_anchors <= 0 || p.line_anchors >= 1 << 9) return fail("lwdetr_zones_create: line_anchors must be a non-zero mask below 1 << 9");
+  std::unique_ptr<lwdetr_zones> z(new (std::nothrow) lwdetr_zones{});
+  if (!z) return fail("lwdetr_zones_create: out of memory");
+  z->params = p;
+  z->n_lines.assign(static_cast<size_t>(num_streams), 0);
+  z->n_polys.assign(static_cast<size_t>(num_streams), 0);
+  lwb::ZoneTable& t = z->table;
+  t.num_streams = num_streams;
+  t.capacity = p.capacity;
+  t.num_classes = p.num_classes;
+  t.forget_after = p.forget_after;
+  t.zone_anchor = p.zone_anchor;
+  t.line_anchors = p.line_anchors;
+  const size_t ns = static_cast<size_t>(num_streams), cap = static_cast<size_t>(p.capacity), ncol = static_cast<size_t>(p.num_classes) + 1;
+  const std::vector<lwb::ZoneHead> h(ns, lwb::ZoneHead{1, 0, 0, 0});    // every stream at frame 1, no records
+  const auto layout = [&](Carver& c) {
+    c.take(t.head, ns);
+    c.take(t.geom, ns);
+    c.take(t.verts, ns * lwb::ZONE_VERTS);
+    c.take(t.index, ns * cap);
+    c.take(t.rec, ns * cap);
+    c.take(t.line_counts, ns * lwb::ZONE_LINES * ncol * 2);
+    c.take(t.entries, ns * lwb::ZONE_POLYS * ncol);
+  };
+  const auto init = [&] {
+    cudaError_t e = cudaMemcpyAsync(t.head, h.data(), ns * sizeof(lwb::ZoneHead), cudaMemcpyHostToDevice, z->state.copy);
+    if (e == cudaSuccess) e = cudaMemsetAsync(t.geom, 0, ns * sizeof(lwb::ZoneGeom), z->state.copy);     // no lines, no polygons
+    if (e == cudaSuccess) e = cudaMemsetAsync(t.line_counts, 0, ns * lwb::ZONE_LINES * ncol * 2 * sizeof(int32_t), z->state.copy);
+    if (e == cudaSuccess) e = cudaMemsetAsync(t.entries, 0, ns * lwb::ZONE_POLYS * ncol * sizeof(int32_t), z->state.copy);
+    return e;
+  };
+  if (int rc = z->state.create("lwdetr_zones_create", layout, init)) return rc;
+  *out = z.release();
+  return 0;
+}
+
+void lwdetr_zones_destroy(lwdetr_zones* z) { delete z; }
+
+int lwdetr_zones_set(lwdetr_zones* z, int stream_id, const double* lines, int n_lines, const int32_t* polygon_sizes, int n_polygons,
+                     const double* vertices) {
+  if (!z || (n_lines > 0 && !lines) || (n_polygons > 0 && (!polygon_sizes || !vertices))) return fail("lwdetr_zones_set: null pointer");
+  const lwb::ZoneTable& t = z->table;
+  if (stream_id < 0 || stream_id >= t.num_streams) return fail("lwdetr_zones_set: stream id outside [0, num_streams)");
+  if (n_lines < 0 || n_lines > lwb::ZONE_LINES) return fail("lwdetr_zones_set: n_lines must be in [0, 32]");
+  if (n_polygons < 0 || n_polygons > lwb::ZONE_POLYS) return fail("lwdetr_zones_set: n_polygons must be in [0, 32]");
+  lwb::ZoneGeom g{};
+  g.n_lines = n_lines;
+  g.n_polys = n_polygons;
+  for (int l = 0; l < n_lines; ++l) {
+    for (int c = 0; c < 4; ++c) {
+      g.line[l][c] = lines[4 * l + c];
+      if (!std::isfinite(g.line[l][c])) return fail("lwdetr_zones_set: line " + std::to_string(l) + " has a non-finite coordinate");
+    }
+    if (g.line[l][0] == g.line[l][2] && g.line[l][1] == g.line[l][3]) return fail("lwdetr_zones_set: line " + std::to_string(l) + " has zero length");
+  }
+  for (int q = 0; q < n_polygons; ++q) {
+    if (polygon_sizes[q] < 3 || polygon_sizes[q] > lwb::ZONE_POLY_VERTS)
+      return fail("lwdetr_zones_set: polygon " + std::to_string(q) + " must have 3 to 256 vertices");
+    g.start[q + 1] = g.start[q] + polygon_sizes[q];
+    if (g.start[q + 1] > lwb::ZONE_VERTS) return fail("lwdetr_zones_set: more than 2048 vertices");
+  }
+  const int nv = g.start[n_polygons];
+  for (int i = 0; i < 2 * nv; ++i)
+    if (!std::isfinite(vertices[i])) return fail("lwdetr_zones_set: vertex " + std::to_string(i / 2) + " has a non-finite coordinate");
+  // after the object's last launch: the frame count goes on, the records and counters are cleared
+  lwb::ZoneHead h;
+  if (int rc = z->state.read_head("lwdetr_zones_set", t.head, t.num_streams, stream_id, &h)) return rc;
+  h.n = 0;
+  h.overflow = 0;
+  const size_t s = static_cast<size_t>(stream_id), ncol = static_cast<size_t>(t.num_classes) + 1;
+  lwb::DeviceGuard guard(z->state.device);
+  const cudaStream_t cs = z->state.copy;
+  cudaError_t e = cudaMemcpyAsync(t.geom + s, &g, sizeof(g), cudaMemcpyHostToDevice, cs);
+  if (e == cudaSuccess && nv) e = cudaMemcpyAsync(t.verts + s * lwb::ZONE_VERTS, vertices, nv * sizeof(double2), cudaMemcpyHostToDevice, cs);
+  if (e == cudaSuccess) e = cudaMemsetAsync(t.line_counts + s * lwb::ZONE_LINES * ncol * 2, 0, lwb::ZONE_LINES * ncol * 2 * sizeof(int32_t), cs);
+  if (e == cudaSuccess) e = cudaMemsetAsync(t.entries + s * lwb::ZONE_POLYS * ncol, 0, lwb::ZONE_POLYS * ncol * sizeof(int32_t), cs);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(t.head + s, &h, sizeof(h), cudaMemcpyHostToDevice, cs);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(cs);
+  if (e != cudaSuccess) return cuda_fail(e, "lwdetr_zones_set");
+  z->n_lines[s] = n_lines;
+  z->n_polys[s] = n_polygons;
+  return 0;
+}
+
+int lwdetr_zones_reset(lwdetr_zones* z, const int32_t* streams, int n, void* stream) {
+  if (!z || (n > 0 && !streams)) return fail("lwdetr_zones_reset: null pointer");
+  if (n < 0) return fail("lwdetr_zones_reset: n must be >= 0");
+  const std::string err = check_ids(z->table.num_streams, streams, n);
+  if (!err.empty()) return fail("lwdetr_zones_reset: " + err);
+  if (n == 0) return 0;
+  lwb::DeviceGuard g(z->state.device);
+  int e = lwb::zones_reset_launch(z->table, streams, n, static_cast<cudaStream_t>(stream));
+  if (!e) e = z->state.mark(stream);
+  if (e) return cuda_fail(e, "lwdetr_zones_reset launch");
+  return 0;
+}
+
+int lwdetr_zones_update(lwdetr_zones* z, const int32_t* ids, const int32_t* labels, const float* boxes, const int32_t* counts, int B,
+                        int max_out, const int32_t* stream_ids, uint32_t* inside, int32_t* occupancy, int32_t* events, int max_events,
+                        int32_t* event_counts, void* stream) {
+  if (!z || !ids || !labels || !boxes || !counts || !stream_ids || !inside || !occupancy || !event_counts || (max_events > 0 && !events))
+    return fail("lwdetr_zones_update: null pointer");
+  if (B < 1 || max_out < 1 || max_out > lwb::ZONE_MAX_OUT || max_events < 0)
+    return fail("lwdetr_zones_update: need B >= 1, max_out in [1, 1024] and max_events >= 0");
+  if (reinterpret_cast<uintptr_t>(boxes) % 16) return fail("lwdetr_zones_update: boxes must be 16-byte aligned");
+  const std::string err = check_ids(z->table.num_streams, stream_ids, B);
+  if (!err.empty()) return fail("lwdetr_zones_update: " + err);
+  lwb::DeviceGuard g(z->state.device);
+  int e = lwb::zones_launch(z->table, ids, labels, boxes, counts, B, max_out, stream_ids, inside, occupancy, events, max_events,
+                            event_counts, static_cast<cudaStream_t>(stream));
+  if (!e) e = z->state.mark(stream);
+  if (e) return cuda_fail(e, "lwdetr_zones_update launch");
+  return 0;
+}
+
+int lwdetr_zones_export(lwdetr_zones* z, int stream_id, int32_t frame_overflow[2], int32_t info[3], int32_t* line_counts, int32_t* entries,
+                        lwdetr_zone_record* records, int cap) {
+  if (!z || !frame_overflow || !info || !line_counts || !entries || (cap > 0 && !records)) return fail("lwdetr_zones_export: null pointer");
+  const lwb::ZoneTable& t = z->table;
+  lwb::ZoneHead h;
+  if (int rc = z->state.read_head("lwdetr_zones_export", t.head, t.num_streams, stream_id, &h)) return rc;
+  const size_t s = static_cast<size_t>(stream_id), C = static_cast<size_t>(t.capacity), ncol = static_cast<size_t>(t.num_classes) + 1;
+  const int L = z->n_lines[s], Z = z->n_polys[s];
+  std::vector<lwb::ZoneIndex> idx(static_cast<size_t>(h.n));
+  std::vector<lwb::ZoneRec> rec(C);
+  const cudaError_t e = z->state.read({{line_counts, t.line_counts + s * lwb::ZONE_LINES * ncol * 2, L * ncol * 2 * sizeof(int32_t)},
+                                       {entries, t.entries + s * lwb::ZONE_POLYS * ncol, Z * ncol * sizeof(int32_t)},
+                                       {idx.data(), t.index + s * C, idx.size() * sizeof(lwb::ZoneIndex)},
+                                       {rec.data(), t.rec + s * C, h.n ? C * sizeof(lwb::ZoneRec) : 0}});
+  if (e != cudaSuccess) return cuda_fail(e, "lwdetr_zones_export");
+  for (int i = 0; i < h.n && i < cap; ++i) {
+    const lwb::ZoneRec& r = rec[static_cast<size_t>(idx[i].slot)];
+    lwdetr_zone_record& o = records[i];
+    o = lwdetr_zone_record{};
+    o.id = idx[i].id;
+    o.last_seen = idx[i].last_seen;
+    o.label = r.label;
+    o.inside = r.inside;
+    for (int l = 0; l < L; ++l) o.sides[l] = static_cast<int8_t>(r.side_set >> l & 1 ? (r.side_pos >> l & 1 ? 1 : -1) : 0);
+    for (int q = 0; q < Z; ++q) o.entry[q] = r.entry[q];
+  }
+  frame_overflow[0] = h.frame;
+  frame_overflow[1] = h.overflow;
+  info[0] = L;
+  info[1] = Z;
+  info[2] = h.n;
   return 0;
 }
 

@@ -207,7 +207,7 @@ class LWDETR(nn.Module):
     @torch.no_grad()
     def track(self, frames, tracker, streams=None, size=None, fit="stretch", short_side=None, max_side=None, colorspace=None,
               max_out=None, motion=None, appearance=False, reid=None, reid_size=(256, 128), reid_filter="bilinear", reid_mean=None,
-              reid_std=None, reid_normalize=True):
+              reid_std=None, reid_normalize=True, zones=None):
         """Multi-object tracking of video streams: frames (RGB or NV12, taken exactly as detect() takes them) run as one
         forward; each query gives one detection, its best class (capi.query_best, boxes in the frame's original pixels);
         then capi.Tracker `tracker` (ByteTrack on the device, include/lwdetr_b200.h) updates each frame's stream.
@@ -231,6 +231,11 @@ class LWDETR(nn.Module):
         reid_normalize=False (capi.crops, float32); reid runs once on all of them under no_grad, and its rows are scattered
         back to their entries (zeros elsewhere: no appearance).  Zero crops: reid is not called.  This costs one extra
         synchronisation per call, the read-back of the crop count that sizes reid's batch.
+        zones: a capi.Zones over the same streams; after each round's tracker update it takes the tracker's outputs as they
+        are (Zones.update), and each frame's dict gains "inside" (int64 [c], each track's zone bit mask), "occupancy" (int32
+        [32], present tracks per zone) and "events" (int32 [e, 5] rows (id, kind, index, label, dwell), the frame's first
+        Zones.update max_events).  The event counts come back in the read-back of the track counts: no extra
+        synchronisation.  With motion= the zones stay fixed in frame pixels: they are image regions, not world regions.
         How ByteTrack's thresholds (tuned on YOLOX scores) suit LW-DETR's score distribution, and whether the decoder's features tell identities apart on real footage, in MOTA / IDF1 / HOTA, is
         not measured here."""
         if self.training:
@@ -273,7 +278,7 @@ class LWDETR(nn.Module):
             if r == len(rounds):
                 rounds.append([])
             rounds[r].append(i)
-        res, counts = [None] * n, []
+        res, counts, ev_counts = [None] * n, [], []
         for rows in rounds:
             idx = torch.tensor(rows, device=dev)
             ids = [streams[i] for i in rows]
@@ -284,17 +289,26 @@ class LWDETR(nn.Module):
             got = tracker.update(scores[idx], labels[idx], boxes[idx], ids, self.num_queries if max_out is None else max_out, motion=mo,
                                  embeddings=em)
             counts.append(got[5])
+            zo = None
+            if zones is not None:
+                inside, occupancy, events, n_ev = zones.update(got[0], got[2], got[3], got[5], ids)
+                zo = (inside.long() & 0xFFFFFFFF, occupancy, events)      # the uint32 masks widened once per round
+                ev_counts.append(n_ev)
             for j, i in enumerate(rows):
-                res[i] = (got, j)
-        counts = torch.cat(counts).cpu().tolist()
+                res[i] = (got, zo, j)
+        both = torch.cat(counts + ev_counts).cpu().tolist()     # track and event counts in one read-back
         order = [i for rows in rounds for i in rows]
-        cnt = {i: c for i, c in zip(order, counts)}
+        cnt = {i: c for i, c in zip(order, both[:n])}
+        ecnt = {i: c for i, c in zip(order, both[n:])}
         dets = []
         for i in range(n):
-            (ids, sc, lab, bx, q, _), j = res[i]
+            (ids, sc, lab, bx, q, _), zo, j = res[i]
             c = cnt[i]
-            dets.append({"ids": ids[j, :c], "scores": sc[j, :c], "labels": lab[j, :c].long(), "boxes": bx[j, :c],
-                         "queries": q[j, :c].long()})
+            d = {"ids": ids[j, :c], "scores": sc[j, :c], "labels": lab[j, :c].long(), "boxes": bx[j, :c], "queries": q[j, :c].long()}
+            if zo is not None:
+                inside, occupancy, events = zo
+                d.update(inside=inside[j, :c], occupancy=occupancy[j], events=events[j, :min(ecnt[i], events.shape[1])])
+            dets.append(d)
         return dets
 
     def _reid_embeddings(self, fb, scores, boxes, tracker, reid, size, filter, mean, std, normalize):
