@@ -525,6 +525,95 @@ LWDETR_API int lwdetr_gmc_reset(lwdetr_gmc* g, const int32_t* streams, int n, vo
 LWDETR_API int lwdetr_gmc_export(lwdetr_gmc* g, int stream_id, uint8_t* levels, int64_t levels_bytes, float* corners, float* flow,
                                  int8_t* found, int32_t info[6]);
 
+/* Tracking between detections: the detector runs on every N-th frame of a stream and the frames between are tracked by
+ * per-object optical flow on the device - the Median Flow tracker (Kalal et al., 2010; OpenCV's TrackerMedianFlow) for
+ * every track of every stream, on the camera-motion estimator's pyramids.  The C composition per call: the streams whose
+ * frame is a keyframe go lwdetr_forward_frames (or _nv12) -> lwdetr_query_best -> lwdetr_track (or _ex with
+ * lwdetr_gmc_estimate); the others go lwdetr_gmc_observe (or lwdetr_gmc_estimate, with a moving camera) ->
+ * lwdetr_track_flow; both then -> lwdetr_zones_update.  tools/flow_spec.py restates the flow in numpy and
+ * tools/track_spec.py (Stream.update_flow) the tracker step.
+ * lwdetr_gmc_observe / _nv12 (declared after the frame descriptors): lwdetr_gmc_estimate's steps 1-3 only (grey, pyramid,
+ *   corners); no Lucas-Kanade, no fit, no outputs.  The stream's chain of pyramids and corners stays current at a lower
+ *   cost, so an estimate or a flow may follow on its next frame.
+ * The flow of one stream, d = the estimator's downscale, every float64 operation rounded on its own:
+ *   1. tracks: the activated records of the tracked list (state Tracked), in list order, as the tracker holds them after the
+ *      stream's previous frame; track j >= max_tracks gets LWDETR_FLOW_SKIPPED.  When the estimator has no previous frame of
+ *      the same size for the stream (its last two frames must be this one and the one before, through estimate or observe),
+ *      every track gets LWDETR_FLOW_NO_PREVIOUS.
+ *   2. seeds: box (x1, y1, w, h) of the track's state (w = a h, x1 = cx - w / 2, y1 = cy - h / 2); seed (i, k) of the
+ *      grid x grid lattice, q = k grid + i: x_f = x1 + ((i + 0.5) w) / grid, y_f = y1 + ((k + 0.5) h) / grid, to level 0 by
+ *      x_0 = (x_f + 0.5) / d - 0.5, rounded to fp32.
+ *   3. forward Lucas-Kanade of each seed from the previous pyramid into the current one, then backward from the forward
+ *      point, with lwdetr_gmc_estimate's step-4 iteration (the estimator's levels; the flow's window, iterations, eps and
+ *      min_eig).  A seed is valid when both end with status 1.
+ *   4. per valid seed, in frame pixels (x_f = d (x_0 + 0.5) - 0.5 of the fp32 points): FB = |p - p_back|; NCC of the
+ *      ncc_window^2 patches of level 0 around round(p) in the previous frame and round(p_fwd) in the current one (round half
+ *      to even, BORDER_REFLECT_101), from exact int64 sums: (n S_ab - S_a S_b) / sqrt((double)(n S_aa - S_a^2) * (double)(n
+ *      S_bb - S_b^2)), -1 when either variance is 0.  OpenCV samples the patches at sub-pixel positions (getRectSubPix); the
+ *      rounding is a deviation.
+ *   5. "median" is the lower median: element (n - 1) / 2 of the ascending order.  Selected: the valid seeds with FB <=
+ *      median(FB) and NCC >= median(NCC), both medians over the valid seeds.
+ *   6. status, in this order: fewer than min_points selected: LWDETR_FLOW_FEW_POINTS; median FB > fb_max: LWDETR_FLOW_FB.
+ *      Else dx, dy = the medians of the selected displacements p_fwd - p; s = the median over the selected pairs i < j (seed
+ *      order) with |p_i - p_j| > 0 of |q_i - q_j| / |p_i - p_j| (each norm sqrt(ex * ex + ey * ey)); no such pair, or s not
+ *      in [scale_min, scale_max]: LWDETR_FLOW_SCALE.  Else the measurement z = (cx + dx, cy + dy, a, h * s) of the state
+ *      (cx, cy, a, h): centre moved, size scaled; a box under 2 level-0 pixels on a side (a (h s) or h s < 2 d):
+ *      LWDETR_FLOW_SMALL.  Else LWDETR_FLOW_OK.
+ *   Deviations from OpenCV's TrackerMedianFlow: the seeds are the state's box, not the last measured one; the scale is the
+ *   lower median of the ratios (OpenCV: the median of the sorted vector's middle element); the status rules are the ones
+ *   above.
+ *   Limits, measured on rendered textured sprites (tests/test_flow_cpu.py, cv2's Lucas-Kanade on this contract): a sprite
+ *   that nothing covers is measured to within 1.1 px on every side, not 0.5 px (the worst of three scenes is 0.96 px off;
+ *   80-100 % of its frames are within 0.5 px); the cause was not isolated (leaving out the outer ring of seeds, whose windows
+ *   see the background, does not remove it).  The failure statuses do not catch every bad measurement: a texture-less
+ *   object on a textured background is measured from the seeds near its outline, and an object partly covered by a flat
+ *   bar or by another textured object from the seeds on the cover; both can get LWDETR_FLOW_OK with a box 1-14 px off.
+ *   Through the tracker (32 streams of rendered 1080p sprites, detections every 4th frame): no identity changes for
+ *   uncovered sprites; the output box (the Kalman state after the flow's update) has IoU >= 0.9 with the truth on 99.7 % of
+ *   the flow frames and 0.88 at worst.
+ * lwdetr_flow_params_default: grid 10 (in [2, 16]), window 15 (odd, [5, 31]), iterations 30, eps 0.01, min_eig 1e-4 (the
+ *   estimator's defaults), ncc_window 11 (odd, [3, 31]), min_points 8 (in [1, grid^2]), fb_max 10 frame pixels (> 0),
+ *   scale_min 0.5, scale_max 2 (0 < scale_min <= 1 <= scale_max), max_tracks 256 per stream (in [1, 1024]).
+ * lwdetr_flow_create: a flow bound to the estimator gmc (which must outlive it) with its stream count; one device allocation
+ *   of num_streams * max_tracks * grid^2 seeds (about 41 bytes each) on the estimator's device.  Synchronous.
+ * lwdetr_track_flow: one flow frame for each of B streams (stream_ids HOST, distinct, in [0, num_streams) of both the
+ *   tracker and the flow's estimator); outputs as lwdetr_track's.  Per stream, float64 as the tracker contract:
+ *   1. the pool (confirmed tracks, then lost) is predicted as in step 1; with motion (DEVICE [B, 4], or NULL) every record
+ *      is then warped as lwdetr_track_ex does: the flow already carries the camera motion of the tracks it measures, the
+ *      warp keeps the lost tracks aligned for the next keyframe;
+ *   2. the flow above runs on the records as they were before this step (so on the states after the previous frame);
+ *   3. a confirmed Tracked track whose status is LWDETR_FLOW_OK is updated with the Kalman update by z; it keeps its score
+ *      and label, takes index -1 and end_frame = frame.  A confirmed Tracked track with any other status becomes Lost;
+ *   4. unconfirmed tracks are carried unchanged: not updated, not removed, not output;
+ *   5. ageing (step 5), the new lists (tracked = previous tracked still Tracked; lost = previous lost not removed, then the
+ *      new lost), duplicates (step 8) and the output (step 9, index -1) as the contract.  No births; the frame counter
+ *      advances.
+ *   Asynchronous, nothing allocated or copied per call, safe to capture in a CUDA graph.  A tracker with appearance keeps its
+ *   embeddings: a flow frame neither updates nor moves them.
+ * lwdetr_flow_export (tests), synchronous: waits for the flow's last lwdetr_track_flow; one stream's last call.
+ *   info = (tracks found by step 1, tracks measured = min(that, max_tracks), grid); per measured track j and seed q (index
+ *   j * grid^2 + q): seeds, fwd, bwd float [.., 2] (level 0), valid int8, fb, ncc float64 (NaN where not valid); per track:
+ *   status int32 and meas float64 [.., 8] = (dx, dy, s, z[4], unused), NaN where the status came before them.  cap: the
+ *   room in tracks; the arrays hold min(cap, info[1]) tracks. */
+enum { LWDETR_FLOW_OK = 0, LWDETR_FLOW_FEW_POINTS = 1, LWDETR_FLOW_FB = 2, LWDETR_FLOW_SCALE = 3, LWDETR_FLOW_SMALL = 4,
+       LWDETR_FLOW_SKIPPED = 5, LWDETR_FLOW_NO_PREVIOUS = 6 };
+typedef struct {
+  int32_t grid, window, iterations;
+  float eps, min_eig;
+  int32_t ncc_window, min_points;
+  float fb_max, scale_min, scale_max;
+  int32_t max_tracks;
+} lwdetr_flow_params;
+typedef struct lwdetr_flow lwdetr_flow;
+LWDETR_API void lwdetr_flow_params_default(lwdetr_flow_params* p);
+LWDETR_API int lwdetr_flow_create(lwdetr_gmc* gmc, const lwdetr_flow_params* params, lwdetr_flow** out);
+LWDETR_API void lwdetr_flow_destroy(lwdetr_flow* f);
+LWDETR_API int lwdetr_track_flow(lwdetr_tracker* t, lwdetr_flow* flow, const double* motion, int B, const int32_t* stream_ids, int max_out,
+                                 int32_t* out_ids, float* out_scores, int32_t* out_labels, float* out_boxes, int32_t* out_index,
+                                 int32_t* counts, void* stream);
+LWDETR_API int lwdetr_flow_export(lwdetr_flow* f, int stream_id, int cap, float* seeds, float* fwd, float* bwd, int8_t* valid, double* fb,
+                                  double* ncc, int32_t* status, double* meas, int32_t info[3]);
+
 /* Line crossings and zone occupancy per camera stream, on the tracker's outputs (what DeepStream's nvdsanalytics and
  * supervision's LineZone / PolygonZone compute after a tracker).  The C composition per batch of frames: ... ->
  * lwdetr_track (or _ex / _reid) -> lwdetr_zones_update on its out_ids, out_labels, out_boxes and counts with the same
@@ -784,6 +873,9 @@ LWDETR_API int lwdetr_gmc_estimate(lwdetr_gmc* g, const lwdetr_frame* frames, in
                                    int32_t* status, int32_t* inliers, void* stream);
 LWDETR_API int lwdetr_gmc_estimate_nv12(lwdetr_gmc* g, const lwdetr_frame_nv12* frames, int B, const int32_t* stream_ids,
                                         double* motion, int32_t* status, int32_t* inliers, void* stream);
+/* Pyramids and corners only (lwdetr_gmc_observe above), for the frames tracked by flow. */
+LWDETR_API int lwdetr_gmc_observe(lwdetr_gmc* g, const lwdetr_frame* frames, int B, const int32_t* stream_ids, void* stream);
+LWDETR_API int lwdetr_gmc_observe_nv12(lwdetr_gmc* g, const lwdetr_frame_nv12* frames, int B, const int32_t* stream_ids, void* stream);
 
 /* Detection crops for second-stage networks (ReID, attribute, vehicle-type or plate models, a second detector pass): each
  * box cut out of its frame on the device and resized to one out_h x out_w size, so no frame leaves the device and no host

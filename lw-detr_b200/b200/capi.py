@@ -53,6 +53,13 @@ _SIGNATURES = {
     "lwdetr_gmc_export": (_i, [_vp, _i, _vp, _i64, _vp, _vp, _vp, _vp]),
     "lwdetr_gmc_estimate": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwdetr_gmc_estimate_nv12": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
+    "lwdetr_gmc_observe": (_i, [_vp, _vp, _i, _vp, _vp]),
+    "lwdetr_gmc_observe_nv12": (_i, [_vp, _vp, _i, _vp, _vp]),
+    "lwdetr_flow_params_default": (None, [_vp]),
+    "lwdetr_flow_create": (_i, [_vp, _vp, _vp]),
+    "lwdetr_flow_destroy": (None, [_vp]),
+    "lwdetr_track_flow": (_i, [_vp, _vp, _vp, _i, _vp, _i] + [_vp] * 7),
+    "lwdetr_flow_export": (_i, [_vp, _i, _i] + [_vp] * 9),
     "lwdetr_zones_params_default": (None, [_vp]),
     "lwdetr_zones_create": (_i, [_i, _vp, _vp]),
     "lwdetr_zones_destroy": (None, [_vp]),
@@ -565,6 +572,15 @@ class Tracker(_DeviceObject):
             super().__init__(num_streams, device, "lwdetr_tracker_create_reid", self.params, self.reid)
         else:
             super().__init__(num_streams, device, "lwdetr_tracker_create", self.params)
+        # frames each stream has had since create or reset, counted on the host by update() and BoxFlow.propagate() (the
+        # keyframe schedule of LWDETR.track(detect_every=)); a replayed CUDA graph of those calls, or a direct C call on this
+        # tracker, advances the device's frame counter without it
+        self.frames = [0] * self.num_streams
+
+    def reset(self, streams):
+        super().reset(streams)
+        for s in streams:
+            self.frames[int(s)] = 0
 
     def update(self, scores, labels, boxes, stream_ids=None, max_out=None, motion=None, embeddings=None):
         """One frame for each of B distinct streams: scores fp32 [B, k], labels int [B, k], xyxy boxes fp32 [B, k, 4] (CUDA;
@@ -622,7 +638,12 @@ class Tracker(_DeviceObject):
         else:
             check(lib().lwdetr_track_ex(self._t, ptr(scores), ptr(labels), ptr(boxes), ptr(motion), B, k, ctypes.cast(ids, _vp), m,
                                         ptr(o_id), ptr(o_s), ptr(o_l), ptr(o_b), ptr(o_i), ptr(counts), stream_ptr(dev)), "lwdetr_track_ex")
+        self._advance(ids, n)
         return o_id, o_s, o_l, o_b, o_i, counts
+
+    def _advance(self, ids, n):
+        for i in range(n):
+            self.frames[ids[i]] += 1
 
     def export(self, stream_id):
         """Synchronous: (records, (frame, next_id, overflow)) of one stream, records a list of dicts in list order (tracked,
@@ -685,10 +706,7 @@ class MotionEstimator(_DeviceObject):
         b y + tx, y' = b x + a y + ty from the stream's previous frame to this one in frame pixels; status int32 [B]
         (GMC_*); inliers int32 [B]).  streams defaults to range(B).  Stream-ordered, no synchronisation."""
         import torch
-        if not isinstance(frames, Frames):
-            nv12 = isinstance(frames, torch.Tensor) and frames.dim() == 3 and frames.shape[2] != 3
-            nv12 = nv12 or (not isinstance(frames, torch.Tensor) and len(frames) > 0 and _is_nv12(frames[0]))
-            frames = Frames(frames, self.device, "bt601" if nv12 else None)
+        frames = self._frames(frames)
         B = len(frames.items)
         ids, n = self._ids(range(B) if streams is None else streams)
         if n != B:
@@ -701,6 +719,25 @@ class MotionEstimator(_DeviceObject):
         name = "lwdetr_gmc_estimate_nv12" if frames.nv12 else "lwdetr_gmc_estimate"
         check(getattr(lib(), name)(self._t, descs, B, ctypes.cast(ids, _vp), ptr(motion), ptr(status), ptr(inliers), stream_ptr(dev)), name)
         return motion, status, inliers
+
+    def observe(self, frames, streams=None):
+        """estimate() without the motion (lwdetr_gmc_observe): the streams' pyramids and corners only, so that the next
+        estimate() or a BoxFlow on the next frame has this one as its previous frame.  Stream-ordered, no synchronisation."""
+        frames = self._frames(frames)
+        B = len(frames.items)
+        ids, n = self._ids(range(B) if streams is None else streams)
+        if n != B:
+            raise RuntimeError("MotionEstimator.observe: %d stream ids for %d frames" % (n, B))
+        name = "lwdetr_gmc_observe_nv12" if frames.nv12 else "lwdetr_gmc_observe"
+        check(getattr(lib(), name)(self._t, frames.descs(frames.sizes), B, ctypes.cast(ids, _vp), stream_ptr(self.device)), name)
+
+    def _frames(self, frames):
+        import torch
+        if isinstance(frames, Frames):
+            return frames
+        nv12 = isinstance(frames, torch.Tensor) and frames.dim() == 3 and frames.shape[2] != 3
+        nv12 = nv12 or (not isinstance(frames, torch.Tensor) and len(frames) > 0 and _is_nv12(frames[0]))
+        return Frames(frames, self.device, "bt601" if nv12 else None)
 
     def export(self, stream_id):
         """Synchronous, waiting for this estimator's last estimate() or reset() and for nothing else on the device: one
@@ -726,6 +763,80 @@ class MotionEstimator(_DeviceObject):
             lh, lw = (lh + 1) // 2, (lw + 1) // 2
         return dict(valid=bool(valid), size=(h, w), levels=levels, corners=corners[:nc].copy(), flow=flow[:nf].copy(),
                     found=found[:nf].astype(bool))
+
+
+class FlowParams(ctypes.Structure):
+    """lwdetr_flow_params (include/lwdetr_b200.h)."""
+    _fields_ = [("grid", ctypes.c_int32), ("window", ctypes.c_int32), ("iterations", ctypes.c_int32), ("eps", _f), ("min_eig", _f),
+                ("ncc_window", ctypes.c_int32), ("min_points", ctypes.c_int32), ("fb_max", _f), ("scale_min", _f), ("scale_max", _f),
+                ("max_tracks", ctypes.c_int32)]
+
+
+FLOW_OK, FLOW_FEW_POINTS, FLOW_FB, FLOW_SCALE, FLOW_SMALL, FLOW_SKIPPED, FLOW_NO_PREVIOUS = range(7)
+
+
+class BoxFlow(_DeviceObject):
+    """Per-object optical flow for the frames between detections (the Median Flow tracker, lwdetr_flow_* and
+    lwdetr_track_flow in include/lwdetr_b200.h), bound to one MotionEstimator whose pyramids it reads (the estimator must
+    have seen each stream's previous frame and its current one, through estimate() or observe()).  Parameters are
+    lwdetr_flow_params' fields (defaults: lwdetr_flow_params_default).  Calls must run on the estimator's CUDA stream."""
+
+    DESTROY = "lwdetr_flow_destroy"
+
+    def __init__(self, estimator, **params):
+        import torch
+        self.params = self._params(FlowParams, "lwdetr_flow_params_default", params)
+        self.estimator = estimator                  # kept alive: the flow reads its tables
+        self.num_streams = estimator.num_streams
+        self.device = estimator.device
+        self._t = _vp()
+        with torch.cuda.device(self.device):
+            check(lib().lwdetr_flow_create(estimator._t, ctypes.byref(self.params), ctypes.byref(self._t)), "lwdetr_flow_create")
+
+    def reset(self, streams):
+        raise RuntimeError("BoxFlow.reset: a flow keeps no per-stream state; reset the tracker and the estimator")
+
+    def propagate(self, tracker, streams, motion=None, max_out=None):
+        """One flow frame for each listed stream (lwdetr_track_flow): the tracker's confirmed tracks move by their measured
+        flow or go Lost, with no detections.  motion: float64 [B, 4] of these frames (MotionEstimator.estimate) or None.
+        Returns Tracker.update's tuple; index is -1 for every track.  Stream-ordered, no synchronisation."""
+        import torch
+        ids, B = self._ids(streams)
+        dev = self.device
+        m = int(tracker.params.capacity) if max_out is None else int(max_out)
+        o_id = torch.empty(B, m, device=dev, dtype=torch.int32)
+        o_s = torch.empty(B, m, device=dev, dtype=torch.float32)
+        o_l = torch.empty(B, m, device=dev, dtype=torch.int32)
+        o_b = torch.empty(B, m, 4, device=dev, dtype=torch.float32)
+        o_i = torch.empty(B, m, device=dev, dtype=torch.int32)
+        counts = torch.empty(B, device=dev, dtype=torch.int32)
+        if motion is not None:
+            if tuple(motion.shape) != (B, 4):
+                raise RuntimeError("BoxFlow.propagate: motion must be [%d, 4], got %s" % (B, tuple(motion.shape)))
+            motion = motion.to(device=dev, dtype=torch.float64).contiguous()
+        check(lib().lwdetr_track_flow(tracker._t, self._t, ptr(motion), B, ctypes.cast(ids, _vp), m, ptr(o_id), ptr(o_s), ptr(o_l),
+                                      ptr(o_b), ptr(o_i), ptr(counts), stream_ptr(dev)), "lwdetr_track_flow")
+        tracker._advance(ids, B)
+        return o_id, o_s, o_l, o_b, o_i, counts
+
+    def export(self, stream_id):
+        """Synchronous: one stream's last flow (lwdetr_flow_export) as a dict of numpy arrays: found (tracks listed), grid,
+        per measured track [n, grid^2, ...] seeds, fwd, bwd (level-0 float32 x, y), valid, fb, ncc; per track status, dx, dy,
+        s and z (the measurement cx, cy, a, h)."""
+        import numpy as np
+        T, g2 = int(self.params.max_tracks), int(self.params.grid) ** 2
+        seeds, fwd, bwd = (np.zeros((T, g2, 2), np.float32) for _ in range(3))
+        valid = np.zeros((T, g2), np.int8)
+        fb, ncc = np.zeros((T, g2)), np.zeros((T, g2))
+        status = np.zeros(T, np.int32)
+        meas = np.zeros((T, 8))
+        info = (ctypes.c_int32 * 3)()
+        arrs = [seeds, fwd, bwd, valid, fb, ncc, status, meas]
+        check(lib().lwdetr_flow_export(self._t, int(stream_id), T, *[a.ctypes.data_as(_vp) for a in arrs], ctypes.cast(info, _vp)),
+              "lwdetr_flow_export")
+        n = info[1]
+        return dict(found=info[0], grid=info[2], seeds=seeds[:n], fwd=fwd[:n], bwd=bwd[:n], valid=valid[:n].astype(bool), fb=fb[:n],
+                    ncc=ncc[:n], status=status[:n], dx=meas[:n, 0], dy=meas[:n, 1], s=meas[:n, 2], z=meas[:n, 3:7])
 
 
 class ZonesParams(ctypes.Structure):

@@ -18,6 +18,7 @@
 #include "attn.h"
 #include "crops.h"
 #include "engine.h"
+#include "flow.h"
 #include "gemm_tc.h"
 #include "gmc.h"
 #include "msda.h"
@@ -886,10 +887,11 @@ int lwdetr_gmc_export(lwdetr_gmc* g, int stream_id, uint8_t* levels, int64_t lev
   return 0;
 }
 
+// lwdetr_gmc_estimate / _nv12, and with observe lwdetr_gmc_observe / _nv12 (no outputs)
 static int gmc_estimate_common(const char* name, lwdetr_gmc* g, const std::vector<lwb::GmcFrameHost>& fr, int B, const int32_t* stream_ids,
-                               double* motion, int32_t* status, int32_t* inliers, void* stream) {
+                               double* motion, int32_t* status, int32_t* inliers, void* stream, bool observe = false) {
   const std::string fn(name);
-  if (!motion || !status || !inliers) return fail(fn + ": null pointer");
+  if (!observe && (!motion || !status || !inliers)) return fail(fn + ": null pointer");
   if (reinterpret_cast<uintptr_t>(motion) % 8) return fail(fn + ": motion must be 8-byte aligned");
   const std::string err = check_ids(g->table.num_streams, stream_ids, B);
   if (!err.empty()) return fail(fn + ": " + err);
@@ -904,7 +906,7 @@ static int gmc_estimate_common(const char* name, lwdetr_gmc* g, const std::vecto
     if (f.pitch < static_cast<long long>(f.w) * (f.nv12 ? 1 : 3)) return fail(fn + ": frame " + std::to_string(i) + ": pitch too small");
   }
   lwb::DeviceGuard dg(g->state.device);
-  int e = lwb::gmc_estimate_launch(g->table, fr.data(), B, stream_ids, motion, status, inliers, static_cast<cudaStream_t>(stream));
+  int e = lwb::gmc_estimate_launch(g->table, fr.data(), B, stream_ids, motion, status, inliers, static_cast<cudaStream_t>(stream), observe);
   if (!e) e = g->state.mark(stream);
   if (e) return cuda_fail(e, (fn + " launch").c_str());
   return 0;
@@ -926,6 +928,133 @@ int lwdetr_gmc_estimate_nv12(lwdetr_gmc* g, const lwdetr_frame_nv12* frames, int
   std::vector<lwb::GmcFrameHost> fr(static_cast<size_t>(B));
   for (int i = 0; i < B; ++i) fr[i] = lwb::GmcFrameHost{frames[i].luma, frames[i].luma_pitch, frames[i].height, frames[i].width, 1};
   return gmc_estimate_common("lwdetr_gmc_estimate_nv12", g, fr, B, stream_ids, motion, status, inliers, stream);
+}
+
+int lwdetr_gmc_observe(lwdetr_gmc* g, const lwdetr_frame* frames, int B, const int32_t* stream_ids, void* stream) {
+  if (!g || !frames || !stream_ids) return fail("lwdetr_gmc_observe: null pointer");
+  if (B < 1) return fail("lwdetr_gmc_observe: B must be >= 1");
+  std::vector<lwb::GmcFrameHost> fr(static_cast<size_t>(B));
+  for (int i = 0; i < B; ++i) fr[i] = lwb::GmcFrameHost{frames[i].data, frames[i].pitch_bytes, frames[i].height, frames[i].width, 0};
+  return gmc_estimate_common("lwdetr_gmc_observe", g, fr, B, stream_ids, nullptr, nullptr, nullptr, stream, true);
+}
+
+int lwdetr_gmc_observe_nv12(lwdetr_gmc* g, const lwdetr_frame_nv12* frames, int B, const int32_t* stream_ids, void* stream) {
+  if (!g || !frames || !stream_ids) return fail("lwdetr_gmc_observe_nv12: null pointer");
+  if (B < 1) return fail("lwdetr_gmc_observe_nv12: B must be >= 1");
+  std::vector<lwb::GmcFrameHost> fr(static_cast<size_t>(B));
+  for (int i = 0; i < B; ++i) fr[i] = lwb::GmcFrameHost{frames[i].luma, frames[i].luma_pitch, frames[i].height, frames[i].width, 1};
+  return gmc_estimate_common("lwdetr_gmc_observe_nv12", g, fr, B, stream_ids, nullptr, nullptr, nullptr, stream, true);
+}
+
+struct lwdetr_flow {
+  lwb::FlowTable table;
+  lwdetr_gmc* gmc;
+  DeviceState state;
+};
+
+void lwdetr_flow_params_default(lwdetr_flow_params* p) {
+  if (!p) return;
+  p->grid = 10;
+  p->window = 15;
+  p->iterations = 30;
+  p->eps = 0.01f;
+  p->min_eig = 1e-4f;
+  p->ncc_window = 11;
+  p->min_points = 8;
+  p->fb_max = 10.f;
+  p->scale_min = 0.5f;
+  p->scale_max = 2.f;
+  p->max_tracks = 256;
+}
+
+int lwdetr_flow_create(lwdetr_gmc* gmc, const lwdetr_flow_params* params, lwdetr_flow** out) {
+  if (!gmc || !params || !out) return fail("lwdetr_flow_create: null pointer");
+  const lwdetr_flow_params& p = *params;
+  if (p.grid < 2 || p.grid > lwb::FLOW_MAX_GRID) return fail("lwdetr_flow_create: grid must be in [2, 16]");
+  if (p.window < 5 || p.window > lwb::GMC_MAX_WINDOW || p.window % 2 == 0) return fail("lwdetr_flow_create: window must be odd in [5, 31]");
+  if (p.iterations < 1 || p.iterations > 100) return fail("lwdetr_flow_create: iterations must be in [1, 100]");
+  if (!(p.eps > 0.f && p.eps < 1e30f) || !(p.min_eig >= 0.f && p.min_eig < 1e30f)) return fail("lwdetr_flow_create: need eps > 0 and min_eig >= 0, both finite");
+  if (p.ncc_window < 3 || p.ncc_window > 31 || p.ncc_window % 2 == 0) return fail("lwdetr_flow_create: ncc_window must be odd in [3, 31]");
+  if (p.min_points < 1 || p.min_points > p.grid * p.grid) return fail("lwdetr_flow_create: min_points must be in [1, grid^2]");
+  if (!(p.fb_max > 0.f && p.fb_max < 1e30f)) return fail("lwdetr_flow_create: fb_max must be > 0 and finite");
+  if (!(p.scale_min > 0.f && p.scale_min <= 1.f && p.scale_max >= 1.f && p.scale_max < 1e30f))
+    return fail("lwdetr_flow_create: need 0 < scale_min <= 1 <= scale_max, finite");
+  if (p.max_tracks < 1 || p.max_tracks > lwb::TRACK_MAX) return fail("lwdetr_flow_create: max_tracks must be in [1, 1024]");
+  std::unique_ptr<lwdetr_flow> f(new (std::nothrow) lwdetr_flow{});
+  if (!f) return fail("lwdetr_flow_create: out of memory");
+  lwb::DeviceGuard dg(gmc->state.device);   // the flow's scratch lives beside the estimator's pyramids, which its kernels read
+  lwb::FlowTable& t = f->table;
+  t.p = p;
+  t.num_streams = gmc->table.num_streams;
+  t.g2 = p.grid * p.grid;
+  f->gmc = gmc;
+  const size_t ns = static_cast<size_t>(t.num_streams), nt = ns * static_cast<size_t>(p.max_tracks), np = nt * static_cast<size_t>(t.g2);
+  const auto layout = [&](Carver& c) {
+    c.take(t.ntracks, ns);
+    c.take(t.slot, nt);
+    c.take(t.status, nt);
+    c.take(t.meas, nt * 8);
+    c.take(t.seed, np);
+    c.take(t.fwd, np);
+    c.take(t.bwd, np);
+    c.take(t.fb, np);
+    c.take(t.ncc, np);
+    c.take(t.valid, np);
+  };
+  const auto init = [&] { return cudaMemsetAsync(t.ntracks, 0, ns * sizeof(int32_t), f->state.copy); };
+  if (int rc = f->state.create("lwdetr_flow_create", layout, init)) return rc;
+  *out = f.release();
+  return 0;
+}
+
+void lwdetr_flow_destroy(lwdetr_flow* f) { delete f; }
+
+int lwdetr_track_flow(lwdetr_tracker* t, lwdetr_flow* flow, const double* motion, int B, const int32_t* stream_ids, int max_out,
+                      int32_t* out_ids, float* out_scores, int32_t* out_labels, float* out_boxes, int32_t* out_index, int32_t* counts,
+                      void* stream) {
+  const std::string fn("lwdetr_track_flow");
+  if (!t || !flow || !stream_ids || !out_ids || !out_scores || !out_labels || !out_boxes || !out_index || !counts)
+    return fail(fn + ": null pointer");
+  if (B < 1 || max_out < 1) return fail(fn + ": need B >= 1 and max_out >= 1");
+  if (reinterpret_cast<uintptr_t>(out_boxes) % 16) return fail(fn + ": out_boxes must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(motion) % 8) return fail(fn + ": motion must be 8-byte aligned");
+  std::string err = check_ids(t->table.num_streams, stream_ids, B);
+  if (err.empty()) err = check_ids(flow->table.num_streams, stream_ids, B);
+  if (!err.empty()) return fail(fn + ": " + err);
+  if (flow->state.device != t->state.device) return fail(fn + ": the tracker and the flow live on different devices");
+  lwb::DeviceGuard g(t->state.device);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int e = lwb::flow_launch(flow->table, flow->gmc->table, t->table, B, stream_ids, st);
+  if (!e) e = lwb::track_flow_launch(t->table, t->params, flow->table, motion, t->reid.slot, B, stream_ids, max_out, out_ids, out_scores,
+                                     out_labels, out_boxes, out_index, counts, st);
+  if (!e) e = flow->state.mark(stream);
+  if (!e) e = t->state.mark(stream);
+  if (e) return cuda_fail(e, (fn + " launch").c_str());
+  return 0;
+}
+
+int lwdetr_flow_export(lwdetr_flow* f, int stream_id, int cap, float* seeds, float* fwd, float* bwd, int8_t* valid, double* fb,
+                       double* ncc, int32_t* status, double* meas, int32_t info[3]) {
+  if (!f || !info || (cap > 0 && (!seeds || !fwd || !bwd || !valid || !fb || !ncc || !status || !meas)))
+    return fail("lwdetr_flow_export: null pointer");
+  const lwb::FlowTable& t = f->table;
+  int32_t n = 0;
+  if (int rc = f->state.read_head("lwdetr_flow_export", t.ntracks, t.num_streams, stream_id, &n)) return rc;
+  const int m = std::min(std::min(n, t.p.max_tracks), std::max(cap, 0));
+  const size_t o = static_cast<size_t>(stream_id) * t.p.max_tracks, g2 = static_cast<size_t>(t.g2), k = static_cast<size_t>(m);
+  if (cudaError_t e = f->state.read({{seeds, t.seed + o * g2, k * g2 * sizeof(float2)},
+                                     {fwd, t.fwd + o * g2, k * g2 * sizeof(float2)},
+                                     {bwd, t.bwd + o * g2, k * g2 * sizeof(float2)},
+                                     {valid, t.valid + o * g2, k * g2},
+                                     {fb, t.fb + o * g2, k * g2 * sizeof(double)},
+                                     {ncc, t.ncc + o * g2, k * g2 * sizeof(double)},
+                                     {status, t.status + o, k * sizeof(int32_t)},
+                                     {meas, t.meas + o * 8, k * 8 * sizeof(double)}}))
+    return cuda_fail(e, "lwdetr_flow_export");
+  info[0] = n;
+  info[1] = std::min(n, t.p.max_tracks);
+  info[2] = t.p.grid;
+  return 0;
 }
 
 int lwdetr_query_best(const float* pred_logits, const float* pred_boxes, const float* target_sizes, int B, int nq, int num_classes,

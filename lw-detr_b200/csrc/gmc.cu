@@ -8,9 +8,11 @@
 //   select_kernel   one CTA per stream: the frame's largest response, the cells that pass the quality test, compacted in
 //                   cell order into the buffer's corner list (used at the stream's next frame);
 //   lk_kernel       one warp per corner of the previous frame: calcOpticalFlowPyrLK's iteration from the previous pyramid
-//                   into this one, window sums in exact int64;
+//                   into this one, window sums in exact int64 (lk_point, lk.cuh);
 //   fit_kernel      one CTA per stream: deterministic RANSAC over 2-point similarity hypotheses, float64 least-squares
 //                   refits, the outputs; it then makes the new buffer current.
+// lwdetr_gmc_observe runs grey, pyramid and corners, then commit_kernel makes the new buffer current (no LK, no fit), so
+// the stream's chain of pyramids and corners stays current for the next estimate or for the per-object flow (flow.cu).
 // Everything reads the current buffer from the device header, so a replayed CUDA graph advances the state.
 #include "gmc.h"
 
@@ -19,6 +21,7 @@
 #include <vector>
 
 #include "launch.h"
+#include "lk.cuh"
 
 namespace lwb {
 namespace {
@@ -50,13 +53,6 @@ __device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a,
 __device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
 __device__ __forceinline__ double ddiv(double a, double b) { return __ddiv_rn(a, b); }
 
-// BORDER_REFLECT_101 (cv::borderInterpolate)
-__device__ __forceinline__ int refl(int p, int n) {
-  if (n == 1) return 0;
-  while (static_cast<unsigned>(p) >= static_cast<unsigned>(n)) p = p < 0 ? -p : 2 * n - 2 - p;
-  return p;
-}
-
 __device__ __forceinline__ void level_sizes(const GmcFrame& f, int d, int* lw, int* lh) {
   lw[0] = f.w / d;
   lh[0] = f.h / d;
@@ -64,10 +60,6 @@ __device__ __forceinline__ void level_sizes(const GmcFrame& f, int d, int* lw, i
     lw[l] = (lw[l - 1] + 1) >> 1;
     lh[l] = (lh[l - 1] + 1) >> 1;
   }
-}
-
-__device__ __forceinline__ uint8_t* level_ptr(const GmcTable& t, int sid, int buf, int l) {
-  return t.pyr + (static_cast<long long>(sid) * 2 + buf) * t.slot_bytes + t.off[l];
 }
 
 // ------------------------------------------------------------------------------------------------ grey and pyramid
@@ -256,24 +248,6 @@ __global__ void __launch_bounds__(SEL_NT) select_kernel(const __grid_constant__ 
 }
 
 // ------------------------------------------------------------------------------------------------ Lucas-Kanade
-constexpr int WB = 14;                   // OpenCV's W_BITS
-constexpr int PP = GMC_MAX_WINDOW + 3;   // previous-image patch side (window + 1 for interpolation + 1 each side)
-constexpr int DP = GMC_MAX_WINDOW + 1;   // derivative patch side
-
-struct LkWarp {
-  uint8_t patch[PP * PP];
-  short2 deriv[DP * DP];
-  short iw[GMC_MAX_WINDOW * GMC_MAX_WINDOW];
-  short2 diw[GMC_MAX_WINDOW * GMC_MAX_WINDOW];
-};
-
-__device__ __forceinline__ int descale(int x, int n) { return (x + (1 << (n - 1))) >> n; }
-
-__device__ __forceinline__ long long warp_sum(long long v) {
-  for (int s = 16; s > 0; s >>= 1) v += __shfl_xor_sync(0xffffffffu, v, s);
-  return v;
-}
-
 __global__ void __launch_bounds__(LK_WARPS * 32) lk_kernel(const __grid_constant__ GmcArgs a) {
   pdl_sync();
   __shared__ LkWarp sw[LK_WARPS];
@@ -283,114 +257,12 @@ __global__ void __launch_bounds__(LK_WARPS * 32) lk_kernel(const __grid_constant
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int pi = blockIdx.x * LK_WARPS + wid;
   if (pi >= hd.npts[hd.cur]) return;
-  LkWarp& S = sw[wid];
   const lwdetr_gmc_params& p = a.t.p;
   int lw[GMC_MAX_LEVELS + 1], lh[GMC_MAX_LEVELS + 1];
   level_sizes(f, p.downscale, lw, lh);
-  const int win = p.window, half = (win - 1) / 2, area = win * win;
-  const float eps2 = p.eps * p.eps;
   const float2 p0 = a.t.pts[(static_cast<long long>(f.sid) * 2 + hd.cur) * p.max_points + pi];
-  float2 nxt = p0;
-  bool ok = true;
-  for (int l = f.nlev; l >= 0; --l) {
-    const int W = lw[l], H = lh[l];
-    const uint8_t* I = level_ptr(a.t, f.sid, hd.cur, l);
-    const uint8_t* J = level_ptr(a.t, f.sid, hd.cur ^ 1, l);
-    const float sc = 1.f / static_cast<float>(1 << l);
-    float2 prev = make_float2(p0.x * sc - half, p0.y * sc - half);
-    nxt = l == f.nlev ? make_float2(p0.x * sc, p0.y * sc) : make_float2(nxt.x * 2.f, nxt.y * 2.f);
-    const int ipx = static_cast<int>(floorf(prev.x)), ipy = static_cast<int>(floorf(prev.y));
-    if (ipx < -win || ipx >= W || ipy < -win || ipy >= H) {
-      if (l == 0) ok = false;
-      continue;
-    }
-    float ax = prev.x - ipx, ay = prev.y - ipy;
-    int w00 = __float2int_rn((1.f - ax) * (1.f - ay) * (1 << WB));
-    int w01 = __float2int_rn(ax * (1.f - ay) * (1 << WB));
-    int w10 = __float2int_rn((1.f - ax) * ay * (1 << WB));
-    int w11 = (1 << WB) - w00 - w01 - w10;
-    // previous image around the window (reflected), its Scharr derivatives (0 outside the image), the window interpolated
-    for (int q = lane; q < (win + 3) * (win + 3); q += 32) {
-      const int qy = q / (win + 3), qx = q - qy * (win + 3);
-      S.patch[qy * PP + qx] = I[static_cast<long long>(refl(ipy - 1 + qy, H)) * W + refl(ipx - 1 + qx, W)];
-    }
-    __syncwarp();
-    for (int q = lane; q < (win + 1) * (win + 1); q += 32) {
-      const int qy = q / (win + 1), qx = q - qy * (win + 1);
-      const int y = ipy + qy, x = ipx + qx;
-      short2 dv = make_short2(0, 0);
-      if (y >= 0 && y < H && x >= 0 && x < W) {
-        const uint8_t* c = S.patch + (qy + 1) * PP + (qx + 1);
-        // the patch holds reflected pixels, which is calcSharrDeriv's border.  t0 = 3 (up + down) + 10 mid, t1 = down - up; dx = t0[x+1] - t0[x-1], dy = 3 (t1[x+1] + t1[x-1]) + 10 t1[x]
-        const auto t0 = [&](int o) { return 3 * (c[o - PP] + c[o + PP]) + 10 * c[o]; };
-        const auto t1 = [&](int o) { return c[o + PP] - c[o - PP]; };
-        dv = make_short2(static_cast<short>(t0(1) - t0(-1)), static_cast<short>(3 * (t1(1) + t1(-1)) + 10 * t1(0)));
-      }
-      S.deriv[qy * DP + qx] = dv;
-    }
-    __syncwarp();
-    long long a11 = 0, a12 = 0, a22 = 0;
-    for (int q = lane; q < area; q += 32) {
-      const int qy = q / win, qx = q - qy * win;
-      const uint8_t* s = S.patch + (qy + 1) * PP + (qx + 1);
-      const int ival = descale(s[0] * w00 + s[1] * w01 + s[PP] * w10 + s[PP + 1] * w11, WB - 5);
-      const short2* ds = S.deriv + qy * DP + qx;
-      const int ixv = descale(ds[0].x * w00 + ds[1].x * w01 + ds[DP].x * w10 + ds[DP + 1].x * w11, WB);
-      const int iyv = descale(ds[0].y * w00 + ds[1].y * w01 + ds[DP].y * w10 + ds[DP + 1].y * w11, WB);
-      S.iw[q] = static_cast<short>(ival);
-      S.diw[q] = make_short2(static_cast<short>(ixv), static_cast<short>(iyv));
-      a11 += static_cast<long long>(ixv) * ixv;
-      a12 += static_cast<long long>(ixv) * iyv;
-      a22 += static_cast<long long>(iyv) * iyv;
-    }
-    const float fs = 1.f / static_cast<float>(1 << 20);
-    const float A11 = static_cast<float>(warp_sum(a11)) * fs, A12 = static_cast<float>(warp_sum(a12)) * fs,
-                A22 = static_cast<float>(warp_sum(a22)) * fs;
-    __syncwarp();
-    float D = A11 * A22 - A12 * A12;
-    const float min_eig = (A22 + A11 - sqrtf((A11 - A22) * (A11 - A22) + 4.f * A12 * A12)) / static_cast<float>(2 * area);
-    if (min_eig < p.min_eig || D < 1.1920929e-7f) {
-      if (l == 0) ok = false;
-      continue;
-    }
-    D = 1.f / D;
-    float2 np_ = make_float2(nxt.x - half, nxt.y - half);
-    float2 pd = make_float2(0.f, 0.f);
-    for (int it = 0; it < p.iterations; ++it) {
-      const int inx = static_cast<int>(floorf(np_.x)), iny = static_cast<int>(floorf(np_.y));
-      if (inx < -win || inx >= W || iny < -win || iny >= H) {
-        if (l == 0) ok = false;
-        break;
-      }
-      ax = np_.x - inx;
-      ay = np_.y - iny;
-      w00 = __float2int_rn((1.f - ax) * (1.f - ay) * (1 << WB));
-      w01 = __float2int_rn(ax * (1.f - ay) * (1 << WB));
-      w10 = __float2int_rn((1.f - ax) * ay * (1 << WB));
-      w11 = (1 << WB) - w00 - w01 - w10;
-      long long b1 = 0, b2 = 0;
-      for (int q = lane; q < area; q += 32) {
-        const int qy = q / win, qx = q - qy * win;
-        const long long r0 = static_cast<long long>(refl(iny + qy, H)) * W, r1 = static_cast<long long>(refl(iny + qy + 1, H)) * W;
-        const int c0 = refl(inx + qx, W), c1 = refl(inx + qx + 1, W);
-        const int diff = descale(J[r0 + c0] * w00 + J[r0 + c1] * w01 + J[r1 + c0] * w10 + J[r1 + c1] * w11, WB - 5) - S.iw[q];
-        b1 += static_cast<long long>(diff) * S.diw[q].x;
-        b2 += static_cast<long long>(diff) * S.diw[q].y;
-      }
-      const float B1 = static_cast<float>(warp_sum(b1)) * fs, B2 = static_cast<float>(warp_sum(b2)) * fs;
-      const float2 delta = make_float2((A12 * B2 - A22 * B1) * D, (A12 * B1 - A11 * B2) * D);
-      np_.x += delta.x;
-      np_.y += delta.y;
-      nxt = make_float2(np_.x + half, np_.y + half);
-      if (delta.x * delta.x + delta.y * delta.y <= eps2) break;
-      if (it > 0 && fabsf(delta.x + pd.x) < 0.01f && fabsf(delta.y + pd.y) < 0.01f) {
-        nxt.x -= delta.x * 0.5f;
-        nxt.y -= delta.y * 0.5f;
-        break;
-      }
-      pd = delta;
-    }
-  }
+  float2 nxt;
+  const bool ok = lk_point(sw[wid], a.t, f.sid, hd.cur, hd.cur ^ 1, lw, lh, f.nlev, p0, p.window, p.iterations, p.eps * p.eps, p.min_eig, &nxt);
   if (lane == 0) {
     const long long o = static_cast<long long>(f.sid) * p.max_points + pi;
     a.t.flow[o] = make_float4(p0.x, p0.y, nxt.x, nxt.y);
@@ -565,10 +437,26 @@ __global__ void __launch_bounds__(FIT_NT) fit_kernel(const __grid_constant__ Gmc
     a.status[row] = st;
     a.inliers[row] = ninl;
     hp->cur = hd.cur ^ 1;
+    hp->prev = hd.valid && hd.h == f.h && hd.w == f.w;
     hp->valid = 1;
     hp->h = f.h;
     hp->w = f.w;
   }
+}
+
+// lwdetr_gmc_observe: what fit_kernel does to the header, one thread per stream, with no motion estimated
+__global__ void commit_kernel(const __grid_constant__ GmcArgs a, int nb) {
+  pdl_sync();
+  const int i = threadIdx.x;
+  if (i >= nb) return;
+  const GmcFrame& f = a.f[i];
+  GmcHead* hp = a.t.head + f.sid;
+  const GmcHead hd = *hp;
+  hp->cur = hd.cur ^ 1;
+  hp->prev = hd.valid && hd.h == f.h && hd.w == f.w;
+  hp->valid = 1;
+  hp->h = f.h;
+  hp->w = f.w;
 }
 
 struct ResetArgs {
@@ -579,7 +467,10 @@ struct ResetArgs {
 
 __global__ void reset_kernel(const __grid_constant__ ResetArgs a) {
   pdl_sync();
-  for (int i = threadIdx.x; i < a.n; i += blockDim.x) a.head[a.stream[i]].valid = 0;
+  for (int i = threadIdx.x; i < a.n; i += blockDim.x) {
+    a.head[a.stream[i]].valid = 0;
+    a.head[a.stream[i]].prev = 0;
+  }
 }
 
 }  // namespace
@@ -603,7 +494,7 @@ void gmc_geometry(int h, int w, const lwdetr_gmc_params& p, GmcGeo* g) {
 }
 
 int gmc_estimate_launch(const GmcTable& t, const GmcFrameHost* frames, int B, const int32_t* streams, double* motion, int32_t* status,
-                        int32_t* inliers, cudaStream_t st) {
+                        int32_t* inliers, cudaStream_t st, bool observe) {
   const int fit_smem = static_cast<int>(sizeof(double4)) * t.p.max_points;
   if (int e = ensure_max_dyn_smem(reinterpret_cast<const void*>(fit_kernel), fit_smem)) return e;
   std::vector<GmcArgs> hold(1);          // ~12 KB of parameters: kept off the stack
@@ -636,8 +527,12 @@ int gmc_estimate_launch(const GmcTable& t, const GmcFrameHost* frames, int B, co
     }
     launch_k(cells_kernel, dim3(max_cells, nb), dim3(256), 0, st, a);
     launch_k(select_kernel, dim3(nb), dim3(SEL_NT), 0, st, a);
-    launch_k(lk_kernel, dim3((t.p.max_points + LK_WARPS - 1) / LK_WARPS, nb), dim3(LK_WARPS * 32), 0, st, a);
-    launch_k(fit_kernel, dim3(nb), dim3(FIT_NT), static_cast<size_t>(fit_smem), st, a);
+    if (observe) {
+      launch_k(commit_kernel, dim3(1), dim3(LAUNCH_STREAMS), 0, st, a, nb);
+    } else {
+      launch_k(lk_kernel, dim3((t.p.max_points + LK_WARPS - 1) / LK_WARPS, nb), dim3(LK_WARPS * 32), 0, st, a);
+      launch_k(fit_kernel, dim3(nb), dim3(FIT_NT), static_cast<size_t>(fit_smem), st, a);
+    }
     if (cudaError_t e = cudaGetLastError()) return static_cast<int>(e);
   }
   return 0;

@@ -21,7 +21,8 @@ struct GmcHead {                         // per stream, on the device
   int32_t valid;                         // a last frame exists
   int32_t h, w;                          // its size
   int32_t npts[2];                       // corner count of each buffer
-  int32_t pad0, pad1;
+  int32_t prev;                          // the other buffer holds the frame before the last one, of the same size
+  int32_t pad1;
 };
 
 struct GmcTable {
@@ -52,9 +53,10 @@ struct GmcFrameHost {
   int h, w, nv12;
 };
 
-// streams: HOST, B distinct ids in [0, num_streams) (checked by the caller); frames validated by the caller.
+// streams: HOST, B distinct ids in [0, num_streams) (checked by the caller); frames validated by the caller.  observe:
+// lwdetr_gmc_observe (grey, pyramid and corners only; motion, status and inliers unused).
 int gmc_estimate_launch(const GmcTable& t, const GmcFrameHost* frames, int B, const int32_t* streams, double* motion, int32_t* status,
-                        int32_t* inliers, cudaStream_t st);
+                        int32_t* inliers, cudaStream_t st, bool observe = false);
 int gmc_reset_launch(const GmcTable& t, const int32_t* streams, int n, cudaStream_t st);
 
 }  // namespace lwb

@@ -21,6 +21,7 @@
 // slot through the compaction (a parallel slot array, double-buffered like the records) and a birth takes the lowest free
 // slot, so a frame moves no embedding; only updates and births write D floats.
 #include "track.h"
+#include "flow.h"
 
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -879,6 +880,122 @@ __global__ void __launch_bounds__(NT, 1) track_kernel(const __grid_constant__ Ar
   }
 }
 
+// lwdetr_track_flow: a frame without detections.  Confirmed Tracked tracks take the flow's measurement or go Lost; the rest
+// of the frame (predict, warp, ageing, lists, duplicates, output) is track_kernel's, without associations and births.
+struct FlowTrackArgs {
+  TrackArgs t;
+  const int32_t* fstatus;                // [streams][max_tracks]
+  const double* fmeas;                   // [streams][max_tracks][8]: z at 3..6
+  int max_tracks;
+  int16_t* slot;                         // the appearance slots, or null
+};
+
+__global__ void __launch_bounds__(NT, 1) track_flow_kernel(const __grid_constant__ FlowTrackArgs fa) {
+  pdl_sync();
+  extern __shared__ __align__(16) uint8_t sm_track[];
+  Smem& S = *reinterpret_cast<Smem*>(sm_track);
+  const TrackArgs& a = fa.t;
+  const int tid = threadIdx.x;
+  const int sid = a.stream[blockIdx.x];
+  const long long row = a.row0 + blockIdx.x;
+  TrackHead* hp = a.head + sid;
+  const int frame = hp->frame, nT = hp->n_tracked, nL = hp->n_lost, parity = hp->parity;
+  const int nS = nT + nL, cap = a.capacity;
+  lwdetr_track_record* cur = a.rec + (static_cast<long long>(sid) * 2 + parity) * cap;
+  lwdetr_track_record* nxt = a.rec + (static_cast<long long>(sid) * 2 + (parity ^ 1)) * cap;
+  if (tid == 0) S.n_removed = 0;
+  for (int sl = tid; sl < nS; sl += NT) {
+    lwdetr_track_record& r = cur[sl];
+    const bool lost = sl >= nT, act = r.activated != 0;
+    KState ks;
+    load_state(r, ks);
+    if (lost || act) predict(ks, !lost);
+    if (a.motion) warp_state(ks, a.motion + row * 4);
+    if (lost || act || a.motion) store_state(r, ks);
+    S.tbox[sl] = state_box(ks.p);
+    S.tlab[sl] = r.label;
+    S.tdiff[sl] = r.end_frame - r.start_frame;
+    S.tf[sl] = static_cast<uint8_t>((act ? TF_ACT : 0) | (lost ? TF_LOSTLIST : 0));
+  }
+  __syncthreads();
+  // the flow's track j is the j-th activated record of the tracked list
+  ordered_scan(S, nT, [&](int sl) { return (S.tf[sl] & TF_ACT) != 0; }, [&](int sl, int j) { S.tdet[sl] = static_cast<int16_t>(j); });
+  const long long fo = static_cast<long long>(sid) * fa.max_tracks;
+  for (int sl = tid; sl < nT; sl += NT) {
+    if (!(S.tf[sl] & TF_ACT)) {
+      S.tf[sl] |= TF_MATCHED;            // unconfirmed: carried
+      continue;
+    }
+    const int j = S.tdet[sl];
+    lwdetr_track_record& r = cur[sl];
+    if (j < fa.max_tracks && fa.fstatus[fo + j] == LWDETR_FLOW_OK) {
+      KState ks;
+      load_state(r, ks);
+      double z[4];
+      for (int q = 0; q < 4; ++q) z[q] = fa.fmeas[(fo + j) * 8 + 3 + q];
+      kalman_update(ks, z);
+      store_state(r, ks);
+      r.end_frame = frame;
+      r.index = -1;
+      S.tbox[sl] = state_box(ks.p);
+      S.tdiff[sl] = frame - r.start_frame;
+      S.tf[sl] |= TF_MATCHED;
+    } else {
+      r.state = LWDETR_TRACK_LOST;
+      S.tf[sl] |= TF_NEWLOST;
+    }
+  }
+  for (int sl = nT + tid; sl < nS; sl += NT)
+    if (frame - cur[sl].end_frame > a.max_time_lost) S.tf[sl] |= TF_REMOVED;
+  __syncthreads();
+  const int ntr = ordered_scan(S, nT, [&](int sl) { return (S.tf[sl] & TF_MATCHED) != 0; },
+                               [&](int sl, int r) { S.tlist[r] = static_cast<int16_t>(sl); });
+  const int nD = ordered_scan(S, nL, [&](int q) { return !(S.tf[nT + q] & TF_REMOVED); },
+                              [&](int q, int r) { S.llist[r] = static_cast<int16_t>(nT + q); });
+  const int nE = ordered_scan(S, nT, [&](int sl) { return (S.tf[sl] & TF_NEWLOST) != 0; },
+                              [&](int sl, int r) { S.llist[nD + r] = static_cast<int16_t>(sl); });
+  const int nlo = nD + nE;
+  const double dup = a.dup_thresh;
+  for (int idx = tid; idx < ntr * nlo; idx += NT) {
+    const int i = idx / nlo, j = idx - i * nlo;
+    const int x = S.tlist[i], y = S.llist[j];
+    if (a.class_aware && S.tlab[x] != S.tlab[y]) continue;
+    if (dsub(1.0, iou_d(S.tbox[x], S.tbox[y])) < dup) {
+      if (S.tdiff[x] > S.tdiff[y]) S.tf[y] |= TF_DROP;
+      else S.tf[x] |= TF_DROP;
+    }
+  }
+  __syncthreads();
+  int16_t* slot_cur = fa.slot ? fa.slot + (static_cast<long long>(sid) * 2 + parity) * cap : nullptr;
+  int16_t* slot_nxt = fa.slot ? fa.slot + (static_cast<long long>(sid) * 2 + (parity ^ 1)) * cap : nullptr;
+  const int newT = ordered_scan(S, ntr, [&](int i) { return !(S.tf[S.tlist[i]] & TF_DROP); }, [&](int i, int r) {
+    nxt[r] = cur[S.tlist[i]];
+    if (slot_nxt) slot_nxt[r] = slot_cur[S.tlist[i]];
+  });
+  const int newL = ordered_scan(S, nlo, [&](int j) { return !(S.tf[S.llist[j]] & TF_DROP); }, [&](int j, int r) {
+    nxt[newT + r] = cur[S.llist[j]];
+    if (slot_nxt) slot_nxt[newT + r] = slot_cur[S.llist[j]];
+  });
+  const long long ob = row * a.max_out;
+  const int nout = ordered_scan(S, ntr, [&](int i) {
+    const int x = S.tlist[i];
+    return !(S.tf[x] & TF_DROP) && (S.tf[x] & TF_ACT);
+  }, [&](int i, int r) {
+    if (r >= a.max_out) return;
+    const lwdetr_track_record& t = cur[S.tlist[i]];
+    write_output(a, ob + r, t.id, t.score, t.label, narrow(S.tbox[S.tlist[i]]), -1);
+  });
+  const int cnt = min(nout, a.max_out);
+  for (int r = cnt + tid; r < a.max_out; r += NT) write_output(a, ob + r, 0, 0.f, -1, make_float4(0.f, 0.f, 0.f, 0.f), -1);
+  if (tid == 0) {
+    a.counts[row] = cnt;
+    hp->frame = frame + 1;
+    hp->n_tracked = newT;
+    hp->n_lost = newL;
+    hp->parity = parity ^ 1;
+  }
+}
+
 struct ResetArgs {
   TrackHead* head;
   int n;
@@ -977,6 +1094,42 @@ int track_launch(const TrackTable& t, const lwdetr_track_params& p, const float*
     for (int i = 0; i < nb; ++i) a.stream[i] = streams[b0 + i];
     if (reid) launch_k(track_kernel<ReidArgs>, dim3(nb), dim3(NT), static_cast<size_t>(smem), st, r);
     else launch_k(track_kernel<TrackArgs>, dim3(nb), dim3(NT), static_cast<size_t>(smem), st, a);
+    if (cudaError_t e = cudaGetLastError()) return static_cast<int>(e);
+  }
+  return 0;
+}
+
+int track_flow_launch(const TrackTable& t, const lwdetr_track_params& p, const FlowTable& f, const double* motion, int16_t* slot, int B,
+                      const int32_t* streams, int max_out, int32_t* out_ids, float* out_scores, int32_t* out_labels, float* out_boxes,
+                      int32_t* out_index, int32_t* counts, cudaStream_t st) {
+  const int smem = static_cast<int>(sizeof(Smem));
+  if (int e = ensure_max_dyn_smem(reinterpret_cast<const void*>(track_flow_kernel), smem)) return e;
+  std::vector<FlowTrackArgs> hold(1);
+  FlowTrackArgs& fa = hold[0];
+  TrackArgs& a = fa.t;
+  a.out_ids = out_ids;
+  a.out_scores = out_scores;
+  a.out_labels = out_labels;
+  a.out_boxes = reinterpret_cast<float4*>(out_boxes);
+  a.out_index = out_index;
+  a.counts = counts;
+  a.head = t.head;
+  a.rec = t.rec;
+  a.motion = motion;
+  a.dup_thresh = p.duplicate_thresh;
+  a.max_out = max_out;
+  a.capacity = t.capacity;
+  a.max_time_lost = static_cast<int>(p.frame_rate / 30.0 * p.track_buffer);
+  a.class_aware = p.class_aware;
+  fa.fstatus = f.status;
+  fa.fmeas = f.meas;
+  fa.max_tracks = f.p.max_tracks;
+  fa.slot = slot;
+  for (int b0 = 0; b0 < B; b0 += LAUNCH_STREAMS) {
+    const int nb = B - b0 < LAUNCH_STREAMS ? B - b0 : LAUNCH_STREAMS;
+    a.row0 = b0;
+    for (int i = 0; i < nb; ++i) a.stream[i] = streams[b0 + i];
+    launch_k(track_flow_kernel, dim3(nb), dim3(NT), static_cast<size_t>(smem), st, fa);
     if (cudaError_t e = cudaGetLastError()) return static_cast<int>(e);
   }
   return 0;

@@ -207,7 +207,7 @@ class LWDETR(nn.Module):
     @torch.no_grad()
     def track(self, frames, tracker, streams=None, size=None, fit="stretch", short_side=None, max_side=None, colorspace=None,
               max_out=None, motion=None, appearance=False, reid=None, reid_size=(256, 128), reid_filter="bilinear", reid_mean=None,
-              reid_std=None, reid_normalize=True, zones=None):
+              reid_std=None, reid_normalize=True, zones=None, detect_every=1, flow=None):
         """Multi-object tracking of video streams: frames (RGB or NV12, taken exactly as detect() takes them) run as one
         forward; each query gives one detection, its best class (capi.query_best, boxes in the frame's original pixels);
         then capi.Tracker `tracker` (ByteTrack on the device, include/lwdetr_b200.h) updates each frame's stream.
@@ -236,6 +236,13 @@ class LWDETR(nn.Module):
         [32], present tracks per zone) and "events" (int32 [e, 5] rows (id, kind, index, label, dwell), the frame's first
         Zones.update max_events).  The event counts come back in the read-back of the track counts: no extra
         synchronisation.  With motion= the zones stay fixed in frame pixels: they are image regions, not world regions.
+        detect_every N > 1 runs the detector on every N-th frame of each stream only and tracks the frames between by
+        per-object optical flow (flow: a capi.BoxFlow, required; with motion= it must be the flow's own estimator, the one
+        that holds each stream's chain of pyramids).  A stream's first frame after a tracker reset is a keyframe; after that
+        stream s detects on its t-th frame (t from 0, counted by the tracker) when (t + s) % N == 0, which staggers the
+        streams so that the forward's batch keeps its size from call to call.  Keyframes take the path above; the other
+        frames go MotionEstimator.estimate (with motion=) or observe, then BoxFlow.propagate.  zones= follows both kinds of
+        frame, appearance= and reid= the keyframes only; on a flow frame "queries" is -1.  detect_every=1 is the path above.
         How ByteTrack's thresholds (tuned on YOLOX scores) suit LW-DETR's score distribution, and whether the decoder's features tell identities apart on real footage, in MOTA / IDF1 / HOTA, is
         not measured here."""
         if self.training:
@@ -263,41 +270,73 @@ class LWDETR(nn.Module):
         if appearance is True and tracker.embedding_dim != self.cfg.hidden_dim:
             raise RuntimeError("lwdetr_b200: appearance=True feeds the decoder's %d-wide features, but the tracker's embedding_dim is %s"
                                % (self.cfg.hidden_dim, tracker.embedding_dim))
-        out = self.engine().forward_frames(fb, size=size, fit=fit, short_side=short_side, max_side=max_side, want_aux=False,
-                                           want_hidden=appearance is True)
-        if appearance is True:
-            emb = out["hidden"]
-        sizes = torch.tensor(fb.sizes, dtype=torch.float32, device=dev)
-        scores, labels, boxes = capi.query_best(out["pred_logits"], out["pred_boxes"], sizes)
-        if reid is not None:
-            emb = self._reid_embeddings(fb, scores, boxes, tracker, reid, reid_size, reid_filter, reid_mean, reid_std, reid_normalize)
+        detect_every = int(detect_every)
+        if detect_every < 1:
+            raise RuntimeError("lwdetr_b200: detect_every must be >= 1")
+        if detect_every > 1 and flow is None:
+            raise RuntimeError("lwdetr_b200: detect_every > 1 needs flow= (a capi.BoxFlow)")
+        if flow is not None and motion is not None and motion is not flow.estimator:
+            raise RuntimeError("lwdetr_b200: motion= must be the flow's own estimator (only one estimator can hold a stream's pyramids)")
         rounds, seen = [], {}
+        key = [True] * n
         for i, s in enumerate(streams):
             r = seen.get(s, 0)
             seen[s] = r + 1
             if r == len(rounds):
                 rounds.append([])
             rounds[r].append(i)
+            if detect_every > 1:
+                t = tracker.frames[s] + r
+                key[i] = t == 0 or (t + s) % detect_every == 0
+        krows = [i for i in range(n) if key[i]]
+        pos = {i: p for p, i in enumerate(krows)}        # a keyframe's row in the forward's batch
+        if krows:
+            fk = fb if len(krows) == n else fb.select(krows)
+            out = self.engine().forward_frames(fk, size=size, fit=fit, short_side=short_side, max_side=max_side, want_aux=False,
+                                               want_hidden=appearance is True)
+            if appearance is True:
+                emb = out["hidden"]
+            elif emb is not None and len(krows) < n:
+                emb = emb[torch.tensor(krows, device=emb.device)]
+            sizes = torch.tensor(fk.sizes, dtype=torch.float32, device=dev)
+            scores, labels, boxes = capi.query_best(out["pred_logits"], out["pred_boxes"], sizes)
+            if reid is not None:
+                emb = self._reid_embeddings(fk, scores, boxes, tracker, reid, reid_size, reid_filter, reid_mean, reid_std, reid_normalize)
+        mout = self.num_queries if max_out is None else max_out
         res, counts, ev_counts = [None] * n, [], []
-        for rows in rounds:
-            idx = torch.tensor(rows, device=dev)
-            ids = [streams[i] for i in rows]
-            mo = None if motion is None else motion.estimate(fb.select(rows), ids)[0]
-            em = None
-            if emb is not None:     # consecutive frames (one round, the usual case) as a view: no copy
-                em = emb[rows[0]:rows[-1] + 1] if rows == list(range(rows[0], rows[-1] + 1)) else emb[idx]
-            got = tracker.update(scores[idx], labels[idx], boxes[idx], ids, self.num_queries if max_out is None else max_out, motion=mo,
-                                 embeddings=em)
-            counts.append(got[5])
-            zo = None
-            if zones is not None:
-                inside, occupancy, events, n_ev = zones.update(got[0], got[2], got[3], got[5], ids)
-                zo = (inside.long() & 0xFFFFFFFF, occupancy, events)      # the uint32 masks widened once per round
-                ev_counts.append(n_ev)
-            for j, i in enumerate(rows):
-                res[i] = (got, zo, j)
+        for round_rows in rounds:
+            parts = [[i for i in round_rows if key[i]], [i for i in round_rows if not key[i]]]
+            for kind, rows in enumerate(parts):
+                if not rows:
+                    continue
+                ids = [streams[i] for i in rows]
+                if kind == 0:
+                    kp = [pos[i] for i in rows]
+                    idx = torch.tensor(kp, device=dev)
+                    mo = None
+                    if motion is not None:
+                        mo = motion.estimate(fb.select(rows), ids)[0]
+                    elif flow is not None:
+                        flow.estimator.observe(fb.select(rows), ids)
+                    em = None
+                    if emb is not None:     # consecutive frames (one round, the usual case) as a view: no copy
+                        em = emb[kp[0]:kp[-1] + 1] if kp == list(range(kp[0], kp[-1] + 1)) else emb[idx]
+                    got = tracker.update(scores[idx], labels[idx], boxes[idx], ids, mout, motion=mo, embeddings=em)
+                else:
+                    mo = motion.estimate(fb.select(rows), ids)[0] if motion is not None else None
+                    if mo is None:
+                        flow.estimator.observe(fb.select(rows), ids)
+                    got = flow.propagate(tracker, ids, motion=mo, max_out=mout)
+                counts.append(got[5])
+                zo = None
+                if zones is not None:
+                    inside, occupancy, events, n_ev = zones.update(got[0], got[2], got[3], got[5], ids)
+                    zo = (inside.long() & 0xFFFFFFFF, occupancy, events)      # the uint32 masks widened once per round
+                    ev_counts.append(n_ev)
+                for j, i in enumerate(rows):
+                    res[i] = (got, zo, j)
         both = torch.cat(counts + ev_counts).cpu().tolist()     # track and event counts in one read-back
-        order = [i for rows in rounds for i in rows]
+        order = [i for rows in rounds for part in ([i for i in rows if key[i]], [i for i in rows if not key[i]]) for i in part]
         cnt = {i: c for i, c in zip(order, both[:n])}
         ecnt = {i: c for i, c in zip(order, both[n:])}
         dets = []

@@ -482,6 +482,45 @@ class Stream:
         self.frame += 1
         return [(t.id, np.float32(t.score), int(t.label), t.box().astype(np.float32), t.index) for t in tracked if t.activated]
 
+    def update_flow(self, measurements, motion=None):
+        """One flow frame (lwdetr_track_flow): measurements[j] = (status, z) for the j-th activated track of the tracked
+        list, z the float64 xyah measurement (flow_spec.measure); a track past the list given is SKIPPED.  Status 0 (OK)
+        updates the track (score and label kept, index -1, end = frame); any other makes it Lost.  Unconfirmed tracks are
+        carried; no births.  Returns the output tracks as update() does."""
+        p, frame = self.p, self.frame
+        conf = [t for t in self.tracked if t.activated]
+        for t in conf + self.lost:
+            predict(t)
+        if motion is not None:
+            for t in self.tracked + self.lost:
+                warp(t, motion)
+        new_lost = []
+        for j, t in enumerate(conf):
+            st, z = measurements[j] if j < len(measurements) else (5, None)
+            if st == 0:
+                kalman_update(t, np.asarray(z, np.float64))
+                t.end, t.index = frame, -1
+            else:
+                t.state = LOST
+                new_lost.append(t)
+        tracked = [t for t in self.tracked if t.state == TRACKED]
+        lost = [t for t in self.lost if not frame - t.end > p["max_time_lost"]] + new_lost
+        if tracked and lost:
+            dup = (1.0 - iou(np.array([t.box() for t in tracked]), np.array([t.box() for t in lost]))) < np.float64(p["duplicate_thresh"])
+            if p["class_aware"]:
+                dup &= np.array([t.label for t in tracked])[:, None] == np.array([t.label for t in lost])[None, :]
+            da, db = set(), set()
+            for a, b in zip(*np.nonzero(dup)):
+                if tracked[a].end - tracked[a].start > lost[b].end - lost[b].start:
+                    db.add(b)
+                else:
+                    da.add(a)
+            tracked = [t for i, t in enumerate(tracked) if i not in da]
+            lost = [t for i, t in enumerate(lost) if i not in db]
+        self.tracked, self.lost = tracked, lost
+        self.frame += 1
+        return [(t.id, np.float32(t.score), int(t.label), t.box().astype(np.float32), -1) for t in tracked if t.activated]
+
     def export(self):
         """Every record in list order (tracked, then lost) as dicts with the float64 state."""
         return [dict(id=t.id, state=t.state, activated=int(t.activated), start=t.start, end=t.end, score=np.float32(t.score),
