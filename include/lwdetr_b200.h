@@ -768,7 +768,9 @@ LWDETR_API int lwdetr_load_weights(lwdetr_handle* h, int n, const char* const* n
 
 /* images: DEVICE [B, 3, S, S], fp32 (images_fp32 = 1) or the compute dtype; outputs: DEVICE fp32
  * pred_logits [B, nq, num_classes], pred_boxes [B, nq, 4]; aux may be NULL.  topk_override: DEVICE
- * int32 [B, nq] or NULL - test hook that forces the two-stage selection (SURVEY.md 8c tier T2). */
+ * int32 [B, nq] or NULL - test hook that forces the two-stage selection (SURVEY.md 8c tier T2).  Every index must lie in
+ * [0, S), S the memory length of this input size; the C entry points do not check that (b200.capi.Engine does, before
+ * the call), and an index outside it makes the forward read outside its buffers. */
 LWDETR_API int lwdetr_forward(lwdetr_handle* h, const void* images, int images_fp32, int B, float* pred_logits,
                               float* pred_boxes, const lwdetr_aux_out* aux, const int32_t* topk_override,
                               void* stream);
@@ -945,7 +947,14 @@ LWDETR_API int64_t lwdetr_weight_arena_bytes(lwdetr_handle* h);
 LWDETR_API int lwdetr_set_option(lwdetr_handle* h, const char* name, int value);
 
 /* Debug captures (tests): after the op labelled `label` runs in the next forward, its output is copied to
- * the HOST buffer dst as fp32 (row-major, dense).  lwdetr_capture_result returns the element count. */
+ * the HOST buffer dst as fp32 (row-major, dense).  lwdetr_capture_result returns the element count (-1: no such output,
+ * -2: larger than capacity).  Ops that write more than one buffer expose the others as "<label>.<name>":
+ *   mask_setup              proposals [B*S, 4];  mask_setup.invalid, mask_setup.pad [B*S] (0 / 1);  mask_setup.valid_ratio [B*L, 2] (w, h)
+ *   topk                    the selected memory rows [B*nq] (int32, exact in fp32)
+ *   gather_topk             the selected encoder rows [B*nq, hidden_dim];  gather_topk.enc_logits [B*nq, num_classes]
+ *   query_init              the decoder reference boxes [B*nq, 4];  query_init.box_ts [B*nq, 4] (enc_outputs boxes);
+ *                           query_init.sine [B*nq, 2*hidden_dim] (the sine embedding of the reference, compute dtype)
+ * Captures run the forward eagerly and synchronise after every captured op; without any, nothing of this is done. */
 LWDETR_API int lwdetr_add_capture(lwdetr_handle* h, const char* label, float* dst, int64_t capacity);
 LWDETR_API int64_t lwdetr_capture_result(lwdetr_handle* h, int index);
 LWDETR_API void lwdetr_clear_captures(lwdetr_handle* h);

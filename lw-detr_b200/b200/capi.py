@@ -1347,6 +1347,28 @@ def config_struct(cfg):
     return c
 
 
+def check_topk_override(ov, B, nq, S, device):
+    """The forced two-stage selection of one forward, checked: an integer tensor [B, nq] on the host or on the engine's
+    `device` (not on any other device) whose every index lies in [0, S), S the memory length of the input size.  The engine
+    gathers the encoder rows, class logits and proposals at these indices without a check of its own.  Returns it as
+    contiguous int32 on `device` (a host tensor is copied there); RuntimeError naming the limit otherwise.  Costs one
+    read-back of the minimum and maximum."""
+    import torch
+    if tuple(ov.shape) != (B, nq):
+        raise RuntimeError("lwdetr_b200: topk_override must be [B, num_queries] = [%d, %d], got %s" % (B, nq, tuple(ov.shape)))
+    if ov.dtype.is_floating_point or ov.dtype.is_complex or ov.dtype == torch.bool:
+        raise RuntimeError("lwdetr_b200: topk_override must be an integer tensor, got %s" % (ov.dtype,))
+    device = torch.device(device)
+    if ov.device != device and ov.device.type != "cpu":
+        raise RuntimeError("lwdetr_b200: topk_override is on %s but the engine lives on %s (pass it there or on the host)"
+                           % (ov.device, device))
+    lo, hi = torch.stack(torch.aminmax(ov.reshape(-1).long())).tolist()
+    if lo < 0 or hi >= S:
+        raise RuntimeError("lwdetr_b200: topk_override indices must lie in [0, %d) (the memory length of this input size), got "
+                           "[%d, %d]" % (S, lo, hi))
+    return ov.to(device=device, dtype=torch.int32).contiguous()
+
+
 class Engine:
     """Owns one lwdetr_handle: packed weights + kernel schedule on the current CUDA device."""
 
@@ -1440,7 +1462,7 @@ class Engine:
         res, logits, boxes, aux = self._outputs(B, dev, want_aux)
         ov = None
         if topk_override is not None:
-            ov = topk_override.to(device=dev, dtype=torch.int32).contiguous()
+            ov = check_topk_override(topk_override, B, self.cfg.num_queries, self.cfg.memory_len_at(H, W), self.device)
         check(lib().lwdetr_forward_hw(self._h, ctypes.byref(desc), B, H, W, ptr(logits), ptr(boxes),
                                       ctypes.byref(aux) if aux is not None else None, ptr(ov), stream_ptr(self.device)), "lwdetr_forward_hw")
         self._last_inputs = (images, ov, mk)    # keep alive until the stream has consumed them
@@ -1500,8 +1522,8 @@ class Engine:
         res, logits, boxes, aux = self._outputs(B, self.device, want_aux)
         ov = None
         if topk_override is not None:
-            ov = topk_override.to(device=self.device, dtype=torch.int32).contiguous()
-        name = "lwdetr_forward_frames_nv12" if fb.nv12 else "lwdetr_forward_frames"
+            ov = check_topk_override(topk_override, B, self.cfg.num_queries, self.cfg.memory_len_at(H, W), self.device)
+        name ="lwdetr_forward_frames_nv12" if fb.nv12 else "lwdetr_forward_frames"
         check(getattr(lib(), name)(self._h, fb.descs(dsts), ctypes.cast(_norm3(mean), _vp), ctypes.cast(_norm3(std), _vp), B, H, W,
                                    ptr(logits), ptr(boxes), ctypes.byref(aux) if aux is not None else None, ptr(ov),
                                    stream_ptr(self.device)), name)

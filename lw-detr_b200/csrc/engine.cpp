@@ -31,13 +31,6 @@ struct Mat {
 inline char* cptr(void* p) { return static_cast<char*>(p); }
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-// What a debug capture of an op copies back: rows x cols of a [*, ld] matrix, fp32 or in the compute dtype.
-struct OutView {
-  const void* p;
-  long long rows;
-  int cols, ld, fp32;
-};
-
 // One pass of Engine::plan.  Pass 0 sizes the workspace: allocations only advance the bump offset (and return null),
 // weight lookups return null and nothing is recorded.  Pass 1 lays the same allocations out from the arena base, resolves
 // the packed weights and records the ops.  The first error is kept.
@@ -69,9 +62,14 @@ class OpBuilder {
     if (pass_ == 0 || failed_) return;
     Op op;
     op.label = label; op.run = std::move(run);
-    op.out = out.p; op.rows = out.rows; op.cols = out.cols; op.ld = out.ld; op.fp32 = out.fp32;
+    op.out = out;
     op.flops = flops; op.bytes = bytes; op.reads_input = reads_input;
     ops_->push_back(std::move(op));
+  }
+  // a further output of the op recorded last, captured as "<label>.<name>"
+  void also(const std::string& name, const OutView& v) {
+    if (pass_ == 0 || failed_) return;
+    ops_->back().extra.emplace_back(name, v);
   }
   void op(const std::string& label, std::function<int(cudaStream_t)> run, const OutView& out, double bytes, bool reads_input = false) {
     record(label, std::move(run), out, 0.0, bytes, reads_input);
@@ -638,7 +636,10 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
           }
         }
         return mask_setup_launch(mask, B, IH, IW, L, S, lh, lw, ls, prop_b, invalid_b, pad_b, vr_b, st);
-      }, {prop_b, BS, 4, 4, 1}, 24.0 * BS, /*reads_input=*/true);
+      }, {prop_b, BS, 4, 4, EL_F32}, 24.0 * BS, /*reads_input=*/true);
+      b.also("invalid", {invalid_b, BS, 1, 1, EL_U8});
+      b.also("pad", {pad_b, BS, 1, 1, EL_U8});
+      b.also("valid_ratio", {vr_b, 1LL * B * L, 2, 2, EL_F32});
     }
     // ================================================================ ViT encoder
     Mat a0 = b.buf16(BT, 768);
@@ -796,12 +797,13 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
       if (in_topk_override_ != nullptr)
         return static_cast<int>(cudaMemcpyAsync(topk_idx, in_topk_override_, static_cast<size_t>(B) * nq * 4, cudaMemcpyDeviceToDevice, st));
       return topk_launch(score, B, S, nq, topk_idx, st);
-    }, {nullptr, 0, 0, 0, 0}, 4.0 * BS);
+    }, {topk_idx, BQ, 1, 1, EL_I32}, 4.0 * BS);
     {
       void* omp = omn.p; void* selp = sel.p;
       b.op("gather_topk", [omp, d, cls_all, ncls, ldc, topk_idx, B, S, nq, selp, enc_logits, dt](cudaStream_t st) {
         return gather_topk_launch(dt, omp, d, cls_all, ldc, ncls, topk_idx, B, S, nq, d, selp, enc_logits, st);
-      }, {sel.p, BQ, d, d, 0}, 4.0 * BQ * d);
+      }, {sel.p, BQ, d, d, EL_16}, 4.0 * BQ * d);
+      b.also("enc_logits", {enc_logits, BQ, ncls, ncls, EL_F32});
     }
     b.gemm("enc_box0", act(ACT_RELU), sel, BQ, d, "enc_box0", d, h1);
     b.gemm("enc_box1", act(ACT_RELU), h1, BQ, d, "enc_box1", d, h2);
@@ -811,7 +813,9 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
       void* sp = sine.p;
       b.op("query_init", [delta_ts, prop_b, topk_idx, rpe, B, nq, d, enc_boxes, refpoint, sp, dt, S, L, vr_b](cudaStream_t st) {
         return query_init_launch(dt, delta_ts, prop_b, topk_idx, rpe, B, nq, d, enc_boxes, refpoint, sp, S, L, vr_b, st);
-      }, {refpoint, BQ, 4, 4, 1}, 4.0 * BQ * d);
+      }, {refpoint, BQ, 4, 4, EL_F32}, 4.0 * BQ * d);
+      b.also("box_ts", {enc_boxes, BQ, 4, 4, EL_F32});
+      b.also("sine", {sine.p, BQ, 2 * d, 2 * d, EL_16});
     }
     b.gemm("ref_point_head0", act(ACT_RELU), sine, BQ, 2 * d, "rph0", d, h1);
     b.gemm("query_pos", GemmDesc{}, h1, BQ, d, "rph1", d, qpos);
@@ -888,19 +892,32 @@ int Engine::plan(int B, int IH, int IW, std::string* err) {
   return 0;
 }
 
+int Engine::copy_view(const OutView& v, Capture* c) {
+  const long long n = v.rows * v.cols;
+  if (n > c->capacity) { c->written = -2; return 0; }
+  const size_t esz = v.kind == EL_U8 ? 1 : (v.kind == EL_16 ? 2 : 4);
+  std::vector<uint8_t> raw(static_cast<size_t>(n) * esz);
+  if (cudaMemcpy2D(raw.data(), v.cols * esz, v.p, static_cast<size_t>(v.ld) * esz, v.cols * esz, static_cast<size_t>(v.rows), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
+  float* dst = c->dst;
+  if (v.kind == EL_F32) std::memcpy(dst, raw.data(), raw.size());
+  else if (v.kind == EL_I32) for (long long i = 0; i < n; ++i) { int32_t x; std::memcpy(&x, &raw[i * 4], 4); dst[i] = static_cast<float>(x); }
+  else if (v.kind == EL_U8) for (long long i = 0; i < n; ++i) dst[i] = static_cast<float>(raw[i]);
+  else if (dtype_ == DT_BF16) for (long long i = 0; i < n; ++i) { __nv_bfloat16 x; std::memcpy(&x, &raw[i * 2], 2); dst[i] = __bfloat162float(x); }
+  else for (long long i = 0; i < n; ++i) { __half x; std::memcpy(&x, &raw[i * 2], 2); dst[i] = __half2float(x); }
+  c->written = n;
+  return 0;
+}
+
 int Engine::do_capture(const Op& op, cudaStream_t st) {
+  bool synced = false;
   for (auto& c : captures_) {
-    if (c.label != op.label || op.out == nullptr) continue;
-    if (cudaStreamSynchronize(st) != cudaSuccess) return -1;
-    const long long n = op.rows * op.cols;
-    if (n > c.capacity) { c.written = -2; continue; }
-    const size_t esz = op.fp32 ? 4 : 2;
-    std::vector<uint8_t> raw(static_cast<size_t>(n) * esz);
-    if (cudaMemcpy2D(raw.data(), op.cols * esz, op.out, static_cast<size_t>(op.ld) * esz, op.cols * esz, static_cast<size_t>(op.rows), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
-    if (op.fp32) std::memcpy(c.dst, raw.data(), raw.size());
-    else if (dtype_ == DT_BF16) for (long long i = 0; i < n; ++i) { __nv_bfloat16 v; std::memcpy(&v, &raw[i * 2], 2); c.dst[i] = __bfloat162float(v); }
-    else for (long long i = 0; i < n; ++i) { __half v; std::memcpy(&v, &raw[i * 2], 2); c.dst[i] = __half2float(v); }
-    c.written = n;
+    const OutView* v = c.label == op.label ? &op.out : nullptr;
+    for (const auto& e : op.extra)
+      if (!v && c.label == op.label + "." + e.first) v = &e.second;
+    if (!v || v->p == nullptr) continue;
+    if (!synced && cudaStreamSynchronize(st) != cudaSuccess) return -1;
+    synced = true;
+    if (copy_view(*v, &c)) return -1;
   }
   return 0;
 }

@@ -26,13 +26,21 @@ struct Capture {
   long long written;    // rows*cols actually written (or -1 if label not found)
 };
 
+// Element kinds of a captured view; do_capture converts each to fp32 on the host (exact for uint8 and for int32 below 2^24).
+enum : int { EL_16 = 0, EL_F32 = 1, EL_I32 = 2, EL_U8 = 3 };
+// What a debug capture of an op copies back: rows x cols of a [*, ld] matrix of `kind` elements (EL_16: the compute dtype).
+struct OutView {
+  const void* p = nullptr;
+  long long rows = 0;
+  int cols = 0, ld = 0, kind = EL_16;
+};
+
 struct Op {
   std::string label;
   std::function<int(cudaStream_t)> run;
-  // output description for debug captures
-  const void* out = nullptr;
-  long long rows = 0;
-  int cols = 0, ld = 0, fp32 = 0;
+  // outputs for debug captures: the primary one under `label`, any further ones under "<label>.<name>"
+  OutView out;
+  std::vector<std::pair<std::string, OutView>> extra;
   double flops = 0, bytes = 0;
   bool reads_input = false;   // consumes caller-owned pointers (images, mask): launched eagerly, never captured in the graph
 };
@@ -125,6 +133,7 @@ class Engine {
   float* upload32(const std::vector<float>& v);
   void* upload8(const std::vector<uint8_t>& v);
   int do_capture(const Op& op, cudaStream_t st);
+  int copy_view(const OutView& v, Capture* c);
 
   lwdetr_config cfg_;
   int dtype_;

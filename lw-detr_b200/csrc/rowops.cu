@@ -757,8 +757,10 @@ __global__ void __launch_bounds__(256) query_init_kernel(const float* __restrict
     const int coord_slot = i / dim;             // output order (y, x, w, h)
     const int e = i % dim;
     const float c = rp[coord_slot == 0 ? 1 : (coord_slot == 1 ? 0 : coord_slot)];
-    // 1 / dim_t = 10000^(-2*(e/2)/dim) by exp2 (13.2877 = log2 1e4); |v| <= 2*pi*1.2: the fast sin/cos are exact to ~1e-6 there,
-    // far below the 16-bit rounding of the embedding
+    // 1 / dim_t = 10000^(-2*(e/2)/dim) by exp2 (13.2877 = log2 1e4).  |v| is not bounded: the reference's width is
+    // exp(refpoint_embed) times the encoder box's, so |v| = 2*pi*|rp| can reach hundreds.  The fast sin/cos stay within
+    // 2^-21.41 plus the argument's own fp32 error there: tests/test_query_select_gpu.py holds every element of the embedding
+    // to that plus half a 16-bit ulp for |v| up to ~560, and the 16-bit rounding dominates
     const float inv_dim_t = exp2f(-13.287712379549449f * static_cast<float>(2 * (e / 2)) / static_cast<float>(dim));
     const float v = c * two_pi * inv_dim_t;
     sine[row * (2 * d) + i] = Cvt<T>::from_f((e & 1) ? __cosf(v) : __sinf(v));
