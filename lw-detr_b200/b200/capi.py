@@ -1,10 +1,13 @@
 """ctypes binding of include/lwdetr_b200.h.
 
-The shared library is built in-tree by tools/build.py (``__graft_entry__.build()``).  There is no
-fallback: if the library is missing or a call fails, a RuntimeError is raised.
+Every function signature and struct layout is read from the header when this module loads, so the header is the only
+description of the ABI; a form the reader does not know is an error.  The shared library is built in-tree by
+tools/build.py (``__graft_entry__.build()``).  There is no fallback: if the header or the library is missing or a call
+fails, a RuntimeError is raised.
 """
 import ctypes
 import os
+import re
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), "lib", "liblwdetr_b200.so")
@@ -14,91 +17,61 @@ ACT_NONE, ACT_RELU, ACT_GELU, ACT_SILU = 0, 1, 2, 3
 
 _lib = None
 
-_vp, _i, _f, _i64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_int64
+_vp = ctypes.c_void_p
+HEADER_PATH = os.path.join(os.path.dirname(os.path.dirname(_HERE)), "include", "lwdetr_b200.h")
+_SCALARS = {"int": ctypes.c_int, "int8_t": ctypes.c_int8, "int16_t": ctypes.c_int16, "int32_t": ctypes.c_int32,
+            "int64_t": ctypes.c_int64, "uint8_t": ctypes.c_uint8, "uint32_t": ctypes.c_uint32, "float": ctypes.c_float,
+            "double": ctypes.c_double}
 
-_SIGNATURES = {
-    "lwdetr_last_error": (ctypes.c_char_p, []),
-    "lwdetr_abi_version": (_i, []),
-    "lwdetr_gemm": (_i, [_i, _vp, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
-    "lwdetr_gemm_ex": (_i, [_vp, _vp]),
-    "lwdetr_conv3x3": (_i, [_i, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp]),
-    "lwdetr_layernorm": (_i, [_i, _vp, _i, _vp, _i, _vp, _vp, _f, _i64, _i, _vp]),
-    "lwdetr_layernorm_ex": (_i, [_i, _vp, _vp]),
-    "lwdetr_attention": (_i, [_i, _vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _i, _f, _vp]),
-    "lwdetr_attention_ex": (_i, [_vp, _vp]),
-    "lwdetr_ms_deform_attn_forward": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
-    "lwdetr_ms_deform_attn_backward": (_i, [_vp] * 9 + [_i] * 8 + [_vp]),
-    "lwdetr_msda_forward": (_i, [_i, _vp, _i64, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
-    "lwdetr_msda_plan": (_i, [_i, _vp, _vp, _i, _vp, _vp]),
-    "lwdetr_conv3x3_plan": (_i, [_i, _i, _vp, _vp]),
-    "lwdetr_topk": (_i, [_vp, _i, _i, _i, _vp, _vp]),
-    "lwdetr_postprocess": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
-    "lwdetr_tile_merge": (_i, [_vp, _vp, _vp, _i, _i, _vp, _i, _f, _f, _i, _i, _vp, _vp, _vp, _vp, _vp]),
-    "lwdetr_track_params_default": (None, [_vp]),
-    "lwdetr_tracker_create": (_i, [_i, _vp, _vp]),
-    "lwdetr_tracker_destroy": (None, [_vp]),
-    "lwdetr_tracker_reset": (_i, [_vp, _vp, _i, _vp]),
-    "lwdetr_track": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "lwdetr_tracker_export": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
-    "lwdetr_track_ex": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "lwdetr_reid_params_default": (None, [_vp]),
-    "lwdetr_tracker_create_reid": (_i, [_i, _vp, _vp, _vp]),
-    "lwdetr_track_reid": (_i, [_vp] * 6 + [_i] * 4 + [_vp, _i] + [_vp] * 7),
-    "lwdetr_tracker_export_embeddings": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
-    "lwdetr_last_hidden": (_i, [_vp, _vp, _i, _vp]),
-    "lwdetr_gmc_params_default": (None, [_vp]),
-    "lwdetr_gmc_create": (_i, [_i, _vp, _vp]),
-    "lwdetr_gmc_destroy": (None, [_vp]),
-    "lwdetr_gmc_reset": (_i, [_vp, _vp, _i, _vp]),
-    "lwdetr_gmc_export": (_i, [_vp, _i, _vp, _i64, _vp, _vp, _vp, _vp]),
-    "lwdetr_gmc_estimate": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
-    "lwdetr_gmc_estimate_nv12": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
-    "lwdetr_gmc_observe": (_i, [_vp, _vp, _i, _vp, _vp]),
-    "lwdetr_gmc_observe_nv12": (_i, [_vp, _vp, _i, _vp, _vp]),
-    "lwdetr_flow_params_default": (None, [_vp]),
-    "lwdetr_flow_create": (_i, [_vp, _vp, _vp]),
-    "lwdetr_flow_destroy": (None, [_vp]),
-    "lwdetr_track_flow": (_i, [_vp, _vp, _vp, _i, _vp, _i] + [_vp] * 7),
-    "lwdetr_flow_export": (_i, [_vp, _i, _i] + [_vp] * 9),
-    "lwdetr_zones_params_default": (None, [_vp]),
-    "lwdetr_zones_create": (_i, [_i, _vp, _vp]),
-    "lwdetr_zones_destroy": (None, [_vp]),
-    "lwdetr_zones_set": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp]),
-    "lwdetr_zones_reset": (_i, [_vp, _vp, _i, _vp]),
-    "lwdetr_zones_update": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp]),
-    "lwdetr_zones_export": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _i]),
-    "lwdetr_query_best": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    "lwdetr_crops": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
-    "lwdetr_crops_nv12": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
-    "lwdetr_crop_select": (_i, [_vp, _vp, _i, _i, _vp, _f, _vp, _vp, _vp, _vp, _vp]),
-    "lwdetr_scatter_rows": (_i, [_i, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp]),
-    "lwdetr_layernorm_e4m3": (_i, [_vp, _i, _i64, _i, _f, _vp, _i, _vp, _vp]),
-    "lwdetr_gemm_e4m3": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _i, _vp]),
-    "lwdetr_vit_mlp": (_i, [_i, _vp, _i, _i, _vp, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp]),
-    "lwdetr_host_quant_e4m3_rows": (_i, [_vp, _i64, _i, _vp, _vp]),
-    "lwdetr_host_bicubic": (_i, [_vp, _i, _i, _i, _vp]),
-    "lwdetr_host_bicubic_hw": (_i, [_vp, _i, _i, _i, _i, _vp]),
-    "lwdetr_create": (_i, [_vp, _i, _vp]),
-    "lwdetr_destroy": (None, [_vp]),
-    "lwdetr_load_weights": (_i, [_vp, _i, _vp, _vp, _vp]),
-    "lwdetr_forward": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
-    "lwdetr_broadcast_weights": (_i, [_vp, _vp, _i, _vp]),
-    "lwdetr_weight_arena_bytes": (_i64, [_vp]),
-    "lwdetr_forward_ex": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
-    "lwdetr_forward_hw": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
-    "lwdetr_forward_frames": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
-    "lwdetr_resize_patches": (_i, [_i, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
-    "lwdetr_forward_frames_nv12": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
-    "lwdetr_resize_patches_nv12": (_i, [_i, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
-    "lwdetr_set_option": (_i, [_vp, ctypes.c_char_p, _i]),
-    "lwdetr_add_capture": (_i, [_vp, ctypes.c_char_p, _vp, _i64]),
-    "lwdetr_capture_result": (_i64, [_vp, _i]),
-    "lwdetr_clear_captures": (None, [_vp]),
-    "lwdetr_num_ops": (_i, [_vp]),
-    "lwdetr_op_label": (ctypes.c_char_p, [_vp, _i]),
-    "lwdetr_op_cost": (_i, [_vp, _i, _vp, _vp]),
-    "lwdetr_profile_ops": (_i, [_vp, _i, _vp, _vp]),
-}
+
+def _unreadable(decl, where):
+    raise RuntimeError("lwdetr_b200: cannot read `%s` (%s) in include/lwdetr_b200.h" % (" ".join(decl.split()), where))
+
+
+def _ctype(decl, where, field=False):
+    """(name, ctypes type) of one declaration of the header: a parameter, a return type (no name) or a struct field.
+    Pointers and array parameters are c_void_p, except a lone char* (a C string); a field array is a ctypes array."""
+    m = re.fullmatch(r"\s*(?:const\s+)?(\w+)\s*((?:\*\s*(?:const\b\s*)?)*)(\w*)\s*(?:\[(\d+)\])?\s*", decl)
+    if m and not (m.group(2) and m.group(4)):
+        base, stars, name, n = m.group(1), m.group(2).count("*"), m.group(3), m.group(4)
+        if stars or (n and not field):
+            return name, ctypes.c_char_p if (base, stars) == ("char", 1) else _vp
+        if base in _SCALARS:
+            return name, _SCALARS[base] * int(n) if n else _SCALARS[base]
+        if base == "void" and not name and not field:
+            return name, None
+    _unreadable(decl, where)
+
+
+def _read_header(path):
+    """The C ABI as the header declares it: ({function: (restype, argtypes)}, {struct typedef name: ctypes.Structure}).
+    It reads the header's own forms only: `LWDETR_API <ret> lwdetr_x(<args>);` and `typedef struct { ... } lwdetr_y;` of
+    scalars, pointers and fixed arrays (and opaque `typedef struct x x;` handles); anything else there is an error."""
+    if not os.path.exists(path):
+        raise RuntimeError("lwdetr_b200: %s not found - the C ABI is read from it (there is no copy of it in Python)" % path)
+    with open(path) as f:
+        src = re.sub(r"^\s*#.*$", " ", re.sub(r"/\*.*?\*/", " ", f.read(), flags=re.S), flags=re.M)
+    structs = {}
+    for decl in re.findall(r"\btypedef\b[^;{]*(?:\{[^}]*\})?[^;]*;", src):
+        m = re.fullmatch(r"typedef\s+struct\s*\{([^}]*)\}\s*(\w+)\s*;", decl)
+        if m is None:
+            if not re.fullmatch(r"typedef\s+struct\s+(\w+)\s+\1\s*;", decl):
+                _unreadable(decl, "typedef")
+            continue
+        fields = []
+        for stmt in filter(str.strip, m.group(1).split(";")):
+            t = re.match(r"\s*(?:const\s+)?\w+", stmt) or _unreadable(stmt, m.group(2))
+            fields += [_ctype(t.group(0) + " " + d, m.group(2), True) for d in stmt[t.end():].split(",")]
+        structs[m.group(2)] = type(m.group(2), (ctypes.Structure,), {"_fields_": fields})
+    sigs = {}
+    for decl in re.findall(r"\bLWDETR_API\b[^;]*;", src):
+        m = re.fullmatch(r"LWDETR_API\s+([^;(]*?)\s*\b(lwdetr_\w+)\s*\(([^()]*)\)\s*;", decl) or _unreadable(decl, "prototype")
+        args = [] if m.group(3).strip() == "void" else [_ctype(a, m.group(2))[1] for a in m.group(3).split(",")]
+        sigs[m.group(2)] = (_ctype(m.group(1), m.group(2))[1], args)
+    return sigs, structs
+
+
+_SIGNATURES, _STRUCTS = _read_header(HEADER_PATH)
 
 
 def lib():
@@ -185,14 +158,7 @@ def gemm(A, W, out, bias=None, gamma=None, resid=None, resid_mod=0, act=ACT_NONE
 EP_NAMES = {0: "EP_GENERIC", 1: "EP_BIAS", 2: "EP_BIAS_ACT", 3: "EP_LN", 4: "EP_LN_GELU", 5: "EP_RESID"}
 
 
-class GemmArgs(ctypes.Structure):
-    """lwdetr_gemm_args (include/lwdetr_b200.h)."""
-    _fields_ = [("dtype", _i), ("A", _vp), ("lda", _i), ("M", _i), ("K", _i), ("W", _vp), ("N", _i), ("bias", _vp), ("gamma", _vp),
-                ("resid", _vp), ("ld_resid", _i), ("resid_mod", _i), ("act", _i), ("out", _vp), ("ld_out", _i), ("out_fp32", _i),
-                ("rows_in", _i), ("remap_rows", _i), ("shuffle_cout", _i), ("IH", _i), ("IW", _i),
-                ("stats_in", _vp), ("stats_parts_in", _i), ("colsum", _vp), ("ln_C", _i), ("ln_eps", _f), ("stats_out", _vp),
-                ("hm_S", _i), ("hm_heads", _i), ("hm_slices", _i), ("row_zero", _vp), ("dry_run", _i),
-                ("bn", _i), ("epilogue", _i), ("stats_parts_out", _i)]
+GemmArgs = _STRUCTS["lwdetr_gemm_args"]
 
 
 def gemm_ex(A, W, out, bias=None, gamma=None, resid=None, resid_mod=0, act=ACT_NONE, M=None, K=None, N=None,
@@ -222,12 +188,7 @@ def gemm_ex(A, W, out, bias=None, gamma=None, resid=None, resid_mod=0, act=ACT_N
     return a.bn, EP_NAMES[a.epilogue], a.stats_parts_out
 
 
-class LayerNormArgs(ctypes.Structure):
-    """lwdetr_layernorm_args (include/lwdetr_b200.h)."""
-    _fields_ = [("x", _vp), ("ldx", _i), ("y", _vp), ("ldy", _i), ("w", _vp), ("b", _vp), ("eps", _f), ("rows", _i64), ("C", _i),
-                ("row_flag", _vp), ("flag_mod", _i), ("override_vec", _vp), ("add_src", _vp), ("ld_add", _i), ("y2", _vp), ("ldy2", _i),
-                ("y_group", _i64), ("y_group_stride", _i64), ("y_row_off", _i64),
-                ("w3", _vp), ("b3", _vp), ("eps3", _f), ("y3", _vp), ("ldy3", _i), ("rows_per_warp", _i)]
+LayerNormArgs = _STRUCTS["lwdetr_layernorm_args"]
 
 
 def layernorm_ex(x, y, w, b, eps, rows=None, C=None, row_flag=None, override=None, add=None, y2=None,
@@ -276,11 +237,7 @@ def attention(q, k, v, out, nseq, seqlen, heads, dh, scale):
 ATTN_KERNELS = {0: "wg", 1: "mma", 2: "mma_short"}
 
 
-class AttentionArgs(ctypes.Structure):
-    """lwdetr_attention_args (include/lwdetr_b200.h)."""
-    _fields_ = [("dtype", _i), ("q", _vp), ("ldq", _i), ("k", _vp), ("ldk", _i), ("v", _vp), ("ldv", _i), ("out", _vp), ("ldo", _i),
-                ("nseq", _i), ("seqlen", _i), ("heads", _i), ("dh", _i), ("scale", _f), ("dry_run", _i),
-                ("kernel", _i), ("warps", _i), ("poly_mask", _i)]
+AttentionArgs = _STRUCTS["lwdetr_attention_args"]
 
 
 def attention_ex(q, k, v, out, nseq, seqlen, heads, dh, scale, dry_run=False, dtype=None):
@@ -345,6 +302,15 @@ def msda_forward(value_hm, offs_logits, ref, out, B, S, Lq, M, L, P, shapes, val
 
 
 ET_F32, ET_F16, ET_BF16 = 0, 1, 2
+_ET_OF = {"float32": ET_F32, "float16": ET_F16, "bfloat16": ET_BF16}
+
+
+def _et_code(dtype, what):
+    """LWDETR_ET_* of a float32, float16 or bfloat16 dtype; else RuntimeError "<what> must be float32, float16 or ..."."""
+    code = _ET_OF.get(str(dtype).replace("torch.", ""))
+    if code is None:
+        raise RuntimeError("%s must be float32, float16 or bfloat16, got %s" % (what, dtype))
+    return code
 
 
 def ms_deform_attn_forward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, im2col_step=64):
@@ -352,9 +318,7 @@ def ms_deform_attn_forward(value, spatial_shapes, level_start_index, sampling_lo
     spatial_shapes int64 [L,2], level_start_index int64 [L], sampling_loc [B,Lq,M,L,P,2], attn_weight [B,Lq,M,L,P], all
     CUDA and contiguous; returns [B, Lq, M*D] in value's dtype (fp32, fp16 or bf16)."""
     import torch
-    et = {torch.float32: ET_F32, torch.float16: ET_F16, torch.bfloat16: ET_BF16}.get(value.dtype)
-    if et is None:
-        raise RuntimeError("ms_deform_attn_forward: value must be float32, float16 or bfloat16, got %s" % value.dtype)
+    et = _et_code(value.dtype, "ms_deform_attn_forward: value")
     for name, t in (("value", value), ("spatial_shapes", spatial_shapes), ("level_start_index", level_start_index),
                     ("sampling_loc", sampling_loc), ("attn_weight", attn_weight)):
         if not t.is_cuda:
@@ -401,13 +365,20 @@ def topk(score, k):
     return idx
 
 
-def postprocess(pred_logits, pred_boxes, target_sizes, num_select):
-    """Fused PostProcess (lwdetr.py:515-544) on CUDA fp32 tensors -> (scores [B,k] fp32, labels [B,k] int32, boxes [B,k,4] fp32)."""
+def _detector_outputs(pred_logits, pred_boxes, target_sizes):
+    """What postprocess() and query_best() read: (B, nq, num_classes, logits, boxes, target sizes), contiguous fp32 on the
+    logits' device."""
     import torch
     B, nq, ncls = pred_logits.shape
     logits = pred_logits.float().contiguous()
     boxes = pred_boxes.float().contiguous()
-    ts = target_sizes.to(device=logits.device, dtype=torch.float32).contiguous()
+    return B, nq, ncls, logits, boxes, target_sizes.to(device=logits.device, dtype=torch.float32).contiguous()
+
+
+def postprocess(pred_logits, pred_boxes, target_sizes, num_select):
+    """Fused PostProcess (lwdetr.py:515-544) on CUDA fp32 tensors -> (scores [B,k] fp32, labels [B,k] int32, boxes [B,k,4] fp32)."""
+    import torch
+    B, nq, ncls, logits, boxes, ts = _detector_outputs(pred_logits, pred_boxes, target_sizes)
     parts = (nq * ncls + 16383) // 16384
     work = torch.empty(B * parts * num_select, device=logits.device, dtype=torch.int32)
     scores = torch.empty(B, num_select, device=logits.device, dtype=torch.float32)
@@ -421,9 +392,7 @@ def postprocess(pred_logits, pred_boxes, target_sizes, num_select):
 TILE_METRICS = {"iou": 0, "ios": 1}     # LWDETR_TILE_IOU / LWDETR_TILE_IOS
 
 
-class TileViewStruct(ctypes.Structure):
-    """lwdetr_tile_view (include/lwdetr_b200.h)."""
-    _fields_ = [("frame", ctypes.c_int32), ("x0", ctypes.c_int32), ("y0", ctypes.c_int32)]
+TileViewStruct = _STRUCTS["lwdetr_tile_view"]
 
 
 def tile_merge(scores, labels, boxes, views, num_frames, score_threshold=0.0, iou_threshold=0.5, metric="ios", max_det=300):
@@ -459,11 +428,8 @@ def query_best(pred_logits, pred_boxes, target_sizes):
     [B, nq], labels int32 [B, nq], boxes fp32 [B, nq, 4]), each entry with the bits postprocess() gives that (query, class)
     pair."""
     import torch
-    B, nq, ncls = pred_logits.shape
-    logits = pred_logits.float().contiguous()
-    boxes = pred_boxes.float().contiguous()
+    B, nq, ncls, logits, boxes, ts = _detector_outputs(pred_logits, pred_boxes, target_sizes)
     dev = logits.device
-    ts = target_sizes.to(device=dev, dtype=torch.float32).contiguous()
     scores = torch.empty(B, nq, device=dev, dtype=torch.float32)
     labels = torch.empty(B, nq, device=dev, dtype=torch.int32)
     out = torch.empty(B, nq, 4, device=dev, dtype=torch.float32)
@@ -472,30 +438,28 @@ def query_best(pred_logits, pred_boxes, target_sizes):
     return scores, labels, out
 
 
-class TrackParams(ctypes.Structure):
-    """lwdetr_track_params (include/lwdetr_b200.h)."""
-    _fields_ = [(n, _f) for n in ("track_thresh", "low_thresh", "new_track_thresh", "match_thresh", "second_thresh",
-                                  "unconfirmed_thresh", "duplicate_thresh")] + \
-               [(n, ctypes.c_int32) for n in ("track_buffer", "frame_rate", "fuse_score", "class_aware", "capacity")]
+TrackParams = _STRUCTS["lwdetr_track_params"]
+TrackRecord = _STRUCTS["lwdetr_track_record"]
+ReidParams = _STRUCTS["lwdetr_reid_params"]
 
 
-class TrackRecord(ctypes.Structure):
-    """lwdetr_track_record (include/lwdetr_b200.h)."""
-    _fields_ = [(n, ctypes.c_int32) for n in ("id", "state", "activated", "start_frame", "end_frame", "label")] + \
-               [("score", _f), ("index", ctypes.c_int32), ("mean", ctypes.c_double * 8), ("cov", ctypes.c_double * 12)]
-
-
-class ReidParams(ctypes.Structure):
-    """lwdetr_reid_params (include/lwdetr_b200.h)."""
-    _fields_ = [("embedding_dim", ctypes.c_int32), ("proximity_thresh", _f), ("appearance_thresh", _f), ("ema_alpha", _f)]
-
-
-def _emb_dtype(dtype):
+def _track_outputs(B, m, dev):
+    """The outputs of one tracker step on dev: ids int32 [B, m], scores fp32, labels int32, boxes fp32 [B, m, 4], index
+    int32 and counts int32 [B], in the C calls' order."""
     import torch
-    codes = {torch.float32: ET_F32, torch.float16: ET_F16, torch.bfloat16: ET_BF16}
-    if dtype not in codes:
-        raise RuntimeError("Tracker.update: embeddings must be float32, float16 or bfloat16, got %s" % dtype)
-    return codes[dtype]
+    return (torch.empty(B, m, device=dev, dtype=torch.int32), torch.empty(B, m, device=dev, dtype=torch.float32),
+            torch.empty(B, m, device=dev, dtype=torch.int32), torch.empty(B, m, 4, device=dev, dtype=torch.float32),
+            torch.empty(B, m, device=dev, dtype=torch.int32), torch.empty(B, device=dev, dtype=torch.int32))
+
+
+def _motion(motion, B, dev, what):
+    """The camera motion of B frames as contiguous float64 [B, 4] on dev, or None."""
+    import torch
+    if motion is None:
+        return None
+    if tuple(motion.shape) != (B, 4):
+        raise RuntimeError("%s: motion must be [%d, 4], got %s" % (what, B, tuple(motion.shape)))
+    return motion.to(device=dev, dtype=torch.float64).contiguous()
 
 
 class _DeviceObject:
@@ -538,6 +502,13 @@ class _DeviceObject:
     def _ids(ids):
         ids = [int(x) for x in ids]
         return (ctypes.c_int32 * max(len(ids), 1))(*ids), len(ids)
+
+    def _stream_ids(self, ids, B, what):
+        """The HOST int32 array of the stream ids of B frames (default range(B)); RuntimeError naming `what` unless B are given."""
+        arr, n = self._ids(range(B) if ids is None else ids)
+        if n != B:
+            raise RuntimeError("%s: %d stream ids for %d frames" % (what, n, B))
+        return arr
 
     def reset(self, streams):
         """The streams start again (stream-ordered): a tracker's at frame 1 and id 1 with empty lists, an estimator's at
@@ -600,20 +571,10 @@ class Tracker(_DeviceObject):
         scores = scores.to(device=dev, dtype=torch.float32).contiguous()
         labels = labels.to(device=dev, dtype=torch.int32).contiguous()
         boxes = boxes.to(device=dev, dtype=torch.float32).contiguous()
-        ids, n = self._ids(range(B) if stream_ids is None else stream_ids)
-        if n != B:
-            raise RuntimeError("Tracker.update: %d stream ids for %d frames" % (n, B))
+        ids = self._stream_ids(stream_ids, B, "Tracker.update")
         m = k if max_out is None else int(max_out)
-        o_id = torch.empty(B, m, device=dev, dtype=torch.int32)
-        o_s = torch.empty(B, m, device=dev, dtype=torch.float32)
-        o_l = torch.empty(B, m, device=dev, dtype=torch.int32)
-        o_b = torch.empty(B, m, 4, device=dev, dtype=torch.float32)
-        o_i = torch.empty(B, m, device=dev, dtype=torch.int32)
-        counts = torch.empty(B, device=dev, dtype=torch.int32)
-        if motion is not None:
-            if tuple(motion.shape) != (B, 4):
-                raise RuntimeError("Tracker.update: motion must be [%d, 4], got %s" % (B, tuple(motion.shape)))
-            motion = motion.to(device=dev, dtype=torch.float64).contiguous()
+        out = _track_outputs(B, m, dev)
+        motion = _motion(motion, B, dev, "Tracker.update")
         if self.reid is not None:
             code, ld = ET_F32, 0
             if embeddings is not None:
@@ -622,24 +583,23 @@ class Tracker(_DeviceObject):
                     raise RuntimeError("Tracker.update: embeddings must be [%d, %d, %d], got %s" % (B, k, D, tuple(embeddings.shape)))
                 if embeddings.device != dev:
                     raise RuntimeError("Tracker.update: embeddings are on %s but the tracker lives on %s" % (embeddings.device, dev))
-                code = _emb_dtype(embeddings.dtype)
+                code = _et_code(embeddings.dtype, "Tracker.update: embeddings")
                 if embeddings.stride(2) != 1 or embeddings.stride(0) != k * embeddings.stride(1):
                     embeddings = embeddings.contiguous()
                 ld = embeddings.stride(1)
             check(lib().lwdetr_track_reid(self._t, ptr(scores), ptr(labels), ptr(boxes), ptr(motion), ptr(embeddings), code, ld, B, k,
-                                          ctypes.cast(ids, _vp), m, ptr(o_id), ptr(o_s), ptr(o_l), ptr(o_b), ptr(o_i), ptr(counts),
-                                          stream_ptr(dev)), "lwdetr_track_reid")
+                                          ctypes.cast(ids, _vp), m, *map(ptr, out), stream_ptr(dev)), "lwdetr_track_reid")
             self._last_embeddings = embeddings      # keep alive until the stream has consumed it
         elif embeddings is not None:
             raise RuntimeError("Tracker.update: embeddings need a tracker made with embedding_dim")
         elif motion is None:
-            check(lib().lwdetr_track(self._t, ptr(scores), ptr(labels), ptr(boxes), B, k, ctypes.cast(ids, _vp), m, ptr(o_id), ptr(o_s),
-                                     ptr(o_l), ptr(o_b), ptr(o_i), ptr(counts), stream_ptr(dev)), "lwdetr_track")
+            check(lib().lwdetr_track(self._t, ptr(scores), ptr(labels), ptr(boxes), B, k, ctypes.cast(ids, _vp), m, *map(ptr, out),
+                                     stream_ptr(dev)), "lwdetr_track")
         else:
             check(lib().lwdetr_track_ex(self._t, ptr(scores), ptr(labels), ptr(boxes), ptr(motion), B, k, ctypes.cast(ids, _vp), m,
-                                        ptr(o_id), ptr(o_s), ptr(o_l), ptr(o_b), ptr(o_i), ptr(counts), stream_ptr(dev)), "lwdetr_track_ex")
-        self._advance(ids, n)
-        return o_id, o_s, o_l, o_b, o_i, counts
+                                        *map(ptr, out), stream_ptr(dev)), "lwdetr_track_ex")
+        self._advance(ids, B)
+        return out
 
     def _advance(self, ids, n):
         for i in range(n):
@@ -677,12 +637,7 @@ class Tracker(_DeviceObject):
         return emb[:n], has[:n].astype(bool)
 
 
-class GmcParams(ctypes.Structure):
-    """lwdetr_gmc_params (include/lwdetr_b200.h)."""
-    _fields_ = [("downscale", ctypes.c_int32), ("max_points", ctypes.c_int32), ("quality", _f), ("levels", ctypes.c_int32),
-                ("window", ctypes.c_int32), ("iterations", ctypes.c_int32), ("eps", _f), ("min_eig", _f), ("ransac_thresh", _f),
-                ("hypotheses", ctypes.c_int32), ("min_inliers", ctypes.c_int32), ("max_height", ctypes.c_int32),
-                ("max_width", ctypes.c_int32)]
+GmcParams = _STRUCTS["lwdetr_gmc_params"]
 
 
 GMC_OK, GMC_FIRST_FRAME, GMC_SIZE_CHANGED, GMC_FEW_POINTS, GMC_FEW_INLIERS = 0, 1, 2, 3, 4
@@ -705,39 +660,27 @@ class MotionEstimator(_DeviceObject):
         through its luma plane only, so its colorspace does not matter) -> (motion float64 [B, 4] (a, b, tx, ty): x' = a x -
         b y + tx, y' = b x + a y + ty from the stream's previous frame to this one in frame pixels; status int32 [B]
         (GMC_*); inliers int32 [B]).  streams defaults to range(B).  Stream-ordered, no synchronisation."""
-        import torch
-        frames = self._frames(frames)
-        B = len(frames.items)
-        ids, n = self._ids(range(B) if streams is None else streams)
-        if n != B:
-            raise RuntimeError("MotionEstimator.estimate: %d stream ids for %d frames" % (n, B))
-        dev = self.device
-        motion = torch.empty(B, 4, device=dev, dtype=torch.float64)
-        status = torch.empty(B, device=dev, dtype=torch.int32)
-        inliers = torch.empty(B, device=dev, dtype=torch.int32)
-        descs = frames.descs(frames.sizes)
-        name = "lwdetr_gmc_estimate_nv12" if frames.nv12 else "lwdetr_gmc_estimate"
-        check(getattr(lib(), name)(self._t, descs, B, ctypes.cast(ids, _vp), ptr(motion), ptr(status), ptr(inliers), stream_ptr(dev)), name)
-        return motion, status, inliers
+        return self._call("estimate", frames, streams)
 
     def observe(self, frames, streams=None):
         """estimate() without the motion (lwdetr_gmc_observe): the streams' pyramids and corners only, so that the next
         estimate() or a BoxFlow on the next frame has this one as its previous frame.  Stream-ordered, no synchronisation."""
-        frames = self._frames(frames)
-        B = len(frames.items)
-        ids, n = self._ids(range(B) if streams is None else streams)
-        if n != B:
-            raise RuntimeError("MotionEstimator.observe: %d stream ids for %d frames" % (n, B))
-        name = "lwdetr_gmc_observe_nv12" if frames.nv12 else "lwdetr_gmc_observe"
-        check(getattr(lib(), name)(self._t, frames.descs(frames.sizes), B, ctypes.cast(ids, _vp), stream_ptr(self.device)), name)
+        self._call("observe", frames, streams)
 
-    def _frames(self, frames):
+    def _call(self, what, frames, streams):
+        """lwdetr_gmc_<what>(_nv12) on one frame per stream; the outputs of an estimate, () for an observe."""
         import torch
-        if isinstance(frames, Frames):
-            return frames
-        nv12 = isinstance(frames, torch.Tensor) and frames.dim() == 3 and frames.shape[2] != 3
-        nv12 = nv12 or (not isinstance(frames, torch.Tensor) and len(frames) > 0 and _is_nv12(frames[0]))
-        return Frames(frames, self.device, "bt601" if nv12 else None)
+        if not isinstance(frames, Frames):
+            nv12 = isinstance(frames, torch.Tensor) and frames.dim() == 3 and frames.shape[2] != 3
+            nv12 = nv12 or (not isinstance(frames, torch.Tensor) and len(frames) > 0 and _is_nv12(frames[0]))
+            frames = Frames(frames, self.device, "bt601" if nv12 else None)
+        B, dev = len(frames.items), self.device
+        ids = self._stream_ids(streams, B, "MotionEstimator." + what)
+        out = () if what == "observe" else (torch.empty(B, 4, device=dev, dtype=torch.float64), torch.empty(B, device=dev, dtype=torch.int32),
+                                           torch.empty(B, device=dev, dtype=torch.int32))
+        name = "lwdetr_gmc_%s%s" % (what, "_nv12" if frames.nv12 else "")
+        check(getattr(lib(), name)(self._t, frames.descs(frames.sizes), B, ctypes.cast(ids, _vp), *map(ptr, out), stream_ptr(dev)), name)
+        return out
 
     def export(self, stream_id):
         """Synchronous, waiting for this estimator's last estimate() or reset() and for nothing else on the device: one
@@ -765,11 +708,7 @@ class MotionEstimator(_DeviceObject):
                     found=found[:nf].astype(bool))
 
 
-class FlowParams(ctypes.Structure):
-    """lwdetr_flow_params (include/lwdetr_b200.h)."""
-    _fields_ = [("grid", ctypes.c_int32), ("window", ctypes.c_int32), ("iterations", ctypes.c_int32), ("eps", _f), ("min_eig", _f),
-                ("ncc_window", ctypes.c_int32), ("min_points", ctypes.c_int32), ("fb_max", _f), ("scale_min", _f), ("scale_max", _f),
-                ("max_tracks", ctypes.c_int32)]
+FlowParams = _STRUCTS["lwdetr_flow_params"]
 
 
 FLOW_OK, FLOW_FEW_POINTS, FLOW_FB, FLOW_SCALE, FLOW_SMALL, FLOW_SKIPPED, FLOW_NO_PREVIOUS = range(7)
@@ -800,24 +739,15 @@ class BoxFlow(_DeviceObject):
         """One flow frame for each listed stream (lwdetr_track_flow): the tracker's confirmed tracks move by their measured
         flow or go Lost, with no detections.  motion: float64 [B, 4] of these frames (MotionEstimator.estimate) or None.
         Returns Tracker.update's tuple; index is -1 for every track.  Stream-ordered, no synchronisation."""
-        import torch
         ids, B = self._ids(streams)
         dev = self.device
         m = int(tracker.params.capacity) if max_out is None else int(max_out)
-        o_id = torch.empty(B, m, device=dev, dtype=torch.int32)
-        o_s = torch.empty(B, m, device=dev, dtype=torch.float32)
-        o_l = torch.empty(B, m, device=dev, dtype=torch.int32)
-        o_b = torch.empty(B, m, 4, device=dev, dtype=torch.float32)
-        o_i = torch.empty(B, m, device=dev, dtype=torch.int32)
-        counts = torch.empty(B, device=dev, dtype=torch.int32)
-        if motion is not None:
-            if tuple(motion.shape) != (B, 4):
-                raise RuntimeError("BoxFlow.propagate: motion must be [%d, 4], got %s" % (B, tuple(motion.shape)))
-            motion = motion.to(device=dev, dtype=torch.float64).contiguous()
-        check(lib().lwdetr_track_flow(tracker._t, self._t, ptr(motion), B, ctypes.cast(ids, _vp), m, ptr(o_id), ptr(o_s), ptr(o_l),
-                                      ptr(o_b), ptr(o_i), ptr(counts), stream_ptr(dev)), "lwdetr_track_flow")
+        out = _track_outputs(B, m, dev)
+        motion = _motion(motion, B, dev, "BoxFlow.propagate")
+        check(lib().lwdetr_track_flow(tracker._t, self._t, ptr(motion), B, ctypes.cast(ids, _vp), m, *map(ptr, out), stream_ptr(dev)),
+              "lwdetr_track_flow")
         tracker._advance(ids, B)
-        return o_id, o_s, o_l, o_b, o_i, counts
+        return out
 
     def export(self, stream_id):
         """Synchronous: one stream's last flow (lwdetr_flow_export) as a dict of numpy arrays: found (tracks listed), grid,
@@ -839,15 +769,10 @@ class BoxFlow(_DeviceObject):
                     ncc=ncc[:n], status=status[:n], dx=meas[:n, 0], dy=meas[:n, 1], s=meas[:n, 2], z=meas[:n, 3:7])
 
 
-class ZonesParams(ctypes.Structure):
-    """lwdetr_zones_params (include/lwdetr_b200.h)."""
-    _fields_ = [(n, ctypes.c_int32) for n in ("num_classes", "capacity", "forget_after", "zone_anchor", "line_anchors")]
+ZonesParams = _STRUCTS["lwdetr_zones_params"]
 
 
-class ZoneRecord(ctypes.Structure):
-    """lwdetr_zone_record (include/lwdetr_b200.h)."""
-    _fields_ = [("id", ctypes.c_int32), ("last_seen", ctypes.c_int32), ("label", ctypes.c_int32), ("inside", ctypes.c_uint32),
-                ("sides", ctypes.c_int8 * 32), ("entry", ctypes.c_int32 * 32)]
+ZoneRecord = _STRUCTS["lwdetr_zone_record"]
 
 
 ANCHORS = ("top_left", "top_center", "top_right", "center_left", "center", "center_right", "bottom_left", "bottom_center",
@@ -930,9 +855,7 @@ class Zones(_DeviceObject):
         labels = labels.to(device=dev, dtype=torch.int32).contiguous()
         boxes = boxes.to(device=dev, dtype=torch.float32).contiguous()
         counts = counts.to(device=dev, dtype=torch.int32).contiguous()
-        sids, n = self._ids(range(B) if stream_ids is None else stream_ids)
-        if n != B:
-            raise RuntimeError("Zones.update: %d stream ids for %d frames" % (n, B))
+        sids = self._stream_ids(stream_ids, B, "Zones.update")
         E = int(max_events)
         inside = torch.empty(B, m, device=dev, dtype=torch.int32)
         occupancy = torch.empty(B, 32, device=dev, dtype=torch.int32)
@@ -959,8 +882,7 @@ class Zones(_DeviceObject):
         check(lib().lwdetr_zones_export(self._t, int(stream), ctypes.cast(fo, _vp), ctypes.cast(info, _vp), lc.ctypes.data_as(_vp),
                                         en.ctypes.data_as(_vp), ctypes.cast(recs, _vp), cap), "lwdetr_zones_export")
         L, Z, n = list(info)
-        raw = np.frombuffer(recs, np.dtype([("id", "<i4"), ("last_seen", "<i4"), ("label", "<i4"), ("inside", "<u4"), ("sides", "i1", 32),
-                                            ("entry", "<i4", 32)]))[:n]
+        raw = np.ctypeslib.as_array(recs)[:n]
         return dict(frame=fo[0], overflow=fo[1], line_counts=lc.reshape(-1)[:L * nc * 2].reshape(L, nc, 2).copy(),
                     entries=en.reshape(-1)[:Z * nc].reshape(Z, nc).copy(), ids=raw["id"].copy(), last_seen=raw["last_seen"].copy(),
                     labels=raw["label"].copy(), sides=raw["sides"][:, :L].copy(), inside=raw["inside"].copy(),
@@ -1039,24 +961,17 @@ def host_bicubic_hw(src, out_h, out_w):
     return dst
 
 
-class ConfigStruct(ctypes.Structure):
-    _fields_ = [(n, ctypes.c_int32) for n in ("vit_dim", "vit_depth", "vit_heads", "window_block_mask", "n_taps")] + \
-               [("taps", ctypes.c_int32 * 4), ("n_levels", ctypes.c_int32), ("level_scale_log2", ctypes.c_int32 * 2)] + \
-               [(n, ctypes.c_int32) for n in ("hidden_dim", "sa_heads", "ca_heads", "dec_points", "num_queries",
-                                              "dec_layers", "dim_feedforward", "num_classes", "group_detr", "img_size")]
+ConfigStruct = _STRUCTS["lwdetr_config"]
 
 
-class InputDesc(ctypes.Structure):
-    _fields_ = [("images", _vp), ("format", ctypes.c_int32), ("padding_mask", _vp), ("mean", ctypes.c_float * 3), ("std", ctypes.c_float * 3)]
+InputDesc = _STRUCTS["lwdetr_input"]
 
 
 IN_F32_NCHW, IN_16_NCHW, IN_U8_NHWC = 0, 1, 2
 IMAGENET_MEAN, IMAGENET_STD = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)      # demo/demo.py:150-153, datasets/coco.py
 
 
-class FrameStruct(ctypes.Structure):
-    _fields_ = [("data", _vp), ("height", ctypes.c_int32), ("width", ctypes.c_int32), ("pitch_bytes", ctypes.c_int64),
-                ("dst_h", ctypes.c_int32), ("dst_w", ctypes.c_int32)]
+FrameStruct = _STRUCTS["lwdetr_frame"]
 
 
 def frame_list(frames, device=None):
@@ -1092,10 +1007,7 @@ def frame_descs(frames, dsts):
     return arr
 
 
-class FrameNV12Struct(ctypes.Structure):
-    _fields_ = [("luma", _vp), ("luma_pitch", ctypes.c_int64), ("chroma", _vp), ("chroma_pitch", ctypes.c_int64),
-                ("height", ctypes.c_int32), ("width", ctypes.c_int32), ("dst_h", ctypes.c_int32), ("dst_w", ctypes.c_int32),
-                ("colorspace", ctypes.c_int32)]
+FrameNV12Struct = _STRUCTS["lwdetr_frame_nv12"]
 
 
 # colorspace names of NV12 frames -> LWDETR_CSC_* (include/lwdetr_b200.h): limited (studio) range unless "_full"
@@ -1234,14 +1146,6 @@ def resize_patches(frames, dsts, size, dtype, mean=None, std=None, want_mask=Fal
 
 
 CROP_FILTERS = {"bilinear": 0, "antialias": 1}     # LWDETR_CROP_BILINEAR (cv2 INTER_LINEAR) / LWDETR_CROP_ANTIALIAS (PIL triangle)
-_ET_OF = {"float32": ET_F32, "float16": ET_F16, "bfloat16": ET_BF16}
-
-
-def _et_code(dtype, what):
-    code = _ET_OF.get(str(dtype).replace("torch.", ""))
-    if code is None:
-        raise RuntimeError("%s: dtype must be float32, float16 or bfloat16, got %s" % (what, dtype))
-    return code
 
 
 def crops(frames, boxes, frame_index, size=(256, 128), filter="bilinear", mean=None, std=None, normalize=True, dtype=None,
@@ -1259,7 +1163,7 @@ def crops(frames, boxes, frame_index, size=(256, 128), filter="bilinear", mean=N
     fb = frames if isinstance(frames, Frames) else Frames(frames, colorspace=colorspace)
     dev, B = fb.device, len(fb.items)
     dtype = torch.float32 if dtype is None else dtype
-    code = _et_code(dtype, "crops")
+    code = _et_code(dtype, "crops: dtype")
     if boxes.dim() != 2 or boxes.shape[1] != 4 or tuple(frame_index.shape) != (boxes.shape[0],):
         raise RuntimeError("crops: boxes must be [N, 4] and frame_index [N], got %s and %s" % (tuple(boxes.shape), tuple(frame_index.shape)))
     N = boxes.shape[0]
@@ -1312,7 +1216,7 @@ def scatter_rows(rows, entry, num_out, count=None):
     N, D = rows.shape
     if rows.stride(1) != 1:
         rows = rows.contiguous()
-    code = _et_code(rows.dtype, "scatter_rows")
+    code = _et_code(rows.dtype, "scatter_rows: dtype")
     entry = entry.to(device=rows.device, dtype=torch.int32).contiguous()
     if entry.numel() < N:
         raise RuntimeError("scatter_rows: %d entries for %d rows" % (entry.numel(), N))
@@ -1326,8 +1230,7 @@ def scatter_rows(rows, entry, num_out, count=None):
     return out
 
 
-class AuxOut(ctypes.Structure):
-    _fields_ = [(n, _vp) for n in ("aux_logits", "aux_boxes", "enc_logits", "enc_boxes", "topk_index")]
+AuxOut = _STRUCTS["lwdetr_aux_out"]
 
 
 def config_struct(cfg):

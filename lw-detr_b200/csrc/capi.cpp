@@ -133,6 +133,16 @@ struct DeviceState {
                                                                 : cudaEventRecord(done, st));
   }
 
+  // the call sequence of every launch on the object: run(stream) (0 or a CUDA error) on the object's device, then mark() on
+  // this state and on `also` (a second object the launch wrote), in that order.  0, or -1 with "<fn> launch: <error>" set
+  template <class Run> int launch(const std::string& fn, void* stream, Run run, const DeviceState* also = nullptr) const {
+    lwb::DeviceGuard g(device);
+    int e = run(static_cast<cudaStream_t>(stream));
+    if (!e) e = mark(stream);
+    if (!e && also) e = also->mark(stream);
+    return e ? cuda_fail(e, (fn + " launch").c_str()) : 0;
+  }
+
   struct Copy { void* dst; const void* src; size_t bytes; };
   // device-to-host copies once the last marked launch is done, all on `copy`, waited for once
   cudaError_t read(const std::vector<Copy>& parts) const {
@@ -162,6 +172,34 @@ struct DeviceState {
     cudaEventDestroy(done);
   }
 };
+
+// lwdetr_tracker_reset, lwdetr_gmc_reset and lwdetr_zones_reset: the listed streams of obj start again through
+// reset_launch(obj->table, streams, n, stream)
+template <class T, class Launch> int reset_call(const char* name, T* obj, const int32_t* streams, int n, void* stream, Launch reset_launch) {
+  const std::string fn(name);
+  if (!obj || (n > 0 && !streams)) return fail(fn + ": null pointer");
+  if (n < 0) return fail(fn + ": n must be >= 0");
+  const std::string err = check_ids(obj->table.num_streams, streams, n);
+  if (!err.empty()) return fail(fn + ": " + err);
+  if (n == 0) return 0;
+  return obj->state.launch(fn, stream, [&](cudaStream_t st) { return reset_launch(obj->table, streams, n, st); });
+}
+
+// lwdetr_layernorm and lwdetr_layernorm_ex, once each has checked its arguments: fill, launch, report the kernel instance
+int layernorm_call(const char* name, int dtype, lwdetr_layernorm_args* p, void* stream) {
+  const std::string fn(name);
+  lwb::LayerNormArgs a{};
+  a.x = p->x; a.ldx = p->ldx; a.y = p->y; a.ldy = p->ldy; a.w = p->w; a.b = p->b; a.eps = p->eps; a.rows = p->rows; a.C = p->C;
+  a.row_flag = p->row_flag; a.flag_mod = p->row_flag ? p->flag_mod : 1; a.override_vec = p->override_vec;
+  a.add_src = p->add_src; a.ld_add = p->ld_add; a.y2 = p->y2; a.ldy2 = p->ldy2;
+  a.y_group = p->y_group; a.y_group_stride = p->y_group_stride; a.y_row_off = p->y_row_off;
+  a.w3 = p->w3; a.b3 = p->b3; a.eps3 = p->eps3; a.y3 = p->y3; a.ldy3 = p->ldy3;
+  int e = lwb::layernorm_launch(dtype, a, static_cast<cudaStream_t>(stream));
+  if (e == -2) return fail(fn + ": C must be a multiple of 8 and <= 1024");
+  if (e) return cuda_fail(e, (fn + " launch").c_str());
+  p->rows_per_warp = lwb::layernorm_rows_per_warp(p->rows, p->C);
+  return 0;
+}
 }  // namespace
 
 static_assert(LWDETR_ATTN_WG == lwb::ATTN_WG && LWDETR_ATTN_MMA == lwb::ATTN_MMA && LWDETR_ATTN_MMA_SHORT == lwb::ATTN_MMA_SHORT, "attention kernel codes");
@@ -233,12 +271,8 @@ int lwdetr_conv3x3_plan(int OH, int OW, int32_t* tw, int32_t* th) {
 int lwdetr_layernorm(int dtype, const void* x, int ldx, void* y, int ldy, const float* w, const float* b, float eps,
                      int64_t rows, int C, void* stream) {
   if (!x || !y || !w || !b) return fail("lwdetr_layernorm: null pointer");
-  lwb::LayerNormArgs a{};
-  a.x = x; a.ldx = ldx; a.y = y; a.ldy = ldy; a.w = w; a.b = b; a.eps = eps; a.rows = rows; a.C = C; a.flag_mod = 1;
-  int e = lwb::layernorm_launch(dtype, a, static_cast<cudaStream_t>(stream));
-  if (e == -2) return fail("lwdetr_layernorm: C must be a multiple of 8 and <= 1024");
-  if (e) return cuda_fail(e, "lwdetr_layernorm launch");
-  return 0;
+  lwdetr_layernorm_args a = {x, ldx, y, ldy, w, b, eps, rows, C};
+  return layernorm_call("lwdetr_layernorm", dtype, &a, stream);
 }
 
 int lwdetr_layernorm_ex(int dtype, lwdetr_layernorm_args* p, void* stream) {
@@ -248,17 +282,7 @@ int lwdetr_layernorm_ex(int dtype, lwdetr_layernorm_args* p, void* stream) {
   if (p->y3 && (!p->w3 || !p->b3)) return fail("lwdetr_layernorm_ex: y3 needs w3 and b3");
   if ((p->ldx | p->ldy | (p->y2 ? p->ld_add | p->ldy2 : 0) | (p->y3 ? p->ldy3 : 0)) % 8) return fail("lwdetr_layernorm_ex: leading dimensions must be multiples of 8");
   if (p->rows < 1) return fail("lwdetr_layernorm_ex: rows must be positive");
-  lwb::LayerNormArgs a{};
-  a.x = p->x; a.ldx = p->ldx; a.y = p->y; a.ldy = p->ldy; a.w = p->w; a.b = p->b; a.eps = p->eps; a.rows = p->rows; a.C = p->C;
-  a.row_flag = p->row_flag; a.flag_mod = p->row_flag ? p->flag_mod : 1; a.override_vec = p->override_vec;
-  a.add_src = p->add_src; a.ld_add = p->ld_add; a.y2 = p->y2; a.ldy2 = p->ldy2;
-  a.y_group = p->y_group; a.y_group_stride = p->y_group_stride; a.y_row_off = p->y_row_off;
-  a.w3 = p->w3; a.b3 = p->b3; a.eps3 = p->eps3; a.y3 = p->y3; a.ldy3 = p->ldy3;
-  int e = lwb::layernorm_launch(dtype, a, static_cast<cudaStream_t>(stream));
-  if (e == -2) return fail("lwdetr_layernorm_ex: C must be a multiple of 8 and <= 1024");
-  if (e) return cuda_fail(e, "lwdetr_layernorm_ex launch");
-  p->rows_per_warp = lwb::layernorm_rows_per_warp(p->rows, p->C);
-  return 0;
+  return layernorm_call("lwdetr_layernorm_ex", dtype, p, stream);
 }
 
 int lwdetr_attention(int dtype, const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, void* out, int ldo,
@@ -466,16 +490,7 @@ int lwdetr_tracker_create(int num_streams, const lwdetr_track_params* params, lw
 void lwdetr_tracker_destroy(lwdetr_tracker* t) { delete t; }
 
 int lwdetr_tracker_reset(lwdetr_tracker* t, const int32_t* streams, int n, void* stream) {
-  if (!t || (n > 0 && !streams)) return fail("lwdetr_tracker_reset: null pointer");
-  if (n < 0) return fail("lwdetr_tracker_reset: n must be >= 0");
-  const std::string err = check_ids(t->table.num_streams, streams, n);
-  if (!err.empty()) return fail("lwdetr_tracker_reset: " + err);
-  if (n == 0) return 0;
-  lwb::DeviceGuard g(t->state.device);
-  int e = lwb::track_reset_launch(t->table, streams, n, static_cast<cudaStream_t>(stream));
-  if (!e) e = t->state.mark(stream);
-  if (e) return cuda_fail(e, "lwdetr_tracker_reset launch");
-  return 0;
+  return reset_call("lwdetr_tracker_reset", t, streams, n, stream, lwb::track_reset_launch);
 }
 
 static int track_common(const char* name, lwdetr_tracker* t, const float* scores, const int32_t* labels, const float* boxes,
@@ -495,13 +510,10 @@ static int track_common(const char* name, lwdetr_tracker* t, const float* scores
   // bits), which keeps each record's embedding slot; the ByteTrack one would leave the slot array stale
   const lwb::ReidInput none{&t->reid, nullptr, LWDETR_ET_F32, 0};
   if (!reid && t->reid.emb) reid = &none;
-  lwb::DeviceGuard g(t->state.device);
-  int e = lwb::track_launch(t->table, t->params, scores, labels, boxes, motion, B, k, stream_ids, max_out, out_ids, out_scores, out_labels,
-                            out_boxes, out_index, counts, static_cast<cudaStream_t>(stream), reid);
-  if (e == -2) return fail(fn + ": a limit is exceeded");
-  if (!e) e = t->state.mark(stream);
-  if (e) return cuda_fail(e, (fn + " launch").c_str());
-  return 0;
+  return t->state.launch(fn, stream, [&](cudaStream_t st) {
+    return lwb::track_launch(t->table, t->params, scores, labels, boxes, motion, B, k, stream_ids, max_out, out_ids, out_scores, out_labels,
+                             out_boxes, out_index, counts, st, reid);
+  });
 }
 
 int lwdetr_track(lwdetr_tracker* t, const float* scores, const int32_t* labels, const float* boxes, int B, int k, const int32_t* stream_ids,
@@ -706,16 +718,7 @@ int lwdetr_zones_set(lwdetr_zones* z, int stream_id, const double* lines, int n_
 }
 
 int lwdetr_zones_reset(lwdetr_zones* z, const int32_t* streams, int n, void* stream) {
-  if (!z || (n > 0 && !streams)) return fail("lwdetr_zones_reset: null pointer");
-  if (n < 0) return fail("lwdetr_zones_reset: n must be >= 0");
-  const std::string err = check_ids(z->table.num_streams, streams, n);
-  if (!err.empty()) return fail("lwdetr_zones_reset: " + err);
-  if (n == 0) return 0;
-  lwb::DeviceGuard g(z->state.device);
-  int e = lwb::zones_reset_launch(z->table, streams, n, static_cast<cudaStream_t>(stream));
-  if (!e) e = z->state.mark(stream);
-  if (e) return cuda_fail(e, "lwdetr_zones_reset launch");
-  return 0;
+  return reset_call("lwdetr_zones_reset", z, streams, n, stream, lwb::zones_reset_launch);
 }
 
 int lwdetr_zones_update(lwdetr_zones* z, const int32_t* ids, const int32_t* labels, const float* boxes, const int32_t* counts, int B,
@@ -728,12 +731,10 @@ int lwdetr_zones_update(lwdetr_zones* z, const int32_t* ids, const int32_t* labe
   if (reinterpret_cast<uintptr_t>(boxes) % 16) return fail("lwdetr_zones_update: boxes must be 16-byte aligned");
   const std::string err = check_ids(z->table.num_streams, stream_ids, B);
   if (!err.empty()) return fail("lwdetr_zones_update: " + err);
-  lwb::DeviceGuard g(z->state.device);
-  int e = lwb::zones_launch(z->table, ids, labels, boxes, counts, B, max_out, stream_ids, inside, occupancy, events, max_events,
-                            event_counts, static_cast<cudaStream_t>(stream));
-  if (!e) e = z->state.mark(stream);
-  if (e) return cuda_fail(e, "lwdetr_zones_update launch");
-  return 0;
+  return z->state.launch("lwdetr_zones_update", stream, [&](cudaStream_t st) {
+    return lwb::zones_launch(z->table, ids, labels, boxes, counts, B, max_out, stream_ids, inside, occupancy, events, max_events,
+                             event_counts, st);
+  });
 }
 
 int lwdetr_zones_export(lwdetr_zones* z, int stream_id, int32_t frame_overflow[2], int32_t info[3], int32_t* line_counts, int32_t* entries,
@@ -841,16 +842,7 @@ int lwdetr_gmc_create(int num_streams, const lwdetr_gmc_params* params, lwdetr_g
 void lwdetr_gmc_destroy(lwdetr_gmc* g) { delete g; }
 
 int lwdetr_gmc_reset(lwdetr_gmc* g, const int32_t* streams, int n, void* stream) {
-  if (!g || (n > 0 && !streams)) return fail("lwdetr_gmc_reset: null pointer");
-  if (n < 0) return fail("lwdetr_gmc_reset: n must be >= 0");
-  const std::string err = check_ids(g->table.num_streams, streams, n);
-  if (!err.empty()) return fail("lwdetr_gmc_reset: " + err);
-  if (n == 0) return 0;
-  lwb::DeviceGuard dg(g->state.device);
-  int e = lwb::gmc_reset_launch(g->table, streams, n, static_cast<cudaStream_t>(stream));
-  if (!e) e = g->state.mark(stream);
-  if (e) return cuda_fail(e, "lwdetr_gmc_reset launch");
-  return 0;
+  return reset_call("lwdetr_gmc_reset", g, streams, n, stream, lwb::gmc_reset_launch);
 }
 
 int lwdetr_gmc_export(lwdetr_gmc* g, int stream_id, uint8_t* levels, int64_t levels_bytes, float* corners, float* flow, int8_t* found,
@@ -887,63 +879,57 @@ int lwdetr_gmc_export(lwdetr_gmc* g, int stream_id, uint8_t* levels, int64_t lev
   return 0;
 }
 
+}  // extern "C"
+
+// a frame as the estimator reads it: RGB, or NV12 through its luma plane
+static lwb::GmcFrameHost gmc_frame(const lwdetr_frame& f) { return {f.data, f.pitch_bytes, f.height, f.width, 0}; }
+static lwb::GmcFrameHost gmc_frame(const lwdetr_frame_nv12& f) { return {f.luma, f.luma_pitch, f.height, f.width, 1}; }
+
 // lwdetr_gmc_estimate / _nv12, and with observe lwdetr_gmc_observe / _nv12 (no outputs)
-static int gmc_estimate_common(const char* name, lwdetr_gmc* g, const std::vector<lwb::GmcFrameHost>& fr, int B, const int32_t* stream_ids,
-                               double* motion, int32_t* status, int32_t* inliers, void* stream, bool observe = false) {
+template <typename F>
+static int gmc_call(const char* name, lwdetr_gmc* g, const F* frames, int B, const int32_t* stream_ids, double* motion, int32_t* status,
+                    int32_t* inliers, void* stream, bool observe) {
   const std::string fn(name);
+  if (!g || !frames || !stream_ids) return fail(fn + ": null pointer");
+  if (B < 1) return fail(fn + ": B must be >= 1");
   if (!observe && (!motion || !status || !inliers)) return fail(fn + ": null pointer");
   if (reinterpret_cast<uintptr_t>(motion) % 8) return fail(fn + ": motion must be 8-byte aligned");
   const std::string err = check_ids(g->table.num_streams, stream_ids, B);
   if (!err.empty()) return fail(fn + ": " + err);
   const lwdetr_gmc_params& p = g->table.p;
   const int lo = lwb::GMC_MIN_SIDE * p.downscale;
+  std::vector<lwb::GmcFrameHost> fr(static_cast<size_t>(B));
   for (int i = 0; i < B; ++i) {
-    const lwb::GmcFrameHost& f = fr[i];
+    const lwb::GmcFrameHost& f = fr[i] = gmc_frame(frames[i]);
     if (!f.data) return fail(fn + ": null frame pointer");
     if (f.h < lo || f.w < lo || f.h > p.max_height || f.w > p.max_width)
       return fail(fn + ": frame " + std::to_string(i) + " is " + std::to_string(f.h) + " x " + std::to_string(f.w) + "; sides must be in [" +
                   std::to_string(lo) + ", max_height / max_width = " + std::to_string(p.max_height) + " x " + std::to_string(p.max_width) + "]");
     if (f.pitch < static_cast<long long>(f.w) * (f.nv12 ? 1 : 3)) return fail(fn + ": frame " + std::to_string(i) + ": pitch too small");
   }
-  lwb::DeviceGuard dg(g->state.device);
-  int e = lwb::gmc_estimate_launch(g->table, fr.data(), B, stream_ids, motion, status, inliers, static_cast<cudaStream_t>(stream), observe);
-  if (!e) e = g->state.mark(stream);
-  if (e) return cuda_fail(e, (fn + " launch").c_str());
-  return 0;
+  return g->state.launch(fn, stream, [&](cudaStream_t st) {
+    return lwb::gmc_estimate_launch(g->table, fr.data(), B, stream_ids, motion, status, inliers, st, observe);
+  });
 }
+
+extern "C" {
 
 int lwdetr_gmc_estimate(lwdetr_gmc* g, const lwdetr_frame* frames, int B, const int32_t* stream_ids, double* motion, int32_t* status,
                         int32_t* inliers, void* stream) {
-  if (!g || !frames || !stream_ids) return fail("lwdetr_gmc_estimate: null pointer");
-  if (B < 1) return fail("lwdetr_gmc_estimate: B must be >= 1");
-  std::vector<lwb::GmcFrameHost> fr(static_cast<size_t>(B));
-  for (int i = 0; i < B; ++i) fr[i] = lwb::GmcFrameHost{frames[i].data, frames[i].pitch_bytes, frames[i].height, frames[i].width, 0};
-  return gmc_estimate_common("lwdetr_gmc_estimate", g, fr, B, stream_ids, motion, status, inliers, stream);
+  return gmc_call("lwdetr_gmc_estimate", g, frames, B, stream_ids, motion, status, inliers, stream, false);
 }
 
 int lwdetr_gmc_estimate_nv12(lwdetr_gmc* g, const lwdetr_frame_nv12* frames, int B, const int32_t* stream_ids, double* motion,
                              int32_t* status, int32_t* inliers, void* stream) {
-  if (!g || !frames || !stream_ids) return fail("lwdetr_gmc_estimate_nv12: null pointer");
-  if (B < 1) return fail("lwdetr_gmc_estimate_nv12: B must be >= 1");
-  std::vector<lwb::GmcFrameHost> fr(static_cast<size_t>(B));
-  for (int i = 0; i < B; ++i) fr[i] = lwb::GmcFrameHost{frames[i].luma, frames[i].luma_pitch, frames[i].height, frames[i].width, 1};
-  return gmc_estimate_common("lwdetr_gmc_estimate_nv12", g, fr, B, stream_ids, motion, status, inliers, stream);
+  return gmc_call("lwdetr_gmc_estimate_nv12", g, frames, B, stream_ids, motion, status, inliers, stream, false);
 }
 
 int lwdetr_gmc_observe(lwdetr_gmc* g, const lwdetr_frame* frames, int B, const int32_t* stream_ids, void* stream) {
-  if (!g || !frames || !stream_ids) return fail("lwdetr_gmc_observe: null pointer");
-  if (B < 1) return fail("lwdetr_gmc_observe: B must be >= 1");
-  std::vector<lwb::GmcFrameHost> fr(static_cast<size_t>(B));
-  for (int i = 0; i < B; ++i) fr[i] = lwb::GmcFrameHost{frames[i].data, frames[i].pitch_bytes, frames[i].height, frames[i].width, 0};
-  return gmc_estimate_common("lwdetr_gmc_observe", g, fr, B, stream_ids, nullptr, nullptr, nullptr, stream, true);
+  return gmc_call("lwdetr_gmc_observe", g, frames, B, stream_ids, nullptr, nullptr, nullptr, stream, true);
 }
 
 int lwdetr_gmc_observe_nv12(lwdetr_gmc* g, const lwdetr_frame_nv12* frames, int B, const int32_t* stream_ids, void* stream) {
-  if (!g || !frames || !stream_ids) return fail("lwdetr_gmc_observe_nv12: null pointer");
-  if (B < 1) return fail("lwdetr_gmc_observe_nv12: B must be >= 1");
-  std::vector<lwb::GmcFrameHost> fr(static_cast<size_t>(B));
-  for (int i = 0; i < B; ++i) fr[i] = lwb::GmcFrameHost{frames[i].luma, frames[i].luma_pitch, frames[i].height, frames[i].width, 1};
-  return gmc_estimate_common("lwdetr_gmc_observe_nv12", g, fr, B, stream_ids, nullptr, nullptr, nullptr, stream, true);
+  return gmc_call("lwdetr_gmc_observe_nv12", g, frames, B, stream_ids, nullptr, nullptr, nullptr, stream, true);
 }
 
 struct lwdetr_flow {
@@ -1022,15 +1008,13 @@ int lwdetr_track_flow(lwdetr_tracker* t, lwdetr_flow* flow, const double* motion
   if (err.empty()) err = check_ids(flow->table.num_streams, stream_ids, B);
   if (!err.empty()) return fail(fn + ": " + err);
   if (flow->state.device != t->state.device) return fail(fn + ": the tracker and the flow live on different devices");
-  lwb::DeviceGuard g(t->state.device);
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int e = lwb::flow_launch(flow->table, flow->gmc->table, t->table, B, stream_ids, st);
-  if (!e) e = lwb::track_flow_launch(t->table, t->params, flow->table, motion, t->reid.slot, B, stream_ids, max_out, out_ids, out_scores,
-                                     out_labels, out_boxes, out_index, counts, st);
-  if (!e) e = flow->state.mark(stream);
-  if (!e) e = t->state.mark(stream);
-  if (e) return cuda_fail(e, (fn + " launch").c_str());
-  return 0;
+  const auto run = [&](cudaStream_t st) {
+    int e = lwb::flow_launch(flow->table, flow->gmc->table, t->table, B, stream_ids, st);
+    if (!e) e = lwb::track_flow_launch(t->table, t->params, flow->table, motion, t->reid.slot, B, stream_ids, max_out, out_ids, out_scores,
+                                       out_labels, out_boxes, out_index, counts, st);
+    return e;
+  };
+  return flow->state.launch(fn, stream, run, &t->state);   // the devices are one: checked above
 }
 
 int lwdetr_flow_export(lwdetr_flow* f, int stream_id, int cap, float* seeds, float* fwd, float* bwd, int8_t* valid, double* fb,
