@@ -655,7 +655,8 @@ LWDETR_API int lwdetr_flow_export(lwdetr_flow* f, int stream_id, int cap, float*
  * lwdetr_zones_set: one stream's geometry from HOST arrays, lines [n_lines][4], polygons' vertex counts [n_polygons] and
  *   vertices [sum of counts][2]; replaces the geometry and clears the stream's records, counters and overflow (the frame
  *   count goes on).  A limit overrun, a non-finite coordinate or a zero-length line is an error and nothing changes.
- *   Synchronous: it waits for the object's last launch and nothing else on the device; not callable during a stream capture.
+ *   Synchronous: it waits for the object's last launch (an lwdetr_zones_update, _reset, or an lwdetr_annotate that read the
+ *   object) and nothing else on the device; not callable during a stream capture.
  * lwdetr_zones_reset: the n streams listed (HOST; ids distinct and in [0, num_streams), else an error and nothing happens)
  *   back to frame 1 with no records, zero counters and overflow; their geometry is kept.  Stream-ordered.
  * lwdetr_zones_update: one frame for each of B streams (stream_ids HOST, distinct and in [0, num_streams)); ids, labels int32
@@ -664,7 +665,8 @@ LWDETR_API int lwdetr_flow_export(lwdetr_flow* f, int stream_id, int cap, float*
  *   stream's polygons), events int32 [B, max_events, 5] (the first max_events of the frame's events in order, unused rows
  *   zero; may be NULL when max_events = 0) and event_counts int32 [B], the true number.  The counters count every event.
  *   All DEVICE; asynchronous, nothing allocated or copied per call, safe to capture in a CUDA graph.
- * lwdetr_zones_export: one stream, synchronous: it waits for the object's last launch and nothing else on the device.
+ * lwdetr_zones_export: one stream, synchronous: it waits for the object's last launch (as lwdetr_zones_set) and nothing else
+ *   on the device.
  *   frame_overflow = (frame, overflow); line_counts int32 [n_lines][num_classes + 1][2] and entries int32
  *   [n_polygons][num_classes + 1] (n_* of the stream's geometry: info = (n_lines, n_polygons, records)); then up to cap
  *   records in ascending id: lwdetr_zone_record with sides[l] in {-1, 0, +1} and entry[z] the entry frame (0 when
@@ -931,6 +933,97 @@ LWDETR_API int lwdetr_crop_select(const float* scores, const float* boxes, int B
                                   int32_t* frame_of, int32_t* entry, float* sel_boxes, int32_t* count, void* stream);
 LWDETR_API int lwdetr_scatter_rows(int etype, const void* rows, int ld_rows, int D, const int32_t* entry, const int32_t* count, int N,
                                    void* out, int num_out, void* stream);
+
+/* Drawing into the frames on the device (what DeepStream's nvdsosd and supervision's box, label, zone and pixelate annotators
+ * do): boxes, labels, zones and their counts, and privacy pixelation, written IN PLACE into RGB or NV12 frames, so that
+ * lwdetr_forward_frames -> lwdetr_query_best -> lwdetr_track -> lwdetr_zones_update -> lwdetr_annotate stays one chain with
+ * no read-back, capturable in one CUDA graph.  tools/annotate_spec.py restates this contract in numpy.
+ * lwdetr_annotate WRITES the pixels of the frames it is given, through the `data` (RGB) or `luma` / `chroma` (NV12) pointers
+ * of the descriptors: their `const` is the promise of the readers (the forward, crops, motion), not of this call.  dst_h and
+ * dst_w are ignored.  A byte that no primitive below covers is never written: not the pitch padding, not the rest of a
+ * larger surface around a frame.
+ * The object: lwdetr_annotator_create(num_classes in [1, 1024]) makes one device allocation on the current device (palette,
+ *   class names, privacy mask and a fixed scratch for 32 frames of 1024 entries, reused group after group in stream order).
+ *   Synchronous.  lwdetr_annotator_set_option (name, value), validated, takes effect at the next lwdetr_annotate (a CUDA
+ *   graph keeps the options it was captured with):
+ *     "thickness" [1, 32], default 2; "text_scale" [1, 8], default 2; "box_fill_alpha" [0, 256], default 0;
+ *     "label" mask of LWDETR_LABEL_NAME | _ID | _SCORE, default all (0: no labels); "zone_fill_alpha" [0, 256], default 64;
+ *     "zone_thickness" [1, 32], default 2; "privacy_block" 2, 4, 8, 16, 32 or 64, default 16.
+ *   lwdetr_annotator_set_names: '\n'-separated class names for classes 0, 1, ... (at most num_classes, each at most 31
+ *   characters; more is an error); a class without a name (or an empty one) is named by its id in decimal, the default for
+ *   all.  lwdetr_annotator_set_palette: n in [1, 256] RGB triples.  Default palette (n = 16): (230,25,75) (60,180,75)
+ *   (255,225,25) (0,130,200) (245,130,48) (145,30,180) (70,240,240) (240,50,230) (210,245,60) (250,190,212) (0,128,128)
+ *   (220,190,255) (170,110,40) (255,250,200) (128,0,0) (170,255,195).  lwdetr_annotator_set_privacy: the labels in
+ *   [0, num_classes) whose boxes are pixelated instead of drawn (n = 0: none, the default).  The three setters replace the
+ *   table, synchronously: they wait for the object's last lwdetr_annotate and nothing else; not during a stream capture.
+ *   Replays of a captured graph read the tables as they are.
+ * lwdetr_annotate / _nv12: frames a HOST array of B descriptors, B in [1, 1024], sides in [8, 8192], any pitch and alignment,
+ *   odd sizes allowed (the caller may reuse the array on return).  Entries [B, k], k in [1, 1024], DEVICE: scores fp32,
+ *   labels int32, boxes fp32 xyxy [B, k, 4] in frame pixels; ids int32 or NULL; counts int32 [B] or NULL (k each).
+ *   lwdetr_track's outputs as they are (k = max_out); with ids NULL, lwdetr_query_best / lwdetr_postprocess /
+ *   lwdetr_tile_merge output.  zones (may be NULL) with stream_ids (HOST, one per frame, in [0, zones' num_streams)): each
+ *   frame also gets its stream's lines and polygons, the line totals read from the zones object's device counters, and with
+ *   occupancy (DEVICE int32 [B, 32], lwdetr_zones_update's output; may be NULL: no occupancy text) each polygon's count.
+ *   The zones object must live on the annotator's device, and its calls must be ordered on the annotator's CUDA stream;
+ *   lwdetr_zones_set and _export wait for the call, which reads the object.  Calls on one annotator must be ordered on one
+ *   CUDA stream.  Asynchronous, nothing allocated or copied per call, safe to
+ *   capture in a CUDA graph.
+ * The drawing contract, per frame (h x w); float64 operations are rounded each on its own, in the order written:
+ *   entry j is drawn when j < count, score >= score_threshold and its rectangle is valid: lwdetr_crops' rule,
+ *     [clamp(floor(x1), 0, w), clamp(floor(x2), 0, w)) x [.. y ..), non-empty and from finite coordinates.
+ *   colour: palette[i mod n] (non-negative remainder) with i = id, or the label when ids is NULL, or the line / polygon index.
+ *   primitives, each with a colour, an alpha a in [0, 256] and a set of covered pixels (those in the frame only):
+ *     rect fill: the rectangle; outline: the rectangle's pixels with x < x0 + t, x >= x1 - t, y < y0 + t or y >= y1 - t
+ *       (t = thickness);
+ *     segment A-B, radius r = t / 2 (t = zone_thickness), pixel centre (cx, cy) = (x + 0.5, y + 0.5): dx = bx - ax,
+ *       dy = by - ay, L2 = dx * dx + dy * dy, qx = cx - ax, qy = cy - ay, u = qx * dx + qy * dy; d2 = qx * qx + qy * qy when
+ *       u <= 0, else (cx - bx)^2 + (cy - by)^2 (each square a product) when u >= L2, else c * c / L2 with
+ *       c = dx * qy - dy * qx; covered when d2 <= r * r;
+ *     polygon fill: pixel centres inside by lwdetr_zones' even-odd rule, exactly (what is drawn inside is what Zones counts);
+ *     text at origin (ox, oy), scale s: character i of the string occupies the cell [ox + 6 s i, ox + 6 s (i + 1)) x
+ *       [oy, oy + 8 s); pixel (x, y) of it is glyph pixel (gx, gy) = ((x - ox) / s - 6 i, (y - oy) / s) of the 5x7 font of
+ *       csrc/font5x7.cuh (characters outside 0x20..0x7E drawn as '?'); a text background is the rect fill of all cells.
+ *   blending of colour c: RGB, per channel, out = (src * (256 - a) + c * a + 128) >> 8.  NV12: c is converted to Y'CbCr by
+ *     the frame's colorspace, Y = clamp(((kYR R + kYG G + kYB B + 2^15) >> 16) + o, 0, 255) with o = 16 (limited range) or
+ *     0 (full), Cb and Cr likewise with their rows and o = 128:
+ *       colorspace               kYR    kYG    kYB    kUR     kUG     kUB    kVR    kVG     kVB
+ *       LWDETR_CSC_BT601_LIMITED 16840  33058  6405   -9713   -19068  28781  28781  -24110  -4671
+ *       LWDETR_CSC_BT709_LIMITED 11966  40254  4064   -6596   -22189  28784  28784  -26145  -2639
+ *       LWDETR_CSC_BT601_FULL    19595  38470  7471   -11058  -21710  32768  32768  -27439  -5329
+ *       LWDETR_CSC_BT709_FULL    13933  46871  4732   -7509   -25259  32768  32768  -29763  -3005
+ *     (round(2^16 m) of the inverse m of each lwdetr_frame_nv12 row).  Luma is blended per covered pixel; a chroma sample with
+ *     n > 0 of its in-frame 2x2 luma pixels covered by the primitive is blended with a' = (a * n + 2) >> 2, per primitive.
+ *   privacy: the covered set is the union of the rectangles of the drawn entries whose label is in the privacy set; with
+ *     P = privacy_block, the blocks of P x P pixels on the frame's grid (cut by its edges); each covered pixel takes the
+ *     rounded mean (sum + cnt / 2) / cnt of its block's cnt covered pixels, per channel; NV12 luma the same, chroma on the
+ *     chroma grid with blocks of P / 2 samples, a sample covered when its top-left luma pixel is.  Those entries get no box
+ *     and no label.
+ *   labels (option "label" != 0): the parts name (or the class id in decimal), "#id" (with ids) and the score as "0.xx" /
+ *     "1.00" from p = clamp(floor(score * 100 + 0.5), 0, 100) in fp32, in that order, joined by one space.  A text of n
+ *     characters at scale s is 6 s n x 8 s; its origin is (x0, y0 - 8 s) above the rectangle's top-left corner, or (x0, y0)
+ *     just inside the top edge when y0 - 8 s < 0.  Background: the colour, opaque; text: black when the colour's grey
+ *     (9798 R + 19235 G + 3735 B + 16384) >> 15 is at least 128, else white, opaque.
+ *   zone texts: "in N out M" of each line (N, M its in and out totals over all classes) with its origin at
+ *     (floor((ax + bx) * 0.5), floor((ay + by) * 0.5)); the occupancy of each polygon in decimal at (floor(x0), floor(y0)) of
+ *     its first vertex (origins clamped to [-2^20, 2^20]); background and text as the labels', with the line's or polygon's colour.
+ *   painter's order: 1. privacy; 2. polygon fills (zone_fill_alpha) in polygon order; 3. polygon outlines (each edge i ->
+ *     i + 1 a segment of its own, in order), then lines (opaque); 4. box fills (box_fill_alpha; none at 0) in entry order,
+ *     then box outlines (opaque) in entry order; 5. labels in entry order (background, then text); 6. line texts, then
+ *     polygon texts. */
+enum { LWDETR_LABEL_NAME = 1, LWDETR_LABEL_ID = 2, LWDETR_LABEL_SCORE = 4 };
+typedef struct lwdetr_annotator lwdetr_annotator;
+LWDETR_API int lwdetr_annotator_create(int num_classes, lwdetr_annotator** out);
+LWDETR_API void lwdetr_annotator_destroy(lwdetr_annotator* a);
+LWDETR_API int lwdetr_annotator_set_option(lwdetr_annotator* a, const char* name, int value);
+LWDETR_API int lwdetr_annotator_set_names(lwdetr_annotator* a, const char* names);
+LWDETR_API int lwdetr_annotator_set_palette(lwdetr_annotator* a, const uint8_t* rgb, int n);
+LWDETR_API int lwdetr_annotator_set_privacy(lwdetr_annotator* a, const int32_t* classes, int n);
+LWDETR_API int lwdetr_annotate(lwdetr_annotator* a, const lwdetr_frame* frames, int B, const int32_t* ids, const float* scores,
+                               const int32_t* labels, const float* boxes, const int32_t* counts, int k, float score_threshold,
+                               lwdetr_zones* zones, const int32_t* stream_ids, const int32_t* occupancy, void* stream);
+LWDETR_API int lwdetr_annotate_nv12(lwdetr_annotator* a, const lwdetr_frame_nv12* frames, int B, const int32_t* ids, const float* scores,
+                                    const int32_t* labels, const float* boxes, const int32_t* counts, int k, float score_threshold,
+                                    lwdetr_zones* zones, const int32_t* stream_ids, const int32_t* occupancy, void* stream);
 
 /* Multi-GPU init (SURVEY.md 8e): ONE ncclBroadcast of the packed weight arena from rank `root`, stream-ordered on
  * `stream`; the only collective of the path (images shard across ranks as independent replicas, nothing on the hot path).

@@ -889,6 +889,126 @@ class Zones(_DeviceObject):
                     entry=raw["entry"][:, :Z].copy())
 
 
+LABEL_NAME, LABEL_ID, LABEL_SCORE = 1, 2, 4
+ANNOTATOR_OPTIONS = ("thickness", "text_scale", "box_fill_alpha", "label", "zone_fill_alpha", "zone_thickness", "privacy_block")
+
+
+class Annotator(_DeviceObject):
+    """Draws detections, tracks and zones into RGB or NV12 frames in place on the device, with privacy pixelation
+    (lwdetr_annotator_* / lwdetr_annotate, the contract in include/lwdetr_b200.h, restated in tools/annotate_spec.py).
+    names: class names (list, at most 31 ASCII characters each; default the class id); palette: RGB triples (1 to 256;
+    default the header's 16); privacy: labels whose boxes are pixelated instead of drawn; options: thickness, text_scale,
+    box_fill_alpha, label (a mask of LABEL_*), zone_fill_alpha, zone_thickness, privacy_block.  All calls of one object must
+    run on one CUDA stream (the current one at each call)."""
+
+    DESTROY = "lwdetr_annotator_destroy"
+
+    def __init__(self, num_classes, names=None, palette=None, privacy=(), device=None, **options):
+        import torch
+        bad = set(options) - set(ANNOTATOR_OPTIONS)
+        if bad:
+            raise RuntimeError("Annotator: unknown options %s" % ", ".join(sorted(bad)))
+        self.num_classes = int(num_classes)
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self._t = _vp()
+        with torch.cuda.device(self.device):
+            check(lib().lwdetr_annotator_create(self.num_classes, ctypes.byref(self._t)), "lwdetr_annotator_create")
+        for n, v in options.items():
+            self.set_option(n, v)
+        if names is not None:
+            self.set_names(names)
+        if palette is not None:
+            self.set_palette(palette)
+        if privacy:
+            self.set_privacy(privacy)
+
+    def set_option(self, name, value):
+        check(lib().lwdetr_annotator_set_option(self._t, name.encode(), int(value)), "lwdetr_annotator_set_option")
+
+    def set_names(self, names):
+        """Synchronous (waits for this object's last draw only)."""
+        names = list(names)
+        if any("\n" in n for n in names):
+            raise RuntimeError("Annotator.set_names: a name cannot hold a newline")
+        check(lib().lwdetr_annotator_set_names(self._t, "\n".join(names).encode("ascii", "replace")), "lwdetr_annotator_set_names")
+
+    def set_palette(self, palette):
+        import numpy as np
+        arr = np.ascontiguousarray(np.asarray(palette, np.uint8).reshape(-1, 3))
+        check(lib().lwdetr_annotator_set_palette(self._t, arr.ctypes.data_as(_vp), len(arr)), "lwdetr_annotator_set_palette")
+
+    def set_privacy(self, classes):
+        arr, n = self._ids(classes)
+        check(lib().lwdetr_annotator_set_privacy(self._t, ctypes.cast(arr, _vp), n), "lwdetr_annotator_set_privacy")
+
+    def annotate(self, frames, scores, labels, boxes, ids=None, counts=None, streams=None, zones=None, occupancy=None,
+                 score_threshold=0.0, colorspace=None):
+        """lwdetr_annotate(_nv12) on device arrays as they are: scores fp32 [B, k], labels int32 [B, k], boxes fp32 [B, k, 4],
+        ids int32 [B, k] or None, counts int32 [B] or None, occupancy int32 [B, 32] or None (Zones.update's), all CUDA; the
+        frames (RGB or NV12 as capi.Frames takes them, CUDA, never copied) are drawn in place.  streams: the frames' stream
+        ids in zones (default range(B)).  Stream-ordered, no synchronisation; graph-safe."""
+        import torch
+        fb = frames if isinstance(frames, Frames) else Frames(frames, self.device, colorspace)
+        if fb.device != self.device:
+            raise RuntimeError("Annotator: frames on %s, the annotator on %s" % (fb.device, self.device))
+        B = len(fb.items)
+        if scores.dim() != 2 or scores.shape[0] != B:
+            raise RuntimeError("Annotator: scores must be [%d, k], got %s" % (B, tuple(scores.shape)))
+        k = scores.shape[1]
+        shapes = [(labels, (B, k)), (boxes, (B, k, 4))] + [(t, sh) for t, sh in ((ids, (B, k)), (counts, (B,)), (occupancy, (B, 32)))
+                                                           if t is not None]
+        for t, sh in shapes:
+            if tuple(t.shape) != sh:
+                raise RuntimeError("Annotator: expected %s, got %s" % (sh, tuple(t.shape)))
+        args = [t if t is None else t.to(device=self.device, dtype=dt).contiguous()
+                for t, dt in ((ids, torch.int32), (scores, torch.float32), (labels, torch.int32), (boxes, torch.float32),
+                              (counts, torch.int32), (occupancy, torch.int32))]
+        sids = None
+        if zones is not None:
+            arr, n = self._ids(range(B) if streams is None else streams)
+            if n != B:
+                raise RuntimeError("Annotator: %d stream ids for %d frames" % (n, B))
+            sids = ctypes.cast(arr, _vp)
+        name = "lwdetr_annotate_nv12" if fb.nv12 else "lwdetr_annotate"
+        ids_, sc, lab, bx, cn, occ = args
+        check(getattr(lib(), name)(self._t, fb.descs(fb.sizes), B, ptr(ids_), ptr(sc), ptr(lab), ptr(bx), ptr(cn), k,
+                                   float(score_threshold), zones._t if zones is not None else None, sids, ptr(occ),
+                                   stream_ptr(self.device)), name)
+
+    def draw(self, frames, dets, streams=None, zones=None, score_threshold=0.0, colorspace=None):
+        """Draws detect() / detect_tiled() / track()'s per-frame lists into the frames in place: each dict's "scores",
+        "labels", "boxes" and, when present, "ids" (colour by track id and "#id" in the label; otherwise colour by class)
+        and "occupancy" (with zones).  The lists are packed on the device; nothing is read back."""
+        import torch
+        fb = frames if isinstance(frames, Frames) else Frames(frames, self.device, colorspace)
+        B = len(fb.items)
+        if len(dets) != B:
+            raise RuntimeError("Annotator.draw: %d detection lists for %d frames" % (len(dets), B))
+        dev = self.device
+        n = [int(d["scores"].shape[0]) for d in dets]
+        k = max(max(n), 1)
+        if k > 1024:
+            raise RuntimeError("Annotator.draw: at most 1024 entries per frame, got %d" % k)
+        with_ids = all("ids" in d for d in dets)
+        scores = torch.zeros(B, k, device=dev, dtype=torch.float32)
+        labels = torch.zeros(B, k, device=dev, dtype=torch.int32)
+        boxes = torch.zeros(B, k, 4, device=dev, dtype=torch.float32)
+        ids = torch.zeros(B, k, device=dev, dtype=torch.int32) if with_ids else None
+        for b, d in enumerate(dets):
+            c = n[b]
+            scores[b, :c] = d["scores"]
+            labels[b, :c] = d["labels"].to(torch.int32)
+            boxes[b, :c] = d["boxes"].reshape(-1, 4)
+            if with_ids:
+                ids[b, :c] = d["ids"].to(torch.int32)
+        counts = torch.tensor(n, dtype=torch.int32).to(dev)
+        occ = None
+        if zones is not None and all("occupancy" in d for d in dets):
+            occ = torch.stack([d["occupancy"].to(device=dev, dtype=torch.int32) for d in dets])
+        self.annotate(fb, scores, labels, boxes, ids=ids, counts=counts, streams=streams, zones=zones, occupancy=occ,
+                      score_threshold=score_threshold)
+
+
 def layernorm_e4m3(x, eps=1e-6):
     """x: CUDA fp16 [rows, C] (any row stride) -> (e4m3 codes uint8 [rows, C], fp32 row scales [rows]); see
     lwdetr_layernorm_e4m3."""

@@ -15,6 +15,7 @@
 #include <type_traits>
 #include <vector>
 
+#include "annotate.h"
 #include "attn.h"
 #include "crops.h"
 #include "engine.h"
@@ -150,6 +151,16 @@ struct DeviceState {
     cudaError_t e = cudaStreamWaitEvent(copy, done, 0);
     for (size_t i = 0; i < parts.size() && e == cudaSuccess; ++i)
       if (parts[i].bytes) e = cudaMemcpyAsync(parts[i].dst, parts[i].src, parts[i].bytes, cudaMemcpyDeviceToHost, copy);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(copy);
+    return e;
+  }
+
+  // host-to-device copies once the last marked launch is done, all on `copy`, waited for once
+  cudaError_t write(const std::vector<Copy>& parts) const {
+    lwb::DeviceGuard g(device);
+    cudaError_t e = cudaStreamWaitEvent(copy, done, 0);
+    for (size_t i = 0; i < parts.size() && e == cudaSuccess; ++i)
+      if (parts[i].bytes) e = cudaMemcpyAsync(parts[i].dst, parts[i].src, parts[i].bytes, cudaMemcpyHostToDevice, copy);
     if (e == cudaSuccess) e = cudaStreamSynchronize(copy);
     return e;
   }
@@ -771,6 +782,115 @@ int lwdetr_zones_export(lwdetr_zones* z, int stream_id, int32_t frame_overflow[2
   return 0;
 }
 
+// the annotator's default palette (include/lwdetr_b200.h)
+static const uint8_t kAnnPalette[16][3] = {{230, 25, 75},   {60, 180, 75},  {255, 225, 25},  {0, 130, 200},  {245, 130, 48}, {145, 30, 180},
+                                           {70, 240, 240},  {240, 50, 230}, {210, 245, 60},  {250, 190, 212}, {0, 128, 128},  {220, 190, 255},
+                                           {170, 110, 40},  {255, 250, 200}, {128, 0, 0},    {170, 255, 195}};
+
+struct lwdetr_annotator {
+  lwb::AnnTable table;
+  lwb::AnnOptions options;
+  DeviceState state;
+};
+
+int lwdetr_annotator_create(int num_classes, lwdetr_annotator** out) {
+  if (!out) return fail("lwdetr_annotator_create: null pointer");
+  if (num_classes < 1 || num_classes > lwb::ANN_CLASSES) return fail("lwdetr_annotator_create: num_classes must be in [1, 1024]");
+  std::unique_ptr<lwdetr_annotator> a(new (std::nothrow) lwdetr_annotator{});
+  if (!a) return fail("lwdetr_annotator_create: out of memory");
+  a->options = lwb::AnnOptions{2, 2, 0, LWDETR_LABEL_NAME | LWDETR_LABEL_ID | LWDETR_LABEL_SCORE, 64, 2, 16};
+  lwb::AnnTable& t = a->table;
+  t.num_classes = num_classes;
+  const size_t nc = static_cast<size_t>(num_classes);
+  const int32_t n16 = 16;
+  const auto layout = [&](Carver& c) {
+    c.take(t.palette, lwb::ANN_PALETTE * 3);
+    c.take(t.palette_n, 1);
+    c.take(t.names, nc * lwb::ANN_NAME);
+    c.take(t.privacy, nc);
+    c.take(t.prims, static_cast<size_t>(lwb::ANN_GROUP) * lwb::ANN_PRIMS);
+    c.take(t.nprims, static_cast<size_t>(lwb::ANN_GROUP) * 2);
+    c.take(t.texts, static_cast<size_t>(lwb::ANN_GROUP) * lwb::ANN_TEXTS * lwb::ANN_TEXT);
+  };
+  const auto init = [&] {
+    cudaError_t e = cudaMemcpyAsync(t.palette, kAnnPalette, sizeof(kAnnPalette), cudaMemcpyHostToDevice, a->state.copy);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(t.palette_n, &n16, sizeof(n16), cudaMemcpyHostToDevice, a->state.copy);
+    if (e == cudaSuccess) e = cudaMemsetAsync(t.names, 0, nc * lwb::ANN_NAME, a->state.copy);     // every class named by its id
+    if (e == cudaSuccess) e = cudaMemsetAsync(t.privacy, 0, nc, a->state.copy);
+    return e;
+  };
+  if (int rc = a->state.create("lwdetr_annotator_create", layout, init)) return rc;
+  *out = a.release();
+  return 0;
+}
+
+void lwdetr_annotator_destroy(lwdetr_annotator* a) { delete a; }
+
+int lwdetr_annotator_set_option(lwdetr_annotator* a, const char* name, int value) {
+  if (!a || !name) return fail("lwdetr_annotator_set_option: null pointer");
+  const std::string n(name), fn = "lwdetr_annotator_set_option: ";
+  lwb::AnnOptions& o = a->options;
+  const auto in = [&](int lo, int hi, int* dst) {
+    if (value < lo || value > hi) return fail(fn + n + " must be in [" + std::to_string(lo) + ", " + std::to_string(hi) + "], got " + std::to_string(value));
+    *dst = value;
+    return 0;
+  };
+  if (n == "thickness") return in(1, 32, &o.thickness);
+  if (n == "text_scale") return in(1, 8, &o.text_scale);
+  if (n == "box_fill_alpha") return in(0, 256, &o.box_fill_alpha);
+  if (n == "label") return in(0, 7, &o.label);
+  if (n == "zone_fill_alpha") return in(0, 256, &o.zone_fill_alpha);
+  if (n == "zone_thickness") return in(1, 32, &o.zone_thickness);
+  if (n == "privacy_block") {
+    if (value < 2 || value > 64 || (value & (value - 1))) return fail(fn + "privacy_block must be 2, 4, 8, 16, 32 or 64, got " + std::to_string(value));
+    o.privacy_block = value;
+    return 0;
+  }
+  return fail(fn + "unknown option " + n + " (thickness, text_scale, box_fill_alpha, label, zone_fill_alpha, zone_thickness, privacy_block)");
+}
+
+int lwdetr_annotator_set_names(lwdetr_annotator* a, const char* names) {
+  if (!a || !names) return fail("lwdetr_annotator_set_names: null pointer");
+  const lwb::AnnTable& t = a->table;
+  std::vector<char> tab(static_cast<size_t>(t.num_classes) * lwb::ANN_NAME, 0);
+  int cls = 0, len = 0;
+  for (const char* c = names; *c; ++c) {
+    if (*c == '\n') {
+      ++cls;
+      len = 0;
+      continue;
+    }
+    if (cls >= t.num_classes) return fail("lwdetr_annotator_set_names: more than num_classes = " + std::to_string(t.num_classes) + " names");
+    if (len == lwb::ANN_NAME - 1) return fail("lwdetr_annotator_set_names: the name of class " + std::to_string(cls) + " is longer than 31 characters");
+    tab[static_cast<size_t>(cls) * lwb::ANN_NAME + len++] = *c;
+  }
+  if (cudaError_t e = a->state.write({{t.names, tab.data(), tab.size()}})) return cuda_fail(e, "lwdetr_annotator_set_names");
+  return 0;
+}
+
+int lwdetr_annotator_set_palette(lwdetr_annotator* a, const uint8_t* rgb, int n) {
+  if (!a || !rgb) return fail("lwdetr_annotator_set_palette: null pointer");
+  if (n < 1 || n > lwb::ANN_PALETTE) return fail("lwdetr_annotator_set_palette: n must be in [1, 256]");
+  const int32_t nn = n;
+  if (cudaError_t e = a->state.write({{a->table.palette, rgb, 3 * static_cast<size_t>(n)}, {a->table.palette_n, &nn, sizeof(nn)}}))
+    return cuda_fail(e, "lwdetr_annotator_set_palette");
+  return 0;
+}
+
+int lwdetr_annotator_set_privacy(lwdetr_annotator* a, const int32_t* classes, int n) {
+  if (!a || (n > 0 && !classes)) return fail("lwdetr_annotator_set_privacy: null pointer");
+  if (n < 0) return fail("lwdetr_annotator_set_privacy: n must be >= 0");
+  const lwb::AnnTable& t = a->table;
+  std::vector<uint8_t> mask(static_cast<size_t>(t.num_classes), 0);
+  for (int i = 0; i < n; ++i) {
+    if (classes[i] < 0 || classes[i] >= t.num_classes)
+      return fail("lwdetr_annotator_set_privacy: class " + std::to_string(classes[i]) + " outside [0, " + std::to_string(t.num_classes) + ")");
+    mask[static_cast<size_t>(classes[i])] = 1;
+  }
+  if (cudaError_t e = a->state.write({{t.privacy, mask.data(), mask.size()}})) return cuda_fail(e, "lwdetr_annotator_set_privacy");
+  return 0;
+}
+
 struct lwdetr_gmc {
   lwb::GmcTable table;
   DeviceState state;
@@ -1222,6 +1342,37 @@ static int resize_patches(const char* fn, int dtype, const F* frames, int B, int
   return 0;
 }
 
+// lwdetr_annotate and lwdetr_annotate_nv12
+template <typename F>
+static int annotate_call(const char* fn, lwdetr_annotator* a, const F* frames, int B, const int32_t* ids, const float* scores,
+                         const int32_t* labels, const float* boxes, const int32_t* counts, int k, float score_threshold, lwdetr_zones* zones,
+                         const int32_t* stream_ids, const int32_t* occupancy, void* stream) {
+  const std::string f(fn);
+  if (!a || !frames || !scores || !labels || !boxes || (zones && !stream_ids)) return fail(f + ": null pointer");
+  if (B < 1 || B > lwb::ANN_FRAMES) return fail(f + ": B must be in [1, 1024]");
+  if (k < 1 || k > lwb::ANN_K) return fail(f + ": k must be in [1, 1024]");
+  if (score_threshold != score_threshold) return fail(f + ": score_threshold is NaN");
+  if (occupancy && !zones) return fail(f + ": occupancy needs zones");
+  if (zones && zones->state.device != a->state.device) return fail(f + ": the annotator and the zones object live on different devices");
+  if (zones)
+    for (int b = 0; b < B; ++b)
+      if (stream_ids[b] < 0 || stream_ids[b] >= zones->table.num_streams)
+        return fail(f + ": stream id " + std::to_string(stream_ids[b]) + " outside [0, " + std::to_string(zones->table.num_streams) + ")");
+  const uintptr_t mis = reinterpret_cast<uintptr_t>(ids) | reinterpret_cast<uintptr_t>(scores) | reinterpret_cast<uintptr_t>(labels) |
+                        reinterpret_cast<uintptr_t>(boxes) | reinterpret_cast<uintptr_t>(counts) | reinterpret_cast<uintptr_t>(occupancy);
+  if (mis % 4) return fail(f + ": ids, scores, labels, boxes, counts and occupancy must be 4-byte aligned");
+  std::string err;
+  if (lwb::crop_frames_check(frames, B, &err)) return fail(f + ": " + err);
+  lwb::AnnCall c = {};
+  c.ids = ids; c.scores = scores; c.labels = labels; c.boxes = boxes; c.counts = counts; c.k = k; c.threshold = score_threshold;
+  c.zones = zones ? &zones->table : nullptr;
+  c.streams = stream_ids;
+  c.occupancy = occupancy;
+  // the kernels read the zones object's geometry and counters, so its later set / export waits for this launch too
+  return a->state.launch(f, stream, [&](cudaStream_t st) { return lwb::annotate_launch(a->table, a->options, frames, B, c, st); },
+                         zones ? &zones->state : nullptr);
+}
+
 // lwdetr_crops and lwdetr_crops_nv12
 template <typename F>
 static int crops_call(const char* fn, const F* frames, int B, const float* boxes, const int32_t* frame_index, int N, const int32_t* count,
@@ -1293,6 +1444,20 @@ int lwdetr_scatter_rows(int etype, const void* rows, int ld_rows, int D, const i
   const int e = lwb::scatter_rows_launch(etype, rows, ld_rows, D, entry, count, N, out, num_out, static_cast<cudaStream_t>(stream));
   if (e) return cuda_fail(e, "lwdetr_scatter_rows launch");
   return 0;
+}
+
+int lwdetr_annotate(lwdetr_annotator* a, const lwdetr_frame* frames, int B, const int32_t* ids, const float* scores, const int32_t* labels,
+                    const float* boxes, const int32_t* counts, int k, float score_threshold, lwdetr_zones* zones, const int32_t* stream_ids,
+                    const int32_t* occupancy, void* stream) {
+  return annotate_call("lwdetr_annotate", a, frames, B, ids, scores, labels, boxes, counts, k, score_threshold, zones, stream_ids, occupancy,
+                       stream);
+}
+
+int lwdetr_annotate_nv12(lwdetr_annotator* a, const lwdetr_frame_nv12* frames, int B, const int32_t* ids, const float* scores,
+                         const int32_t* labels, const float* boxes, const int32_t* counts, int k, float score_threshold, lwdetr_zones* zones,
+                         const int32_t* stream_ids, const int32_t* occupancy, void* stream) {
+  return annotate_call("lwdetr_annotate_nv12", a, frames, B, ids, scores, labels, boxes, counts, k, score_threshold, zones, stream_ids,
+                       occupancy, stream);
 }
 
 int lwdetr_forward_frames(lwdetr_handle* h, const lwdetr_frame* frames, const float mean[3], const float std[3], int B, int height,

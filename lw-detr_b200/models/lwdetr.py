@@ -207,7 +207,7 @@ class LWDETR(nn.Module):
     @torch.no_grad()
     def track(self, frames, tracker, streams=None, size=None, fit="stretch", short_side=None, max_side=None, colorspace=None,
               max_out=None, motion=None, appearance=False, reid=None, reid_size=(256, 128), reid_filter="bilinear", reid_mean=None,
-              reid_std=None, reid_normalize=True, zones=None, detect_every=1, flow=None):
+              reid_std=None, reid_normalize=True, zones=None, detect_every=1, flow=None, annotate=None):
         """Multi-object tracking of video streams: frames (RGB or NV12, taken exactly as detect() takes them) run as one
         forward; each query gives one detection, its best class (capi.query_best, boxes in the frame's original pixels);
         then capi.Tracker `tracker` (ByteTrack on the device, include/lwdetr_b200.h) updates each frame's stream.
@@ -243,6 +243,10 @@ class LWDETR(nn.Module):
         streams so that the forward's batch keeps its size from call to call.  Keyframes take the path above; the other
         frames go MotionEstimator.estimate (with motion=) or observe, then BoxFlow.propagate.  zones= follows both kinds of
         frame, appearance= and reid= the keyframes only; on a flow frame "queries" is -1.  detect_every=1 is the path above.
+        annotate: a capi.Annotator; after each round's tracker (and zones) update it draws that round's tracks into the
+        round's frames in place, from the device outputs as they are (Annotator.annotate: ids, labels and scores, and with
+        zones= the lines, polygons, line totals and occupancy).  It adds no synchronisation; on flow frames it draws the
+        flow's tracks.  The returned lists are the same with and without it.
         How ByteTrack's thresholds (tuned on YOLOX scores) suit LW-DETR's score distribution, and whether the decoder's features tell identities apart on real footage, in MOTA / IDF1 / HOTA, is
         not measured here."""
         if self.training:
@@ -333,6 +337,9 @@ class LWDETR(nn.Module):
                     inside, occupancy, events, n_ev = zones.update(got[0], got[2], got[3], got[5], ids)
                     zo = (inside.long() & 0xFFFFFFFF, occupancy, events)      # the uint32 masks widened once per round
                     ev_counts.append(n_ev)
+                if annotate is not None:
+                    annotate.annotate(fb.select(rows), got[1], got[2], got[3], ids=got[0], counts=got[5], streams=ids, zones=zones,
+                                      occupancy=None if zones is None else occupancy)
                 for j, i in enumerate(rows):
                     res[i] = (got, zo, j)
         both = torch.cat(counts + ev_counts).cpu().tolist()     # track and event counts in one read-back
