@@ -699,6 +699,72 @@ LWDETR_API int lwdetr_zones_update(lwdetr_zones* z, const int32_t* ids, const in
 LWDETR_API int lwdetr_zones_export(lwdetr_zones* z, int stream_id, int32_t frame_overflow[2], int32_t info[3], int32_t* line_counts,
                                    int32_t* entries, lwdetr_zone_record* records, int cap);
 
+/* Ground-plane position, velocity and speed of each track per camera stream, on the tracker's outputs (what supervision's
+ * speed-estimation example and the road-analytics stages of DeepStream-style pipelines compute after a tracker).  The C
+ * composition per batch of frames: ... -> lwdetr_track (or _ex / _reid / lwdetr_track_flow) -> lwdetr_zones_update ->
+ * lwdetr_speed_update on the same out_ids, out_boxes and counts with the same stream_ids, on the same CUDA stream; nothing
+ * is read back in between, so the chain can be captured in one CUDA graph.  Calls on one speed object must be ordered on
+ * one CUDA stream.  tools/speed_spec.py restates this contract in numpy.
+ * Per stream: a 3x3 float64 homography H (row-major, h0..h8) from frame pixels to ground units (default the identity:
+ *   pixels and pixels per second); a frame counter from 1; the last timestamp t_last (-inf at first); overflow and
+ *   clock-error counters; up to capacity records, one per track id, each a ring of its last `window` samples (t, x, y),
+ *   x and y the track's anchor in frame PIXELS (float64).  The ring keeps pixels, so lwdetr_speed_set can replace H
+ *   without dropping any history: every estimate projects the ring with the current H.  H is fixed: it describes a still
+ *   camera over a ground plane (with lwdetr_track_ex's moving cameras it has no meaning).
+ * Parameters (lwdetr_speed_create): capacity in [1, 4096] (default 1024), window in [2, 64] (default 30: one second at
+ *   30 fps), min_samples in [2, window] (default 15), forget_after >= 0 (default 30), anchor in [0, 9) (default
+ *   LWDETR_ANCHOR_BOTTOM_CENTER, the ground-contact point; the zones' anchor rule), frame_rate finite and > 0 (default 30).
+ * Everything is float64 with each operation rounded on its own (no FMA), in the order written; outputs are rounded to
+ *   fp32 once at the end.
+ * Projection of (x, y): w = (h6 * x + h7 * y) + h8, X = ((h0 * x + h1 * y) + h2) / w, Y = ((h3 * x + h4 * y) + h5) / w.
+ *   The point is valid iff w > 0 and X and Y are finite: points on or beyond the horizon are invalid, so H must give
+ *   w > 0 on the ground (capi.homography normalises the sign).
+ * Time: timestamps DEVICE float64 [B] in seconds, or NULL: then t = frame / frame_rate, frame the stream's own update
+ *   count, so a stream whose caller skips real frames runs slow.  A frame whose t is not finite or not greater than the
+ *   stream's t_last adds no samples; it is otherwise a normal frame, and adds 1 to the stream's clock errors.  Else
+ *   t_last = t.
+ * A frame of a stream (a stream absent from a call does not advance):
+ *   - entries at index >= min(counts[b], max_out), with id <= 0 or a non-finite box are absent; a repeated id's later
+ *     entries are ignored (the zones' rule);
+ *   - present tracks in input order: a track without a record takes one if the stream holds fewer than capacity records
+ *     (else it is not recorded and adds 1 to the overflow).  A recorded track appends (t, anchor) to its ring (unless the
+ *     clock is bad), dropping the oldest sample once the ring holds `window`; its record takes the frame as last_seen;
+ *   - the fit runs over the ring's samples whose projection is valid (n of them), oldest first, with tau_i = t_i - t of
+ *     the newest of them: mt = (sum tau_i) / n, mX = (sum X_i) / n, mY likewise, each sum left to right from 0.0;
+ *     Stt = sum (tau_i - mt) * (tau_i - mt), StX = sum (tau_i - mt) * (X_i - mX), StY likewise; vX = StX / Stt,
+ *     vY = StY / Stt, speed = sqrt(vX * vX + vY * vY).  There is an estimate iff n >= min_samples and Stt > 0;
+ *   - then every record with frame - last_seen > forget_after is dropped.
+ * Outputs per entry [B, max_out]: kin fp32 [B, max_out, 5] = (X, Y, vX, vY, speed): X, Y this frame's anchor projected
+ *   (NaN when invalid or absent), vX, vY, speed NaN without an estimate; samples int32 = n for a recorded present track,
+ *   else 0.
+ * lwdetr_speed_create: num_streams >= 1, parameters validated; one device allocation on the current device (the rings
+ *   take num_streams * capacity * window * 24 bytes), every stream at frame 1 with H the identity.  Synchronous.
+ * lwdetr_speed_destroy: frees the object.
+ * lwdetr_speed_set: one stream's H from a HOST [9] array; a non-finite H or a singular one (its determinant
+ *   h0 (h4 h8 - h5 h7) - h1 (h3 h8 - h5 h6) + h2 (h3 h7 - h4 h6) is 0 or not finite) is an error and nothing changes.
+ *   The history is kept.  Synchronous: it waits for the object's last launch and nothing else on the device; not callable
+ *   during a stream capture.
+ * lwdetr_speed_reset: the n streams listed (HOST; distinct and in [0, num_streams), else an error and nothing happens)
+ *   back to frame 1, no records, zero counters, t_last = -inf; H is kept.  Stream-ordered.
+ * lwdetr_speed_update: one frame for each of B streams (stream_ids HOST, distinct and in [0, num_streams)); ids int32
+ *   [B, max_out], boxes fp32 [B, max_out, 4] (16-byte aligned), counts int32 [B]: lwdetr_track's outputs; max_out in
+ *   [1, 1024]; timestamps as above.  All DEVICE; asynchronous, nothing allocated or copied per call, safe to capture in a
+ *   CUDA graph.
+ * lwdetr_speed_export: one stream, synchronous: it waits for the object's last launch and nothing else on the device.
+ *   head = (frame, records, overflow, clock_errors), last_t, homography [9]; then up to cap records in ascending id:
+ *   ids, last_seen, counts (samples in the ring) int32 [cap] and samples float64 [cap][window][3] (t, x, y), oldest
+ *   first, the rest of each record's rows untouched. */
+typedef struct lwdetr_speed lwdetr_speed;
+LWDETR_API int lwdetr_speed_create(int num_streams, int capacity, int window, int min_samples, int forget_after, int anchor,
+                                   double frame_rate, lwdetr_speed** out);
+LWDETR_API void lwdetr_speed_destroy(lwdetr_speed* s);
+LWDETR_API int lwdetr_speed_set(lwdetr_speed* s, int stream_id, const double* homography);
+LWDETR_API int lwdetr_speed_reset(lwdetr_speed* s, const int32_t* streams, int n, void* stream);
+LWDETR_API int lwdetr_speed_update(lwdetr_speed* s, const int32_t* ids, const float* boxes, const int32_t* counts, int B, int max_out,
+                                   const int32_t* stream_ids, const double* timestamps, float* kin, int32_t* samples, void* stream);
+LWDETR_API int lwdetr_speed_export(lwdetr_speed* s, int stream_id, int32_t head[4], double* last_t, double* homography, int32_t* ids,
+                                   int32_t* last_seen, int32_t* counts, double* samples, int cap);
+
 /* The LWDETR_F16_E4M3 mode's two kernels.
  * lwdetr_layernorm_e4m3: fp16 rows x [rows, ldx] -> e4m3 codes q [rows, ldq] (uint8) and fp32 row_scale [rows], as the mode's
  *   activation contract above (x^ without the LayerNorm affine, eps as given).  C % 8 == 0, C <= 1024, ldx and ldq

@@ -889,6 +889,135 @@ class Zones(_DeviceObject):
                     entry=raw["entry"][:, :Z].copy())
 
 
+def homography(src, dst):
+    """The 3x3 float64 homography H that maps four (x, y) frame pixels `src` to four ground points `dst` (metres, say):
+    the 8x8 system of cv2.getPerspectiveTransform (h8 = 1) solved in float64, then H scaled by -1 if needed so that
+    w = h6 x + h7 y + h8 > 0 at the centroid of src (lwdetr_speed's side of the horizon).  ValueError unless both are
+    four finite points with no three of either collinear."""
+    import numpy as np
+    src, dst = np.asarray(src, np.float64), np.asarray(dst, np.float64)
+    for name, p in (("src", src), ("dst", dst)):
+        if p.shape != (4, 2) or not np.isfinite(p).all():
+            raise ValueError("homography: %s must be four finite (x, y) points, got shape %s" % (name, p.shape))
+        for i in range(4):
+            a, b, c = (p[k] for k in range(4) if k != i)
+            if (b[0] - a[0]) * (c[1] - a[1]) - (b[1] - a[1]) * (c[0] - a[0]) == 0:
+                raise ValueError("homography: three points of %s are collinear" % name)
+    A = np.zeros((8, 8))
+    rhs = np.zeros(8)
+    for i, ((x, y), (u, v)) in enumerate(zip(src, dst)):
+        A[i] = (x, y, 1, 0, 0, 0, -x * u, -y * u)
+        A[i + 4] = (0, 0, 0, x, y, 1, -x * v, -y * v)
+        rhs[i], rhs[i + 4] = u, v
+    try:
+        H = np.append(np.linalg.solve(A, rhs), 1.0).reshape(3, 3)
+    except np.linalg.LinAlgError:
+        raise ValueError("homography: the points give a singular system") from None
+    cx, cy = src.mean(0)
+    if H[2, 0] * cx + H[2, 1] * cy + H[2, 2] < 0:
+        H = -H
+    return H
+
+
+def _check_homography(H):
+    """H as a contiguous float64 [3, 3] array, with lwdetr_speed_set's checks (finite, determinant neither 0 nor
+    non-finite, in the header's order of operations); else ValueError."""
+    import numpy as np
+    h = np.ascontiguousarray(np.asarray(H, np.float64))
+    if h.shape != (3, 3):
+        raise ValueError("SpeedEstimator.set: the homography must be [3, 3], got %s" % (h.shape,))
+    if not np.isfinite(h).all():
+        raise ValueError("SpeedEstimator.set: the homography has a non-finite entry")
+    f = [float(v) for v in h.reshape(-1)]
+    det = f[0] * (f[4] * f[8] - f[5] * f[7]) - f[1] * (f[3] * f[8] - f[5] * f[6]) + f[2] * (f[3] * f[7] - f[4] * f[6])
+    if det == 0.0 or not np.isfinite(det):
+        raise ValueError("SpeedEstimator.set: the homography is singular")
+    return h
+
+
+class SpeedEstimator(_DeviceObject):
+    """Ground-plane position, velocity and speed of each track per camera stream on the device (lwdetr_speed_*, the
+    contract in include/lwdetr_b200.h, restated in tools/speed_spec.py): supervision's speed estimation, fed by
+    Tracker.update.  capacity (records per stream, default 1024), window (samples per track, default 30), min_samples
+    (default 15), forget_after (frames, default 30), anchor (an anchor index or a name of ANCHORS, default
+    "bottom_center"), frame_rate (the clock of frames without timestamps, default 30).  Each stream's homography maps
+    frame pixels to ground units (set(); default the identity: pixels per second).  All calls of one object must run on
+    one CUDA stream (the current one at each call)."""
+
+    RESET, DESTROY = "lwdetr_speed_reset", "lwdetr_speed_destroy"
+
+    def __init__(self, num_streams, device=None, capacity=1024, window=30, min_samples=15, forget_after=30, anchor="bottom_center",
+                 frame_rate=30.0):
+        import torch
+        if isinstance(anchor, str):
+            anchor = ANCHORS.index(anchor)
+        self.num_streams = int(num_streams)
+        self.capacity, self.window = int(capacity), int(window)
+        self.min_samples, self.forget_after, self.anchor = int(min_samples), int(forget_after), int(anchor)
+        self.frame_rate = float(frame_rate)
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self._t = _vp()
+        with torch.cuda.device(self.device):
+            check(lib().lwdetr_speed_create(self.num_streams, self.capacity, self.window, self.min_samples, self.forget_after,
+                                            self.anchor, self.frame_rate, ctypes.byref(self._t)), "lwdetr_speed_create")
+
+    def set(self, stream, homography):
+        """Replaces one stream's homography (a [3, 3] array, frame pixels -> ground units; checked before any device call).
+        The history is kept.  Synchronous: waits for this object's last launch only.  Not during a stream capture."""
+        stream = int(stream)
+        if not 0 <= stream < self.num_streams:
+            raise ValueError("SpeedEstimator.set: stream %d outside [0, %d)" % (stream, self.num_streams))
+        h = _check_homography(homography)
+        check(lib().lwdetr_speed_set(self._t, stream, h.ctypes.data_as(_vp)), "lwdetr_speed_set")
+
+    def update(self, ids, boxes, counts, stream_ids=None, timestamps=None):
+        """One frame for each of B distinct streams, on Tracker.update's outputs as they are: ids int32 [B, max_out], xyxy
+        boxes fp32 [B, max_out, 4], counts [B] (CUDA; stream_ids default range(B)); timestamps: float64 [B] seconds (CUDA
+        tensor, or a host sequence) or None (frame / frame_rate) -> (kin fp32 [B, max_out, 5] = (X, Y, vX, vY, speed),
+        samples int32 [B, max_out]).  Stream-ordered, no synchronisation (a host timestamps sequence is copied to the
+        device first); graph-safe with a CUDA tensor or None."""
+        import torch
+        B, m = ids.shape
+        if tuple(boxes.shape) != (B, m, 4) or tuple(counts.shape) != (B,):
+            raise RuntimeError("SpeedEstimator.update: ids %s, boxes %s and counts %s do not describe one [B, max_out] set"
+                               % (tuple(ids.shape), tuple(boxes.shape), tuple(counts.shape)))
+        dev = self.device
+        ids = ids.to(device=dev, dtype=torch.int32).contiguous()
+        boxes = boxes.to(device=dev, dtype=torch.float32).contiguous()
+        counts = counts.to(device=dev, dtype=torch.int32).contiguous()
+        if timestamps is not None:
+            timestamps = torch.as_tensor(timestamps, dtype=torch.float64).to(dev).contiguous()
+            if tuple(timestamps.shape) != (B,):
+                raise RuntimeError("SpeedEstimator.update: timestamps must be [%d], got %s" % (B, tuple(timestamps.shape)))
+        sids = self._stream_ids(stream_ids, B, "SpeedEstimator.update")
+        kin = torch.empty(B, m, 5, device=dev, dtype=torch.float32)
+        samples = torch.empty(B, m, device=dev, dtype=torch.int32)
+        check(lib().lwdetr_speed_update(self._t, ptr(ids), ptr(boxes), ptr(counts), B, m, ctypes.cast(sids, _vp),
+                                        ptr(timestamps) if timestamps is not None else None, ptr(kin), ptr(samples), stream_ptr(dev)),
+              "lwdetr_speed_update")
+        return kin, samples
+
+    def export(self, stream):
+        """Synchronous, waiting for this object's last update() or reset() and for nothing else on the device: one stream's
+        state as a dict: frame, records, overflow, clock_errors, last_t, homography float64 [3, 3], and the records in
+        ascending id: ids, last_seen int32 [n], and samples, a list of float64 [n_i, 3] arrays (t, x, y), oldest first."""
+        import numpy as np
+        cap, W = self.capacity, self.window
+        head = (ctypes.c_int32 * 4)()
+        last_t = ctypes.c_double()
+        H = np.zeros(9, np.float64)
+        ids = np.zeros(cap, np.int32)
+        seen = np.zeros(cap, np.int32)
+        counts = np.zeros(cap, np.int32)
+        samples = np.zeros((cap, W, 3), np.float64)
+        check(lib().lwdetr_speed_export(self._t, int(stream), ctypes.cast(head, _vp), ctypes.byref(last_t), H.ctypes.data_as(_vp),
+                                        ids.ctypes.data_as(_vp), seen.ctypes.data_as(_vp), counts.ctypes.data_as(_vp),
+                                        samples.ctypes.data_as(_vp), cap), "lwdetr_speed_export")
+        n = head[1]
+        return dict(frame=head[0], records=n, overflow=head[2], clock_errors=head[3], last_t=last_t.value, homography=H.reshape(3, 3),
+                    ids=ids[:n].copy(), last_seen=seen[:n].copy(), samples=[samples[i, :counts[i]].copy() for i in range(n)])
+
+
 LABEL_NAME, LABEL_ID, LABEL_SCORE = 1, 2, 4
 ANNOTATOR_OPTIONS = ("thickness", "text_scale", "box_fill_alpha", "label", "zone_fill_alpha", "zone_thickness", "privacy_block")
 

@@ -25,6 +25,7 @@
 #include "msda.h"
 #include "resize.h"
 #include "rowops.h"
+#include "speed.h"
 #include "tiles.h"
 #include "track.h"
 #include "zones.h"
@@ -779,6 +780,117 @@ int lwdetr_zones_export(lwdetr_zones* z, int stream_id, int32_t frame_overflow[2
   info[0] = L;
   info[1] = Z;
   info[2] = h.n;
+  return 0;
+}
+
+struct lwdetr_speed {
+  lwb::SpeedTable table;
+  DeviceState state;
+};
+
+int lwdetr_speed_create(int num_streams, int capacity, int window, int min_samples, int forget_after, int anchor, double frame_rate,
+                        lwdetr_speed** out) {
+  if (!out) return fail("lwdetr_speed_create: null pointer");
+  if (num_streams < 1) return fail("lwdetr_speed_create: num_streams must be >= 1");
+  if (capacity < 1 || capacity > lwb::SPEED_CAPACITY) return fail("lwdetr_speed_create: capacity must be in [1, 4096]");
+  if (window < 2 || window > lwb::SPEED_WINDOW) return fail("lwdetr_speed_create: window must be in [2, 64]");
+  if (min_samples < 2 || min_samples > window) return fail("lwdetr_speed_create: min_samples must be in [2, window]");
+  if (forget_after < 0) return fail("lwdetr_speed_create: forget_after must be >= 0");
+  if (anchor < 0 || anchor > 8) return fail("lwdetr_speed_create: anchor must be in [0, 9)");
+  if (!std::isfinite(frame_rate) || frame_rate <= 0.0) return fail("lwdetr_speed_create: frame_rate must be finite and > 0");
+  std::unique_ptr<lwdetr_speed> s(new (std::nothrow) lwdetr_speed{});
+  if (!s) return fail("lwdetr_speed_create: out of memory");
+  lwb::SpeedTable& t = s->table;
+  t.num_streams = num_streams;
+  t.capacity = capacity;
+  t.window = window;
+  t.min_samples = min_samples;
+  t.forget_after = forget_after;
+  t.anchor = anchor;
+  t.frame_rate = frame_rate;
+  const size_t ns = static_cast<size_t>(num_streams), cap = static_cast<size_t>(capacity);
+  // every stream at frame 1, no records, no timestamp yet, H the identity
+  const std::vector<lwb::SpeedHead> h(ns, lwb::SpeedHead{1, 0, 0, 0, -HUGE_VAL});
+  std::vector<double> H(ns * 9, 0.0);
+  for (size_t i = 0; i < ns; ++i) H[i * 9] = H[i * 9 + 4] = H[i * 9 + 8] = 1.0;
+  const auto layout = [&](Carver& c) {
+    c.take(t.head, ns);
+    c.take(t.homography, ns * 9);
+    c.take(t.index, ns * cap);
+    c.take(t.rec, ns * cap);
+    c.take(t.ring, ns * cap * static_cast<size_t>(window) * 3);
+  };
+  const auto init = [&] {
+    cudaError_t e = cudaMemcpyAsync(t.head, h.data(), ns * sizeof(lwb::SpeedHead), cudaMemcpyHostToDevice, s->state.copy);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(t.homography, H.data(), H.size() * sizeof(double), cudaMemcpyHostToDevice, s->state.copy);
+    return e;
+  };
+  if (int rc = s->state.create("lwdetr_speed_create", layout, init)) return rc;
+  *out = s.release();
+  return 0;
+}
+
+void lwdetr_speed_destroy(lwdetr_speed* s) { delete s; }
+
+int lwdetr_speed_set(lwdetr_speed* s, int stream_id, const double* homography) {
+  if (!s || !homography) return fail("lwdetr_speed_set: null pointer");
+  const lwb::SpeedTable& t = s->table;
+  if (stream_id < 0 || stream_id >= t.num_streams) return fail("lwdetr_speed_set: stream id outside [0, num_streams)");
+  const double* h = homography;
+  for (int i = 0; i < 9; ++i)
+    if (!std::isfinite(h[i])) return fail("lwdetr_speed_set: the homography has a non-finite entry");
+  const double det = h[0] * (h[4] * h[8] - h[5] * h[7]) - h[1] * (h[3] * h[8] - h[5] * h[6]) + h[2] * (h[3] * h[7] - h[4] * h[6]);
+  if (det == 0.0 || !std::isfinite(det)) return fail("lwdetr_speed_set: the homography is singular");
+  const cudaError_t e = s->state.write({{t.homography + static_cast<size_t>(stream_id) * 9, h, 9 * sizeof(double)}});
+  return e == cudaSuccess ? 0 : cuda_fail(e, "lwdetr_speed_set");
+}
+
+int lwdetr_speed_reset(lwdetr_speed* s, const int32_t* streams, int n, void* stream) {
+  return reset_call("lwdetr_speed_reset", s, streams, n, stream, lwb::speed_reset_launch);
+}
+
+int lwdetr_speed_update(lwdetr_speed* s, const int32_t* ids, const float* boxes, const int32_t* counts, int B, int max_out,
+                        const int32_t* stream_ids, const double* timestamps, float* kin, int32_t* samples, void* stream) {
+  if (!s || !ids || !boxes || !counts || !stream_ids || !kin || !samples) return fail("lwdetr_speed_update: null pointer");
+  if (B < 1 || max_out < 1 || max_out > lwb::SPEED_MAX_OUT) return fail("lwdetr_speed_update: need B >= 1 and max_out in [1, 1024]");
+  if (reinterpret_cast<uintptr_t>(boxes) % 16) return fail("lwdetr_speed_update: boxes must be 16-byte aligned");
+  const std::string err = check_ids(s->table.num_streams, stream_ids, B);
+  if (!err.empty()) return fail("lwdetr_speed_update: " + err);
+  return s->state.launch("lwdetr_speed_update", stream, [&](cudaStream_t st) {
+    return lwb::speed_launch(s->table, ids, boxes, counts, B, max_out, stream_ids, timestamps, kin, samples, st);
+  });
+}
+
+int lwdetr_speed_export(lwdetr_speed* s, int stream_id, int32_t head[4], double* last_t, double* homography, int32_t* ids,
+                        int32_t* last_seen, int32_t* counts, double* samples, int cap) {
+  if (!s || !head || !last_t || !homography || (cap > 0 && (!ids || !last_seen || !counts || !samples)))
+    return fail("lwdetr_speed_export: null pointer");
+  const lwb::SpeedTable& t = s->table;
+  lwb::SpeedHead h;
+  if (int rc = s->state.read_head("lwdetr_speed_export", t.head, t.num_streams, stream_id, &h)) return rc;
+  const size_t st = static_cast<size_t>(stream_id), C = static_cast<size_t>(t.capacity), W = static_cast<size_t>(t.window);
+  std::vector<lwb::RecordIndex> idx(static_cast<size_t>(h.n));
+  std::vector<lwb::SpeedRec> rec(h.n ? C : 0);
+  std::vector<double> ring(h.n ? C * W * 3 : 0);
+  const cudaError_t e = s->state.read({{homography, t.homography + st * 9, 9 * sizeof(double)},
+                                       {idx.data(), t.index + st * C, idx.size() * sizeof(lwb::RecordIndex)},
+                                       {rec.data(), t.rec + st * C, rec.size() * sizeof(lwb::SpeedRec)},
+                                       {ring.data(), t.ring + st * C * W * 3, ring.size() * sizeof(double)}});
+  if (e != cudaSuccess) return cuda_fail(e, "lwdetr_speed_export");
+  for (int i = 0; i < h.n && i < cap; ++i) {
+    const size_t slot = static_cast<size_t>(idx[i].slot);
+    const lwb::SpeedRec r = rec[slot];
+    ids[i] = idx[i].id;
+    last_seen[i] = idx[i].last_seen;
+    counts[i] = r.n;
+    for (int k = 0; k < r.n; ++k)
+      for (int c = 0; c < 3; ++c) samples[(i * W + k) * 3 + c] = ring[(slot * W + (r.pos + k) % W) * 3 + c];
+  }
+  head[0] = h.frame;
+  head[1] = h.n;
+  head[2] = h.overflow;
+  head[3] = h.clock_errors;
+  *last_t = h.last_t;
   return 0;
 }
 

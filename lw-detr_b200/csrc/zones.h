@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "records.h"
+
 namespace lwb {
 
 constexpr int ZONE_LINES = 32, ZONE_POLYS = 32, ZONE_POLY_VERTS = 256, ZONE_VERTS = 2048;
@@ -19,9 +21,7 @@ struct ZoneGeom {                        // per stream; vertices in ZoneTable::v
   int32_t start[ZONE_POLYS + 1];         // polygon p: vertices [start[p], start[p + 1])
 };
 
-struct ZoneIndex {                       // per record, sorted by id
-  int32_t id, slot, last_seen;
-};
+using ZoneIndex = RecordIndex;           // per record, sorted by id
 
 struct ZoneRec {                         // per slot
   uint32_t inside, side_set, side_pos;   // side of line l: 0 unless bit l of side_set, else +1 / -1 by bit l of side_pos

@@ -207,7 +207,7 @@ class LWDETR(nn.Module):
     @torch.no_grad()
     def track(self, frames, tracker, streams=None, size=None, fit="stretch", short_side=None, max_side=None, colorspace=None,
               max_out=None, motion=None, appearance=False, reid=None, reid_size=(256, 128), reid_filter="bilinear", reid_mean=None,
-              reid_std=None, reid_normalize=True, zones=None, detect_every=1, flow=None, annotate=None):
+              reid_std=None, reid_normalize=True, zones=None, detect_every=1, flow=None, annotate=None, speed=None, timestamps=None):
         """Multi-object tracking of video streams: frames (RGB or NV12, taken exactly as detect() takes them) run as one
         forward; each query gives one detection, its best class (capi.query_best, boxes in the frame's original pixels);
         then capi.Tracker `tracker` (ByteTrack on the device, include/lwdetr_b200.h) updates each frame's stream.
@@ -247,6 +247,12 @@ class LWDETR(nn.Module):
         round's frames in place, from the device outputs as they are (Annotator.annotate: ids, labels and scores, and with
         zones= the lines, polygons, line totals and occupancy).  It adds no synchronisation; on flow frames it draws the
         flow's tracks.  The returned lists are the same with and without it.
+        speed: a capi.SpeedEstimator over the same streams; after each round's tracker (and zones) update it takes the
+        tracker's outputs as they are (SpeedEstimator.update) with that round's timestamps (timestamps: one per frame in
+        seconds, a host list or a CUDA float64 tensor; None: each stream's frame count / frame_rate), and each frame's dict
+        gains "position" (fp32 [c, 2], the ground point of each track's anchor, NaN beyond the horizon), "velocity" (fp32
+        [c, 2]) and "speed" (fp32 [c]; NaN before the track has min_samples samples).  No extra synchronisation; keyframes
+        and flow frames alike.  Not with motion=: a fixed image-to-ground homography has no meaning for a moving camera.
         How ByteTrack's thresholds (tuned on YOLOX scores) suit LW-DETR's score distribution, and whether the decoder's features tell identities apart on real footage, in MOTA / IDF1 / HOTA, is
         not measured here."""
         if self.training:
@@ -281,6 +287,14 @@ class LWDETR(nn.Module):
             raise RuntimeError("lwdetr_b200: detect_every > 1 needs flow= (a capi.BoxFlow)")
         if flow is not None and motion is not None and motion is not flow.estimator:
             raise RuntimeError("lwdetr_b200: motion= must be the flow's own estimator (only one estimator can hold a stream's pyramids)")
+        if speed is not None and motion is not None:
+            raise RuntimeError("lwdetr_b200: speed= needs a still camera (a fixed homography); it cannot go with motion=")
+        if timestamps is not None:
+            if speed is None:
+                raise RuntimeError("lwdetr_b200: timestamps= is for speed=")
+            timestamps = torch.as_tensor(timestamps, dtype=torch.float64).to(dev)
+            if tuple(timestamps.shape) != (n,):
+                raise RuntimeError("lwdetr_b200: %d timestamps for %d frames" % (timestamps.numel(), n))
         rounds, seen = [], {}
         key = [True] * n
         for i, s in enumerate(streams):
@@ -337,23 +351,32 @@ class LWDETR(nn.Module):
                     inside, occupancy, events, n_ev = zones.update(got[0], got[2], got[3], got[5], ids)
                     zo = (inside.long() & 0xFFFFFFFF, occupancy, events)      # the uint32 masks widened once per round
                     ev_counts.append(n_ev)
+                sp = None
+                if speed is not None:
+                    ts_rows = None
+                    if timestamps is not None:    # consecutive frames as a view: no copy
+                        ts_rows = timestamps[rows[0]:rows[-1] + 1] if rows == list(range(rows[0], rows[-1] + 1)) \
+                            else timestamps[torch.tensor(rows, device=dev)]
+                    sp = speed.update(got[0], got[3], got[5], ids, ts_rows)[0]
                 if annotate is not None:
                     annotate.annotate(fb.select(rows), got[1], got[2], got[3], ids=got[0], counts=got[5], streams=ids, zones=zones,
                                       occupancy=None if zones is None else occupancy)
                 for j, i in enumerate(rows):
-                    res[i] = (got, zo, j)
+                    res[i] = (got, zo, sp, j)
         both = torch.cat(counts + ev_counts).cpu().tolist()     # track and event counts in one read-back
         order = [i for rows in rounds for part in ([i for i in rows if key[i]], [i for i in rows if not key[i]]) for i in part]
         cnt = {i: c for i, c in zip(order, both[:n])}
         ecnt = {i: c for i, c in zip(order, both[n:])}
         dets = []
         for i in range(n):
-            (ids, sc, lab, bx, q, _), zo, j = res[i]
+            (ids, sc, lab, bx, q, _), zo, sp, j = res[i]
             c = cnt[i]
             d = {"ids": ids[j, :c], "scores": sc[j, :c], "labels": lab[j, :c].long(), "boxes": bx[j, :c], "queries": q[j, :c].long()}
             if zo is not None:
                 inside, occupancy, events = zo
                 d.update(inside=inside[j, :c], occupancy=occupancy[j], events=events[j, :min(ecnt[i], events.shape[1])])
+            if sp is not None:
+                d.update(position=sp[j, :c, 0:2], velocity=sp[j, :c, 2:4], speed=sp[j, :c, 4])
             dets.append(d)
         return dets
 
